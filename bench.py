@@ -39,7 +39,7 @@ def static_config(world: int) -> dict:
     return {"workload": WORKLOAD, "streams_per_gpu": 1, "kv_tokens_start": KV_START, "tokens_per_step": 11,
             "vit_dtype": "fp16 operands / fp32 accumulate",
             "parallelism": f"replicas x{world} (weights broadcast at init, no hot-path collective)",
-            "l2": "inputs larger than L2: every step streams 15.0 GB of weights + 1.6 GB of KV (L2 = 126 MB)",
+            "l2": "inputs larger than L2: every step streams 15.0 GB of weights + 1.6 GB of KV (L2 = 50 MB)",
             "pipelining": "ViT+connector of the NEXT frames on a side CUDA stream during the decoder steps of the current ones "
                           "(same work per frame; --encode-ahead frames per ViT pass, default 1: the next frame, as a live "
                           "camera delivers it)"}
@@ -64,11 +64,11 @@ def _peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1468.8))), "measured"
-    return 6650.0, 1400.0, "fallback"
+    return 3350.0, 989.0, "datasheet (H100 SXM, 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -241,6 +241,21 @@ def run_reference_arm(args):
     return line
 
 
+def dump_outputs(out_dir, step_out, frame_embeds, dec):
+    """The last timed step's results as a caller of Engine.step receives them, as float32 / float64 .npy files
+    (about 0.7 MB for Llama-3-8B): the last-position logits [1, vocab], the 10 frame-token embeddings the step
+    consumed [10, hidden] (ViT + connector of the last frame) and the on-device decision."""
+    import numpy as np
+    import torch
+    d = pathlib.Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(d / "logits.npy", step_out[0].float().cpu().numpy())
+    np.save(d / "frame_embeds.npy", frame_embeds.float().cpu().numpy())
+    np.save(d / "decision.npy", np.array([dec.argmax_id, dec.argmax_excl_id, dec.argmax_prob_id, dec.p_interval, dec.max_logit,
+                                          dec.top2_margin, dec.lse], dtype=np.float64))
+
+
 # ----------------------------------------------------------------------------- our arm
 def run_engine_arm(args):
     import torch
@@ -334,6 +349,7 @@ def run_engine_arm(args):
             evs[slot].record(side)
 
     pre_evs = [torch.cuda.Event(), torch.cuda.Event()]
+    last_out = [None]     # (logits, decisions) returned by the most recent Engine.step of pipelined()
 
     def pipelined(n, base, from_host=False, read_back=False, step_fn=None):
         """n frame steps; the ViT runs D frames at a time on the side stream, one group ahead of the decoder"""
@@ -354,7 +370,7 @@ def run_engine_arm(args):
                 step_fn(i, fe[10 * j:10 * j + 10])
             else:
                 packed[1:] = fe[10 * j:10 * j + 10]
-                eng.step([sid], [11], packed, row_ids=prefix, want_logits=True)
+                last_out[0] = eng.step([sid], [11], packed, row_ids=prefix, want_logits=True)
             if j == 0 and g + 1 < n_groups:
                 encode_on_side(base + (g + 1) * D, (g + 1) & 1, from_host, after=pre_evs[g & 1], count=min(D, n - (g + 1) * D))
             if read_back:
@@ -378,6 +394,8 @@ def run_engine_arm(args):
     launches = eng.launch_count() - l0
     clocks = sampler.stop() if rank == 0 else None
     kv_end = eng.kv_len(sid)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out[0], packed[1:], eng.read_decisions(1)[0])
 
     # ---- end-to-end timing through the public API with host frames (e2e): pinned-host frame copied in and the
     #      32-byte decision read back (one sync) every step
@@ -489,9 +507,9 @@ def run_engine_arm(args):
                 "method": "CUDA events around 4 back-to-back passes of the 128 decoder GEMM launches (q|k|v, o, gate|up, down of all 32 layers) on the engine's buffers, T=11",
                 "in_step_event_bracketed": {"achieved": gs["achieved_gbs"], "avg_us_per_launch": gs["avg_us_per_launch"],
                                             "note": "per-launch event pairs inside the step (PDL off): includes ~3-5 us bracket overhead per launch"}}
-        roof_attn = {"bound": "hbm", "kernel": "attn_tc_kernel + attn_merge_kernel (KV-append attention on tcgen05, one launch pair per layer; attn_tc2_kernel, P in TMEM + key-sliced softmax, takes over from 24k keys)",
+        roof_attn = {"bound": "hbm", "kernel": "attn_kvappend_kernel + attn_merge_kernel (KV-append attention, TMA-fed mma.sync, one launch pair per layer)",
                      "achieved": micro_attn["achieved_gbs"], "peak": hbm_peak, "unit": "GB/s", "frac": micro_attn["achieved_gbs"] / hbm_peak,
-                     "peak_source": which, "traffic": _ncu_traffic("attn_tc")[0], "traffic_commit": _ncu_traffic("attn_tc")[1], "avg_us_per_launch": micro_attn["us_per_launch_incl_merge"],
+                     "peak_source": which, "traffic": _ncu_traffic("attn_kvappend")[0], "traffic_commit": _ncu_traffic("attn_kvappend")[1], "avg_us_per_launch": micro_attn["us_per_launch_incl_merge"],
                      "algo_bytes_per_launch": micro_attn["algo_bytes_per_launch"],
                      "method": "CUDA events around 4x32 back-to-back launch pairs over the 32 layers' caches (1.6 GB, > L2), q=11, kv=12011; merge kernel time included",
                      "main_kernel_only": {"achieved": micro_attn["achieved_gbs_main_only"], "frac": micro_attn["achieved_gbs_main_only"] / hbm_peak,
@@ -765,9 +783,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", dest="no_cpu_baseline", action="store_true")
     ap.add_argument("--encode-ahead", dest="encode_ahead", type=int, default=1,
                     help="frames per encode-ahead ViT pass on the side stream (1 = one frame at a time: the small-tile ViT "
-                         "co-resides with the decoder step; >= 3 = 2-CTA tensor-bound GEMMs, serialised against the step)")
+                         "runs next to the decoder step; >= 3 = wider token tiles for the tensor-bound batch)")
     ap.add_argument("--no-extras", dest="extras", action="store_false", help="skip the side measurements of the other BASELINE configs")
     ap.add_argument("--quick-extras", dest="quick_extras", action="store_true", help="shorter side measurements (dev runs)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (last-position logits, the frame "
+                         "embeddings it consumed, the decision) as DIR/<name>.npy, to compare two builds output for output")
     args = ap.parse_args()
     with _StdoutToStderr() as guard:
         line = run_reference_arm(args) if args.impl == "reference" else run_engine_arm(args)

@@ -1,5 +1,5 @@
 /*
- * vlo_b200.h — C ABI of libvlo_b200.so, the B200-native (sm_100a) engine for the per-frame hot
+ * vlo_b200.h — C ABI of libvlo_b200.so, the native CUDA engine (H100, sm_90a) for the per-frame hot
  * loop of showlab/videollm-online.
  *
  * The reference has no FFI: its seam is the Python duck-typed API of demo/inference.py and
@@ -71,7 +71,7 @@ long long vlo_launch_count(void);
 #define VLO_PROF_NUM_CLASSES 6
 int vlo_profile_enable(int on);
 int vlo_profile_read(double* ms, long long* launches, double* algo_bytes, int n_classes);
-/* 1 when the device is an sm_100 part the kernels can run on */
+/* 1 when the device is an sm_90 (Hopper) part the kernels can run on */
 int vlo_device_supported(int device);
 
 /* ------------------------------------------------------------------ engine life cycle
@@ -156,7 +156,7 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
 
 /* ------------------------------------------------------------------ kernel-level entry points
  * (used by the parity tests and micro-benchmarks; same kernels the engine launches) */
-/* C = A[rows_a,k] * B[rows_b,k]^T on tcgen05; see csrc/gemm.cuh for fmt/epi/act codes */
+/* C = A[rows_a,k] * B[rows_b,k]^T on wgmma; see csrc/gemm.cuh for fmt/epi/act codes */
 int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a, const void* d_b, int rows_b, int k,
                 void* d_out, int ld_out, const float* d_bias, const float* d_pos, int pos_rows, int splits,
                 long long split_stride, int bn, void* cuda_stream);
@@ -168,24 +168,14 @@ int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
                    void* cuda_stream);
-/* 2-CTA (tcgen05 cta_group::2) tensor-bound GEMM of the ViT trunk at batch >= 3 (csrc/gemm2.cuh), fp16:
- *   epi 0: out16[rows_x][ld_out] = act(fp16(X W^T + bias));  epi 1: out32[rows_x][ld_out] += fp16(X W^T + bias)
- *   (the fp32 residual stream).  bn = 256 | 128 features per CTA-pair tile; rows_w % 32 == 0; d_bias required.
- * Replaces the cuBLAS GEMMs of HF:models/siglip/modeling_siglip.py:285-287, 309, 323-327. */
-int vlo_op_gemm2(const void* d_x, int rows_x, const void* d_w, int rows_w, int k, void* d_out, int ld_out, const float* d_bias,
-                 int act, int epi, int bn, void* cuda_stream);
 /* KV-append attention over one layer's cache (the graded kernel, K15):
  *   d_q bf16 [n_tok, n_heads, head_dim] (RoPE applied); d_k/d_v bf16 [n_kv_heads, kv_stride, head_dim];
  *   keys 0..kv_len-1 valid, the n_tok query tokens sit at positions kv_len-n_tok .. kv_len-1 (causal with
  *   offset, HF:masking_utils.py:263-272); d_out bf16 [n_tok, n_heads*head_dim]; d_ws fp32 scratch of
  *   vlo_op_attn_ws_bytes(). Replaces HF:models/llama/modeling_llama.py:272-285 (SDPA / flash-attn 2). */
-/* which generation of the KV-append attention kernel runs for this head layout: 3 = tcgen05 with P in TMEM and a
- * 192 KB K/V ring (csrc/attn_tc2.cuh, default), 2 = tcgen05 with P in shared memory (csrc/attn_tc.cuh, VLO_ATTN=2),
- * 1 = mma.sync (csrc/attn.cuh; forced by VLO_ATTN=1, or when n_heads/n_kv_heads does not divide 128) */
+/* which generation of the KV-append attention kernel runs for this head layout: 1 = mma.sync over TMA-loaded
+ * K / V blocks (csrc/attn.cuh), the only one */
 int vlo_op_attn_version(int n_heads, int n_kv_heads);
-/* developer aid: with VLO_ATTN_TRACE=1 the tcgen05 attention kernel records clock64 stamps per CTA and role
- * ([cta][3 roles][64]); this copies the first n values to the host (tools/gpu_attn_trace.py). */
-int vlo_debug_attn_trace(long long* h_out, int n);
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len);
 int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void* d_out, float* d_ws, int n_tok,
                          int n_heads, int n_kv_heads, int head_dim, int kv_len, long long kv_stride, void* cuda_stream);

@@ -9,7 +9,7 @@ import vlo_bootstrap  # noqa: E402,F401  registers `videollm_online_b200`
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 @pytest.fixture(scope="session")

@@ -308,5 +308,30 @@ def main():
         print(k, tuple(v.shape) if isinstance(v, torch.Tensor) else v)
 
 
+@torch.no_grad()
+def host_delta():
+    """tests/golden/host_reference_delta.pt: the reference's chunked-forward logits, last-layer K / V and joint-forward logits
+    computed on THIS host, stored as the elements that differ from tiny_reference.pt (index, value) per tensor."""
+    g = torch.load(OUT / "tiny_reference.pt", weights_only=False)
+    cfg = tiny_config()
+    llm_state = W.synthetic_llm_state(cfg, seed=0)
+    llm_state["lm_head.weight"] = (llm_state["lm_head.weight"].float() * 8).to(torch.bfloat16)
+    model, _, _ = build_reference_model(cfg, llm_state, W.synthetic_vision_state(cfg, seed=1))
+    cache, off, logits = None, 0, []
+    for c in g["step_chunks"].tolist():
+        out = model(inputs_embeds=g["step_embeds"][None, off:off + c], use_cache=True, past_key_values=cache)
+        cache = out.past_key_values
+        logits.append(out.logits[0].clone())
+        off += c
+    L = cfg.num_hidden_layers - 1
+    here = {"step_logits": torch.cat(logits, 0), "kv_kL": cache.layers[L].keys[0].clone(), "kv_vL": cache.layers[L].values[0].clone(),
+            "joint_logits": model(input_ids=g["joint_ids"], frames=g["frames"][:2], use_cache=False).logits[0].clone()}
+    fx = {}
+    for k, v in here.items():
+        idx = (v != g[k]).flatten().nonzero().flatten()
+        fx[k] = (idx.to(torch.int32), v.flatten()[idx].clone())
+    torch.save(fx, OUT / "host_reference_delta.pt")
+
+
 if __name__ == "__main__":
-    main()
+    host_delta() if "--host-delta" in sys.argv else main()

@@ -1,5 +1,5 @@
 """Dev tool: the decoder step ALONE (no ViT) at a 12k-token cache: q = 11 frame steps and q = 1 AR steps, device-timed.
-One JSON line; run once per environment setting (VLO_FUSE, VLO_WS_STAGES, VLO_WSF_STAGES, VLO_ATTN, ...)."""
+One JSON line; run once per environment setting (VLO_FUSE, VLO_WS_STAGES, VLO_WSF_STAGES, ...)."""
 import json, os, pathlib, sys
 import torch
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parents[1]))

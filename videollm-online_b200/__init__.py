@@ -1,4 +1,4 @@
-"""videollm_online_b200 — B200-native (sm_100a) engine for VideoLLM-online's per-frame hot loop.
+"""videollm_online_b200 — native CUDA (H100, sm_90a) engine for VideoLLM-online's per-frame hot loop.
 
 The directory is named `videollm-online_b200/`; import it as `videollm_online_b200` via the
 repo-root bootstrap (`import vlo_bootstrap`), which registers this package under that name.

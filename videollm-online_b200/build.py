@@ -1,8 +1,8 @@
-"""In-tree build of libvlo_b200.so (hand-written sm_100a CUDA behind a C ABI).
+"""In-tree build of libvlo_b200.so (hand-written sm_90a CUDA for the H100 behind a C ABI).
 
-nvcc cross-compiles for sm_100a without a GPU, so this runs in the CPU-only dev
-container; the resulting .so is git-ignored but travels to the GPU box with the
-gpurun snapshot.  Also builds nothing else: the oracle is pure Python/torch.
+nvcc cross-compiles for sm_90a without a GPU, so the library can be built on a machine
+without one; the resulting .so is git-ignored.  Builds nothing else: the oracle is pure
+Python/torch.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ LIB = PKG / "libvlo_b200.so"
 INCLUDE = PKG.parent / "include"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -44,14 +44,14 @@ def _stale(target: pathlib.Path, deps: list[pathlib.Path]) -> bool:
 
 def build(force: bool = False, verbose: bool = False, debug: bool = False) -> pathlib.Path:
     """debug=True: a second library (libvlo_b200_dbg.so, objects in build_dbg/) whose bounded mbarrier waits trap after
-    2^16 polls instead of 2^24, so a protocol dead-lock reports the stuck (block, thread) within seconds; select it with
-    VLO_LIB=.../libvlo_b200_dbg.so."""
+    2^16 polls instead of 2^24 and print the stuck (block, thread) first, so a protocol dead-lock is reported within
+    seconds; select it with VLO_LIB=.../libvlo_b200_dbg.so."""
     global OBJ, LIB
     nvcc = _nvcc()
     flags_extra = []
     if debug:
         OBJ, LIB = PKG / "build_dbg", PKG / "libvlo_b200_dbg.so"
-        flags_extra = ["-DVLO_MBAR_BOUND_LOG2=16"]
+        flags_extra = ["-DVLO_MBAR_BOUND_LOG2=16", "-DVLO_MBAR_TRACE=1"]
     OBJ.mkdir(exist_ok=True)
     headers = sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + sorted(INCLUDE.glob("*.h"))
     sources = sorted(CSRC.glob("*.cu"))

@@ -1,10 +1,8 @@
 // Host side of the KV-append attention: chunking of sequences into <=64-row work items,
-// split-KV planning (one wave of CTAs over the 148 SMs), workspace layout and launches.
+// split-KV planning (one wave of CTAs over the SMs), workspace layout and launches.
 // The plan depends only on (q_len, kv_len) of the sequences, so a decoder step builds and
 // uploads it once and reuses it for all layers.
 #include "attn.cuh"
-#include "attn_tc.cuh"
-#include "attn_tc2.cuh"
 
 #include <cmath>
 #include <cstdlib>
@@ -16,57 +14,34 @@
 namespace vlo {
 
 namespace {
-constexpr int kNumSMs = 148;
 constexpr size_t kAlign = 256;
 size_t align_up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
 
 int max_chunks(int total_tokens, int n_seqs, int G) {
-  const int per = std::max(1, 64 / G);  // v1 chunking (v2 packs twice as many tokens per item)
+  const int per = std::max(1, 64 / G);
   return total_tokens / per + n_seqs + 1;
 }
-// kernel generation: 3 = tcgen05 with P in TMEM and the deep K/V ring (attn_tc2.cuh, default), 2 = tcgen05 with P in
-// shared memory (attn_tc.cuh), 1 = mma.sync (attn.cuh).  VLO_ATTN=1|2 forces the older kernels (A/B checks).
-// Default (VLO_ATTN unset): by context length.  Same-box A/B (tools/gpu_r2_call6.sh / call7.sh): at 12k keys the two
-// tcgen05 kernels tie in the back-to-back loop (14.6 us) and generation 2 is 9 % faster inside the step (generation 3's
-// 192 KB prefetch before the grid dependency competes with the tail of the QKV GEMM); at 66k keys generation 3 wins
-// (46.1 vs 49.9 us, 0.90 of the HBM peak).
-int attn_version_impl(int G, int max_kv_len = 0) {
-  static int forced = -1;
-  if (forced < 0) {
-    const char* e = getenv("VLO_ATTN");
-    forced = (e != nullptr && e[0] == '1') ? 1 : ((e != nullptr && e[0] == '2') ? 2 : ((e != nullptr && e[0] == '3') ? 3 : 0));
-  }
-  if (128 % G != 0) return 1;
-  if (forced > 0) return forced;
-  return max_kv_len >= 24576 ? 3 : 2;
-}
-// keys per pipeline block of the generation-3 kernel (64-key blocks were measured slower: per-block latency dominates)
-int attn_tc2_blk() { return 128; }
-size_t max_ctas(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
-  return static_cast<size_t>(kNumSMs) + static_cast<size_t>(n_kv_heads) * max_chunks(total_tokens, n_seqs, n_heads / n_kv_heads);
-}
-// Per item n_splits <= max(1, 148 / (n_kv_heads * n_items)) and rows <= 64, so the sum of
-// n_kv_heads * n_splits * rows over all items is bounded by (148 + n_kv_heads * n_items) * 64.
+// Per item n_splits <= max(1, n_sms / (n_kv_heads * n_items)) and rows <= 64, so the sum of
+// n_kv_heads * n_splits * rows over all items is bounded by (n_sms + n_kv_heads * n_items) * 64.
 size_t cap_slots_for(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
   const int G = n_heads / n_kv_heads;
-  return static_cast<size_t>(kNumSMs + n_kv_heads * max_chunks(total_tokens, n_seqs, G)) * 128;
+  return static_cast<size_t>(num_sms() + n_kv_heads * max_chunks(total_tokens, n_seqs, G)) * 128;
 }
 }  // namespace
 
-int attn_version(int n_heads, int n_kv_heads) { return attn_version_impl(n_heads / n_kv_heads); }
+// one kernel generation: mma.sync m16n8k16 over TMA-loaded K / V blocks (attn.cuh)
+int attn_version(int, int) { return 1; }
 
 size_t attn_stage_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
   const int G = n_heads / n_kv_heads;
-  return align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens) +
-         align_up(sizeof(int) * max_ctas(total_tokens, n_seqs, n_heads, n_kv_heads));
+  return align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens);
 }
 
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
   const int G = n_heads / n_kv_heads;
   const size_t slots = cap_slots_for(total_tokens, n_seqs, n_heads, n_kv_heads);
   return align_up(slots * kAttnHD * 4) + align_up(slots * 2 * 4) +
-         align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens) +
-         align_up(sizeof(int) * max_ctas(total_tokens, n_seqs, n_heads, n_kv_heads));
+         align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens);
 }
 
 int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, int n_seqs, int total_tokens,
@@ -75,12 +50,8 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   VLO_CHECK(n_heads % n_kv_heads == 0, "n_heads must be a multiple of n_kv_heads");
   const int G = n_heads / n_kv_heads;
   VLO_CHECK(G <= 64, "GQA group too large");
-  int max_kv = 0;
-  for (int s = 0; s < n_seqs; ++s) max_kv = std::max(max_kv, seqs[s].kv_len);
-  const int version = attn_version_impl(G, max_kv);
-  const int per = (version >= 2 ? 128 : 64) / G;   // query tokens per work item
-  const int blk = version == 3 ? attn_tc2_blk() : (version == 2 ? kTcBlk : kAttnBlk);  // keys per pipeline block
-  plan->version = version;
+  const int per = 64 / G;        // query tokens per work item
+  const int blk = kAttnBlk;      // keys per pipeline block
   plan->blk = blk;
 
   std::vector<AttnItem> items;
@@ -101,7 +72,7 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
     }
   }
   const int n_items = static_cast<int>(items.size());
-  const int want = std::max(1, kNumSMs / (n_kv_heads * n_items));
+  const int want = std::max(1, num_sms() / (n_kv_heads * n_items));
   int max_splits = 1;
   size_t slots = 0;
   double algo = 0.0;
@@ -109,47 +80,15 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
     algo += static_cast<double>(it.q_pos0 + it.q_count) * n_kv_heads * kAttnHD * 2 * 2 +
             static_cast<double>(it.q_count) * n_heads * kAttnHD * 2 * 2;
   plan->algo_bytes = algo;
-  std::vector<int> cta_tab;
-  if (version == 3) {
-    // Deal the split budget (one wave: floor(148 / n_kv_heads) splits over all items) greedily to the item whose
-    // largest split is currently the longest; splits of an item are as even as its block count allows (the kernel
-    // derives blk0 = split * nblk / n_splits).  One stream, 8 kv heads: 18 splits -> 144 CTAs.
-    std::vector<int> nblk(n_items), ns(n_items, 1);
-    for (int i = 0; i < n_items; ++i) nblk[i] = (items[i].q_pos0 + items[i].q_count + blk - 1) / blk;
-    int budget = kNumSMs / n_kv_heads - n_items;
-    while (budget > 0) {
-      int best = -1, best_len = 1;
-      for (int i = 0; i < n_items; ++i) {
-        const int len = (nblk[i] + ns[i] - 1) / ns[i];
-        if (ns[i] < nblk[i] && ns[i] < 255 && len > best_len) best = i, best_len = len;
-      }
-      if (best < 0) break;
-      ++ns[best];
-      --budget;
-    }
-    for (int i = 0; i < n_items; ++i) {
-      AttnItem& it = items[i];
-      it.blocks_per_split = 0;  // even distribution
-      it.n_splits = ns[i];
-      it.ws_slot0 = static_cast<int>(slots);
-      slots += static_cast<size_t>(n_kv_heads) * it.n_splits * it.q_count * G;
-      max_splits = std::max(max_splits, it.n_splits);
-      for (int h = 0; h < n_kv_heads; ++h)
-        for (int sp = 0; sp < it.n_splits; ++sp) cta_tab.push_back((i << 16) | (h << 8) | sp);
-    }
-    VLO_CHECK(n_kv_heads <= 255 && n_items < 32768, "attention CTA table field overflow");
-    VLO_CHECK(cta_tab.size() <= max_ctas(total_tokens, n_seqs, n_heads, n_kv_heads), "attention CTA table overflow");
-  } else {
-    for (AttnItem& it : items) {
-      const int nblk = (it.q_pos0 + it.q_count + blk - 1) / blk;
-      int bps = (nblk + want - 1) / want;
-      if (version == 1) bps = std::max(2, bps + (bps & 1));  // even: both warp groups get the same number of blocks
-      it.blocks_per_split = bps;
-      it.n_splits = (nblk + bps - 1) / bps;
-      it.ws_slot0 = static_cast<int>(slots);
-      slots += static_cast<size_t>(n_kv_heads) * it.n_splits * it.q_count * G;
-      max_splits = std::max(max_splits, it.n_splits);
-    }
+  for (AttnItem& it : items) {
+    const int nblk = (it.q_pos0 + it.q_count + blk - 1) / blk;
+    int bps = (nblk + want - 1) / want;
+    bps = std::max(2, bps + (bps & 1));  // even: both warp groups get the same number of blocks
+    it.blocks_per_split = bps;
+    it.n_splits = (nblk + bps - 1) / bps;
+    it.ws_slot0 = static_cast<int>(slots);
+    slots += static_cast<size_t>(n_kv_heads) * it.n_splits * it.q_count * G;
+    max_splits = std::max(max_splits, it.n_splits);
   }
   const size_t cap_slots = cap_slots_for(total_tokens, n_seqs, n_heads, n_kv_heads);
   VLO_CHECK(slots <= cap_slots, "attention workspace plan overflow");
@@ -164,9 +103,6 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   plan->d_items = w;
   w += align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G));
   plan->d_tok_item = reinterpret_cast<int*>(w);
-  w += align_up(sizeof(int) * total_tokens);
-  plan->d_cta_tab = reinterpret_cast<int*>(w);
-  plan->n_ctas = static_cast<int>(cta_tab.size());
   plan->n_items = n_items;
   plan->max_splits = max_splits;
   plan->total_tokens = total_tokens;
@@ -177,16 +113,8 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   std::memcpy(hs2, tok_item.data(), sizeof(int) * total_tokens);
   VLO_CUDA(cudaMemcpyAsync(plan->d_items, hs, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, stream));
   VLO_CUDA(cudaMemcpyAsync(plan->d_tok_item, hs2, sizeof(int) * total_tokens, cudaMemcpyHostToDevice, stream));
-  if (!cta_tab.empty()) {
-    uint8_t* hs3 = hs2 + align_up(sizeof(int) * total_tokens);
-    std::memcpy(hs3, cta_tab.data(), sizeof(int) * cta_tab.size());
-    VLO_CUDA(cudaMemcpyAsync(plan->d_cta_tab, hs3, sizeof(int) * cta_tab.size(), cudaMemcpyHostToDevice, stream));
-  }
   return 0;
 }
-
-static long long* g_attn_trace = nullptr;
-long long* attn_trace_buffer() { return g_attn_trace; }
 
 static int launch_merge(const AttnPlan& plan, void* d_out, int n_heads, int n_kv_heads, float scale_log2, cudaStream_t stream) {
   AttnMergeParams mp{};
@@ -205,98 +133,9 @@ static int launch_merge(const AttnPlan& plan, void* d_out, int n_heads, int n_kv
   return 0;
 }
 
-// VLO_ATTN_TRACE=1: per-CTA clock64 timeline into a device buffer dumped by tools/gpu_attn_trace.py
-static long long* attn_trace_buffer_for_launch() {
-  static long long* dbg = nullptr;
-  static int want = -1;
-  if (want < 0) {
-    const char* e = getenv("VLO_ATTN_TRACE");
-    want = (e != nullptr && e[0] == '1') ? 1 : 0;
-    if (want) {
-      if (cudaMalloc(&dbg, sizeof(long long) * 192 * 4096) != cudaSuccess) dbg = nullptr;
-      if (dbg != nullptr) cudaMemset(dbg, 0, sizeof(long long) * 192 * 4096);
-    }
-  }
-  g_attn_trace = dbg;
-  return dbg;
-}
-
-template <int BLK>
-static int launch_tc2(const AttnPlan& plan, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap* tq,
-                      const AttnTc2Params& p, cudaStream_t stream) {
-  auto kern = attn_tc2_kernel<BLK>;
-  if (ensure_max_smem(reinterpret_cast<const void*>(kern), Tc2Cfg<BLK>::kSmemBytes)) return -1;
-  prof_begin(PROF_ATTN, stream, plan.algo_bytes);
-  VLO_CUDA(launch_pdl(kern, dim3(plan.n_ctas), dim3(kTcThreads), Tc2Cfg<BLK>::kSmemBytes, stream, tk, tv, tq[0], tq[1], tq[2], p));
-  prof_end(stream);
-  count_launch();
-  return 0;
-}
-
-static int attn_run_tc2(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows,
-                        void* d_out, int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream) {
-  const int blk = plan.blk;
-  CUtensorMap tk, tv, tq[3];
-  if (tmap_2d_sw128(d_k, static_cast<int>(kv_rows), kAttnHD, blk, 1, &tk) != 0) return -1;
-  if (tmap_2d_sw128(d_v, static_cast<int>(kv_rows), kAttnHD, blk, 1, &tv) != 0) return -1;
-  const int G = n_heads / n_kv_heads;
-  for (int i = 0; i < 3; ++i) {   // Q boxes of 32 / 64 / 128 tile rows (key slicing); a box is at least one token
-    const int rows = std::max(32 << i, G);
-    if (tmap_q3d_sw128(d_q, plan.total_tokens, n_heads, G, &tq[i], rows) != 0) return -1;
-  }
-  const float scale_log2 = static_cast<float>(1.4426950408889634 / std::sqrt(static_cast<double>(head_dim)));
-  AttnTc2Params p{};
-  p.base.q = static_cast<const __nv_bfloat16*>(d_q);
-  p.base.ws_o = plan.ws_o;
-  p.base.ws_ml = plan.ws_ml;
-  p.base.items = static_cast<const AttnItem*>(plan.d_items);
-  p.base.n_heads = n_heads;
-  p.base.n_kv_heads = n_kv_heads;
-  p.base.scale_log2 = scale_log2;
-  p.cta_tab = plan.d_cta_tab;
-  p.dbg = attn_trace_buffer_for_launch();
-  // V tile = MN-major B operand: 64-d halves one sub-tile apart (LBO), 8-key groups 1 KB apart (SBO)
-  p.v_lbo = static_cast<uint32_t>(blk * 128);
-  p.v_sbo = 1024u;
-  if (launch_tc2<128>(plan, tk, tv, tq, p, stream)) return -1;
-  if (plan.skip_merge) return 0;
-  return launch_merge(plan, d_out, n_heads, n_kv_heads, scale_log2, stream);
-}
-
-static int attn_run_tc(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows,
-                       void* d_out, int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream) {
-  CUtensorMap tk, tv, tq;
-  if (tmap_2d_sw128(d_k, static_cast<int>(kv_rows), kAttnHD, kTcBlk, 1, &tk) != 0) return -1;
-  if (tmap_2d_sw128(d_v, static_cast<int>(kv_rows), kAttnHD, kTcBlk, 1, &tv) != 0) return -1;
-  if (tmap_q3d_sw128(d_q, plan.total_tokens, n_heads, n_heads / n_kv_heads, &tq) != 0) return -1;
-  if (ensure_max_smem(reinterpret_cast<const void*>(attn_tc_kernel), kTcSmemBytes)) return -1;
-  const float scale_log2 = static_cast<float>(1.4426950408889634 / std::sqrt(static_cast<double>(head_dim)));
-  AttnTcParams p{};
-  p.base.q = static_cast<const __nv_bfloat16*>(d_q);
-  p.base.ws_o = plan.ws_o;
-  p.base.ws_ml = plan.ws_ml;
-  p.base.items = static_cast<const AttnItem*>(plan.d_items);
-  p.base.n_heads = n_heads;
-  p.base.n_kv_heads = n_kv_heads;
-  p.base.scale_log2 = scale_log2;
-  // V tile = MN-major B operand: 64-d halves 16 KB apart (LBO), 8-key groups 1 KB apart (SBO)
-  p.dbg = attn_trace_buffer_for_launch();
-  p.v_lbo = static_cast<uint32_t>(kTcSub);
-  p.v_sbo = 1024u;
-  prof_begin(PROF_ATTN, stream, plan.algo_bytes);
-  VLO_CUDA(launch_pdl(attn_tc_kernel, dim3(plan.max_splits, n_kv_heads, plan.n_items), dim3(kTcThreads), kTcSmemBytes, stream,
-                      tk, tv, tq, p));
-  prof_end(stream);
-  count_launch();
-  if (plan.skip_merge) return 0;
-  return launch_merge(plan, d_out, n_heads, n_kv_heads, scale_log2, stream);
-}
-
 int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows, void* d_out,
              int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream) {
   VLO_CHECK(kv_rows > 0 && kv_rows < (1ll << 31), "KV matrix rows out of range for a TMA map");
-  if (plan.version == 3) return attn_run_tc2(plan, d_q, d_k, d_v, kv_rows, d_out, n_heads, n_kv_heads, head_dim, stream);
-  if (plan.version == 2) return attn_run_tc(plan, d_q, d_k, d_v, kv_rows, d_out, n_heads, n_kv_heads, head_dim, stream);
   CUtensorMap tk, tv;
   if (tmap_2d_sw128(d_k, static_cast<int>(kv_rows), kAttnHD, kAttnBlk, 1, &tk) != 0) return -1;
   if (tmap_2d_sw128(d_v, static_cast<int>(kv_rows), kAttnHD, kAttnBlk, 1, &tv) != 0) return -1;
@@ -314,20 +153,9 @@ int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void*
   VLO_CUDA(launch_pdl(attn_kvappend_kernel, dim3(plan.max_splits, n_kv_heads, plan.n_items), dim3(kAttnThreads),
                       kAttnSmemBytes, stream, tk, tv, p));
   prof_end(stream);
-  AttnMergeParams mp{};
-  mp.ws_o = plan.ws_o;
-  mp.ws_ml = plan.ws_ml;
-  mp.items = static_cast<const AttnItem*>(plan.d_items);
-  mp.tok_item = plan.d_tok_item;
-  mp.out = static_cast<__nv_bfloat16*>(d_out);
-  mp.n_heads = n_heads;
-  mp.n_kv_heads = n_kv_heads;
-  mp.scale_log2 = scale_log2;
-  prof_begin(PROF_ATTN_MERGE, stream, 0.0);
-  VLO_CUDA(launch_pdl(attn_merge_kernel, dim3(n_heads, plan.total_tokens), dim3(128), 0, stream, mp));
-  prof_end(stream);
-  count_launch(2);
-  return 0;
+  count_launch();
+  if (plan.skip_merge) return 0;
+  return launch_merge(plan, d_out, n_heads, n_kv_heads, scale_log2, stream);
 }
 
 }  // namespace vlo

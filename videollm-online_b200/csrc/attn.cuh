@@ -355,7 +355,7 @@ __global__ void __launch_bounds__(128) attn_merge_kernel(const AttnMergeParams p
   const int r = (tok - it.q_tok0) * G + g;
   const float c = p.scale_log2;
   const size_t slot0 = static_cast<size_t>(it.ws_slot0) + static_cast<size_t>(kvh) * it.n_splits * rows + r;
-  const int ns = it.n_splits;  // <= 148
+  const int ns = it.n_splits;  // <= number of SMs
   const float* o = p.ws_o + slot0 * kAttnHD + d;
   const size_t stride = static_cast<size_t>(rows) * kAttnHD;
   __nv_bfloat16* dst = p.out + (static_cast<size_t>(tok) * p.n_heads + head) * kAttnHD + d;

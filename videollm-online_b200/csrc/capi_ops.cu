@@ -26,7 +26,7 @@ int vlo_device_supported(int device) {
     cudaGetLastError();
     return 0;
   }
-  return prop.major == 10 ? 1 : 0;
+  return (prop.major == 9 && prop.minor == 0) ? 1 : 0;
 }
 
 int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a, const void* d_b,
@@ -60,23 +60,6 @@ int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a
 
 extern "C" {
 
-int vlo_op_gemm2(const void* d_x, int rows_x, const void* d_w, int rows_w, int k, void* d_out, int ld_out, const float* d_bias,
-                 int act, int epi, int bn, void* cuda_stream) {
-  Gemm2Call c{};
-  c.x = d_x;
-  c.rows_x = rows_x;
-  c.w = d_w;
-  c.rows_w = rows_w;
-  c.k = k;
-  c.out = d_out;
-  c.ld_out = ld_out;
-  c.bias = d_bias;
-  c.act = act;
-  c.epi = epi;
-  c.bn = bn;
-  return gemm2_launch(c, static_cast<cudaStream_t>(cuda_stream));
-}
-
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
                    void* cuda_stream) {
@@ -101,14 +84,6 @@ int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d
   if (h_max_planes) *h_max_planes = planes;
   if (d_out == nullptr) return 0;  // planning query only
   return gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream));
-}
-
-/* debug: copy the VLO_ATTN_TRACE timeline (n int64 values) to the host; returns -1 when tracing is off */
-int vlo_debug_attn_trace(long long* h_out, int n) {
-  long long* d = attn_trace_buffer();
-  if (d == nullptr) return fail("attention tracing is off (set VLO_ATTN_TRACE=1)");
-  VLO_CUDA(cudaMemcpy(h_out, d, sizeof(long long) * n, cudaMemcpyDeviceToHost));
-  return 0;
 }
 
 int vlo_op_attn_version(int n_heads, int n_kv_heads) { return attn_version(n_heads, n_kv_heads); }

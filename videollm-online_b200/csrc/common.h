@@ -53,6 +53,8 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
+int num_sms();  // multiprocessors of the current device (queried once)
+
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device function attribute: set it once per (device, kernel).
 int ensure_max_smem(const void* func, int bytes);
 
@@ -123,22 +125,6 @@ struct GemmWsCall {
 int gemm_ws_plan(int rows_w, int k, int mode, int n_ctas, SkInfo* sk, int* max_planes, int x_tiles = 1);
 int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream);
 
-// ---- 2-CTA (cta_group::2) tensor-bound GEMM for the ViT trunk (gemm2.cuh / gemm.cu): tokens on MMA-M, 256 x bn tiles per CTA pair
-struct Gemm2Call {
-  const void* x;      // [rows_x, k] fp16 activations
-  int rows_x;
-  const void* w;      // [rows_w, k] fp16 weights, rows_w a multiple of 32
-  int rows_w;
-  int k;
-  void* out;          // epi 0: fp16 [rows_x, ld_out] = act(fp16(acc + bias));  epi 1: fp32 [rows_x, ld_out] += fp16(acc + bias)
-  int ld_out;
-  const float* bias;
-  int act;
-  int epi;
-  int bn;             // 256 or 128 features per tile
-};
-int gemm2_launch(const Gemm2Call& c, cudaStream_t stream);
-
 // ---- stream-K GEMM with the fused finisher epilogue (gemm_wsf.cuh / gemm.cu); args struct defined in gemm_wsf.cuh
 struct GemmWsfArgs;
 int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, int epi, cudaStream_t stream);
@@ -154,18 +140,14 @@ struct AttnSeq {
 // bytes of scratch attn_launch needs for these sequences (upper bound)
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads);
 size_t attn_stage_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads);
-int attn_version(int n_heads, int n_kv_heads);
-long long* attn_trace_buffer();  // device buffer of the VLO_ATTN_TRACE timeline (nullptr when off)  // 2 = tcgen05 kernel, 1 = mma.sync kernel (VLO_ATTN=1 or G not dividing 128)
+int attn_version(int n_heads, int n_kv_heads);  // 1: the mma.sync kernel (attn.cuh)
 struct AttnPlan {
   float* ws_o;
   float* ws_ml;
   void* d_items;
   int* d_tok_item;
   int n_items, max_splits, total_tokens;
-  int* d_cta_tab;     // v3: flat (item, kv head, split) table, one entry per CTA
-  int n_ctas;
   int blk;            // keys per pipeline block
-  int version;        // 1 = mma.sync kernel, 2 = tcgen05 kernel (P in smem), 3 = tcgen05 kernel (P in TMEM, deep ring)
   int skip_merge;     // measurement only: launch the main kernel without the split-KV merge
   double algo_bytes;  // algorithmic HBM bytes of one attn_run over this plan (K+V rows read, Q read, out written)
 };

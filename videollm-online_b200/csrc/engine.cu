@@ -12,15 +12,12 @@
 #include "gemm.cuh"
 #include "gemm_wsf.cuh"
 #include "vit_kernels.cuh"
-#include "vit_attn_tc.cuh"
-#include "vit_attn_tc2.cuh"
 #include "vlo_b200.h"
 
 using namespace vlo;
 
 namespace {
 
-constexpr int kNumSMs = 148;
 constexpr int kStageSlots = 16;
 
 using bf16 = __nv_bfloat16;
@@ -40,12 +37,6 @@ size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 struct vlo_engine {
   vlo_config cfg{};
   int device = 0;
-  // Cluster kernels (the 2-CTA ViT GEMMs) never run concurrently with a decoder step: next to the step's deep PDL chain
-  // (several kernels resident early, all SM shared memory taken) a pending CTA pair was observed to stall both streams.
-  // A step enqueued on another stream than the last pair-GEMM ViT pass waits for that pass, and vice versa (events below).
-  cudaEvent_t ev_step = nullptr, ev_pair = nullptr;
-  cudaStream_t step_stream = nullptr, pair_stream = nullptr;
-  bool step_seen = false, pair_seen = false;
   std::map<std::string, std::pair<const void*, int64_t>> tensors;
   bool finalized = false;
 
@@ -168,13 +159,12 @@ int gemm_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, 
 }
 
 // Which stream-K fix-ups run inside the GEMM's finisher CTAs (gemm_wsf.cuh) instead of a separate kernel.  A finisher's
-// epilogue (flag acquire -> plane loads -> table loads -> stores) is a ~3 us tail at the end of EVERY CTA during which its SM
-// streams nothing, while a separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling: fusing all
-// four is slower than fusing none.
+// epilogue (flag acquire -> plane loads -> table loads -> stores) is a tail at the end of EVERY CTA during which its SM
+// streams nothing, while a separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling.  Only
+// the gate|up GEMM has enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB
+// plane round trip of its fix-up.
 // VLO_FUSE bit mask: 1 = q|k|v (+RoPE +append), 2 = o_proj (+residual), 4 = gate|up (+SwiGLU), 8 = down_proj (+residual);
-// "all" = 15.  Default 4, by measurement (tools/gpu_r2_call18.sh, decoder frame step alone at 12k, ms): 0 -> 4.14, 15 -> 4.47,
-// 1 -> 4.39, 2 -> 4.32, 4 -> 3.98, 8 -> 4.30, 5 -> 4.18, 10 -> 4.46.  Only the gate|up GEMM gains: it is the one with enough
-// tiles (224, 1.5 per CTA) to amortise the finisher's tail, and fusing it removes the 3.6 MB plane round trip of its fix-up.
+// "all" = 15.  Default 4 (H100 measurements in DESIGN.md section 3.2).
 int fuse_mask() {
   static int v = -1;
   if (v < 0) {
@@ -244,11 +234,11 @@ int gemm_store16(int fmt, int swap, const void* a, int rows_a, const void* b, in
 int vit_bn(int rows, int n_out) {
   const int mt = (rows + 127) / 128;
   const int t64 = mt * ((n_out + 63) / 64), t128 = mt * ((n_out + 127) / 128);
-  if (t64 <= kNumSMs) return 64;     // everything fits in one wave even with the narrow tile
-  if (t128 <= kNumSMs) return 128;   // one wave with the wide tile
+  if (t64 <= num_sms()) return 64;     // everything fits in one wave even with the narrow tile
+  if (t128 <= num_sms()) return 128;   // one wave with the wide tile
   // multi-wave: wide tiles (better operand reuse) unless the narrow ones waste much less of the last wave
-  const double e64 = static_cast<double>(t64) / (((t64 + kNumSMs - 1) / kNumSMs) * kNumSMs);
-  const double e128 = static_cast<double>(t128) / (((t128 + kNumSMs - 1) / kNumSMs) * kNumSMs);
+  const double e64 = static_cast<double>(t64) / (((t64 + num_sms() - 1) / num_sms()) * num_sms());
+  const double e128 = static_cast<double>(t128) / (((t128 + num_sms() - 1) / num_sms()) * num_sms());
   return e64 > e128 + 0.15 ? 64 : 128;
 }
 
@@ -308,7 +298,7 @@ int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out) {
   int prev_dev = -1;
   cudaGetDevice(&prev_dev);
   VLO_CUDA(cudaSetDevice(device));
-  if (!vlo_device_supported(device)) return fail("device is not an sm_100 (Blackwell) GPU; there is no fallback path");
+  if (!vlo_device_supported(device)) return fail("device is not an sm_90 (Hopper) GPU; there is no fallback path");
   const vlo_config& c = *cfg;
   VLO_CHECK(c.head_dim == 128, "decoder head_dim must be 128");
   VLO_CHECK(c.vocab_size % 8 == 0, "vocab_size must be a multiple of 8 (16-byte aligned logits rows)");
@@ -408,8 +398,6 @@ int vlo_engine_destroy(vlo_engine* e) {
   if (e->stage) cudaFreeHost(e->stage);
   for (int i = 0; i < kStageSlots; ++i)
     if (e->stage_events[i]) cudaEventDestroy(e->stage_events[i]);
-  if (e->ev_step) cudaEventDestroy(e->ev_step);
-  if (e->ev_pair) cudaEventDestroy(e->ev_pair);
   delete e;
   return 0;
 }
@@ -650,52 +638,27 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     g.bn = vit_bn(rows, C);
     if (gemm_launch(g, st)) return -1;
   }
+  // ViT attention: mma.sync m16n8k16 over TMA-loaded Q / K / V tiles (vit_kernels.cuh)
   if (ensure_max_smem(reinterpret_cast<const void*>(vit_attn_kernel), kVitSmemBytes)) return -1;
-  // attention kernel generation: tcgen05 (vit_attn_tc.cuh) whenever the frame's K / V fit its resident ring;
-  // VLO_VIT_ATTN=1 forces the mma.sync kernel (A/B checks)
-  static int vit_attn_gen = -1;
-  if (vit_attn_gen < 0) {
-    const char* ev = getenv("VLO_VIT_ATTN");
-    vit_attn_gen = (ev != nullptr && ev[0] == '1') ? 1 : ((ev != nullptr && ev[0] == '2') ? 2 : ((ev != nullptr && ev[0] == '3') ? 3 : 0));
-  }
-  // default: the two-tile tcgen05 kernel for the tensor-bound batches (>= 3 frames: 0.95 vs 1.2 ms per pass at batch 8),
-  // the mma.sync kernel for 1-2 frames, where a launch is latency-bound (80 CTAs, 12.8 vs 14.7 us) and hidden behind the
-  // decoder step it overlaps
-  const int attn_gen = vit_attn_gen > 0 ? vit_attn_gen : (B >= 3 ? 3 : 1);
-  const bool attn_tc = attn_gen >= 2 && (P + kVitTcBlk - 1) / kVitTcBlk <= kVitTcMaxBlk;
-  // generation 3 (vit_attn_tc2.cuh): two query tiles in flight per CTA, K / V loaded once per CTA.  Query tiles per CTA:
-  // as many as keeps >= ~120 CTAs in the grid (all 5 at batch 8: one CTA per (frame, head)).
-  const bool attn_tc2 = attn_tc && attn_gen == 3;
-  const int vit_qtiles = (P + 127) / 128;
-  int vit_tpc = vit_qtiles;
-  while (vit_tpc > 2 && c.vit_heads * B * ((vit_qtiles + vit_tpc - 1) / vit_tpc) < 120) --vit_tpc;
-  if (attn_tc2 && ensure_max_smem(reinterpret_cast<const void*>(vit_attn_tc2_kernel), kVit2SmemBytes)) return -1;
   CUtensorMap tm_qkv;
-  if (tmap_2d_sw128(e->v_qkv, rows, 3 * C, attn_tc ? kVitTcBlk : kVitBlk, FMT_F16, &tm_qkv)) return -1;
+  if (tmap_2d_sw128(e->v_qkv, rows, 3 * C, kVitBlk, FMT_F16, &tm_qkv)) return -1;
   const float scale_log2 = 1.4426950408889634f / 8.0f;  // head_dim 64
   auto launch_vit_attn = [&]() -> int {
     prof_begin(PROF_VIT_ATTN, st, 4.0 * rows * C * 2);
-    if (attn_tc2)
-      VLO_CUDA(launch_pdl(vit_attn_tc2_kernel, dim3((vit_qtiles + vit_tpc - 1) / vit_tpc, c.vit_heads, B), dim3(kVit2Threads),
-                          kVit2SmemBytes, st, tm_qkv, e->v_attn, P, C, scale_log2, vit_tpc));
-    else if (attn_tc)
-      VLO_CUDA(launch_pdl(vit_attn_tc_kernel, dim3((P + kVitTcBlk - 1) / kVitTcBlk, c.vit_heads, B), dim3(kVitTcThreads),
-                          kVitTcSmemBytes, st, tm_qkv, e->v_attn, P, C, scale_log2));
-    else
-      VLO_CUDA(launch_pdl(vit_attn_kernel, dim3((P + kVitBlk - 1) / kVitBlk, c.vit_heads, B), dim3(kVitThreads), kVitSmemBytes, st,
-                          tm_qkv, e->v_attn, P, C, scale_log2));
+    VLO_CUDA(launch_pdl(vit_attn_kernel, dim3((P + kVitBlk - 1) / kVitBlk, c.vit_heads, B), dim3(kVitThreads), kVitSmemBytes, st,
+                        tm_qkv, e->v_attn, P, C, scale_log2));
     prof_end(st);
     count_launch();
     return 0;
   };
-  if (attn_tc && ensure_max_smem(reinterpret_cast<const void*>(vit_attn_tc_kernel), kVitTcSmemBytes)) return -1;
   // Trunk GEMMs on the persistent swap-AB kernel (weights ride MMA-M, the 576*B token rows are tiled along
   // MMA-N): QKV and fc1 run whole tiles with the fused bias / GELU fp16 epilogue; out_proj and fc2 (few
   // output tiles) run stream-K over all SMs and their partial planes are folded into the fp32 residual
   // stream together with the NEXT LayerNorm by vit_fix_ln_kernel.
-  // Small batches (the single-stream case) run the trunk GEMMs with 64-token tiles and a shallow ring (~75 KB of
-  // shared memory): such a CTA fits on an SM NEXT TO a decoder weight-streaming CTA (145 KB), so the tensor-bound
-  // ViT of frame i+1 and the HBM-bound decoder step of frame i really execute concurrently (two CUDA streams).
+  // Small batches (the single-stream case) run the trunk GEMMs with 64-token tiles and a shallow ring (83 KB of
+  // shared memory): such a CTA fits on an SM NEXT TO a decoder weight-streaming CTA (119 KB; gemm.cu checks the sum),
+  // so the tensor-bound ViT of frame i+1 and the HBM-bound decoder step of frame i can execute concurrently (two CUDA
+  // streams).
   static int coreside = -1;
   if (coreside < 0) {
     const char* ev = getenv("VLO_VIT_CORESIDE");
@@ -703,12 +666,12 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   }
   const bool small = coreside && B <= 2;
   // token-tile width of the co-resident configuration (VLO_VIT_SMALL_BN=64|96; ring = 3 stages of 16 KB + bn * 128 B).
-  // 96 divides the 576 tokens of a frame (no padded tile, 144 tiles = one wave): the pass alone takes 2.22 instead of
-  // 2.46 ms (batch 2: 2.99 vs 3.43); next to the decoder step it is a wash (202-204 frames/s either way).
+  // 64 by measurement on the H100 (pipelined frame step 1.3 % faster than with 96, DESIGN.md section 5); both divide
+  // the 576 tokens of a frame.
   static int small_bn = 0;
   if (small_bn == 0) {
     const char* ev = getenv("VLO_VIT_SMALL_BN");
-    small_bn = (ev != nullptr && atoi(ev) == 64) ? 64 : 96;
+    small_bn = (ev != nullptr && atoi(ev) == 96) ? 96 : 64;
   }
   auto pick_bn = [&](int n_out, int mode) {
     if (small) return small_bn;
@@ -719,7 +682,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
       const int xt = (rows + bn - 1) / bn;
       const int tiles = ((n_out + 127) / 128) * xt;
       double eff = static_cast<double>(rows) / (static_cast<double>(xt) * bn);          // padding waste
-      if (mode == 1) eff *= static_cast<double>(tiles) / (((tiles + kNumSMs - 1) / kNumSMs) * kNumSMs);  // wave quantisation
+      if (mode == 1) eff *= static_cast<double>(tiles) / (((tiles + num_sms() - 1) / num_sms()) * num_sms());  // wave quantisation
       if (eff >= best_eff - 1e-9) {  // ties -> wider tile (better operand reuse)
         best_eff = eff;
         best = bn;
@@ -793,57 +756,9 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   VLO_CUDA(launch_pdl(layernorm_kernel<float>, dim3(rows), dim3(256), ln_smem, st, static_cast<const float*>(e->v_h),
                       e->vit[0].ln1_w, e->vit[0].ln1_b, e->v_xn, static_cast<float*>(nullptr), C, c.vit_ln_eps));
   count_launch();
-  // Batches of >= 3 frames (encode-ahead groups, multi-stream ticks, offline extraction) are tensor-bound: their trunk
-  // GEMMs run on CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles, gemm2.cuh) with tokens on MMA-M; out_proj / fc2 add
-  // straight into the fp32 residual stream and a plain LayerNorm kernel follows.  VLO_VIT_GEMM2=0: single-CTA path.
-  static int use_gemm2 = -1;
-  if (use_gemm2 < 0) {
-    const char* ev = getenv("VLO_VIT_GEMM2");
-    use_gemm2 = (ev != nullptr && ev[0] == '0') ? 0 : 1;
-  }
-  const bool pair_gemm = use_gemm2 && B >= 3 && C % 128 == 0 && M % 128 == 0;
-  if (pair_gemm) {
-    if (e->ev_pair == nullptr) VLO_CUDA(cudaEventCreateWithFlags(&e->ev_pair, cudaEventDisableTiming));
-    if (e->step_seen && e->step_stream != st) VLO_CUDA(cudaStreamWaitEvent(st, e->ev_step, 0));   // behind the last decoder step
-  }
-  auto gemm2 = [&](const __half* x, const __half* w, int n_out, int k, void* out, const float* bias, int act, int epi) -> int {
-    Gemm2Call g{};
-    g.x = x;
-    g.rows_x = rows;
-    g.w = w;
-    g.rows_w = n_out;
-    g.k = k;
-    g.out = out;
-    g.ld_out = n_out;
-    g.bias = bias;
-    g.act = act;
-    g.epi = epi;
-    // 256-wide tiles unless they leave most CTA pairs idle (the two C-wide GEMMs at small batch)
-    const int mt = (rows + 255) / 256;
-    g.bn = (n_out % 256 == 0 && mt * (n_out / 256) >= 60) ? 256 : 128;
-    return gemm2_launch(g, st);
-  };
-  auto plain_ln = [&](const float* lw, const float* lb, float* out32) -> int {
-    VLO_CUDA(launch_pdl(layernorm_kernel<float>, dim3(rows), dim3(256), ln_smem, st, static_cast<const float*>(e->v_h), lw, lb,
-                        e->v_xn, out32, C, c.vit_ln_eps));
-    count_launch();
-    return 0;
-  };
   for (int l = 0; l < c.vit_layers; ++l) {
     const VitLayer& v = e->vit[l];
     SkCall sc{};
-    if (pair_gemm) {
-      if (gemm2(e->v_xn, v.qkv_w, 3 * C, C, e->v_qkv, v.qkv_b, ACT_NONE, 0)) return -1;
-      if (launch_vit_attn()) return -1;
-      if (gemm2(e->v_attn, v.out_w, C, C, e->v_h, v.out_b, ACT_NONE, 1)) return -1;
-      if (plain_ln(v.ln2_w, v.ln2_b, nullptr)) return -1;
-      if (gemm2(e->v_xn, v.fc1_w, M, C, e->v_mlp, v.fc1_b, ACT_GELU_TANH, 0)) return -1;
-      if (gemm2(e->v_mlp, v.fc2_w, C, M, e->v_h, v.fc2_b, ACT_NONE, 1)) return -1;
-      const bool last2 = (l == c.vit_layers - 1);
-      if (plain_ln(last2 ? e->post_ln_w : e->vit[l + 1].ln1_w, last2 ? e->post_ln_b : e->vit[l + 1].ln1_b, last2 ? e->v_ln32 : nullptr))
-        return -1;
-      continue;
-    }
     if (tiles_gemm(e->v_xn, v.qkv_w, 3 * C, C, e->v_qkv, v.qkv_b, ACT_NONE)) return -1;
     if (launch_vit_attn()) return -1;
     if (partial_gemm(e->v_attn, v.out_w, C, &sc)) return -1;
@@ -856,11 +771,6 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     if (fix_ln(sc, v.fc2_b, last ? e->post_ln_w : e->vit[l + 1].ln1_w, last ? e->post_ln_b : e->vit[l + 1].ln1_b,
                last ? e->v_ln32 : nullptr))
       return -1;
-  }
-  if (pair_gemm) {   // decoder steps on other streams queue behind the trunk's cluster kernels
-    VLO_CUDA(cudaEventRecord(e->ev_pair, st));
-    e->pair_stream = st;
-    e->pair_seen = true;
   }
   const int NT = e->n_frame_tokens;
   const int cls = c.frame_token_cls ? 1 : 0;
@@ -921,7 +831,6 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   const vlo_config& c = e->cfg;
   VLO_CHECK(n_seqs > 0 && n_seqs <= c.max_streams, "step: n_seqs out of range");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  if (e->pair_seen && e->pair_stream != st) VLO_CUDA(cudaStreamWaitEvent(st, e->ev_pair, 0));   // see vlo_engine::ev_pair
   const int H = c.hidden_size;
   int T = 0;
   for (int i = 0; i < n_seqs; ++i) {
@@ -1066,7 +975,7 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
       p.T = T;
       p.I = c.intermediate_size;
       const long long n2 = static_cast<long long>(T) * c.intermediate_size / 4;
-      VLO_CUDA(launch_pdl(swiglu_kernel, dim3(static_cast<unsigned>(std::min<long long>((n2 + 255) / 256, 4 * kNumSMs))),
+      VLO_CUDA(launch_pdl(swiglu_kernel, dim3(static_cast<unsigned>(std::min<long long>((n2 + 255) / 256, 4 * num_sms()))),
                           dim3(256), 0, st, p));
       count_launch();
     }
@@ -1091,10 +1000,6 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
 
   for (int i = 0; i < n_seqs; ++i) e->kv_len[h_stream_ids[i]] += h_q_lens[i];
   e->last_step_tokens = T;
-  if (e->ev_step == nullptr) VLO_CUDA(cudaEventCreateWithFlags(&e->ev_step, cudaEventDisableTiming));
-  VLO_CUDA(cudaEventRecord(e->ev_step, st));
-  e->step_stream = st;
-  e->step_seen = true;
   return 0;
 }
 

@@ -1,10 +1,9 @@
-// Host launcher for the tcgen05 GEMM: TMA descriptor construction (driver entry point
+// Host launchers of the wgmma GEMMs: TMA descriptor construction (driver entry point
 // resolved at run time, so the library loads on a box without libcuda), tile-shape
 // selection and kernel dispatch.
 #include "gemm.cuh"
 #include "gemm_ws.cuh"
 #include "gemm_wsf.cuh"
-#include "gemm2.cuh"
 
 #include <cudaTypedefs.h>
 
@@ -231,17 +230,18 @@ int gemm_launch(const GemmCall& c, cudaStream_t stream) {
 
 // ------------------------------------------------------------------------------------------------
 // persistent weight-streaming GEMM (gemm_ws.cuh)
-namespace {
-int num_sms() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
-  }
-  return n;
-}
 
+// The default single-stream frame step runs the ViT of frame i+1 (small-tile configuration: 96- or 64-token tiles,
+// 3 stages) next to the decoder step of frame i (16-token tiles, 6 stages).  One CTA of each fits on one sm_90 SM:
+// 228 KB of shared memory per SM, of which 1 KB is reserved per resident block.  (4 ViT stages, VLO_VIT_STAGES=4, and
+// the 8-stage fused gate|up GEMM do not leave room for the other CTA.)
+constexpr int kSmemPerSm = 233472, kSmemReservedPerBlock = 1024;
+static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<96, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "decoder GEMM CTA and 96-token ViT GEMM CTA no longer share an SM");
+static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
+
+namespace {
 template <int FMT, int BN, int STAGES = ws_default_stages(BN)>
 int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
   auto kern = gemm_ws_kernel<FMT, BN, STAGES>;
@@ -278,7 +278,7 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
   VLO_CHECK(c.k > 0 && c.k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(c.rows_w > 0 && c.rows_x > 0, "empty GEMM operand");
   // token-tile width: the smallest instance covering rows_x (a narrower X tile leaves more of the ring to the weight stream:
-  // 88 tokens = 8 streams x 11 take the 96-wide instance, 7 x 28 KB stages instead of 6 x 32 KB)
+  // 88 tokens = 8 streams x 11 take the 96-wide instance)
   const int bn = c.bn > 0 ? c.bn
                           : (c.rows_x <= 16 ? 16 : (c.rows_x <= 32 ? 32 : (c.rows_x <= 64 ? 64 : ((c.rows_x <= 96 && c.fmt == FMT_BF16) ? 96 : 128))));
   const int x_tiles = (c.rows_x + bn - 1) / bn;
@@ -309,7 +309,7 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
       const char* e = getenv("VLO_WS_STAGES");
       st = e ? atoi(e) : 6;
     }
-    // 6 x 18 KB (measured best in the two-stream pipelined step: leaves room for a co-resident ViT CTA)
+    // default 6 x 18 KB: leaves room on the SM for a co-resident small-tile ViT CTA (static_asserts above)
     if (st == 4) return launch_ws<FMT_BF16, 16, 4>(tw, tx, a, stream);
     if (st == 5) return launch_ws<FMT_BF16, 16, 5>(tw, tx, a, stream);
     if (st == 6) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
@@ -374,10 +374,8 @@ int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, int epi,
   if (get_tmap(w, a.rows_w, a.k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
   if (get_tmap(x, a.rows_x, a.k, bn, FMT_BF16, &tx) != 0) return -1;
   if (bn == 16) {
-    // ring depth (VLO_WSF_STAGES=4|5|6|8|10; default 8 = 144 KB + the 8.7 KB exchange tile).  Same-box A/Bs: the decoder step
-    // alone does not care (3.97-3.99 ms for 6 / 8 / 10 stages; 5 and 4 stages, which let the next GEMM's CTA become resident
-    // beside this one, are slower: 4.02 / 4.07); next to the co-resident ViT 8 stages measure 211 vs 208 frames/s - the ViT's
-    // CTAs then cannot share an SM with the (only) fused GEMM, gate|up, and stop competing with its stream.
+    // ring depth (VLO_WSF_STAGES=4|5|6|8|10; default 8 = 144 KB + the 8.7 KB exchange and 10 KB staging tiles).  With 8
+    // stages a co-resident ViT CTA cannot share an SM with the (only) fused GEMM, gate|up, and stop competing with its stream.
     static int st = 0;
     if (st == 0) {
       const char* e = getenv("VLO_WSF_STAGES");
@@ -390,107 +388,10 @@ int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, int epi,
     if (st == 6) return launch_wsf_epi<16, 6>(epi, tw, tx, a, stream);
     return launch_wsf_epi<16, 8>(epi, tw, tx, a, stream);
   }
-  if (bn == 32) return launch_wsf_epi<32, ws_default_stages(32)>(epi, tw, tx, a, stream);
-  if (bn == 64) return launch_wsf_epi<64, ws_default_stages(64)>(epi, tw, tx, a, stream);
-  if (bn == 96) return launch_wsf_epi<96, 6>(epi, tw, tx, a, stream);
-  return launch_wsf_epi<128, ws_default_stages(128)>(epi, tw, tx, a, stream);
-}
-
-// ------------------------------------------------------------------------------------------------
-// 2-CTA tensor-bound GEMM (gemm2.cuh)
-namespace {
-// output map for the TMA-store epilogue: [rows, cols] row-major, 2- or 4-byte elements, box = 128 rows x 128 bytes, 128B swizzle
-int tmap_out_sw128(const void* ptr, int rows, int cols, int elem_bytes, CUtensorMap* out) {
-  TmapKey key{ptr, rows, cols, -128, 100 + elem_bytes};
-  {
-    std::lock_guard<std::mutex> g(g_tmap_mu);
-    auto it = g_tmaps.find(key);
-    if (it != g_tmaps.end()) {
-      *out = it->second;
-      return 0;
-    }
-  }
-  EncodeFn enc = get_encode();
-  if (enc == nullptr) return fail("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) return fail("TMA operand not 16-byte aligned");
-  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * elem_bytes};
-  cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / elem_bytes), 128};
-  cuuint32_t estr[2] = {1, 1};
-  CUtensorMap m;
-  CUresult r = enc(&m, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr),
-                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (output) failed, CUresult " + std::to_string(r));
-  {
-    std::lock_guard<std::mutex> g(g_tmap_mu);
-    g_tmaps.emplace(key, m);
-  }
-  *out = m;
-  return 0;
-}
-
-template <int BN, int STAGES, int EPI>
-int launch_gemm2(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& to, const Gemm2Args& a, cudaStream_t stream) {
-  auto kern = gemm2_kernel<BN, STAGES, EPI>;
-  using Cfg = Gemm2Cfg<BN, STAGES>;
-  if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
-  const int tiles = a.m_tiles * a.n_tiles;
-  const int n_pairs = std::min(num_sms() / 2, tiles);
-  if (prof_on())
-    prof_begin(PROF_GEMM_VIT, stream, 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x) + (EPI == G2_STORE16 ? 2.0 : 8.0) * a.rows_x * a.rows_w);
-  // VLO_GEMM2_PDL bit 0: launch with the programmatic-serialization attribute (prologue - barrier init, TMEM allocation of
-  // the pair, cluster sync - overlaps the predecessor's tail); bit 1: trigger the successor early.  Default 1.  Measured
-  // (tools/gpu_r2_call11.sh, ViT alone at batch 8): 0 -> 5.07 ms, 2 -> 5.10, 1 -> 4.83; 3 DEAD-LOCKS next to the
-  // non-cluster kernels of the trunk (three kernels deep: a cluster kernel resident early AND its successor resident early;
-  // the gemm2 <-> gemm2 chain alone runs), so a cluster kernel here never triggers early.
-  static int pdl_mode = -1;
-  if (pdl_mode < 0) {
-    const char* e = getenv("VLO_GEMM2_PDL");
-    pdl_mode = e ? atoi(e) : 1;
-  }
-  Gemm2Args a2 = a;
-  a2.pdl_trigger = (pdl_mode & 2) ? 1 : 0;
-  if (pdl_mode & 1) {
-    VLO_CUDA(launch_pdl(kern, dim3(2 * n_pairs), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tx, tw, to, a2));
-  } else {
-    kern<<<dim3(2 * n_pairs), dim3(kGemmThreads), Cfg::kSmemBytes, stream>>>(tx, tw, to, a2);
-    VLO_LAUNCH_CHECK();
-  }
-  prof_end(stream);
-  count_launch();
-  return 0;
-}
-}  // namespace
-
-int gemm2_launch(const Gemm2Call& c, cudaStream_t stream) {
-  VLO_CHECK(c.k > 0 && c.k % kGemmBK == 0, "gemm2: K must be a positive multiple of 64");
-  VLO_CHECK(c.rows_x > 0 && c.rows_w > 0 && c.rows_w % 64 == 0, "gemm2: rows_w must be a positive multiple of 64");
-  VLO_CHECK(c.bn == 256 || c.bn == 128, "gemm2: bn is 256 or 128");
-  VLO_CHECK(c.bias != nullptr && (reinterpret_cast<uintptr_t>(c.bias) & 15) == 0, "gemm2: bias required, 16-byte aligned");
-  VLO_CHECK(c.ld_out % 8 == 0 && (reinterpret_cast<uintptr_t>(c.out) & 15) == 0, "gemm2: output rows must be 16-byte aligned");
-  Gemm2Args a{};
-  a.rows_x = c.rows_x;
-  a.rows_w = c.rows_w;
-  a.k = c.k;
-  a.m_tiles = (c.rows_x + 255) / 256;
-  a.n_tiles = (c.rows_w + c.bn - 1) / c.bn;
-  a.out = c.out;
-  a.ld_out = c.ld_out;
-  a.bias = c.bias;
-  a.act = c.act;
-  CUtensorMap tx, tw;
-  if (get_tmap(c.x, c.rows_x, c.k, 128, FMT_F16, &tx) != 0) return -1;
-  if (get_tmap(c.w, c.rows_w, c.k, c.bn / 2, FMT_F16, &tw) != 0) return -1;
-  CUtensorMap to;
-  VLO_CHECK(c.ld_out == c.rows_w, "gemm2: the output is a dense [rows_x, rows_w] matrix");
-  if (tmap_out_sw128(c.out, c.rows_x, c.rows_w, c.epi == G2_STORE16 ? 2 : 4, &to) != 0) return -1;
-  // ring: 5 x 32 KB (bn 256) / 7 x 24 KB (bn 128) + two 16 KB output panels
-  if (c.bn == 256 && c.epi == G2_STORE16) return launch_gemm2<256, 5, G2_STORE16>(tx, tw, to, a, stream);
-  if (c.bn == 128 && c.epi == G2_STORE16) return launch_gemm2<128, 7, G2_STORE16>(tx, tw, to, a, stream);
-  if (c.bn == 256 && c.epi == G2_RESID32) return launch_gemm2<256, 5, G2_RESID32>(tx, tw, to, a, stream);
-  if (c.bn == 128 && c.epi == G2_RESID32) return launch_gemm2<128, 7, G2_RESID32>(tx, tw, to, a, stream);
-  return fail("gemm2_launch: no kernel instance");
+  if (bn == 32) return launch_wsf_epi<32, wsf_default_stages(32)>(epi, tw, tx, a, stream);
+  if (bn == 64) return launch_wsf_epi<64, wsf_default_stages(64)>(epi, tw, tx, a, stream);
+  if (bn == 96) return launch_wsf_epi<96, wsf_default_stages(96)>(epi, tw, tx, a, stream);
+  return launch_wsf_epi<128, wsf_default_stages(128)>(epi, tw, tx, a, stream);
 }
 
 }  // namespace vlo

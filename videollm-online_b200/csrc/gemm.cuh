@@ -1,18 +1,18 @@
-// tcgen05 / TMA GEMM for sm_100a:   C[i, j] = sum_k A[i, k] * B[j, k]
+// wgmma / TMA GEMM for sm_90a:   C[i, j] = sum_k A[i, k] * B[j, k]
 //
 // Both operands are K-major ("TN"): A is [rows_a, K], B is [rows_b, K], 16-bit
-// (bf16 or fp16), fp32 accumulation in TMEM.  One CTA computes one 128 x BN
+// (bf16 or fp16), fp32 accumulation in registers.  One CTA computes one 128 x BN
 // tile (optionally one K-split of it):
-//   warp 0     TMA producer   (cp.async.bulk.tensor, 128B-swizzled boxes)
-//   warp 1     MMA issuer     (tcgen05.mma cta_group::1 kind::f16, one thread)
-//   warps 2-5  epilogue       (tcgen05.ld 32x32b -> registers -> global)
-// connected by an mbarrier full/empty ring plus one "accumulator ready" barrier.
+//   warps 0-3  one warpgroup: wgmma.mma_async m64nBNk16 on both 64-row halves of the
+//              tile, then the epilogue (accumulators -> shared staging tile -> global)
+//   warp 4     TMA producer   (cp.async.bulk.tensor, 128B-swizzled boxes)
+// connected by an mbarrier full/empty ring.
 //
 // Two orientations share the kernel:
 //   SWAP = false  A = activations [M, K], B = weights [N, K]; out[M, N]   (ViT: M = 576*B rows)
 //   SWAP = true   A = weights [N, K],     B = activations [T, K]; out[T, N]
-//                 "swap-AB": the weight matrix rides the 128-wide MMA-M dimension and
-//                 the (few) tokens are the MMA-N dimension (16..256), so a decoder step
+//                 "swap-AB": the weight matrix rides the 128-row M tile and the (few)
+//                 tokens are the wgmma N dimension (16..128), so a decoder step
 //                 with T = 11..96 tokens streams every weight byte exactly once at full
 //                 tensor-core tile efficiency.  The kernel is then HBM-bound.
 //
@@ -23,6 +23,7 @@
 #pragma once
 #include <cuda.h>
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace vlo {
 
@@ -50,17 +51,101 @@ struct GemmArgs {
 
 constexpr int kGemmBM = 128;
 constexpr int kGemmBK = 64;  // one 128-byte swizzle atom of 16-bit elements
-constexpr int kGemmThreads = 192;
+constexpr int kGemmThreads = 160;  // warps 0-3: MMA + epilogue warpgroup; warp 4: TMA producer
+constexpr int kGemmProducerWarp = 4;
+constexpr int kSmemOptIn = 232448;  // 227 KB: the per-block dynamic shared memory limit of sm_90
+
+// fp32 staging tile the accumulators pass through on their way to the epilogue, 16 columns at a time: [128][16 + 4].
+// 10 KB whatever the tile width, so the small-tile ViT configuration still fits on an SM beside a decoder CTA (gemm.cu).
+constexpr int kWgChunk = 16;
+constexpr int kWgStageLd = kWgChunk + 4;
+constexpr int kWgStageBytes = kGemmBM * kWgStageLd * 4;
+// deepest ring (<= cap stages of `per_stage` bytes) that fits next to `fixed` bytes in one block
+constexpr int fit_stages(int per_stage, int fixed, int cap) {
+  return (kSmemOptIn - fixed) / per_stage < cap ? (kSmemOptIn - fixed) / per_stage : cap;
+}
 
 template <int BN>
 struct GemmCfg {
-  static constexpr int kStages = BN <= 64 ? 8 : (BN <= 128 ? 6 : 4);
   static constexpr int kBytesA = kGemmBM * kGemmBK * 2;
   static constexpr int kBytesB = BN * kGemmBK * 2;
-  static constexpr int kTmemCols = BN < 32 ? 32 : BN;
-  // 1024 B of slack so the tile ring can be aligned for SWIZZLE_128B.
-  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256 + 1024;  // + bias tile
+  // 1024 B of slack so the tile ring can be aligned for SWIZZLE_128B, 256 B of barriers, 1 KB bias tile
+  static constexpr int kFixed = kWgStageBytes + 1024 + 256 + 1024;
+  static constexpr int kStages = fit_stages(kBytesA + kBytesB, kFixed, BN <= 64 ? 8 : 6);
+  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + kFixed;
 };
+
+__device__ __forceinline__ void wg_sync() { asm volatile("bar.sync 1, 128;\n" ::: "memory"); }  // the MMA warpgroup
+
+// The warpgroup's part of the ring protocol: accumulate the nk k-blocks at ring positions i, i+1, ... into acc
+// (zeroed first; acc[h] is the 64-row half h of the 128 x BN tile).  A stage goes back to the producer (one arrival per
+// warp, empty barriers count 4) once the MMAs reading it have retired; one k-block of MMAs stays in flight.
+template <int FMT, int BN, int S>
+__device__ __forceinline__ void wg_mainloop(float (&acc)[2][BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
+                                            uint64_t* full_bar, uint64_t* empty_bar, int& i, int nk) {
+  constexpr int kBytesA = kGemmBM * kGemmBK * 2, kBytesB = BN * kGemmBK * 2;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+  for (int j = 0; j < nk; ++j, ++i) {
+    const int s = i % S;
+    mbar_wait(&full_bar[s], (i / S) & 1);
+    wgmma_fence();
+    const uint64_t da = wgmma_desc_sw128(smem_u32(smem_a + s * kBytesA));
+    const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + s * kBytesB));
+#pragma unroll
+    for (int kk = 0; kk < kGemmBK / 16; ++kk) {
+      // +2 per 16 elements (32 B) along K; the second 64-row half of A starts 8 KB (+512) further
+      Wgmma<FMT, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
+      Wgmma<FMT, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (j > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+    }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  if (nk > 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+  }
+}
+
+// columns c0 .. c0 + 15 of the accumulators -> staging tile (row r of the tile at stage[r * kWgStageLd]); c0 must be a
+// compile-time constant after unrolling, so that acc stays in registers
+template <int BN>
+__device__ __forceinline__ void wg_stage_chunk(const float (&acc)[2][BN / 2], int c0, float* stage) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = 64 * h + 16 * warp + (lane >> 2);
+#pragma unroll
+    for (int c = 0; c < kWgChunk / 8; ++c) {
+      const int g = c0 / 8 + c;  // 8-column group of the accumulator fragment
+      const int col = 8 * c + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(stage + row * kWgStageLd + col) = make_float2(acc[h][4 * g], acc[h][4 * g + 1]);
+      *reinterpret_cast<float2*>(stage + (row + 8) * kWgStageLd + col) = make_float2(acc[h][4 * g + 2], acc[h][4 * g + 3]);
+    }
+  }
+}
+// the staged 16 columns of tile row `row`
+__device__ __forceinline__ void wg_load16(const float* stage, int row, float (&v)[16]) {
+  const float4* p = reinterpret_cast<const float4*>(stage + row * kWgStageLd);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float4 t = p[j];
+    v[4 * j] = t.x;
+    v[4 * j + 1] = t.y;
+    v[4 * j + 2] = t.z;
+    v[4 * j + 3] = t.w;
+  }
+}
 
 template <int FMT>
 __device__ __forceinline__ float r16(float x) {
@@ -110,8 +195,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
   uint8_t* smem_b = smem + S * Cfg::kBytesA;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * (Cfg::kBytesA + Cfg::kBytesB));
   uint64_t* empty_bar = full_bar + S;
-  uint64_t* accum_bar = empty_bar + S;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
+  float* s_bias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
+  float* stage = s_bias + 256;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -121,25 +206,20 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
   const int kb1 = min(kb0 + p.kb_per_split, total_kb);
   const int nkb = kb1 - kb0;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kGemmProducerWarp && lane == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);
     }
-    mbar_init(accum_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_trigger();  // after the TMEM allocation
+  pdl_trigger();
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == kGemmProducerWarp) {
     if (lane == 0) {
       // ------------------------------------------------ TMA producer
       for (int i = 0; i < nkb; ++i) {
@@ -152,60 +232,40 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         tma_load_2d(smem_b + s * Cfg::kBytesB, &tm_b, &full_bar[s], kc, n_tile * BN, p.hint_b);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------ MMA issuer
-      constexpr uint32_t idesc = umma_idesc_f16(FMT, kGemmBM, BN);
-      for (int i = 0; i < nkb; ++i) {
-        const int s = i % S;
-        const uint32_t ph = (i / S) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint64_t da = umma_desc_sw128(smem_u32(smem_a + s * Cfg::kBytesA));
-        const uint64_t db = umma_desc_sw128(smem_u32(smem_b + s * Cfg::kBytesB));
-#pragma unroll
-        for (int kk = 0; kk < kGemmBK / 16; ++kk) {
-          // advance 16 elements (32 B) along K inside the swizzle atom: +2 in 16-B units
-          umma_f16(tmem_base, da + 2 * kk, db + 2 * kk, idesc, (i > 0 || kk > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(accum_bar);
-    }
   } else {
-    // -------------------------------------------------- epilogue warps 2..5
-    const int q = warp & 3;  // TMEM lane quarter this warp may read
-    const int a_row = m_tile * kGemmBM + q * 32 + lane;
-    // per-column bias of this tile -> shared memory while the mainloop runs (SWAP = false only)
-    float* s_bias = reinterpret_cast<float*>(tmem_slot + 4);
+    // -------------------------------------------------- MMA + epilogue warpgroup (warps 0-3)
+    // per-column bias of this tile -> shared memory (SWAP = false only)
     if (!SWAP && EPI != EPI_PARTIAL) {
-      const int et = threadIdx.x - 64;  // 0..127
-      for (int j = et; j < BN; j += 128) {
+      for (int j = threadIdx.x; j < BN; j += 128) {
         const int col = n_tile * BN + j;
         s_bias[j] = (p.bias != nullptr && col < p.rows_b) ? __ldg(p.bias + col) : 0.f;
       }
-      asm volatile("bar.sync 1, 128;\n" ::: "memory");  // epilogue warps only
     }
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
+    float acc[2][BN / 2];
+    int i = 0;
+    wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nkb);
+    const int row = threadIdx.x;  // tile row this thread finishes
+    const int a_row = m_tile * kGemmBM + row;
     const bool a_ok = a_row < p.rows_a;
     float bias_a = 0.f;
     if (SWAP && EPI != EPI_PARTIAL && p.bias != nullptr && a_ok) bias_a = __ldg(p.bias + a_row);
 
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 16) {
-      uint32_t v[16];
-      tmem_ld_x16(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(c0), v);
-      tmem_ld_wait();
+#pragma unroll
+    for (int c0 = 0; c0 < BN; c0 += kWgChunk) {
+      wg_sync();                      // the previous chunk's readers are done with the staging tile
+      wg_stage_chunk<BN>(acc, c0, stage);
+      wg_sync();
       const int b0 = n_tile * BN + c0;
       if (!a_ok || b0 >= p.rows_b) continue;
+      float v[16];
+      wg_load16(stage, row, v);
       if (SWAP) {
         // out[token = b, feature = a]; lanes hold consecutive features -> coalesced.
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int b = b0 + j;
           if (b >= p.rows_b) break;
-          const float acc = __uint_as_float(v[j]);
+          const float acc = v[j];
           const size_t idx = static_cast<size_t>(b) * p.ld_out + a_row;
           if (EPI == EPI_PARTIAL) {
             reinterpret_cast<float*>(p.out)[static_cast<size_t>(split) * p.split_stride + idx] = acc;
@@ -227,7 +287,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         float x[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          float acc = __uint_as_float(v[j]);
+          float acc = v[j];
           if (EPI != EPI_PARTIAL) {
             acc = r16<FMT>(acc + s_bias[c0 + j]);
             if (EPI == EPI_STORE16) acc = apply_act<FMT>(acc, p.act);
@@ -279,12 +339,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 

@@ -1,16 +1,17 @@
 // Persistent weight-streaming GEMM (decoder / connector / lm_head):  out[t, n] = sum_k X[t, k] * W[n, k]
 //
-// Same tcgen05 / TMA machinery as gemm.cuh in its swap-AB orientation (W rows ride MMA-M = 128, the
-// T <= 128 tokens are MMA-N), but scheduled for an HBM-bound problem:
-//   * ONE CTA per SM, resident for the whole GEMM: barrier init, TMEM allocation and descriptor prefetch
+// Same wgmma / TMA machinery as gemm.cuh in its swap-AB orientation (W rows ride the 128-row M tile, the
+// T <= 128 tokens are the wgmma N dimension), but scheduled for an HBM-bound problem:
+//   * ONE CTA per SM, resident for the whole GEMM: barrier init and descriptor prefetch
 //     are paid once and the TMA ring never drains between work items;
 //   * stream-K: the (weight tile, 64-wide k-block) units are dealt out evenly, CTA c owns the contiguous
-//     unit range [c*U/G, (c+1)*U/G), so all 148 SMs stream the same number of bytes (no wave
+//     unit range [c*U/G, (c+1)*U/G), so all SMs stream the same number of bytes (no wave
 //     quantisation, no tail).  A CTA whose range crosses a tile boundary emits one fp32 partial per tile
 //     it touches into plane (c - first_cta_of_tile); the consumer kernels (resid_rmsnorm / qkv_rope /
 //     swiglu) add the planes of each tile in plane order -> deterministic;
 //   * TILES mode (lm_head, connector): whole tiles per CTA, direct 16-bit epilogue, no partials;
-//   * two TMEM accumulator buffers: the epilogue of item i overlaps the MMAs of item i+1.
+//   * the producer warp keeps the ring full across items, so the weight stream continues while the warpgroup
+//     runs the epilogue of an item.
 #pragma once
 #include <cuda.h>
 #include "gemm.cuh"
@@ -32,15 +33,16 @@ struct GemmWsArgs {
   unsigned long long hint_w;  // L2 policy for the weight stream (evict-first when read once per launch)
 };
 
-constexpr int ws_default_stages(int bn) { return bn <= 64 ? 8 : (bn <= 96 ? 7 : (bn <= 128 ? 6 : 5)); }
+// deepest ring of at most 8 stages that fits next to the staging tile
+constexpr int ws_default_stages(int bn) { return fit_stages(kGemmBM * kGemmBK * 2 + bn * kGemmBK * 2, kWgStageBytes + 1024 + 256, 8); }
 
 template <int BN, int STAGES = ws_default_stages(BN)>
 struct GemmWsCfg {
   static constexpr int kStages = STAGES;
   static constexpr int kBytesA = kGemmBM * kGemmBK * 2;
   static constexpr int kBytesB = BN * kGemmBK * 2;
-  static constexpr int kTmemCols = 2 * BN <= 32 ? 32 : (2 * BN <= 64 ? 64 : (2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512)));
-  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256;
+  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256 + kWgStageBytes;
+  static_assert(kSmemBytes <= kSmemOptIn, "ring + staging tile exceed the shared memory of one block");
 };
 
 template <int FMT, int BN, int STAGES = ws_default_stages(BN)>
@@ -56,9 +58,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   uint8_t* smem_b = smem + S * Cfg::kBytesA;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * (Cfg::kBytesA + Cfg::kBytesB));
   uint64_t* empty_bar = full_bar + S;
-  uint64_t* acc_full = empty_bar + S;   // [2]
-  uint64_t* acc_empty = acc_full + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  float* stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = blockIdx.x;
@@ -71,33 +71,24 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     u0 = ((static_cast<long long>(c) * p.tiles) / p.sk.G) * kb;
     u1 = ((static_cast<long long>(c + 1) * p.tiles) / p.sk.G) * kb;
   }
+  const bool producer = warp == kGemmProducerWarp && lane == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (producer) {
     tma_prefetch_desc(&tm_w);
     tma_prefetch_desc(&tm_x);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);
+      mbar_init(&empty_bar[s], 4);
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Our TMEM is allocated: successors may be scheduled now (never before the allocation: a successor that grabbed
-  // this SM's TMEM first while we still had to allocate would dead-lock us).  Early triggering lets the next kernels of
-  // the step become resident and prefetch while this one streams.
+  // Early triggering lets the next kernels of the step become resident and prefetch while this one streams.
   pdl_trigger();
   // The weight operand never depends on any earlier kernel: the producer starts streaming the first S weight
   // k-blocks right away, i.e. while the predecessors are still running.
   int pre = 0;
-  if (warp == 0 && lane == 0) {
+  if (producer) {
     for (long long u = u0; u < u1 && pre < S; ++u, ++pre) {
       const int tile = static_cast<int>(u / kb);
       const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
@@ -109,7 +100,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   // everything above overlapped the predecessors; their results (the activations) are needed from here on
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == kGemmProducerWarp) {
     if (lane == 0) {
       // ------------------------------------------------ TMA producer: one continuous stream of k-blocks
       int i = 0;
@@ -127,50 +118,20 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         tma_load_2d(smem_b + s * Cfg::kBytesB, &tm_x, &full_bar[s], kblk * kGemmBK, xt * BN, kEvictLast);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------ MMA issuer
-      constexpr uint32_t idesc = umma_idesc_f16(FMT, kGemmBM, BN);
-      int i = 0, item = 0;
-      for (long long u = u0; u < u1; ++item) {
-        const int tile = static_cast<int>(u / kb);
-        const int k0 = static_cast<int>(u - static_cast<long long>(tile) * kb);
-        const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
-        const int buf = item & 1;
-        mbar_wait(&acc_empty[buf], (((item >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + static_cast<uint32_t>(buf * BN);
-        for (int j = 0; j < nk; ++j, ++i) {
-          const int s = i % S;
-          const uint32_t ph = (i / S) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(smem_a + s * Cfg::kBytesA));
-          const uint64_t db = umma_desc_sw128(smem_u32(smem_b + s * Cfg::kBytesB));
-#pragma unroll
-          for (int kk = 0; kk < kGemmBK / 16; ++kk)
-            umma_f16(tacc, da + 2 * kk, db + 2 * kk, idesc, (j > 0 || kk > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&acc_full[buf]);
-        u += nk;
-      }
-    }
   } else {
-    // -------------------------------------------------- epilogue warps 2..5
-    const int q = warp & 3;
-    int item = 0;
-    for (long long u = u0; u < u1; ++item) {
+    // -------------------------------------------------- MMA + epilogue warpgroup (warps 0-3)
+    const int row = threadIdx.x;  // tile row (output feature inside the weight tile) this thread finishes
+    int i = 0;
+    for (long long u = u0; u < u1;) {
       const int tile = static_cast<int>(u / kb);
       const int k0 = static_cast<int>(u - static_cast<long long>(tile) * kb);
       const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
       u += nk;
-      const int buf = item & 1;
-      mbar_wait(&acc_full[buf], (item >> 1) & 1);
-      tc_fence_after();
+      float acc[2][BN / 2];
+      wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int wt = tile / p.x_tiles, xt = tile - wt * p.x_tiles;
-      const int n = wt * kGemmBM + q * 32 + lane;  // output feature (row of W)
-      const int t0 = xt * BN;                      // first token row of this tile
+      const int n = wt * kGemmBM + row;  // output feature (row of W)
+      const int t0 = xt * BN;            // first token row of this tile
       const bool n_ok = n < p.rows_w;
       float* plane = nullptr;
       float bias_n = 0.f;
@@ -180,23 +141,19 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       } else if (p.bias != nullptr && n_ok) {
         bias_n = __ldg(p.bias + n);
       }
-      const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(buf * BN);
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld_x16(tacc + static_cast<uint32_t>(c0), v);
-        tmem_ld_wait();
-        if (c0 + 16 >= BN) {  // last chunk is in registers: hand the accumulator buffer back
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[buf]);
-        }
+#pragma unroll
+      for (int c0 = 0; c0 < BN; c0 += kWgChunk) {
+        wg_sync();                            // the previous chunk's readers are done with the staging tile
+        wg_stage_chunk<BN>(acc, c0, stage);
+        wg_sync();
         if (!n_ok || t0 + c0 >= p.rows_x) continue;
+        float v[16];
+        wg_load16(stage, row, v);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int t = t0 + c0 + j;
           if (t >= p.rows_x) break;
-          const float acc = __uint_as_float(v[j]);
+          const float acc = v[j];
           if (p.mode == 0) {
             plane[static_cast<size_t>(t) * p.rows_w + n] = acc;
           } else {
@@ -207,12 +164,6 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 

@@ -1,19 +1,19 @@
 // Persistent stream-K weight-streaming GEMM with the fix-up FUSED into its epilogue (decoder GEMMs, bf16):
 //   out[t, n] = sum_k X[t, k] * W[n, k]      X = the step's <= 128 tokens (MMA-N), W rows ride MMA-M (128-row tiles)
 //
-// Same TMA ring / tcgen05 / stream-K schedule as gemm_ws.cuh (CTA c owns the contiguous unit range [c*U/G, (c+1)*U/G),
+// Same TMA ring / wgmma / stream-K schedule as gemm_ws.cuh (CTA c owns the contiguous unit range [c*U/G, (c+1)*U/G),
 // unit = (weight tile, 64-wide k-block)), but the partial sums of a tile no longer go through a separate fix-up kernel:
 //   * the FIRST contributing CTA of a tile is its finisher.  It works on the tile's k-blocks LAST (the tail of its unit
 //     range), whereas every other contributor meets the tile at the very START of its range - so by the time the
 //     finisher's accumulator is complete the other partials have long been published;
 //   * contributors write their fp32 partial plane, fence, and bump the tile's arrival counter (flags[tile]);
-//   * the finisher waits for the counter (normally already there), adds the planes in plane order to its own TMEM
+//   * the finisher waits for the counter (normally already there), adds the planes in plane order to its own
 //     accumulator (deterministic), resets the counter and applies the fused epilogue:
 //       WSF_RESID   h[t, n] = bf16(h[t, n] + bf16(y))                       (o_proj / down_proj + residual, HF:...llama.py:325,331)
 //       WSF_QKV     RoPE on q / k heads (tile == head), Q -> q_out, K / V appended IN PLACE to the cache
 //                   (HF:...llama.py:262-264, 146-168; cache_utils.py:119-120)
 //       WSF_SWIGLU  act = bf16(bf16(silu(g)) * u)  with gate / up rows interleaved per tile (64 + 64)   (HF:...llama.py:182-184)
-//     the two halves of a head (d, d + 64) and gate / up sit in different lane quadrants: they are exchanged through a
+//     the two halves of a head (d, d + 64) and gate / up are finished by different threads: they are exchanged through a
 //     small shared-memory tile.  Rounding points are those of decoder_kernels.cuh.
 // All CTAs of the grid are co-resident or become so without depending on a waiting CTA (grid <= #SMs, the PDL successor
 // cannot start before every CTA of this grid has started), so the finisher's wait cannot dead-lock; it is bounded anyway.
@@ -57,17 +57,20 @@ struct GemmWsfCfg {
   static constexpr int kStages = STAGES;
   static constexpr int kBytesA = kGemmBM * kGemmBK * 2;
   static constexpr int kBytesB = BN * kGemmBK * 2;
-  static constexpr int kTmemCols = 2 * BN <= 32 ? 32 : (2 * BN <= 64 ? 64 : (2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512)));
   static constexpr int kXchBytes = kGemmBM * kWsfXchStride * 4;
-  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256 + kXchBytes;
+  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256 + kXchBytes + kWgStageBytes;
+  static_assert(kSmemBytes <= kSmemOptIn, "ring + exchange + staging tiles exceed the shared memory of one block");
 };
+// deepest ring of at most 8 stages that fits next to the exchange and staging tiles
+constexpr int wsf_default_stages(int bn) {
+  return fit_stages(kGemmBM * kGemmBK * 2 + bn * kGemmBK * 2, 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 8);
+}
 
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
   asm volatile("ld.acquire.gpu.global.s32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ void epi_group_sync() { asm volatile("bar.sync 1, 128;\n" ::: "memory"); }  // the 4 epilogue warps
 
 template <int BN, int STAGES, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -80,38 +83,29 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
   uint8_t* smem_b = smem + S * Cfg::kBytesA;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * (Cfg::kBytesA + Cfg::kBytesB));
   uint64_t* empty_bar = full_bar + S;
-  uint64_t* acc_full = empty_bar + S;   // [2]
-  uint64_t* acc_empty = acc_full + 2;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float* xch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);   // [128][17] exchange tile
+  float* stage = xch + kGemmBM * kWsfXchStride;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = blockIdx.x;
   const int kb = p.sk.kb;
   const long long u0 = sk_lo(c, p.sk), u1 = sk_lo(c + 1, p.sk);
+  const bool producer = warp == kGemmProducerWarp && lane == 0;
 
-  if (warp == 0 && lane == 0) {
+  if (producer) {
     tma_prefetch_desc(&tm_w);
     tma_prefetch_desc(&tm_x);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&acc_full[b], 1);
-      mbar_init(&acc_empty[b], 4);
+      mbar_init(&empty_bar[s], 4);
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_trigger();   // after the TMEM allocation (see gemm_ws.cuh)
+  pdl_trigger();
   // the weight operand never depends on an earlier kernel: fill the ring while the predecessors are still running
   int pre = 0;
-  if (warp == 0 && lane == 0) {
+  if (producer) {
     for (long long u = u0; u < u1 && pre < S; ++u, ++pre) {
       const int tile = static_cast<int>(u / kb);
       const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
@@ -121,7 +115,7 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
   }
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == kGemmProducerWarp) {
     if (lane == 0) {
       // ------------------------------------------------ TMA producer: one continuous stream of k-blocks
       int i = 0;
@@ -138,76 +132,41 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
         tma_load_2d(smem_b + s * Cfg::kBytesB, &tm_x, &full_bar[s], kblk * kGemmBK, 0, kEvictLast);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------------------------ MMA issuer
-      constexpr uint32_t idesc = umma_idesc_f16(FMT_BF16, kGemmBM, BN);
-      int i = 0, item = 0;
-      for (long long u = u0; u < u1; ++item) {
-        const int tile = static_cast<int>(u / kb);
-        const int k0 = static_cast<int>(u - static_cast<long long>(tile) * kb);
-        const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
-        const int buf = item & 1;
-        mbar_wait(&acc_empty[buf], (((item >> 1) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + static_cast<uint32_t>(buf * BN);
-        for (int j = 0; j < nk; ++j, ++i) {
-          const int s = i % S;
-          const uint32_t ph = (i / S) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint64_t da = umma_desc_sw128(smem_u32(smem_a + s * Cfg::kBytesA));
-          const uint64_t db = umma_desc_sw128(smem_u32(smem_b + s * Cfg::kBytesB));
-#pragma unroll
-          for (int kk = 0; kk < kGemmBK / 16; ++kk)
-            umma_f16(tacc, da + 2 * kk, db + 2 * kk, idesc, (j > 0 || kk > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&acc_full[buf]);
-        u += nk;
-      }
-    }
   } else {
-    // -------------------------------------------------- epilogue warps 2..5: contributor or finisher per item
-    const int q = warp & 3;
-    const int d = q * 32 + lane;          // row of the weight tile (output feature inside the tile)
-    int item = 0;
-    for (long long u = u0; u < u1; ++item) {
+    // -------------------------------------------------- MMA + epilogue warpgroup: contributor or finisher per item
+    const int d = threadIdx.x;            // row of the weight tile (output feature inside the tile)
+    int i = 0;
+    for (long long u = u0; u < u1;) {
       const int tile = static_cast<int>(u / kb);
       const int k0 = static_cast<int>(u - static_cast<long long>(tile) * kb);
       const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
       u += nk;
-      const int buf = item & 1;
+      float acc[2][BN / 2];
+      wg_mainloop<FMT_BF16, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int pl = c - sk_first_cta(tile, p.sk);
       const int n_planes = sk_planes(tile, p.sk);
       const int n = tile * kGemmBM + d;
       const bool n_ok = n < p.rows_w;
-      mbar_wait(&acc_full[buf], (item >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tacc = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(buf * BN);
       if (pl > 0) {
         // ---- contributor: publish the partial plane, then bump the tile's arrival counter
         float* plane = p.planes + static_cast<size_t>(pl - 1) * p.plane_stride;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 16) {
-          uint32_t v[16];
-          tmem_ld_x16(tacc + static_cast<uint32_t>(c0), v);
-          tmem_ld_wait();
-          if (c0 + 16 >= BN) {
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&acc_empty[buf]);
-          }
+#pragma unroll
+        for (int c0 = 0; c0 < BN; c0 += kWgChunk) {
+          wg_sync();                                  // the previous chunk's readers are done with the staging tile
+          wg_stage_chunk<BN>(acc, c0, stage);
+          wg_sync();
           if (!n_ok || c0 >= p.rows_x) continue;
+          float v[16];
+          wg_load16(stage, d, v);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int t = c0 + j;
             if (t >= p.rows_x) break;
-            __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, __uint_as_float(v[j]));
+            __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, v[j]);
           }
         }
         __threadfence();
-        epi_group_sync();
+        wg_sync();
         if (d == 0) atomicAdd(p.flags + tile, 1);
         continue;
       }
@@ -218,29 +177,25 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
           while (ld_acquire_gpu(p.flags + tile) < n_planes - 1) {
             __nanosleep(32);
             if (++spins > (1u << 22)) {
+#if VLO_MBAR_TRACE
               printf("vlo: stream-K finisher timeout cta %d tile %d\n", c, tile);
+#endif
               __trap();
             }
           }
           p.flags[tile] = 0;   // next launch starts from zero again (no other reader or writer is left)
         }
-        epi_group_sync();
+        wg_sync();
         __threadfence();
       }
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t v[16];
-        tmem_ld_x16(tacc + static_cast<uint32_t>(c0), v);
-        tmem_ld_wait();
-        if (c0 + 16 >= BN) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[buf]);
-        }
-        if (c0 >= p.rows_x) continue;    // (uniform over the epilogue group: the barriers below stay aligned)
-        float x[16];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) x[j] = __uint_as_float(v[j]);
+      for (int c0 = 0; c0 < BN; c0 += kWgChunk) {
+        if (c0 >= p.rows_x) continue;    // (uniform over the warpgroup: the barriers below stay aligned)
+        wg_sync();                            // the previous chunk's readers are done with the staging tile
+        wg_stage_chunk<BN>(acc, c0, stage);
+        wg_sync();
+        float x[16];
+        wg_load16(stage, d, x);
         for (int s2 = 1; s2 < n_planes; ++s2) {   // plane order: deterministic
           const float* plane = p.planes + static_cast<size_t>(s2 - 1) * p.plane_stride + n;
           float a[16];
@@ -268,10 +223,10 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
           if (rot) {                                             // partner half (d ^ 64) through shared memory
 #pragma unroll
             for (int j = 0; j < 16; ++j) xch[d * kWsfXchStride + j] = x[j];
-            epi_group_sync();
+            wg_sync();
 #pragma unroll
             for (int j = 0; j < 16; ++j) xp[j] = xch[(d ^ 64) * kWsfXchStride + j];
-            epi_group_sync();
+            wg_sync();
           }
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
@@ -300,7 +255,7 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
 #pragma unroll
             for (int j = 0; j < 16; ++j) xch[(d - 64) * kWsfXchStride + j] = x[j];
           }
-          epi_group_sync();
+          wg_sync();
           if (d < 64) {
             const int f = tile * 64 + d;
 #pragma unroll
@@ -312,16 +267,10 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
               p.act[static_cast<size_t>(t) * p.I + f] = __float2bfloat16_rn(a * up);
             }
           }
-          epi_group_sync();
+          wg_sync();
         }
       }
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::kTmemCols>(tmem_base);
   }
 }
 

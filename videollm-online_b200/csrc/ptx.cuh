@@ -1,7 +1,6 @@
-// Inline-PTX helpers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05
-// (TMEM alloc / mma / commit / ld) and small utilities.  Everything in here is
-// Blackwell-only; the translation units that include it are compiled with
-// -gencode arch=compute_100a,code=sm_100a and nothing else.
+// Inline-PTX helpers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), programmatic dependent launch
+// and small utilities.  The translation units that include it are compiled with
+// -gencode arch=compute_90a,code=sm_90a and nothing else.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -57,6 +56,11 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 #ifndef VLO_MBAR_BOUND_LOG2
 #define VLO_MBAR_BOUND_LOG2 24   // debug builds (build.py --debug -> libvlo_b200_dbg.so, VLO_LIB=...) use 16: a stuck wait traps within seconds
 #endif
+// Debug builds also print the stuck (block, thread) before trapping.  Release builds do not: a printf call anywhere in a
+// kernel makes ptxas serialise its wgmma instructions.
+#ifndef VLO_MBAR_TRACE
+#define VLO_MBAR_TRACE 0
+#endif
 // non-blocking probe (mbarrier.test_wait): true when the phase with this parity has completed
 __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
@@ -75,8 +79,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > (1u << VLO_MBAR_BOUND_LOG2)) {
+#if VLO_MBAR_TRACE
       printf("vlo: mbarrier timeout block(%d,%d,%d) thread %d parity %u\n", blockIdx.x, blockIdx.y,
              blockIdx.z, threadIdx.x, parity);
+#endif
       __trap();
     }
   }
@@ -109,88 +115,14 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_slot)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// All previously issued MMAs arrive on `bar` when they retire (implies
-// tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
-}
-
-// UMMA shared-memory matrix descriptor for a K-major tile stored as rows of
-// 128 B with the 128-byte swizzle (what a TMA box {64 x rows} of 16-bit
-// elements with CU_TENSOR_MAP_SWIZZLE_128B produces).  8-row groups are 1024 B
-// apart (SBO); LBO is unused for swizzled K-major tiles.  Bit layout follows
-// the PTX ISA "matrix descriptor" (start>>4 @0, LBO>>4 @16, SBO>>4 @32,
-// version=1 @46, layout_type=SWIZZLE_128B(2) @61).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor, kind::f16: fp32 accumulate, A and B both K-major.
-// fmt: 0 = fp16, 1 = bf16.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int fmt, int m, int n) {
-  return (1u << 4) | (static_cast<uint32_t>(fmt) << 7) | (static_cast<uint32_t>(fmt) << 10) |
-         (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
-
 // ---------------------------------------------- programmatic dependent launch (PDL)
 // A kernel launched with the programmatic-stream-serialization attribute may start while its
 // predecessor in the stream is still running; it must execute pdl_wait() before touching anything the
 // predecessor produces (the wait returns once the predecessor grid has completed and flushed).
 // pdl_trigger() lets the successor start being scheduled; everything before pdl_wait() in the
-// successor (barrier init, TMEM allocation, descriptor prefetch, weight / old-KV prefetch) then overlaps
+// successor (barrier init, descriptor prefetch, weight / old-KV prefetch) then overlaps
 // this grid.  Rules used throughout the step:
-//   * trigger EARLY (kernel entry, or right after the TMEM allocation for kernels that allocate TMEM — a
-//     successor must never be able to take an SM's TMEM before a CTA of this grid that still has to allocate);
+//   * trigger EARLY (kernel entry or right after the barrier set-up);
 //   * before pdl_wait() a kernel only reads data that no kernel of the current step writes (weights, the
 //     per-step tables uploaded by memcpy before the step's first kernel, K/V rows of earlier steps) and
 //     writes nothing to global memory.

@@ -27,6 +27,17 @@ bool pdl_enabled() {
   return on == 1 && !prof_on();
 }
 
+// SMs of the current device (132 on an H100 SXM): persistent grids and split planning size themselves by it
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+  }
+  return n;
+}
+
 int ensure_max_smem(const void* func, int bytes) {
   static std::mutex mu;
   static std::vector<std::pair<int, const void*>> done;

@@ -1,4 +1,4 @@
-// Vision-tower kernels around the tcgen05 GEMMs: pixel rescale/normalise + patchify, LayerNorm,
+// Vision-tower kernels around the wgmma GEMMs: pixel rescale/normalise + patchify, LayerNorm,
 // the 576-token non-causal self-attention, 3x3 adaptive average pool, the MAP-head probe attention
 // and the final token assembly.  Dtype flow follows the reference's GPU path — fp16 autocast
 // operands, fp32 LayerNorm and residual stream (models/vision_live.py:10-30 under

@@ -52,7 +52,7 @@ class Engine:
         self.cfg = cfg
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise VloError("the vlo_b200 engine runs on a CUDA (sm_100a) device only; there is no CPU path")
+            raise VloError("the vlo_b200 engine runs on a CUDA (sm_90a) device only; there is no CPU path")
         if not torch.cuda.is_available():
             raise VloError("no CUDA device visible: the hot path cannot run (no fallback by design)")
         self.index = self.device.index if self.device.index is not None else torch.cuda.current_device()

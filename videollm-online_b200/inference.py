@@ -64,10 +64,10 @@ class LiveInfer:
         # during the current step anyway).  Set prefetch_next = False for strictly sequential behaviour.
         self.prefetch_next = True
         # frames encoded per encode-ahead call.  1 (default): the next frame only, through the small-tile ViT configuration
-        # that shares the SMs with the decoder step (measured 211 frames/s in the pipelined loop, versus 202 for groups of 4).
+        # that shares the SMs with the decoder step.
         # With a loaded clip a larger depth sends the next `prefetch_depth` frames through ONE batched ViT pass (the
         # reference itself batches every frame between two input_video_stream calls, demo/inference.py:106); from 3 frames
-        # on that pass uses the 2-CTA tensor-bound GEMMs, which the engine serialises against decoder steps.
+        # on that pass uses the wide-tile tensor-bound GEMM configuration.
         self.prefetch_depth = 1
         self._side = torch.cuda.Stream(self.device)
         # demo/app.py drives input_video_stream and __call__ from separate Gradio callbacks (SURVEY 3.2): both touch the

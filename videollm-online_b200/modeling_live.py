@@ -285,7 +285,7 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
     """models/modeling_live.py:184-222 for inference: build config + tokenizer, load (or synthesise)
     weights, merge LoRA, hand everything to the engine."""
     if is_training:
-        raise NotImplementedError("the B200 engine covers the streaming-inference path only")
+        raise NotImplementedError("the vlo_b200 engine covers the streaming-inference path only")
     cfg = config or llama3_8b_siglip_l()
     for k in ("frame_resolution", "frame_token_cls", "frame_token_pooled", "frame_num_tokens", "frame_token_interval",
               "vision_pretrained"):
