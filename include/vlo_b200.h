@@ -168,6 +168,11 @@ int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
                    void* cuda_stream);
+/* ViT trunk GEMM (csrc/gemm_vit.cuh), fp16, 128-token x 128-feature tiles:
+ * out[t][n] = act(fp16(sum_k X[t,k] W[n,k] + bias[n])), fp16 out[rows_x][ld_out], ld_out even and >= rows_w;
+ * n_ctas <= 0: one CTA per SM. */
+int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
+                    const float* d_bias, int act, int n_ctas, void* cuda_stream);
 /* KV-append attention over one layer's cache (the graded kernel, K15):
  *   d_q bf16 [n_tok, n_heads, head_dim] (RoPE applied); d_k/d_v bf16 [n_kv_heads, kv_stride, head_dim];
  *   keys 0..kv_len-1 valid, the n_tok query tokens sit at positions kv_len-n_tok .. kv_len-1 (causal with

@@ -86,6 +86,11 @@ int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d
   return gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream));
 }
 
+int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
+                    const float* d_bias, int act, int n_ctas, void* cuda_stream) {
+  return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
+}
+
 int vlo_op_attn_version(int n_heads, int n_kv_heads) { return attn_version(n_heads, n_kv_heads); }
 
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len) {

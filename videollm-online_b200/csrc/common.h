@@ -125,6 +125,11 @@ struct GemmWsCall {
 int gemm_ws_plan(int rows_w, int k, int mode, int n_ctas, SkInfo* sk, int* max_planes, int x_tiles = 1);
 int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream);
 
+// ---- ViT trunk GEMM, 128-token x 128-feature tiles (gemm_vit.cuh / gemm.cu): fp16 x [rows_x, k], w [rows_w, k] ->
+// fp16 out[rows_x][ld_out] = act(fp16(x w^T + bias)); n_ctas <= 0 -> one CTA per SM
+int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
+                    const float* bias, int act, int n_ctas, cudaStream_t stream);
+
 // ---- stream-K GEMM with the fused finisher epilogue (gemm_wsf.cuh / gemm.cu); args struct defined in gemm_wsf.cuh
 struct GemmWsfArgs;
 int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, int epi, cudaStream_t stream);

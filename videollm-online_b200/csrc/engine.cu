@@ -651,28 +651,28 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     count_launch();
     return 0;
   };
-  // Trunk GEMMs on the persistent swap-AB kernel (weights ride MMA-M, the 576*B token rows are tiled along
-  // MMA-N): QKV and fc1 run whole tiles with the fused bias / GELU fp16 epilogue; out_proj and fc2 (few
-  // output tiles) run stream-K over all SMs and their partial planes are folded into the fp32 residual
-  // stream together with the NEXT LayerNorm by vit_fix_ln_kernel.
-  // Small batches (the single-stream case) run the trunk GEMMs with 64-token tiles and a shallow ring (83 KB of
-  // shared memory): such a CTA fits on an SM NEXT TO a decoder weight-streaming CTA (119 KB; gemm.cu checks the sum),
-  // so the tensor-bound ViT of frame i+1 and the HBM-bound decoder step of frame i can execute concurrently (two CUDA
-  // streams).
+  // Trunk GEMMs: QKV and fc1 run whole tiles with the fused bias / GELU fp16 epilogue; out_proj and fc2 (few
+  // output tiles) run stream-K over all SMs on the persistent swap-AB kernel (weights ride MMA-M, the token rows are
+  // tiled along MMA-N) and their partial planes are folded into the fp32 residual stream together with the NEXT
+  // LayerNorm by vit_fix_ln_kernel.
+  // Small batches (the single-stream case) use CTAs that fit on an SM NEXT TO a decoder weight-streaming CTA (119 KB;
+  // gemm.cu checks the sums), so the tensor-bound ViT of frame i+1 and the HBM-bound decoder step of frame i execute
+  // concurrently (two CUDA streams): QKV and fc1 on gemm_vit_kernel (128-token x 128-feature tiles, tokens on MMA-M,
+  // 97 KB), out_proj and fc2 with 64-token tiles and a 3-stage ring (83 KB).  gemm_vit_kernel gives QKV / fc1 the
+  // same bits as 64-token swap-AB tiles would; the stream-K planes keep the 64-token decomposition, whose summation
+  // order the frame embeddings depend on.  VLO_VIT_SMALL_BN=96 runs all four on 96-token swap-AB tiles (95 KB).
   static int coreside = -1;
   if (coreside < 0) {
     const char* ev = getenv("VLO_VIT_CORESIDE");
     coreside = (ev != nullptr && ev[0] == '0') ? 0 : 1;
   }
   const bool small = coreside && B <= 2;
-  // token-tile width of the co-resident configuration (VLO_VIT_SMALL_BN=64|96; ring = 3 stages of 16 KB + bn * 128 B).
-  // 64 by measurement on the H100 (pipelined frame step 1.3 % faster than with 96, DESIGN.md section 5); both divide
-  // the 576 tokens of a frame.
   static int small_bn = 0;
   if (small_bn == 0) {
     const char* ev = getenv("VLO_VIT_SMALL_BN");
     small_bn = (ev != nullptr && atoi(ev) == 96) ? 96 : 64;
   }
+  const bool trunk_vit = small && small_bn == 64;
   auto pick_bn = [&](int n_out, int mode) {
     if (small) return small_bn;
     const int cands[4] = {64, 96, 128, 192};
@@ -703,6 +703,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     g.ld_out = n_out;
     g.bias = bias;
     g.act = act;
+    if (trunk_vit) return gemm_vit_launch(x, rows, w, n_out, k, out, n_out, bias, act, vit_ctas(), st);
     g.bn = pick_bn(n_out, 1);
     g.weights_hot = 1;
     g.small_smem = small ? 1 : 0;

@@ -2,6 +2,7 @@
 // resolved at run time, so the library loads on a box without libcuda), tile-shape
 // selection and kernel dispatch.
 #include "gemm.cuh"
+#include "gemm_vit.cuh"
 #include "gemm_ws.cuh"
 #include "gemm_wsf.cuh"
 
@@ -231,15 +232,22 @@ int gemm_launch(const GemmCall& c, cudaStream_t stream) {
 // ------------------------------------------------------------------------------------------------
 // persistent weight-streaming GEMM (gemm_ws.cuh)
 
-// The default single-stream frame step runs the ViT of frame i+1 (small-tile configuration: 96- or 64-token tiles,
-// 3 stages) next to the decoder step of frame i (16-token tiles, 6 stages).  One CTA of each fits on one sm_90 SM:
-// 228 KB of shared memory per SM, of which 1 KB is reserved per resident block.  (4 ViT stages, VLO_VIT_STAGES=4, and
-// the 8-stage fused gate|up GEMM do not leave room for the other CTA.)
+// The default single-stream frame step runs the ViT of frame i+1 (gemm_vit_kernel for QKV / fc1, the 64-token
+// small-tile configuration of gemm_ws_kernel for out_proj / fc2; or the 96-token one for all four) next to the
+// decoder step of frame i (16-token tiles, 6 stages).  One CTA of each fits on one sm_90 SM: 228 KB of shared memory
+// per SM, of which 1 KB is reserved per resident block.  The fused gate|up GEMM leaves room for a gemm_vit_kernel CTA
+// with a 6-stage ring, not with 8 (VLO_WSF_STAGES).
 constexpr int kSmemPerSm = 233472, kSmemReservedPerBlock = 1024;
 static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<96, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
               "decoder GEMM CTA and 96-token ViT GEMM CTA no longer share an SM");
 static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
               "decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
+static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
+static_assert(GemmWsfCfg<16, 6>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "6-stage fused decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
+static_assert(GemmWsfCfg<16, 8>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
+              "the 8-stage fused decoder GEMM now shares its SM with a ViT trunk GEMM CTA: update the comment above");
 
 namespace {
 template <int FMT, int BN, int STAGES = ws_default_stages(BN)>
@@ -315,16 +323,8 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
     if (st == 6) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
     if (st == 11) return launch_ws<FMT_BF16, 16, 11>(tw, tx, a, stream);
   }
-  if (c.fmt == FMT_F16 && c.small_smem && bn == 96) return launch_ws<FMT_F16, 96, 3>(tw, tx, a, stream);    // 84 KB ring
-  if (c.fmt == FMT_F16 && bn == 64 && c.small_smem) {
-    static int vst = 0;
-    if (vst == 0) {
-      const char* e = getenv("VLO_VIT_STAGES");
-      vst = e ? atoi(e) : 3;
-    }
-    if (vst == 4) return launch_ws<FMT_F16, 64, 4>(tw, tx, a, stream);
-    return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);
-  }
+  if (c.fmt == FMT_F16 && c.small_smem && bn == 96) return launch_ws<FMT_F16, 96, 3>(tw, tx, a, stream);    // 95 KB
+  if (c.fmt == FMT_F16 && c.small_smem && bn == 64) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
   VLO_WS_CASE(FMT_BF16, 16)
   VLO_WS_CASE(FMT_BF16, 32)
   VLO_WS_CASE(FMT_BF16, 64)
@@ -338,6 +338,38 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
   VLO_WS_CASE(FMT_F16, 192)
 #undef VLO_WS_CASE
   return fail("gemm_ws_launch: no kernel instance");
+}
+
+// ------------------------------------------------------------------------------------------------
+// ViT trunk GEMM, tokens on wgmma M (gemm_vit.cuh)
+
+int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
+                    const float* bias, int act, int n_ctas, cudaStream_t stream) {
+  VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
+  VLO_CHECK(rows_w > 0 && rows_x > 0, "empty GEMM operand");
+  VLO_CHECK(ld_out % 2 == 0 && ld_out >= rows_w, "gemm_vit: even output row stride >= rows_w (pairs of fp16 are stored)");
+  GemmVitArgs a{};
+  a.rows_x = rows_x;
+  a.rows_w = rows_w;
+  a.k = k;
+  a.m_tiles = (rows_x + kGemmBM - 1) / kGemmBM;
+  a.tiles = a.m_tiles * ((rows_w + kGemmBM - 1) / kGemmBM);
+  a.out = static_cast<__half*>(out);
+  a.ld_out = ld_out;
+  a.bias = bias;
+  a.act = act;
+  const int G = std::min(n_ctas > 0 ? n_ctas : num_sms(), a.tiles);
+  CUtensorMap tx, tw;
+  if (get_tmap(x, rows_x, k, kGemmBM, FMT_F16, &tx) != 0) return -1;
+  if (get_tmap(w, rows_w, k, kGemmBM, FMT_F16, &tw) != 0) return -1;
+  auto kern = gemm_vit_kernel;
+  if (ensure_max_smem(reinterpret_cast<const void*>(kern), GemmVitCfg::kSmemBytes)) return -1;
+  if (prof_on())
+    prof_begin(PROF_GEMM_VIT, stream, 2.0 * k * (static_cast<double>(rows_w) + rows_x) + 2.0 * rows_x * rows_w);
+  VLO_CUDA(launch_pdl(kern, dim3(G), dim3(kVitGemmThreads), GemmVitCfg::kSmemBytes, stream, tx, tw, a));
+  prof_end(stream);
+  count_launch();
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------

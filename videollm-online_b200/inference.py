@@ -63,8 +63,8 @@ class LiveInfer:
         # decoder works on the current one (same per-frame arithmetic; a live stream delivers the next frame
         # during the current step anyway).  Set prefetch_next = False for strictly sequential behaviour.
         self.prefetch_next = True
-        # frames encoded per encode-ahead call.  1 (default): the next frame only, through the small-tile ViT configuration
-        # that shares the SMs with the decoder step.
+        # frames encoded per encode-ahead call.  1 (default): the next frame only, through the ViT trunk GEMM whose CTAs
+        # share the SMs with the decoder step.
         # With a loaded clip a larger depth sends the next `prefetch_depth` frames through ONE batched ViT pass (the
         # reference itself batches every frame between two input_video_stream calls, demo/inference.py:106); from 3 frames
         # on that pass uses the wide-tile tensor-bound GEMM configuration.
