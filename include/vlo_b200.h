@@ -156,10 +156,13 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
 
 /* ------------------------------------------------------------------ kernel-level entry points
  * (used by the parity tests and micro-benchmarks; same kernels the engine launches) */
-/* C = A[rows_a,k] * B[rows_b,k]^T on wgmma; see csrc/gemm.cuh for fmt/epi/act codes */
-int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a, const void* d_b, int rows_b, int k,
-                void* d_out, int ld_out, const float* d_bias, const float* d_pos, int pos_rows, int splits,
-                long long split_stride, int bn, void* cuda_stream);
+/* One-tile GEMM of the ViT patch embed and MAP-head K/V projection (csrc/gemm.cuh), fp16:
+ * y[t][n] = fp16(sum_k X[t,k] W[n,k] + bias[n]), X [rows_x, k], W [rows_w, k], k a multiple of 64;
+ * epi 1: fp16 out[rows_x][ld_out] = act(y) (act codes in csrc/gemm.cuh);
+ * epi 3: fp32 out[rows_x][ld_out] = y + pos[t % pos_rows][n], pos fp32 [pos_rows][ld_out].
+ * bn = feature-tile width, 64 or 128 (0: 128). */
+int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, int rows_w, int k, void* d_out, int ld_out,
+                const float* d_bias, const float* d_pos, int pos_rows, int bn, void* cuda_stream);
 /* Persistent weight-streaming GEMM (csrc/gemm_ws.cuh): out[t, n] = sum_k X[t,k] W[n,k].  bn = token-tile width
  * (0: smallest of 16/32/64/128 covering rows_x, which must then be <= 128; 64/96/128/192 tile larger rows_x).
  * mode 0: stream-K over all SMs, fp32 partial planes out[plane][rows_x][rows_w] (the caller zero-fills d_out
@@ -178,9 +181,6 @@ int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, in
  *   keys 0..kv_len-1 valid, the n_tok query tokens sit at positions kv_len-n_tok .. kv_len-1 (causal with
  *   offset, HF:masking_utils.py:263-272); d_out bf16 [n_tok, n_heads*head_dim]; d_ws fp32 scratch of
  *   vlo_op_attn_ws_bytes(). Replaces HF:models/llama/modeling_llama.py:272-285 (SDPA / flash-attn 2). */
-/* which generation of the KV-append attention kernel runs for this head layout: 1 = mma.sync over TMA-loaded
- * K / V blocks (csrc/attn.cuh), the only one */
-int vlo_op_attn_version(int n_heads, int n_kv_heads);
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len);
 int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void* d_out, float* d_ws, int n_tok,
                          int n_heads, int n_kv_heads, int head_dim, int kv_len, long long kv_stride, void* cuda_stream);

@@ -539,21 +539,3 @@ def test_offline_encode_directory_on_the_engine(built, tiny, tmp_path):
         mx, frac = _close(feats, ref, 3e-2 + 8e-3, 2e-2)             # VIT_ATOL + one bf16 ulp of O(1) tokens
         assert frac == 0.0, (name, mx)
 
-
-# ------------------------------------------------------------------------------------------- alternative kernel generations
-@pytest.mark.parametrize("env", ["VLO_FUSE=15", "VLO_FUSE=0", "VLO_WS_STAGES=11", "VLO_WSF_STAGES=4", "VLO_VIT_SMALL_BN=96",
-                                 "VLO_VIT_CORESIDE=0"])
-def test_non_default_kernel_paths_keep_parity(env):
-    """The kernel configurations that are not the default stay selectable (A/B switches, read once per process):
-    fused stream-K finishers (all four / none; the default fuses gate|up only), the deepest decoder GEMM ring (11 stages) and
-    the shallowest fused-GEMM ring (4 stages), the ViT trunk with 96-token co-resident tiles, and without the co-resident
-    configuration.  Each runs the reference-golden parity tests of the tiny model in its own process."""
-    import os
-    import subprocess
-    e = dict(os.environ)
-    for kv in env.split():
-        k, v = kv.split("=")
-        e[k] = v
-    r = subprocess.run([sys.executable, "-m", "pytest", str(ROOT / "tests" / "test_gpu_parity.py"), "-m", "gpu", "-q", "-x", "-p", "no:cacheprovider",
-                        "-k", "chunked or greedy or vit_tokens or batched or state_machine"], env=e, capture_output=True, text=True, timeout=280)
-    assert r.returncode == 0, r.stdout[-1500:] + r.stderr[-500:]

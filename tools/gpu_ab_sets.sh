@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B several environment SETS of one build inside ONE gpurun call (box-to-box variance is ~5-10 %).
-# usage: tools/gpu_ab_sets.sh "" "VLO_DEC_CTAS=132 VLO_VIT_CTAS=16 VLO_WS_STAGES=11 VLO_VIT_CORESIDE=0" ... [-- bench args]
+# usage: tools/gpu_ab_sets.sh "" "VLO_NO_PDL=1" ... [-- bench args]
 set -u
 SETS=()
 while [ $# -gt 0 ] && [ "$1" != "--" ]; do SETS+=("$1"); shift; done

@@ -8,7 +8,6 @@ P, I, LL = C.c_void_p, C.c_int, C.c_longlong
 lib.vlo_op_attn_ws_bytes.argtypes = [I, I, I, I]; lib.vlo_op_attn_ws_bytes.restype = C.c_int64
 lib.vlo_op_attn_kvappend.argtypes = [P, P, P, P, P, I, I, I, I, I, LL, P]; lib.vlo_op_attn_kvappend.restype = I
 dev = "cuda"
-print("attention kernel version:", lib.vlo_op_attn_version(32, 8), flush=True)
 torch.manual_seed(0)
 res = []
 

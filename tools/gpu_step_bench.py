@@ -1,5 +1,5 @@
 """Dev tool: the decoder step ALONE (no ViT) at a 12k-token cache: q = 11 frame steps and q = 1 AR steps, device-timed.
-One JSON line; run once per environment setting (VLO_FUSE, VLO_WS_STAGES, VLO_WSF_STAGES, ...)."""
+One JSON line; run once per library build (VLO_LIB) or environment setting (VLO_NO_PDL)."""
 import json, os, pathlib, sys
 import torch
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parents[1]))

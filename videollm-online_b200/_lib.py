@@ -74,10 +74,9 @@ SIGNATURES = {
     "vlo_last_step_hidden": (_I, [_P, _P, _P]),
     "vlo_bench_attn": (_I, [_P, _I, C.POINTER(C.c_int32), _I, _I, _I, C.POINTER(C.c_double), _P]),
     "vlo_bench_gemm": (_I, [_P, _I, _I, C.POINTER(C.c_double), C.POINTER(_I), _P]),
-    "vlo_op_gemm": (_I, [_I, _I, _I, _I, _P, _I, _P, _I, _I, _P, _I, _P, _P, _I, _I, _LL, _I, _P]),
+    "vlo_op_gemm": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _P, _P, _I, _I, _P]),
     "vlo_op_gemm_ws": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
-    "vlo_op_attn_version": (_I, [_I, _I]),
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
     "vlo_op_attn_kvappend": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),

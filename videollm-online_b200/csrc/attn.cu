@@ -29,9 +29,6 @@ size_t cap_slots_for(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) 
 }
 }  // namespace
 
-// one kernel generation: mma.sync m16n8k16 over TMA-loaded K / V blocks (attn.cuh)
-int attn_version(int, int) { return 1; }
-
 size_t attn_stage_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
   const int G = n_heads / n_kv_heads;
   return align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens);

@@ -29,27 +29,21 @@ int vlo_device_supported(int device) {
   return (prop.major == 9 && prop.minor == 0) ? 1 : 0;
 }
 
-int vlo_op_gemm(int fmt, int swap, int epi, int act, const void* d_a, int rows_a, const void* d_b,
-                int rows_b, int k, void* d_out, int ld_out, const float* d_bias, const float* d_pos,
-                int pos_rows, int splits, long long split_stride, int bn, void* cuda_stream) {
+int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, int rows_w, int k, void* d_out, int ld_out,
+                const float* d_bias, const float* d_pos, int pos_rows, int bn, void* cuda_stream) {
   GemmCall c{};
-  c.fmt = fmt;
-  c.swap = swap;
   c.epi = epi;
   c.act = act;
-  c.a = d_a;
-  c.rows_a = rows_a;
-  c.b = d_b;
-  c.rows_b = rows_b;
+  c.a = d_x;
+  c.rows_a = rows_x;
+  c.b = d_w;
+  c.rows_b = rows_w;
   c.k = k;
   c.out = d_out;
   c.ld_out = ld_out;
   c.bias = d_bias;
   c.pos = d_pos;
   c.pos_rows = pos_rows;
-  c.splits = splits < 1 ? 1 : splits;
-  c.split_stride = split_stride;
-  c.stream_weights = swap;
   c.bn = bn;
   return gemm_launch(c, static_cast<cudaStream_t>(cuda_stream));
 }
@@ -90,8 +84,6 @@ int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, in
                     const float* d_bias, int act, int n_ctas, void* cuda_stream) {
   return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
 }
-
-int vlo_op_attn_version(int n_heads, int n_kv_heads) { return attn_version(n_heads, n_kv_heads); }
 
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len) {
   (void)head_dim;

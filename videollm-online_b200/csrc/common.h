@@ -79,9 +79,8 @@ void prof_end(cudaStream_t st);
 int prof_read(double* ms, long long* n, double* bytes, int ncls);
 
 // ---- GEMM (gemm.cu) ---------------------------------------------------------------
+// fp16 out[rows_a, rows_b] from activations A [rows_a, k] (MMA-M) and weights B [rows_b, k], one CTA per 128 x bn tile
 struct GemmCall {
-  int fmt;   // 0 fp16, 1 bf16
-  int swap;  // 1: A = weights (MMA-M), B = tokens (MMA-N); logical out [rows_b, rows_a]
   int epi;   // GemmEpi
   int act;   // GemmAct
   const void* a;
@@ -94,13 +93,9 @@ struct GemmCall {
   const float* bias;
   const float* pos;
   int pos_rows;
-  int splits;          // >1 only with EPI_PARTIAL; out is then the fp32 workspace
-  long long split_stride;
-  int stream_weights;  // 1: operand A is read once (EVICT_FIRST), B is hot (EVICT_LAST)
-  int bn;              // 0 = choose
+  int bn;    // 64 or 128 (0 = 128)
 };
 int gemm_launch(const GemmCall& c, cudaStream_t stream);
-int gemm_fix_splits(int k, int want);
 
 // ---- persistent weight-streaming GEMM (gemm_ws.cuh / gemm.cu)
 struct GemmWsCall {
@@ -119,7 +114,7 @@ struct GemmWsCall {
   SkInfo sk;          // from gemm_ws_plan
   int bn;             // token-tile width (0 = smallest of 16/32/64/128 covering rows_x); 96 / 192 for the ViT
   int weights_hot;    // 1: weights are re-read by several token tiles (keep them in L2)
-  int small_smem;     // 1: shallow 3-stage ring (~75 KB) so the CTA can share an SM with a decoder weight-streaming CTA
+  int small_smem;     // 1 with bn 64, fp16: shallow 3-stage ring (83 KB) so the CTA can share an SM with a decoder weight-streaming CTA
 };
 // decomposition for (rows_w, k): n_ctas <= 0 -> one CTA per SM; max_planes = fp32 planes the partials need
 int gemm_ws_plan(int rows_w, int k, int mode, int n_ctas, SkInfo* sk, int* max_planes, int x_tiles = 1);
@@ -130,9 +125,9 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream);
 int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
                     const float* bias, int act, int n_ctas, cudaStream_t stream);
 
-// ---- stream-K GEMM with the fused finisher epilogue (gemm_wsf.cuh / gemm.cu); args struct defined in gemm_wsf.cuh
+// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu); args struct defined in gemm_wsf.cuh
 struct GemmWsfArgs;
-int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, int epi, cudaStream_t stream);
+int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, cudaStream_t stream);
 
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {
@@ -145,7 +140,6 @@ struct AttnSeq {
 // bytes of scratch attn_launch needs for these sequences (upper bound)
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads);
 size_t attn_stage_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads);
-int attn_version(int n_heads, int n_kv_heads);  // 1: the mma.sync kernel (attn.cuh)
 struct AttnPlan {
   float* ws_o;
   float* ws_ml;
@@ -166,6 +160,5 @@ int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void*
 
 // 2D TMA map over a row-major 16-bit matrix [rows, k], box 64 x box_rows, 128-byte swizzle (cached).
 int tmap_2d_sw128(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out);
-int tmap_q3d_sw128(const void* ptr, int n_tok, int n_heads, int G, CUtensorMap* out, int box_rows = 128);  // attention Q tile (see gemm.cu)
 
 }  // namespace vlo

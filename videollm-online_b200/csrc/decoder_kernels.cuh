@@ -26,16 +26,15 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Split-K fix-up + residual add + RMSNorm in one pass over a token row:
+// Stream-K fix-up + residual add + RMSNorm in one pass over a token row:
 //   y      = bf16(sum_s part[s][t][:])                (the Linear output, o_proj / down_proj)
 //   h[t]   = bf16(h[t] + y)                           (residual, HF:...llama.py:325,331)
 //   xn[t]  = w * bf16(h * rsqrt(mean(h^2) + eps))     (LlamaRMSNorm.forward, HF:...llama.py:62-67)
-// n_splits == 0: no partials, plain RMSNorm of h (first layer).  `xn_last` (optional) receives
+// part == null: no partials, plain RMSNorm of h (first layer).  `xn_last` (optional) receives
 // compact copies of the rows flagged in last_index (>= 0): the final-norm rows the lm_head needs.
 // grid = T rows, block = 256.
 struct ResidNormParams {
-  const float* part;
-  int n_splits;             // 0: no partials; > 0: that many planes; < 0: stream-K planes per 128-column tile (sk)
+  const float* part;        // stream-K planes per 128-column tile (sk), or null
   long long split_stride;
   SkInfo sk;
   __nv_bfloat16* h;         // [T, H] residual stream, updated in place
@@ -46,8 +45,6 @@ struct ResidNormParams {
   int H;
   float eps;
 };
-
-constexpr int kFixMaxPlanes = 8;  // stream-K never needs more (engine checks)
 
 __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormParams p) {
   // one CTA per token row, 4 contiguous elements per thread per sweep; the plane loads of a sweep are
@@ -63,7 +60,7 @@ __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormPara
   // the last-token index (tables uploaded by the memcpy at the start of the step).
   const int i0 = threadIdx.x * 4;
   const uint2 w_pre = (i0 < p.H) ? *reinterpret_cast<const uint2*>(p.w + i0) : make_uint2(0u, 0u);
-  const int ns_pre = (p.n_splits < 0 && i0 < p.H) ? sk_planes(i0 >> 7, p.sk) : p.n_splits;
+  const int ns_pre = (p.part != nullptr && i0 < p.H) ? sk_planes(i0 >> 7, p.sk) : 0;
   const int li = p.last_index ? p.last_index[t] : -1;
   pdl_wait();
   float ss = 0.f;
@@ -71,8 +68,8 @@ __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormPara
     const uint2 hraw = *reinterpret_cast<const uint2*>(h + i);
     float2 v01 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hraw.x));
     float2 v23 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hraw.y));
-    if (p.n_splits != 0) {
-      const int ns = (i == i0) ? ns_pre : (p.n_splits > 0 ? p.n_splits : sk_planes(i >> 7, p.sk));
+    if (p.part != nullptr) {
+      const int ns = (i == i0) ? ns_pre : sk_planes(i >> 7, p.sk);
       const float* pp = p.part + static_cast<size_t>(t) * p.H + i;
       float4 a[kFixMaxPlanes];
 #pragma unroll
@@ -112,7 +109,7 @@ __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormPara
 }
 
 // ---------------------------------------------------------------------------------------------
-// QKV split-K fix-up + RoPE + KV-cache append (SURVEY K12/K13/K14 fused):
+// QKV stream-K fix-up + RoPE + KV-cache append (SURVEY K12/K13/K14 fused):
 //   q,k,v = bf16(sum_s part)                              (HF:...llama.py:262-264)
 //   q,k   = x*cos + rotate_half(x)*sin in bf16            (apply_rotary_pos_emb, :146-168)
 //   K/V rows written in place at the token's position     (replaces DynamicLayer.update's
@@ -120,8 +117,7 @@ __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormPara
 // cos/sin: bf16 tables [max_pos, head_dim/2] (the two halves of HF's cos/sin are identical).
 // grid = (T, n_heads + 2*n_kv_heads), block = 64 (thread d handles dims d and d+64).
 struct QkvRopeParams {
-  const float* part;       // [S][T][(nh + 2 nkv) * 128]
-  int n_splits;            // > 0 planes, < 0 stream-K (head hh == weight tile hh)
+  const float* part;       // [S][T][(nh + 2 nkv) * 128], stream-K planes (head hh == weight tile hh)
   long long split_stride;
   SkInfo sk;
   const __nv_bfloat16* cos_tab;
@@ -142,7 +138,7 @@ __global__ void __launch_bounds__(64) qkv_rope_append_kernel(const QkvRopeParams
   // the step), the RoPE table entries (static) and the plane count - three dependent round trips off the critical path.
   const int width = (p.n_heads + 2 * p.n_kv_heads) * 128;
   const float* pp = p.part + static_cast<size_t>(t) * width + hh * 128 + d;
-  const int ns = p.n_splits > 0 ? p.n_splits : sk_planes(hh, p.sk);
+  const int ns = sk_planes(hh, p.sk);
   const int pos = p.tok_pos[t];
   const long long kvrow = p.tok_kvrow[t];
   const bool rot = hh < p.n_heads + p.n_kv_heads;
@@ -150,23 +146,16 @@ __global__ void __launch_bounds__(64) qkv_rope_append_kernel(const QkvRopeParams
   const float s = rot ? __bfloat162float(p.sin_tab[static_cast<size_t>(pos) * 64 + d]) : 0.f;
   pdl_wait();
   float x1 = 0.f, x2 = 0.f;
-  if (ns <= kFixMaxPlanes) {  // all plane loads in flight together
-    float a1[kFixMaxPlanes], a2[kFixMaxPlanes];
+  float a1[kFixMaxPlanes], a2[kFixMaxPlanes];  // all plane loads in flight together
 #pragma unroll
-    for (int k = 0; k < kFixMaxPlanes; ++k) {
-      a1[k] = (k < ns) ? pp[k * p.split_stride] : 0.f;
-      a2[k] = (k < ns) ? pp[k * p.split_stride + 64] : 0.f;
-    }
+  for (int k = 0; k < kFixMaxPlanes; ++k) {
+    a1[k] = (k < ns) ? pp[k * p.split_stride] : 0.f;
+    a2[k] = (k < ns) ? pp[k * p.split_stride + 64] : 0.f;
+  }
 #pragma unroll
-    for (int k = 0; k < kFixMaxPlanes; ++k) {  // plane order: deterministic
-      x1 += a1[k];
-      x2 += a2[k];
-    }
-  } else {
-    for (int k = 0; k < ns; ++k) {
-      x1 += pp[k * p.split_stride];
-      x2 += pp[k * p.split_stride + 64];
-    }
+  for (int k = 0; k < kFixMaxPlanes; ++k) {  // plane order: deterministic
+    x1 += a1[k];
+    x2 += a2[k];
   }
   x1 = bf16_round(x1);
   x2 = bf16_round(x2);
@@ -186,65 +175,6 @@ __global__ void __launch_bounds__(64) qkv_rope_append_kernel(const QkvRopeParams
   }
   dst[d] = __float2bfloat16_rn(x1);
   dst[d + 64] = __float2bfloat16_rn(x2);
-}
-
-// ---------------------------------------------------------------------------------------------
-// gate/up split-K fix-up + SwiGLU:  act = bf16(bf16(silu(g)) * u)      (LlamaMLP, :182-184)
-// The fused gate|up weight is stored tile-interleaved: 128-row tile j = gate rows of features 64j..64j+63 followed by
-// the matching up rows (so one tile holds both operands of 64 activations: gemm_wsf.cuh fuses this kernel into the
-// GEMM's finisher; this stand-alone version is the VLO_FUSE=0 fallback).  part column of feature i: gate
-// (i/64)*128 + i%64, up = gate + 64.   grid-stride over T*I/4 quads.
-struct SwigluParams {
-  const float* part;
-  int n_splits;  // > 0 planes, < 0 stream-K
-  long long split_stride;
-  SkInfo sk;
-  __nv_bfloat16* act;  // [T, I]
-  int T, I;
-};
-__global__ void __launch_bounds__(256) swiglu_kernel(const SwigluParams p) {
-  pdl_trigger();
-  const long long n4 = static_cast<long long>(p.T) * p.I / 4;
-  const long long idx0 = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  // index arithmetic and stream-K plane counts of the first element group: before the grid dependency resolves
-  int t0 = 0, c0 = 0, ng0 = 0;
-  if (idx0 < n4) {
-    const long long e = idx0 * 4;
-    t0 = static_cast<int>(e / p.I), c0 = static_cast<int>(e % p.I);
-    ng0 = p.n_splits > 0 ? p.n_splits : sk_planes(c0 >> 6, p.sk);
-  }
-  pdl_wait();
-  for (long long idx = idx0; idx < n4; idx += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const long long e = idx * 4;
-    const bool first = idx == idx0;
-    const int t = first ? t0 : static_cast<int>(e / p.I), i = first ? c0 : static_cast<int>(e % p.I);
-    const float* pg = p.part + static_cast<size_t>(t) * 2 * p.I + (i >> 6) * 128 + (i & 63);
-    const int ng = first ? ng0 : (p.n_splits > 0 ? p.n_splits : sk_planes(i >> 6, p.sk));
-    const int nu = ng;
-    float4 ga[kFixMaxPlanes], ua[kFixMaxPlanes];
-#pragma unroll
-    for (int s = 0; s < kFixMaxPlanes; ++s) {
-      ga[s] = (s < ng) ? *reinterpret_cast<const float4*>(pg + s * p.split_stride) : make_float4(0.f, 0.f, 0.f, 0.f);
-      ua[s] = (s < nu) ? *reinterpret_cast<const float4*>(pg + s * p.split_stride + 64) : make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    float g[4] = {0.f, 0.f, 0.f, 0.f}, u[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-    for (int s = 0; s < kFixMaxPlanes; ++s) {
-      g[0] += ga[s].x; g[1] += ga[s].y; g[2] += ga[s].z; g[3] += ga[s].w;
-      u[0] += ua[s].x; u[1] += ua[s].y; u[2] += ua[s].z; u[3] += ua[s].w;
-    }
-    float o[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float gk = bf16_round(g[k]), uk = bf16_round(u[k]);
-      const float a = bf16_round(gk / (1.0f + expf(-gk)));
-      o[k] = a * uk;
-    }
-    uint2 w;
-    *reinterpret_cast<__nv_bfloat162*>(&w.x) = __floats2bfloat162_rn(o[0], o[1]);
-    *reinterpret_cast<__nv_bfloat162*>(&w.y) = __floats2bfloat162_rn(o[2], o[3]);
-    *reinterpret_cast<uint2*>(p.act + e) = w;
-  }
 }
 
 // ---------------------------------------------------------------------------------------------

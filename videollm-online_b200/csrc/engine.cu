@@ -68,9 +68,7 @@ struct vlo_engine {
        *logits = nullptr;
   float* part = nullptr;
   size_t part_elems = 0;
-  int* sk_flags = nullptr;          // stream-K arrival counters of the fused-finisher GEMMs (zero between launches)
-  bf16* bench_kv = nullptr;         // scratch K / V rows for vlo_bench_gemm's fused QKV epilogue
-  uint8_t* bench_meta = nullptr;    // tok_pos | tok_kvrow of the micro-loop
+  int* sk_flags = nullptr;          // stream-K arrival counters of the fused gate|up GEMM (zero between launches)
   uint8_t* attn_ws = nullptr;
   uint8_t* meta_dev = nullptr;  // tok_pos | tok_kvrow | last_index | first_rows
   size_t meta_bytes = 0;
@@ -117,30 +115,10 @@ int lookup(vlo_engine* e, const std::string& name, int64_t expect_elems, const T
   return 0;
 }
 
-// SM partitioning experiment (DESIGN.md section 8.1a; default off = every persistent GEMM uses all SMs):
-//   VLO_DEC_CTAS=<n>  CTAs of the decoder / lm_head weight-streaming GEMMs (e.g. 132 with VLO_WS_STAGES=11)
-//   VLO_VIT_CTAS=<n>  CTAs of the ViT trunk GEMMs (e.g. 16), so both run side by side on disjoint SMs
-int dec_ctas() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("VLO_DEC_CTAS");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-int vit_ctas() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("VLO_VIT_CTAS");
-    v = e ? atoi(e) : 0;
-  }
-  return v;
-}
-
 // weights [n_out, k] x tokens [T, k] -> stream-K fp32 partial planes in e->part (persistent kernel)
 int gemm_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, SkInfo* sk, cudaStream_t st) {
   int planes = 1;
-  gemm_ws_plan(n_out, k, 0, dec_ctas(), sk, &planes);
+  gemm_ws_plan(n_out, k, 0, 0, sk, &planes);
   VLO_CHECK(static_cast<size_t>(planes) * T * n_out <= e->part_elems, "stream-K workspace too small");
   VLO_CHECK(planes <= kFixMaxPlanes, "stream-K produced more partial planes than the fix-up kernels unroll");
   GemmWsCall c{};
@@ -158,26 +136,15 @@ int gemm_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, 
   return gemm_ws_launch(c, st);
 }
 
-// Which stream-K fix-ups run inside the GEMM's finisher CTAs (gemm_wsf.cuh) instead of a separate kernel.  A finisher's
-// epilogue (flag acquire -> plane loads -> table loads -> stores) is a tail at the end of EVERY CTA during which its SM
-// streams nothing, while a separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling.  Only
-// the gate|up GEMM has enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB
-// plane round trip of its fix-up.
-// VLO_FUSE bit mask: 1 = q|k|v (+RoPE +append), 2 = o_proj (+residual), 4 = gate|up (+SwiGLU), 8 = down_proj (+residual);
-// "all" = 15.  Default 4 (H100 measurements in DESIGN.md section 3.2).
-int fuse_mask() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("VLO_FUSE");
-    v = (e == nullptr) ? 4 : ((e[0] == 'a') ? 15 : (atoi(e) & 15));
-  }
-  return v;
-}
-
-// stream-K GEMM whose finisher CTAs apply the fix-up themselves (gemm_wsf.cuh); `a` carries the epilogue's operands
-int gemm_fused(vlo_engine* e, GemmWsfArgs& a, int epi, const bf16* w, int n_out, const bf16* x, int T, int k, cudaStream_t st) {
+// gate|up GEMM + SwiGLU: the stream-K finisher CTAs apply the fix-up themselves (gemm_wsf.cuh).  A finisher's epilogue
+// (flag acquire -> plane loads -> stores) is a tail at the end of EVERY CTA during which its SM streams nothing, while a
+// separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling.  Only the gate|up GEMM has
+// enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB plane round trip of
+// its fix-up; q|k|v, o_proj and down_proj go through gemm_partial and a fix-up kernel (DESIGN.md section 5).
+int gemm_swiglu(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, cudaStream_t st) {
+  GemmWsfArgs a{};
   int planes = 1;
-  gemm_ws_plan(n_out, k, 0, dec_ctas(), &a.sk, &planes);
+  gemm_ws_plan(n_out, k, 0, 0, &a.sk, &planes);
   VLO_CHECK(static_cast<size_t>(std::max(1, planes - 1)) * T * n_out <= e->part_elems, "stream-K workspace too small");
   VLO_CHECK((n_out + 127) / 128 <= 4096, "stream-K flag array too small");
   a.rows_w = n_out;
@@ -187,7 +154,9 @@ int gemm_fused(vlo_engine* e, GemmWsfArgs& a, int epi, const bf16* w, int n_out,
   a.plane_stride = static_cast<long long>(T) * n_out;
   a.flags = e->sk_flags;
   a.hint_w = kEvictFirst;
-  return gemm_wsf_launch(a, w, x, epi, st);
+  a.act = e->act;
+  a.I = n_out / 2;
+  return gemm_wsf_launch(a, w, x, st);
 }
 
 // whole-tile persistent GEMM with the 16-bit epilogue: out[T, n_out] = act(x W^T + bias)
@@ -205,15 +174,14 @@ int gemm_ws_store16(int fmt, const void* w, int n_out, const void* x, int T, int
   c.ld_out = ld;
   c.bias = bias;
   c.act = act;
-  gemm_ws_plan(n_out, k, 1, fmt == FMT_BF16 ? dec_ctas() : 0, &c.sk, nullptr);
+  gemm_ws_plan(n_out, k, 1, 0, &c.sk, nullptr);
   return gemm_ws_launch(c, st);
 }
 
-int gemm_store16(int fmt, int swap, const void* a, int rows_a, const void* b, int rows_b, int k, void* out, int ld,
-                 const float* bias, int act, int bn, cudaStream_t st) {
+// one-tile fp16 GEMM with the 16-bit epilogue: out[rows_a, rows_b] = act(a b^T + bias)
+int gemm_store16(const void* a, int rows_a, const void* b, int rows_b, int k, void* out, int ld, const float* bias, int act,
+                 int bn, cudaStream_t st) {
   GemmCall c{};
-  c.fmt = fmt;
-  c.swap = swap;
   c.epi = EPI_STORE16;
   c.act = act;
   c.a = a;
@@ -224,8 +192,6 @@ int gemm_store16(int fmt, int swap, const void* a, int rows_a, const void* b, in
   c.out = out;
   c.ld_out = ld;
   c.bias = bias;
-  c.splits = 1;
-  c.stream_weights = swap;
   c.bn = bn;
   return gemm_launch(c, st);
 }
@@ -352,8 +318,6 @@ static int engine_init(vlo_engine* e) {
   e->part_elems = static_cast<size_t>(8) * T * widest;  // stream-K needs <= kb/floor(U/G) + 2 planes (<= 4 in practice)
   if (dev_alloc_t(e, &e->part, e->part_elems)) return -1;
   if (dev_alloc_t(e, &e->sk_flags, 4096, true)) return -1;
-  if (dev_alloc_t(e, &e->bench_kv, static_cast<size_t>(2) * c.num_kv_heads * T * c.head_dim, true)) return -1;
-  if (dev_alloc(e, reinterpret_cast<void**>(&e->bench_meta), align256(sizeof(int) * T) + align256(sizeof(long long) * T), true)) return -1;
   const size_t aws = attn_ws_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads);
   if (dev_alloc(e, reinterpret_cast<void**>(&e->attn_ws), aws, false)) return -1;
   e->meta_bytes = align256(sizeof(int) * T) * 3 + align256(sizeof(long long) * T);
@@ -621,8 +585,6 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
                         d_frames, e->patches, B, c.image_size, c.patch_size));
     count_launch();
     GemmCall g{};
-    g.fmt = FMT_F16;
-    g.swap = 0;
     g.epi = EPI_PATCH32;
     g.a = e->patches;
     g.rows_a = rows;
@@ -634,7 +596,6 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     g.bias = e->patch_b;
     g.pos = e->pos_emb;
     g.pos_rows = P;
-    g.splits = 1;
     g.bn = vit_bn(rows, C);
     if (gemm_launch(g, st)) return -1;
   }
@@ -660,21 +621,10 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   // concurrently (two CUDA streams): QKV and fc1 on gemm_vit_kernel (128-token x 128-feature tiles, tokens on MMA-M,
   // 97 KB), out_proj and fc2 with 64-token tiles and a 3-stage ring (83 KB).  gemm_vit_kernel gives QKV / fc1 the
   // same bits as 64-token swap-AB tiles would; the stream-K planes keep the 64-token decomposition, whose summation
-  // order the frame embeddings depend on.  VLO_VIT_SMALL_BN=96 runs all four on 96-token swap-AB tiles (95 KB).
-  static int coreside = -1;
-  if (coreside < 0) {
-    const char* ev = getenv("VLO_VIT_CORESIDE");
-    coreside = (ev != nullptr && ev[0] == '0') ? 0 : 1;
-  }
-  const bool small = coreside && B <= 2;
-  static int small_bn = 0;
-  if (small_bn == 0) {
-    const char* ev = getenv("VLO_VIT_SMALL_BN");
-    small_bn = (ev != nullptr && atoi(ev) == 96) ? 96 : 64;
-  }
-  const bool trunk_vit = small && small_bn == 64;
+  // order the frame embeddings depend on.
+  const bool small = B <= 2;
   auto pick_bn = [&](int n_out, int mode) {
-    if (small) return small_bn;
+    if (small) return 64;
     const int cands[4] = {64, 96, 128, 192};
     int best = 64;
     double best_eff = -1.0;
@@ -691,6 +641,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     return best;
   };
   auto tiles_gemm = [&](const __half* x, const __half* w, int n_out, int k, __half* out, const float* bias, int act) -> int {
+    if (small) return gemm_vit_launch(x, rows, w, n_out, k, out, n_out, bias, act, 0, st);
     GemmWsCall g{};
     g.fmt = FMT_F16;
     g.mode = 1;
@@ -703,11 +654,9 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     g.ld_out = n_out;
     g.bias = bias;
     g.act = act;
-    if (trunk_vit) return gemm_vit_launch(x, rows, w, n_out, k, out, n_out, bias, act, vit_ctas(), st);
     g.bn = pick_bn(n_out, 1);
     g.weights_hot = 1;
-    g.small_smem = small ? 1 : 0;
-    gemm_ws_plan(n_out, k, 1, vit_ctas(), &g.sk, nullptr, (rows + g.bn - 1) / g.bn);
+    gemm_ws_plan(n_out, k, 1, 0, &g.sk, nullptr, (rows + g.bn - 1) / g.bn);
     return gemm_ws_launch(g, st);
   };
   struct SkCall { SkInfo sk; int bn, xt; };
@@ -729,15 +678,14 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     int planes = 1;
     out->bn = g.bn;
     out->xt = (rows + g.bn - 1) / g.bn;
-    gemm_ws_plan(C, k, 0, vit_ctas(), &g.sk, &planes, out->xt);
-    VLO_CHECK(planes <= 8 && static_cast<size_t>(planes) * rows * C <= e->v_part_elems, "ViT stream-K workspace too small");
+    gemm_ws_plan(C, k, 0, 0, &g.sk, &planes, out->xt);
+    VLO_CHECK(planes <= kFixMaxPlanes && static_cast<size_t>(planes) * rows * C <= e->v_part_elems, "ViT stream-K workspace too small");
     out->sk = g.sk;
     return gemm_ws_launch(g, st);
   };
   auto fix_ln = [&](const SkCall& sc, const float* bias, const float* lw, const float* lb, float* out32) -> int {
     VitFixLnParams p{};
     p.part = e->v_part;
-    p.n_splits = -1;
     p.sk = sc.sk;
     p.sk_bn = sc.bn;
     p.sk_xtiles = sc.xt;
@@ -784,8 +732,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   }
   if (cls) {
     // MAP head: K/V projection of all tokens, 1-query attention, out-proj, LN, MLP, residual
-    if (gemm_store16(FMT_F16, 0, e->v_xn, rows, e->head_kv_w, 2 * C, C, e->v_qkv, 2 * C, e->head_kv_b, ACT_NONE,
-                     vit_bn(rows, 2 * C), st))
+    if (gemm_store16(e->v_xn, rows, e->head_kv_w, 2 * C, C, e->v_qkv, 2 * C, e->head_kv_b, ACT_NONE, vit_bn(rows, 2 * C), st))
       return -1;
     probe_attn_kernel<<<dim3(c.vit_heads, B), 128, static_cast<size_t>(P) * sizeof(float), st>>>(e->v_qkv, e->head_q, e->v_pa, P, C, 0.125f);
     VLO_LAUNCH_CHECK();
@@ -887,12 +834,12 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   }
 
   const size_t norm_smem = static_cast<size_t>(H) * sizeof(float);
-  auto resid_norm = [&](const SkInfo* sk, long long split_stride, const bf16* w, bool last) -> int {
+  // sk == null: no partials (the first layer's input norm)
+  auto resid_norm = [&](const SkInfo* sk, const bf16* w, bool last) -> int {
     ResidNormParams p{};
-    p.part = e->part;
-    p.n_splits = sk ? -1 : 0;
+    p.part = sk ? e->part : nullptr;
     if (sk) p.sk = *sk;
-    p.split_stride = split_stride;
+    p.split_stride = static_cast<long long>(T) * H;
     p.h = e->h;
     p.w = w;
     p.xn = e->xn;
@@ -905,90 +852,41 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     return 0;
   };
 
-  if (resid_norm(nullptr, 0, e->dec[0].in_norm, false)) return -1;
+  if (resid_norm(nullptr, e->dec[0].in_norm, false)) return -1;
   const int attn_width = c.num_heads * c.head_dim;
   for (int l = 0; l < c.num_layers; ++l) {
     const DecLayer& d = e->dec[l];
     SkInfo sk{};
     const bool is_last = (l == c.num_layers - 1);
-    const int fm = fuse_mask();
-    GemmWsfArgs r{};
-    r.h = e->h;
-    // ---- q|k|v projection (+ RoPE + in-place KV append): fused finisher, or planes + fix-up kernel
-    if (fm & 1) {
-      GemmWsfArgs a{};
-      a.cos_tab = e->rope_cos;
-      a.sin_tab = e->rope_sin;
-      a.tok_pos = d_tok_pos;
-      a.tok_kvrow = d_tok_kvrow;
-      a.kv_head_stride = c.max_kv_tokens;
-      a.q_out = e->q;
-      a.k_cache = kv_layer_base(e, l, 0);
-      a.v_cache = kv_layer_base(e, l, 1);
-      a.n_heads = c.num_heads;
-      a.n_kv_heads = c.num_kv_heads;
-      if (gemm_fused(e, a, WSF_QKV, d.qkv, e->qkv_width, e->xn, T, H, st)) return -1;
-    } else {
-      if (gemm_partial(e, d.qkv, e->qkv_width, e->xn, T, H, &sk, st)) return -1;
-      QkvRopeParams p{};
-      p.part = e->part;
-      p.n_splits = -1;
-      p.sk = sk;
-      p.split_stride = static_cast<long long>(T) * e->qkv_width;
-      p.cos_tab = e->rope_cos;
-      p.sin_tab = e->rope_sin;
-      p.tok_pos = d_tok_pos;
-      p.tok_kvrow = d_tok_kvrow;
-      p.kv_head_stride = c.max_kv_tokens;
-      p.q_out = e->q;
-      p.k_cache = kv_layer_base(e, l, 0);
-      p.v_cache = kv_layer_base(e, l, 1);
-      p.n_heads = c.num_heads;
-      p.n_kv_heads = c.num_kv_heads;
-      VLO_CUDA(launch_pdl(qkv_rope_append_kernel, dim3(T, c.num_heads + 2 * c.num_kv_heads), dim3(64), 0, st, p));
-      count_launch();
-    }
+    // ---- q|k|v projection, then RoPE + in-place KV append
+    if (gemm_partial(e, d.qkv, e->qkv_width, e->xn, T, H, &sk, st)) return -1;
+    QkvRopeParams p{};
+    p.part = e->part;
+    p.sk = sk;
+    p.split_stride = static_cast<long long>(T) * e->qkv_width;
+    p.cos_tab = e->rope_cos;
+    p.sin_tab = e->rope_sin;
+    p.tok_pos = d_tok_pos;
+    p.tok_kvrow = d_tok_kvrow;
+    p.kv_head_stride = c.max_kv_tokens;
+    p.q_out = e->q;
+    p.k_cache = kv_layer_base(e, l, 0);
+    p.v_cache = kv_layer_base(e, l, 1);
+    p.n_heads = c.num_heads;
+    p.n_kv_heads = c.num_kv_heads;
+    VLO_CUDA(launch_pdl(qkv_rope_append_kernel, dim3(T, c.num_heads + 2 * c.num_kv_heads), dim3(64), 0, st, p));
+    count_launch();
     if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), kv_rows_per_layer(c), e->attn_out,
                  c.num_heads, c.num_kv_heads, c.head_dim, st))
       return -1;
     // ---- o_proj + residual, then post-attention RMSNorm
-    if (fm & 2) {
-      if (gemm_fused(e, r, WSF_RESID, d.o, H, e->attn_out, T, attn_width, st)) return -1;
-      if (resid_norm(nullptr, 0, d.post_norm, false)) return -1;
-    } else {
-      if (gemm_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
-      if (resid_norm(&sk, static_cast<long long>(T) * H, d.post_norm, false)) return -1;
-    }
+    if (gemm_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
+    if (resid_norm(&sk, d.post_norm, false)) return -1;
     // ---- gate|up + SwiGLU
-    if (fm & 4) {
-      GemmWsfArgs g{};
-      g.act = e->act;
-      g.I = c.intermediate_size;
-      if (gemm_fused(e, g, WSF_SWIGLU, d.gate_up, 2 * c.intermediate_size, e->xn, T, H, st)) return -1;
-    } else {
-      if (gemm_partial(e, d.gate_up, 2 * c.intermediate_size, e->xn, T, H, &sk, st)) return -1;
-      SwigluParams p{};
-      p.part = e->part;
-      p.n_splits = -1;
-      p.sk = sk;
-      p.split_stride = static_cast<long long>(T) * 2 * c.intermediate_size;
-      p.act = e->act;
-      p.T = T;
-      p.I = c.intermediate_size;
-      const long long n2 = static_cast<long long>(T) * c.intermediate_size / 4;
-      VLO_CUDA(launch_pdl(swiglu_kernel, dim3(static_cast<unsigned>(std::min<long long>((n2 + 255) / 256, 4 * num_sms()))),
-                          dim3(256), 0, st, p));
-      count_launch();
-    }
+    if (gemm_swiglu(e, d.gate_up, 2 * c.intermediate_size, e->xn, T, H, st)) return -1;
     // ---- down_proj + residual, then the next RMSNorm (next layer's input norm, or the final norm + last-row compaction)
-    const bf16* next_norm = is_last ? e->final_norm : e->dec[l + 1].in_norm;
-    if (fm & 8) {
-      if (gemm_fused(e, r, WSF_RESID, d.down, H, e->act, T, c.intermediate_size, st)) return -1;
-      if (resid_norm(nullptr, 0, next_norm, is_last)) return -1;
-    } else {
-      if (gemm_partial(e, d.down, H, e->act, T, c.intermediate_size, &sk, st)) return -1;
-      if (resid_norm(&sk, static_cast<long long>(T) * H, next_norm, is_last)) return -1;
-    }
+    if (gemm_partial(e, d.down, H, e->act, T, c.intermediate_size, &sk, st)) return -1;
+    if (resid_norm(&sk, is_last ? e->final_norm : e->dec[l + 1].in_norm, is_last)) return -1;
   }
   // ---- last-position lm_head + on-device decision
   bf16* logits = d_last_logits ? static_cast<bf16*>(d_last_logits) : e->logits;

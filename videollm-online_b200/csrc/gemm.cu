@@ -90,16 +90,16 @@ int get_tmap(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMa
   return 0;
 }
 
-template <int FMT, int BN, bool SWAP, int EPI>
+template <int BN, int EPI>
 int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& args, dim3 grid,
                cudaStream_t stream) {
-  auto kern = gemm_tn_kernel<FMT, BN, SWAP, EPI>;
+  auto kern = gemm_tn_kernel<BN, EPI>;
   if (ensure_max_smem(reinterpret_cast<const void*>(kern), GemmCfg<BN>::kSmemBytes)) return -1;
   if (prof_on()) {
     const double esz = (EPI == EPI_STORE16) ? 2.0 : 4.0;
     const double bytes = 2.0 * args.k * (static_cast<double>(args.rows_a) + args.rows_b) +
-                         esz * static_cast<double>(args.rows_a) * args.rows_b * (EPI == EPI_PARTIAL ? grid.z : 1);
-    prof_begin(SWAP ? PROF_GEMM_STREAM : PROF_GEMM_VIT, stream, bytes);
+                         esz * static_cast<double>(args.rows_a) * args.rows_b;
+    prof_begin(PROF_GEMM_VIT, stream, bytes);
   }
   VLO_CUDA(launch_pdl(kern, grid, dim3(kGemmThreads), GemmCfg<BN>::kSmemBytes, stream, ta, tb, args));
   prof_end(stream);
@@ -109,144 +109,51 @@ int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& arg
 
 }  // namespace
 
-// Query tensor [n_tok][n_heads][128] bf16 as a 3-D map; one box = (64 dims, G heads of one kv head, 128/G tokens)
-// lands in shared memory as 128 rows of 128 B ordered row = token * G + head: the K-major SW128 A tile of the
-// attention kernel.  Tokens past n_tok are zero-filled by the TMA unit.  box_rows (32 / 64 / 128, a multiple of G)
-// selects a smaller box of box_rows / G tokens: the v3 kernel stacks 128 / box_rows copies of it (key slicing).
-int tmap_q3d_sw128(const void* ptr, int n_tok, int n_heads, int G, CUtensorMap* out, int box_rows) {
-  if (box_rows <= 0) box_rows = 128;
-  TmapKey key{ptr, n_tok, n_heads, -G, 3 + 16 * box_rows};
-  {
-    std::lock_guard<std::mutex> g(g_tmap_mu);
-    auto it = g_tmaps.find(key);
-    if (it != g_tmaps.end()) {
-      *out = it->second;
-      return 0;
-    }
-  }
-  EncodeFn enc = get_encode();
-  if (enc == nullptr) return fail("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) return fail("TMA operand not 16-byte aligned");
-  if (G < 1 || 128 % G != 0 || n_heads % G != 0) return fail("tmap_q3d: GQA group must divide 128 and n_heads");
-  if (box_rows % G != 0 || box_rows > 128) return fail("tmap_q3d: box rows must be a multiple of the GQA group, <= 128");
-  cuuint64_t dims[3] = {128, static_cast<cuuint64_t>(n_heads), static_cast<cuuint64_t>(n_tok)};
-  cuuint64_t strides[2] = {256, static_cast<cuuint64_t>(n_heads) * 256};
-  cuuint32_t box[3] = {64, static_cast<cuuint32_t>(G), static_cast<cuuint32_t>(box_rows / G)};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUtensorMap m;
-  CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (Q, 3-D) failed, CUresult " + std::to_string(r));
-  {
-    std::lock_guard<std::mutex> g(g_tmap_mu);
-    g_tmaps.emplace(key, m);
-  }
-  *out = m;
-  return 0;
-}
-
 int tmap_2d_sw128(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out) {
   return get_tmap(ptr, rows, k, box_rows, fmt, out);
-}
-
-// Largest split count <= want for which every split owns at least one 64-wide k-block.
-int gemm_fix_splits(int k, int want) {
-  const int total_kb = k / kGemmBK;
-  int s = want < 1 ? 1 : (want > total_kb ? total_kb : want);
-  for (; s > 1; --s) {
-    const int per = (total_kb + s - 1) / s;
-    if ((total_kb + per - 1) / per == s) break;
-  }
-  return s;
 }
 
 int gemm_launch(const GemmCall& c, cudaStream_t stream) {
   VLO_CHECK(c.k > 0 && c.k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(c.rows_a > 0 && c.rows_b > 0, "empty GEMM operand");
-  VLO_CHECK(c.splits >= 1, "splits >= 1");
-  VLO_CHECK(c.splits == 1 || c.epi == EPI_PARTIAL, "split-K requires the fp32 partial epilogue");
-  const int total_kb = c.k / kGemmBK;
-  const int splits = c.splits > total_kb ? total_kb : c.splits;
-  const int kb_per = (total_kb + splits - 1) / splits;
-  const int eff_splits = (total_kb + kb_per - 1) / kb_per;  // every split gets >= 1 k-block
-  VLO_CHECK(eff_splits == c.splits, "split count leaves an empty split; use gemm_fix_splits()");
-
-  int bn = c.bn;
-  if (bn == 0) {
-    if (c.swap) bn = c.rows_b <= 16 ? 16 : (c.rows_b <= 32 ? 32 : (c.rows_b <= 64 ? 64 : 128));
-    else bn = 128;
-  }
+  const int bn = c.bn == 0 ? 128 : c.bn;
   GemmArgs a{};
   a.rows_a = c.rows_a;
   a.rows_b = c.rows_b;
   a.k = c.k;
-  a.kb_per_split = kb_per;
   a.out = c.out;
   a.ld_out = c.ld_out;
   a.bias = c.bias;
   a.pos = c.pos;
   a.pos_rows = c.pos_rows > 0 ? c.pos_rows : 1;
   a.act = c.act;
-  a.split_stride = c.split_stride;
-  a.hint_a = c.stream_weights ? kEvictFirst : kEvictNormal;
-  a.hint_b = c.stream_weights ? kEvictLast : kEvictNormal;
 
   CUtensorMap ta, tb;
-  if (get_tmap(c.a, c.rows_a, c.k, kGemmBM, c.fmt, &ta) != 0) return -1;
-  if (get_tmap(c.b, c.rows_b, c.k, bn, c.fmt, &tb) != 0) return -1;
-  dim3 grid((c.rows_a + kGemmBM - 1) / kGemmBM, (c.rows_b + bn - 1) / bn, eff_splits);
+  if (get_tmap(c.a, c.rows_a, c.k, kGemmBM, FMT_F16, &ta) != 0) return -1;
+  if (get_tmap(c.b, c.rows_b, c.k, bn, FMT_F16, &tb) != 0) return -1;
+  dim3 grid((c.rows_a + kGemmBM - 1) / kGemmBM, (c.rows_b + bn - 1) / bn);
 
-#define VLO_GEMM_CASE(F, N, SW, E)                                                        \
-  if (c.fmt == F && bn == N && (c.swap != 0) == SW && c.epi == E)                         \
-    return launch_one<F, N, SW, E>(ta, tb, a, grid, stream);
-
-  // decoder / connector: bf16, swap-AB
-  VLO_GEMM_CASE(FMT_BF16, 16, true, EPI_PARTIAL)
-  VLO_GEMM_CASE(FMT_BF16, 32, true, EPI_PARTIAL)
-  VLO_GEMM_CASE(FMT_BF16, 64, true, EPI_PARTIAL)
-  VLO_GEMM_CASE(FMT_BF16, 128, true, EPI_PARTIAL)
-  VLO_GEMM_CASE(FMT_BF16, 16, true, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_BF16, 32, true, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_BF16, 64, true, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_BF16, 128, true, EPI_STORE16)
-  // ViT MAP head (few rows): fp16, swap-AB
-  VLO_GEMM_CASE(FMT_F16, 16, true, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_F16, 32, true, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_F16, 64, true, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_F16, 128, true, EPI_STORE16)
-  // ViT trunk: fp16, activations on MMA-M
-  VLO_GEMM_CASE(FMT_F16, 64, false, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_F16, 128, false, EPI_STORE16)
-  VLO_GEMM_CASE(FMT_F16, 64, false, EPI_RESID32)
-  VLO_GEMM_CASE(FMT_F16, 128, false, EPI_RESID32)
-  VLO_GEMM_CASE(FMT_F16, 64, false, EPI_PARTIAL)
-  VLO_GEMM_CASE(FMT_F16, 128, false, EPI_PARTIAL)
-  VLO_GEMM_CASE(FMT_F16, 64, false, EPI_PATCH32)
-  VLO_GEMM_CASE(FMT_F16, 128, false, EPI_PATCH32)
-#undef VLO_GEMM_CASE
-  return fail("gemm_launch: no kernel instance for fmt=" + std::to_string(c.fmt) + " bn=" +
-              std::to_string(bn) + " swap=" + std::to_string(c.swap) + " epi=" + std::to_string(c.epi));
+  if (bn == 64 && c.epi == EPI_STORE16) return launch_one<64, EPI_STORE16>(ta, tb, a, grid, stream);
+  if (bn == 128 && c.epi == EPI_STORE16) return launch_one<128, EPI_STORE16>(ta, tb, a, grid, stream);
+  if (bn == 64 && c.epi == EPI_PATCH32) return launch_one<64, EPI_PATCH32>(ta, tb, a, grid, stream);
+  if (bn == 128 && c.epi == EPI_PATCH32) return launch_one<128, EPI_PATCH32>(ta, tb, a, grid, stream);
+  return fail("gemm_launch: no kernel instance for bn=" + std::to_string(bn) + " epi=" + std::to_string(c.epi));
 }
 
 // ------------------------------------------------------------------------------------------------
 // persistent weight-streaming GEMM (gemm_ws.cuh)
 
 // The default single-stream frame step runs the ViT of frame i+1 (gemm_vit_kernel for QKV / fc1, the 64-token
-// small-tile configuration of gemm_ws_kernel for out_proj / fc2; or the 96-token one for all four) next to the
-// decoder step of frame i (16-token tiles, 6 stages).  One CTA of each fits on one sm_90 SM: 228 KB of shared memory
-// per SM, of which 1 KB is reserved per resident block.  The fused gate|up GEMM leaves room for a gemm_vit_kernel CTA
-// with a 6-stage ring, not with 8 (VLO_WSF_STAGES).
+// small-tile configuration of gemm_ws_kernel for out_proj / fc2) next to the decoder step of frame i (16-token tiles,
+// 6 stages).  One CTA of each fits on one sm_90 SM: 228 KB of shared memory per SM, of which 1 KB is reserved per
+// resident block.  The fused gate|up GEMM's 8-stage ring leaves no room for a gemm_vit_kernel CTA (a 6-stage ring
+// would, and measured no faster: DESIGN.md section 5).
 constexpr int kSmemPerSm = 233472, kSmemReservedPerBlock = 1024;
-static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<96, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "decoder GEMM CTA and 96-token ViT GEMM CTA no longer share an SM");
 static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
               "decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
 static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
               "decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
-static_assert(GemmWsfCfg<16, 6>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "6-stage fused decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
-static_assert(GemmWsfCfg<16, 8>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
+static_assert(GemmWsfCfg<16, wsf_default_stages(16)>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
               "the 8-stage fused decoder GEMM now shares its SM with a ViT trunk GEMM CTA: update the comment above");
 
 namespace {
@@ -311,21 +218,9 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
   if (get_tmap(c.x, c.rows_x, c.k, bn, c.fmt, &tx) != 0) return -1;
 #define VLO_WS_CASE(F, N) \
   if (c.fmt == F && bn == N) return launch_ws<F, N>(tw, tx, a, stream);
-  if (c.fmt == FMT_BF16 && bn == 16) {  // ring depth of the single-stream decoder GEMM: A/B switch (VLO_WS_STAGES=6|8|11)
-    static int st = 0;
-    if (st == 0) {
-      const char* e = getenv("VLO_WS_STAGES");
-      st = e ? atoi(e) : 6;
-    }
-    // default 6 x 18 KB: leaves room on the SM for a co-resident small-tile ViT CTA (static_asserts above)
-    if (st == 4) return launch_ws<FMT_BF16, 16, 4>(tw, tx, a, stream);
-    if (st == 5) return launch_ws<FMT_BF16, 16, 5>(tw, tx, a, stream);
-    if (st == 6) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
-    if (st == 11) return launch_ws<FMT_BF16, 16, 11>(tw, tx, a, stream);
-  }
-  if (c.fmt == FMT_F16 && c.small_smem && bn == 96) return launch_ws<FMT_F16, 96, 3>(tw, tx, a, stream);    // 95 KB
+  // the single-stream decoder GEMM: 6 x 18 KB leaves room on the SM for a co-resident ViT CTA (static_asserts above)
+  if (c.fmt == FMT_BF16 && bn == 16) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
   if (c.fmt == FMT_F16 && c.small_smem && bn == 64) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
-  VLO_WS_CASE(FMT_BF16, 16)
   VLO_WS_CASE(FMT_BF16, 32)
   VLO_WS_CASE(FMT_BF16, 64)
   VLO_WS_CASE(FMT_BF16, 96)
@@ -373,12 +268,13 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 }
 
 // ------------------------------------------------------------------------------------------------
-// stream-K GEMM with the fused finisher epilogue (gemm_wsf.cuh)
+// stream-K gate|up GEMM with the SwiGLU finisher epilogue (gemm_wsf.cuh)
 namespace {
-template <int BN, int STAGES, int EPI>
+template <int BN>
 int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, cudaStream_t stream) {
-  auto kern = gemm_wsf_kernel<BN, STAGES, EPI>;
-  using Cfg = GemmWsfCfg<BN, STAGES>;
+  constexpr int S = wsf_default_stages(BN);
+  auto kern = gemm_wsf_kernel<BN, S>;
+  using Cfg = GemmWsfCfg<BN, S>;
   if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
   if (prof_on())
     prof_begin(PROF_GEMM_STREAM, stream, 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x) + 2.0 * a.rows_x * a.rows_w);
@@ -387,43 +283,22 @@ int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& 
   count_launch();
   return 0;
 }
-template <int BN, int STAGES>
-int launch_wsf_epi(int epi, const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, cudaStream_t stream) {
-  if (epi == WSF_RESID) return launch_wsf<BN, STAGES, WSF_RESID>(tw, tx, a, stream);
-  if (epi == WSF_QKV) return launch_wsf<BN, STAGES, WSF_QKV>(tw, tx, a, stream);
-  if (epi == WSF_SWIGLU) return launch_wsf<BN, STAGES, WSF_SWIGLU>(tw, tx, a, stream);
-  return fail("gemm_wsf_launch: unknown epilogue");
-}
 }  // namespace
 
-int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, int epi, cudaStream_t stream) {
+int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, cudaStream_t stream) {
   VLO_CHECK(a.k > 0 && a.k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(a.rows_w > 0 && a.rows_x > 0 && a.rows_x <= 128, "gemm_wsf: 1..128 token rows");
-  VLO_CHECK(epi == WSF_RESID || a.rows_w % kGemmBM == 0, "gemm_wsf: QKV / SwiGLU epilogues need whole 128-row tiles");
+  VLO_CHECK(a.rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
   const int bn = a.rows_x <= 16 ? 16 : (a.rows_x <= 32 ? 32 : (a.rows_x <= 64 ? 64 : (a.rows_x <= 96 ? 96 : 128)));
   VLO_CHECK(a.sk.U == static_cast<long long>((a.rows_w + kGemmBM - 1) / kGemmBM) * (a.k / kGemmBK), "gemm_wsf: plan mismatch");
   CUtensorMap tw, tx;
   if (get_tmap(w, a.rows_w, a.k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
   if (get_tmap(x, a.rows_x, a.k, bn, FMT_BF16, &tx) != 0) return -1;
-  if (bn == 16) {
-    // ring depth (VLO_WSF_STAGES=4|5|6|8|10; default 8 = 144 KB + the 8.7 KB exchange and 10 KB staging tiles).  With 8
-    // stages a co-resident ViT CTA cannot share an SM with the (only) fused GEMM, gate|up, and stop competing with its stream.
-    static int st = 0;
-    if (st == 0) {
-      const char* e = getenv("VLO_WSF_STAGES");
-      st = e ? atoi(e) : 8;
-    }
-    if (st == 4) return launch_wsf_epi<16, 4>(epi, tw, tx, a, stream);
-    if (st == 5) return launch_wsf_epi<16, 5>(epi, tw, tx, a, stream);
-    if (st == 8) return launch_wsf_epi<16, 8>(epi, tw, tx, a, stream);
-    if (st == 10) return launch_wsf_epi<16, 10>(epi, tw, tx, a, stream);
-    if (st == 6) return launch_wsf_epi<16, 6>(epi, tw, tx, a, stream);
-    return launch_wsf_epi<16, 8>(epi, tw, tx, a, stream);
-  }
-  if (bn == 32) return launch_wsf_epi<32, wsf_default_stages(32)>(epi, tw, tx, a, stream);
-  if (bn == 64) return launch_wsf_epi<64, wsf_default_stages(64)>(epi, tw, tx, a, stream);
-  if (bn == 96) return launch_wsf_epi<96, wsf_default_stages(96)>(epi, tw, tx, a, stream);
-  return launch_wsf_epi<128, wsf_default_stages(128)>(epi, tw, tx, a, stream);
+  if (bn == 16) return launch_wsf<16>(tw, tx, a, stream);
+  if (bn == 32) return launch_wsf<32>(tw, tx, a, stream);
+  if (bn == 64) return launch_wsf<64>(tw, tx, a, stream);
+  if (bn == 96) return launch_wsf<96>(tw, tx, a, stream);
+  return launch_wsf<128>(tw, tx, a, stream);
 }
 
 }  // namespace vlo

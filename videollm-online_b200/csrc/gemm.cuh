@@ -1,20 +1,13 @@
 // wgmma / TMA GEMM for sm_90a:   C[i, j] = sum_k A[i, k] * B[j, k]
 //
-// Both operands are K-major ("TN"): A is [rows_a, K], B is [rows_b, K], 16-bit
-// (bf16 or fp16), fp32 accumulation in registers.  One CTA computes one 128 x BN
-// tile (optionally one K-split of it):
+// Both operands are K-major ("TN"): A = activations [rows_a, K], B = weights [rows_b, K], fp16, fp32
+// accumulation in registers.  One CTA computes one 128 x BN tile of out[rows_a, rows_b]:
 //   warps 0-3  one warpgroup: wgmma.mma_async m64nBNk16 on both 64-row halves of the
 //              tile, then the epilogue (accumulators -> shared staging tile -> global)
 //   warp 4     TMA producer   (cp.async.bulk.tensor, 128B-swizzled boxes)
-// connected by an mbarrier full/empty ring.
-//
-// Two orientations share the kernel:
-//   SWAP = false  A = activations [M, K], B = weights [N, K]; out[M, N]   (ViT: M = 576*B rows)
-//   SWAP = true   A = weights [N, K],     B = activations [T, K]; out[T, N]
-//                 "swap-AB": the weight matrix rides the 128-row M tile and the (few)
-//                 tokens are the wgmma N dimension (16..128), so a decoder step
-//                 with T = 11..96 tokens streams every weight byte exactly once at full
-//                 tensor-core tile efficiency.  The kernel is then HBM-bound.
+// connected by an mbarrier full/empty ring.  It runs the ViT patch embed (EPI_PATCH32) and the MAP-head K/V
+// projection (EPI_STORE16).  The persistent kernels (gemm_ws.cuh, gemm_wsf.cuh, gemm_vit.cuh) build on the tile
+// constants and helpers defined here.
 //
 // Replaces, for the hot path, the cuBLAS/cuDNN GEMMs reached from
 //   HF:models/llama/modeling_llama.py:262-264,288,182-184,487  (q/k/v/o, MLP, lm_head)
@@ -28,9 +21,7 @@
 namespace vlo {
 
 enum GemmEpi : int {
-  EPI_PARTIAL = 0,  // fp32 raw accumulators -> ws[split][out_row][out_col]   (split-K)
   EPI_STORE16 = 1,  // out16 = r16(act(r16(acc + bias)))
-  EPI_RESID32 = 2,  // out32 += r16(acc + bias)                (fp32 residual stream, ViT)
   EPI_PATCH32 = 3,  // out32  = r16(acc + bias) + pos[out_row % pos_rows]     (ViT patch embed)
 };
 enum GemmAct : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF_PY = 2 };
@@ -38,15 +29,12 @@ enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1 };
 
 struct GemmArgs {
   int rows_a, rows_b, k;
-  int kb_per_split;  // 64-wide k-blocks handled by one split (blockIdx.z)
   void* out;
-  int ld_out;  // row stride of the logical output, elements
+  int ld_out;  // row stride of the output, elements
   const float* bias;  // per output column (feature) or nullptr
   const float* pos;   // EPI_PATCH32: [pos_rows, ld_out] fp32
   int pos_rows;
   int act;
-  long long split_stride;  // EPI_PARTIAL: elements between split planes
-  unsigned long long hint_a, hint_b;  // TMA L2 cache hints
 };
 
 constexpr int kGemmBM = 128;
@@ -182,7 +170,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return v;
 }
 
-template <int FMT, int BN, bool SWAP, int EPI>
+template <int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                const GemmArgs p) {
@@ -200,11 +188,8 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m_tile = blockIdx.x, n_tile = blockIdx.y, split = blockIdx.z;
-  const int total_kb = p.k / kGemmBK;
-  const int kb0 = split * p.kb_per_split;
-  const int kb1 = min(kb0 + p.kb_per_split, total_kb);
-  const int nkb = kb1 - kb0;
+  const int m_tile = blockIdx.x, n_tile = blockIdx.y;
+  const int nkb = p.k / kGemmBK;
 
   if (warp == kGemmProducerWarp && lane == 0) {
     tma_prefetch_desc(&tm_a);
@@ -227,28 +212,24 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
         const uint32_t ph = (i / S) & 1;
         mbar_wait(&empty_bar[s], ph ^ 1);
         mbar_arrive_expect_tx(&full_bar[s], Cfg::kBytesA + Cfg::kBytesB);
-        const int kc = (kb0 + i) * kGemmBK;
-        tma_load_2d(smem_a + s * Cfg::kBytesA, &tm_a, &full_bar[s], kc, m_tile * kGemmBM, p.hint_a);
-        tma_load_2d(smem_b + s * Cfg::kBytesB, &tm_b, &full_bar[s], kc, n_tile * BN, p.hint_b);
+        const int kc = i * kGemmBK;
+        tma_load_2d(smem_a + s * Cfg::kBytesA, &tm_a, &full_bar[s], kc, m_tile * kGemmBM, kEvictNormal);
+        tma_load_2d(smem_b + s * Cfg::kBytesB, &tm_b, &full_bar[s], kc, n_tile * BN, kEvictNormal);
       }
     }
   } else {
     // -------------------------------------------------- MMA + epilogue warpgroup (warps 0-3)
-    // per-column bias of this tile -> shared memory (SWAP = false only)
-    if (!SWAP && EPI != EPI_PARTIAL) {
-      for (int j = threadIdx.x; j < BN; j += 128) {
-        const int col = n_tile * BN + j;
-        s_bias[j] = (p.bias != nullptr && col < p.rows_b) ? __ldg(p.bias + col) : 0.f;
-      }
+    // per-column bias of this tile -> shared memory
+    for (int j = threadIdx.x; j < BN; j += 128) {
+      const int col = n_tile * BN + j;
+      s_bias[j] = (p.bias != nullptr && col < p.rows_b) ? __ldg(p.bias + col) : 0.f;
     }
     float acc[2][BN / 2];
     int i = 0;
-    wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nkb);
+    wg_mainloop<FMT_F16, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nkb);
     const int row = threadIdx.x;  // tile row this thread finishes
     const int a_row = m_tile * kGemmBM + row;
     const bool a_ok = a_row < p.rows_a;
-    float bias_a = 0.f;
-    if (SWAP && EPI != EPI_PARTIAL && p.bias != nullptr && a_ok) bias_a = __ldg(p.bias + a_row);
 
 #pragma unroll
     for (int c0 = 0; c0 < BN; c0 += kWgChunk) {
@@ -259,83 +240,41 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__
       if (!a_ok || b0 >= p.rows_b) continue;
       float v[16];
       wg_load16(stage, row, v);
-      if (SWAP) {
-        // out[token = b, feature = a]; lanes hold consecutive features -> coalesced.
+      // out[row = a, feature = b]; this thread owns 16 consecutive features of one row.
+      const int nvalid = min(16, p.rows_b - b0);
+      float x[16];
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int b = b0 + j;
-          if (b >= p.rows_b) break;
-          const float acc = v[j];
-          const size_t idx = static_cast<size_t>(b) * p.ld_out + a_row;
-          if (EPI == EPI_PARTIAL) {
-            reinterpret_cast<float*>(p.out)[static_cast<size_t>(split) * p.split_stride + idx] = acc;
-          } else if (EPI == EPI_STORE16) {
-            float x = r16<FMT>(acc + bias_a);
-            x = apply_act<FMT>(x, p.act);
-            reinterpret_cast<uint16_t*>(p.out)[idx] = to16<FMT>(x);
-          } else if (EPI == EPI_RESID32) {
-            float* o = reinterpret_cast<float*>(p.out) + idx;
-            *o = *o + r16<FMT>(acc + bias_a);
-          } else {
-            const float pe = __ldg(p.pos + static_cast<size_t>(b % p.pos_rows) * p.ld_out + a_row);
-            reinterpret_cast<float*>(p.out)[idx] = r16<FMT>(acc + bias_a) + pe;
-          }
+      for (int j = 0; j < 16; ++j) {
+        float acc = r16<FMT_F16>(v[j] + s_bias[c0 + j]);
+        if (EPI == EPI_STORE16) acc = apply_act<FMT_F16>(acc, p.act);
+        x[j] = acc;
+      }
+      const size_t idx = static_cast<size_t>(a_row) * p.ld_out + b0;
+      const bool vec_ok = (nvalid == 16) && ((p.ld_out & 7) == 0);
+      if (EPI == EPI_STORE16) {
+        uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + idx;
+        if (vec_ok) {
+          uint32_t w[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            w[j] = static_cast<uint32_t>(to16<FMT_F16>(x[2 * j])) |
+                   (static_cast<uint32_t>(to16<FMT_F16>(x[2 * j + 1])) << 16);
+          reinterpret_cast<uint4*>(o)[0] = make_uint4(w[0], w[1], w[2], w[3]);
+          reinterpret_cast<uint4*>(o)[1] = make_uint4(w[4], w[5], w[6], w[7]);
+        } else {
+          for (int j = 0; j < nvalid; ++j) o[j] = to16<FMT_F16>(x[j]);
         }
       } else {
-        // out[row = a, feature = b]; this thread owns 16 consecutive features of one row.
-        const int nvalid = min(16, p.rows_b - b0);
-        float x[16];
+        float* o = reinterpret_cast<float*>(p.out) + idx;
+        const float* pe = p.pos + static_cast<size_t>(a_row % p.pos_rows) * p.ld_out + b0;
+        if (vec_ok) {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          float acc = v[j];
-          if (EPI != EPI_PARTIAL) {
-            acc = r16<FMT>(acc + s_bias[c0 + j]);
-            if (EPI == EPI_STORE16) acc = apply_act<FMT>(acc, p.act);
-          }
-          x[j] = acc;
-        }
-        const size_t idx = static_cast<size_t>(a_row) * p.ld_out + b0;
-        const bool vec_ok = (nvalid == 16) && ((p.ld_out & 7) == 0);
-        if (EPI == EPI_STORE16) {
-          uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + idx;
-          if (vec_ok) {
-            uint32_t w[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              w[j] = static_cast<uint32_t>(to16<FMT>(x[2 * j])) |
-                     (static_cast<uint32_t>(to16<FMT>(x[2 * j + 1])) << 16);
-            reinterpret_cast<uint4*>(o)[0] = make_uint4(w[0], w[1], w[2], w[3]);
-            reinterpret_cast<uint4*>(o)[1] = make_uint4(w[4], w[5], w[6], w[7]);
-          } else {
-            for (int j = 0; j < nvalid; ++j) o[j] = to16<FMT>(x[j]);
+          for (int j = 0; j < 16; j += 4) {
+            const float4 pp = __ldg(reinterpret_cast<const float4*>(pe + j));
+            reinterpret_cast<float4*>(o + j)[0] = make_float4(x[j] + pp.x, x[j + 1] + pp.y, x[j + 2] + pp.z, x[j + 3] + pp.w);
           }
         } else {
-          float* o = reinterpret_cast<float*>(p.out) + idx +
-                     (EPI == EPI_PARTIAL ? static_cast<size_t>(split) * p.split_stride : 0);
-          const float* pe = nullptr;
-          if (EPI == EPI_PATCH32)
-            pe = p.pos + static_cast<size_t>(a_row % p.pos_rows) * p.ld_out + b0;
-          if (vec_ok) {
-#pragma unroll
-            for (int j = 0; j < 16; j += 4) {
-              float4 t = make_float4(x[j], x[j + 1], x[j + 2], x[j + 3]);
-              if (EPI == EPI_RESID32) {
-                const float4 old = reinterpret_cast<float4*>(o + j)[0];
-                t.x += old.x; t.y += old.y; t.z += old.z; t.w += old.w;
-              } else if (EPI == EPI_PATCH32) {
-                const float4 pp = __ldg(reinterpret_cast<const float4*>(pe + j));
-                t.x += pp.x; t.y += pp.y; t.z += pp.z; t.w += pp.w;
-              }
-              reinterpret_cast<float4*>(o + j)[0] = t;
-            }
-          } else {
-            for (int j = 0; j < nvalid; ++j) {
-              float t = x[j];
-              if (EPI == EPI_RESID32) t += o[j];
-              if (EPI == EPI_PATCH32) t += __ldg(pe + j);
-              o[j] = t;
-            }
-          }
+          for (int j = 0; j < nvalid; ++j) o[j] = x[j] + __ldg(pe + j);
         }
       }
     }

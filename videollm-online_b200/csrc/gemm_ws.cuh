@@ -1,14 +1,14 @@
 // Persistent weight-streaming GEMM (decoder / connector / lm_head):  out[t, n] = sum_k X[t, k] * W[n, k]
 //
-// Same wgmma / TMA machinery as gemm.cuh in its swap-AB orientation (W rows ride the 128-row M tile, the
-// T <= 128 tokens are the wgmma N dimension), but scheduled for an HBM-bound problem:
+// Same wgmma / TMA machinery as gemm.cuh, swap-AB (W rows ride the 128-row M tile, the T <= 128 tokens are
+// the wgmma N dimension) and scheduled for an HBM-bound problem:
 //   * ONE CTA per SM, resident for the whole GEMM: barrier init and descriptor prefetch
 //     are paid once and the TMA ring never drains between work items;
 //   * stream-K: the (weight tile, 64-wide k-block) units are dealt out evenly, CTA c owns the contiguous
 //     unit range [c*U/G, (c+1)*U/G), so all SMs stream the same number of bytes (no wave
 //     quantisation, no tail).  A CTA whose range crosses a tile boundary emits one fp32 partial per tile
 //     it touches into plane (c - first_cta_of_tile); the consumer kernels (resid_rmsnorm / qkv_rope /
-//     swiglu) add the planes of each tile in plane order -> deterministic;
+//     vit_fix_ln) add the planes of each tile in plane order -> deterministic;
 //   * TILES mode (lm_head, connector): whole tiles per CTA, direct 16-bit epilogue, no partials;
 //   * the producer warp keeps the ring full across items, so the weight stream continues while the warpgroup
 //     runs the epilogue of an item.

@@ -1,4 +1,4 @@
-// Persistent stream-K weight-streaming GEMM with the fix-up FUSED into its epilogue (decoder GEMMs, bf16):
+// Persistent stream-K weight-streaming GEMM with the SwiGLU fix-up FUSED into its epilogue (the decoder's gate|up, bf16):
 //   out[t, n] = sum_k X[t, k] * W[n, k]      X = the step's <= 128 tokens (MMA-N), W rows ride MMA-M (128-row tiles)
 //
 // Same TMA ring / wgmma / stream-K schedule as gemm_ws.cuh (CTA c owns the contiguous unit range [c*U/G, (c+1)*U/G),
@@ -8,13 +8,11 @@
 //     finisher's accumulator is complete the other partials have long been published;
 //   * contributors write their fp32 partial plane, fence, and bump the tile's arrival counter (flags[tile]);
 //   * the finisher waits for the counter (normally already there), adds the planes in plane order to its own
-//     accumulator (deterministic), resets the counter and applies the fused epilogue:
-//       WSF_RESID   h[t, n] = bf16(h[t, n] + bf16(y))                       (o_proj / down_proj + residual, HF:...llama.py:325,331)
-//       WSF_QKV     RoPE on q / k heads (tile == head), Q -> q_out, K / V appended IN PLACE to the cache
-//                   (HF:...llama.py:262-264, 146-168; cache_utils.py:119-120)
-//       WSF_SWIGLU  act = bf16(bf16(silu(g)) * u)  with gate / up rows interleaved per tile (64 + 64)   (HF:...llama.py:182-184)
-//     the two halves of a head (d, d + 64) and gate / up are finished by different threads: they are exchanged through a
-//     small shared-memory tile.  Rounding points are those of decoder_kernels.cuh.
+//     accumulator (deterministic), resets the counter and applies SwiGLU:
+//       act = bf16(bf16(silu(g)) * u)  with gate / up rows interleaved per tile (64 + 64)   (HF:...llama.py:182-184)
+//     gate and up are finished by different threads: they are exchanged through a small shared-memory tile.
+// Only gate|up has enough tiles to amortise the finisher tail; q|k|v, o_proj and down_proj leave fp32 planes to the
+// fix-up kernels of decoder_kernels.cuh, whose rounding points this epilogue shares.
 // All CTAs of the grid are co-resident or become so without depending on a waiting CTA (grid <= #SMs, the PDL successor
 // cannot start before every CTA of this grid has started), so the finisher's wait cannot dead-lock; it is bounded anyway.
 #pragma once
@@ -24,8 +22,6 @@
 
 namespace vlo {
 
-enum WsfEpi : int { WSF_RESID = 1, WSF_QKV = 2, WSF_SWIGLU = 3 };
-
 struct GemmWsfArgs {
   int rows_w, rows_x, k;
   SkInfo sk;
@@ -33,19 +29,6 @@ struct GemmWsfArgs {
   long long plane_stride;
   int* flags;                 // [tiles] arrival counters; zero between launches (the finisher resets them)
   unsigned long long hint_w;
-  // WSF_RESID
-  __nv_bfloat16* h;           // [rows_x, rows_w] residual stream, updated in place
-  // WSF_QKV
-  const __nv_bfloat16* cos_tab;
-  const __nv_bfloat16* sin_tab;
-  const int* tok_pos;
-  const long long* tok_kvrow;
-  int kv_head_stride;
-  __nv_bfloat16* q_out;       // [rows_x, n_heads, 128]
-  __nv_bfloat16* k_cache;
-  __nv_bfloat16* v_cache;
-  int n_heads, n_kv_heads;
-  // WSF_SWIGLU
   __nv_bfloat16* act;         // [rows_x, I]
   int I;
 };
@@ -72,9 +55,12 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-template <int BN, int STAGES, int EPI>
+// p is __grid_constant__ so that its fields are read from parameter space where used: ptxas otherwise copies a struct
+// this small up front, which costs the 64- and 128-token instances registers.
+template <int BN, int STAGES>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x, const GemmWsfArgs p) {
+gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
+                const __grid_constant__ GemmWsfArgs p) {
   using Cfg = GemmWsfCfg<BN, STAGES>;
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -206,69 +192,24 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
         }
 #pragma unroll
         for (int j = 0; j < 16; ++j) x[j] = bf16_round(x[j]);    // the Linear output in bf16
-        if (EPI == WSF_RESID) {
-          if (n_ok) {
+        // tile rows 0..63 = gate features 64*tile.., rows 64..127 = the matching up features
+        if (d >= 64) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int t = c0 + j;
-              if (t >= p.rows_x) break;
-              __nv_bfloat16* hp = p.h + static_cast<size_t>(t) * p.rows_w + n;
-              *hp = __float2bfloat16_rn(__bfloat162float(*hp) + x[j]);
-            }
-          }
-        } else if (EPI == WSF_QKV) {
-          const int hh = tile;                                   // one 128-row tile == one head
-          const bool rot = hh < p.n_heads + p.n_kv_heads;
-          float xp[16];
-          if (rot) {                                             // partner half (d ^ 64) through shared memory
-#pragma unroll
-            for (int j = 0; j < 16; ++j) xch[d * kWsfXchStride + j] = x[j];
-            wg_sync();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) xp[j] = xch[(d ^ 64) * kWsfXchStride + j];
-            wg_sync();
-          }
+          for (int j = 0; j < 16; ++j) xch[(d - 64) * kWsfXchStride + j] = x[j];
+        }
+        wg_sync();
+        if (d < 64) {
+          const int f = tile * 64 + d;
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const int t = c0 + j;
             if (t >= p.rows_x) break;
-            const int pos = p.tok_pos[t];
-            float o = x[j];
-            if (rot) {
-              const float cs = __bfloat162float(p.cos_tab[static_cast<size_t>(pos) * 64 + (d & 63)]);
-              const float sn = __bfloat162float(p.sin_tab[static_cast<size_t>(pos) * 64 + (d & 63)]);
-              o = (d < 64) ? bf16_round(bf16_round(x[j] * cs) + bf16_round(-xp[j] * sn))
-                           : bf16_round(bf16_round(x[j] * cs) + bf16_round(xp[j] * sn));
-            }
-            __nv_bfloat16* dst;
-            if (hh < p.n_heads) {
-              dst = p.q_out + (static_cast<size_t>(t) * p.n_heads + hh) * 128;
-            } else {
-              const int kvh = (hh - p.n_heads) % p.n_kv_heads;
-              __nv_bfloat16* base = (hh < p.n_heads + p.n_kv_heads) ? p.k_cache : p.v_cache;
-              dst = base + (p.tok_kvrow[t] + static_cast<long long>(kvh) * p.kv_head_stride + pos) * 128;
-            }
-            dst[d] = __float2bfloat16_rn(o);
+            const float g = x[j], up = xch[d * kWsfXchStride + j];
+            const float a = bf16_round(g / (1.0f + expf(-g)));
+            p.act[static_cast<size_t>(t) * p.I + f] = __float2bfloat16_rn(a * up);
           }
-        } else {  // WSF_SWIGLU: tile rows 0..63 = gate features 64*tile.., rows 64..127 = the matching up features
-          if (d >= 64) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) xch[(d - 64) * kWsfXchStride + j] = x[j];
-          }
-          wg_sync();
-          if (d < 64) {
-            const int f = tile * 64 + d;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int t = c0 + j;
-              if (t >= p.rows_x) break;
-              const float g = x[j], up = xch[d * kWsfXchStride + j];
-              const float a = bf16_round(g / (1.0f + expf(-g)));
-              p.act[static_cast<size_t>(t) * p.I + f] = __float2bfloat16_rn(a * up);
-            }
-          }
-          wg_sync();
         }
+        wg_sync();
       }
     }
   }

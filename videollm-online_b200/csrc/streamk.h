@@ -7,6 +7,9 @@
 
 namespace vlo {
 
+// The fix-up kernels unroll their plane loads to this many planes; the launchers reject plans that need more.
+constexpr int kFixMaxPlanes = 8;
+
 struct SkInfo {
   long long U;  // total units = tiles * kb
   int kb;       // k-blocks per tile

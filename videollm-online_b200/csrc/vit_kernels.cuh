@@ -85,13 +85,12 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const InT* in, const flo
   }
 }
 
-// Split-K fix-up + fp32 residual add + LayerNorm in one pass over a token row:
+// Stream-K fix-up + fp32 residual add + LayerNorm in one pass over a token row:
 //   y    = fp16(sum_s part[s][r][:] + bias)      (the out_proj / fc2 Linear output under fp16 autocast)
 //   h[r] += y                                     (fp32 residual stream, HF:...siglip.py:353,360)
 //   out  = LayerNorm(h[r])                        (the next layer_norm1 / layer_norm2 / post_layernorm)
 struct VitFixLnParams {
-  const float* part;  // [planes][rows][C]
-  int n_splits;       // > 0: that many planes; < 0: stream-K planes of tile (col/128) * sk_xtiles + row / sk_bn
+  const float* part;  // [planes][rows][C], stream-K planes of tile (col/128) * sk_xtiles + row / sk_bn
   SkInfo sk;
   int sk_bn, sk_xtiles;
   long long split_stride;
@@ -107,25 +106,24 @@ struct VitFixLnParams {
 __global__ void __launch_bounds__(256) vit_fix_ln_kernel(const VitFixLnParams p) {
   pdl_trigger();
   pdl_wait();
-  // 4 contiguous channels per thread per sweep; the (<= 8) plane loads of a sweep are independent.
+  // 4 contiguous channels per thread per sweep; the (<= kFixMaxPlanes) plane loads of a sweep are independent.
   extern __shared__ float row[];
   __shared__ float red[32];
   const size_t r = blockIdx.x;
   const int C = p.C;
   float s = 0.f;
   for (int i = threadIdx.x * 4; i < C; i += blockDim.x * 4) {
-    float4 a[8];
-    const int ns = p.n_splits > 0 ? p.n_splits
-                                  : sk_planes((i >> 7) * p.sk_xtiles + static_cast<int>(r) / p.sk_bn, p.sk);
+    float4 a[kFixMaxPlanes];
+    const int ns = sk_planes((i >> 7) * p.sk_xtiles + static_cast<int>(r) / p.sk_bn, p.sk);
 #pragma unroll
-    for (int k = 0; k < 8; ++k)
+    for (int k = 0; k < kFixMaxPlanes; ++k)
       a[k] = (k < ns) ? *reinterpret_cast<const float4*>(p.part + k * p.split_stride + r * C + i)
                               : make_float4(0.f, 0.f, 0.f, 0.f);
     const float4 hv = *reinterpret_cast<const float4*>(p.h + r * C + i);
     const float4 bv = *reinterpret_cast<const float4*>(p.bias + i);
     float4 y = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
+    for (int k = 0; k < kFixMaxPlanes; ++k) {
       y.x += a[k].x; y.y += a[k].y; y.z += a[k].z; y.w += a[k].w;
     }
     float4 v;
