@@ -42,7 +42,7 @@ typedef struct vlo_config {
   int32_t frame_token_cls, pool_h, pool_w;
   /* capacities */
   int32_t max_streams;     /* concurrent video streams (KV caches) on this GPU */
-  int32_t max_kv_tokens;   /* per-stream KV capacity, tokens */
+  int32_t max_kv_tokens;   /* per-stream KV cap, tokens (the pool is shared: see vlo_engine_create_pooled) */
   int32_t max_step_tokens; /* max total new tokens in one vlo_step */
   int32_t max_vit_batch;   /* max frames per vlo_vit_encode */
 } vlo_config;
@@ -78,6 +78,14 @@ int vlo_device_supported(int device);
  * replaces: build_live / LiveLlamaForCausalLM.from_pretrained + model.to('cuda')
  *           (models/modeling_live.py:184-222, demo/inference.py:15-16) */
 int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out);
+/* KV cache = a pool of kv_pool_tokens (rounded up to whole 64-token pages) shared by all streams;
+ * max_kv_tokens stays the per-stream cap.  kv_pool_tokens <= 0: max_streams * max_kv_tokens,
+ * which is what vlo_engine_create reserves.  A stream holds ceil(kv_len / 64) pages; a step (or
+ * vlo_kv_write / vlo_kv_copy_prefix / vlo_kv_fill_synthetic) that needs more pages than are free fails
+ * with a "KV page pool exhausted" message and changes no stream.  max_kv_tokens may not exceed 552 896 (the
+ * attention stages a split's page table in shared memory). */
+int vlo_engine_create_pooled(const vlo_config* cfg, int64_t kv_pool_tokens, int device, vlo_engine** out);
+int vlo_kv_pool_info(vlo_engine* e, int* page_tokens, int64_t* total_pages, int64_t* free_pages);
 int vlo_engine_destroy(vlo_engine* e);
 /* Register one weight tensor that already lives on the device in the ENGINE layout (see
  * DESIGN.md "weight layout"; the Python loader does the HF/peft key mapping, LoRA merge and
@@ -102,7 +110,8 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_stream_id, int dst_stream_id, int 
 /* test/bench hook: fill a stream's KV cache with deterministic pseudo-random values up to n_tokens
  * (pre-fill for the 12k-context measurements without replaying 1200 frames) */
 int vlo_kv_fill_synthetic(vlo_engine* e, int stream_id, int n_tokens, uint64_t seed, void* cuda_stream);
-/* copy one layer's K or V rows [n_kv_heads, len, head_dim] bf16 out of / into the cache (tests) */
+/* copy one layer's K or V rows [n_kv_heads, len, head_dim] bf16 out of / into the cache (tests); d_out / d_in must be
+ * 16-byte aligned (the copy moves 16 bytes per thread) */
 int vlo_kv_read(vlo_engine* e, int stream_id, int layer, int is_v, void* d_out, void* cuda_stream);
 int vlo_kv_write(vlo_engine* e, int stream_id, int layer, int is_v, const void* d_in, int n_tokens, void* cuda_stream);
 
@@ -184,6 +193,12 @@ int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, in
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len);
 int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void* d_out, float* d_ws, int n_tok,
                          int n_heads, int n_kv_heads, int head_dim, int kv_len, long long kv_stride, void* cuda_stream);
+/* kernel-level: the decoder attention over a paged pool [n_pages, n_kv_heads, 64, 128] (tests).  d_page_table: device
+ * int32 [ceil(kv_len / 64)], the page of each 64-key block; other arguments as vlo_op_attn_kvappend.  Rows of the last
+ * page past kv_len must be finite. */
+int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
+                               int n_pages, void* d_out, float* d_ws, int n_tok, int n_heads, int n_kv_heads,
+                               int head_dim, int kv_len, void* cuda_stream);
 /* Micro-loop of the same attention over n_layers separate K / V matrices (working set > L2), iters passes of back-to-back
  * launches on one plan: what bench tools bracket with ONE CUDA-event pair (per-launch time incl. the PDL overlap of a real
  * step).  skip_merge != 0 launches the main kernel only.  Mirrors vlo_bench_attn without an engine. */

@@ -52,6 +52,8 @@ SIGNATURES = {
     "vlo_profile_enable": (_I, [_I]),
     "vlo_profile_read": (_I, [C.POINTER(C.c_double), C.POINTER(_LL), C.POINTER(C.c_double), _I]),
     "vlo_engine_create": (_I, [C.POINTER(VloConfig), _I, C.POINTER(_P)]),
+    "vlo_engine_create_pooled": (_I, [C.POINTER(VloConfig), C.c_int64, _I, C.POINTER(_P)]),
+    "vlo_kv_pool_info": (_I, [_P, C.POINTER(_I), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "vlo_engine_destroy": (_I, [_P]),
     "vlo_load_tensor": (_I, [_P, C.c_char_p, _P, C.c_int64]),
     "vlo_finalize_weights": (_I, [_P]),
@@ -79,6 +81,7 @@ SIGNATURES = {
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
     "vlo_op_attn_kvappend": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P]),
+    "vlo_op_attn_kvappend_paged": (_I, [_P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),
 }
 

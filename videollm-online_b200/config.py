@@ -113,6 +113,7 @@ class LiveArguments:
     # engine-side additions
     device: str = "cuda:0"
     max_streams: int = 1
+    kv_pool_tokens: int = 0  # KV page pool shared by the streams, tokens; 0: max_streams x the per-stream cap
     synthetic_weights: bool = False
     seed: int = 0
 

@@ -10,8 +10,12 @@
 #include <vector>
 
 #include "common.h"
+#include "kv_pages.h"
 
 namespace vlo {
+
+// every 64-key TMA box of the attention lies in one page of the KV pool
+static_assert(kKvPageTokens == kAttnBlk, "KV page size must equal the attention key block");
 
 namespace {
 constexpr size_t kAlign = 256;
@@ -56,21 +60,20 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   for (int s = 0; s < n_seqs; ++s) {
     const AttnSeq& q = seqs[s];
     VLO_CHECK(q.q_len > 0 && q.kv_len >= q.q_len, "bad sequence lengths");
-    VLO_CHECK(q.kv_row0 >= 0 && q.kv_row0 < (1ll << 31), "kv_row0 out of range");
+    VLO_CHECK(q.pt0 >= 0, "page-table offset out of range");
     for (int t0 = 0; t0 < q.q_len; t0 += per) {
       AttnItem it{};
       it.q_tok0 = q.q_tok0 + t0;
       it.q_count = std::min(per, q.q_len - t0);
       it.q_pos0 = q.kv_len - q.q_len + t0;
-      it.kv_row0 = static_cast<int>(q.kv_row0);
-      it.kv_head_stride = q.kv_head_stride;
+      it.pt0 = q.pt0;
       for (int t = 0; t < it.q_count; ++t) tok_item[it.q_tok0 + t] = static_cast<int>(items.size());
       items.push_back(it);
     }
   }
   const int n_items = static_cast<int>(items.size());
   const int want = std::max(1, num_sms() / (n_kv_heads * n_items));
-  int max_splits = 1;
+  int max_splits = 1, max_bps = 2;
   size_t slots = 0;
   double algo = 0.0;
   for (const AttnItem& it : items)  // SURVEY 8(d): K+V rows read once per item, Q read, output written
@@ -82,6 +85,9 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
     int bps = (nblk + want - 1) / want;
     bps = std::max(2, bps + (bps & 1));  // even: both warp groups get the same number of blocks
     it.blocks_per_split = bps;
+    VLO_CHECK(bps <= kAttnPtMax, "attention split of " + std::to_string(bps) + " key blocks exceeds the " +
+                                   std::to_string(kAttnPtMax) + " page-table entries a CTA can stage");
+    max_bps = std::max(max_bps, bps);
     it.n_splits = (nblk + bps - 1) / bps;
     it.ws_slot0 = static_cast<int>(slots);
     slots += static_cast<size_t>(n_kv_heads) * it.n_splits * it.q_count * G;
@@ -102,6 +108,7 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   plan->d_tok_item = reinterpret_cast<int*>(w);
   plan->n_items = n_items;
   plan->max_splits = max_splits;
+  plan->max_blocks_per_split = max_bps;
   plan->total_tokens = total_tokens;
 
   uint8_t* hs = static_cast<uint8_t*>(h_stage);
@@ -112,6 +119,8 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   VLO_CUDA(cudaMemcpyAsync(plan->d_tok_item, hs2, sizeof(int) * total_tokens, cudaMemcpyHostToDevice, stream));
   return 0;
 }
+
+int attn_max_key_blocks() { return kAttnPtMax - 1; }  // blocks_per_split rounds an odd block count up by one
 
 static int launch_merge(const AttnPlan& plan, void* d_out, int n_heads, int n_kv_heads, float scale_log2, cudaStream_t stream) {
   AttnMergeParams mp{};
@@ -130,25 +139,31 @@ static int launch_merge(const AttnPlan& plan, void* d_out, int n_heads, int n_kv
   return 0;
 }
 
-int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows, void* d_out,
-             int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream) {
+int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows,
+             const int* d_page_table, long long page_stride_rows, long long head_stride_rows, void* d_out, int n_heads,
+             int n_kv_heads, int head_dim, cudaStream_t stream) {
   VLO_CHECK(kv_rows > 0 && kv_rows < (1ll << 31), "KV matrix rows out of range for a TMA map");
+  VLO_CHECK(page_stride_rows > 0 && page_stride_rows < (1ll << 31) && head_stride_rows >= 0 && head_stride_rows < (1ll << 31),
+            "KV page strides out of range");
   CUtensorMap tk, tv;
   if (tmap_2d_sw128(d_k, static_cast<int>(kv_rows), kAttnHD, kAttnBlk, 1, &tk) != 0) return -1;
   if (tmap_2d_sw128(d_v, static_cast<int>(kv_rows), kAttnHD, kAttnBlk, 1, &tv) != 0) return -1;
-  if (ensure_max_smem(reinterpret_cast<const void*>(attn_kvappend_kernel), kAttnSmemBytes)) return -1;
+  if (ensure_max_smem(reinterpret_cast<const void*>(attn_kvappend_kernel), kAttnSmemOptIn)) return -1;
   const float scale_log2 = static_cast<float>(1.4426950408889634 / std::sqrt(static_cast<double>(head_dim)));
   AttnParams p{};
   p.q = static_cast<const __nv_bfloat16*>(d_q);
   p.ws_o = plan.ws_o;
   p.ws_ml = plan.ws_ml;
   p.items = static_cast<const AttnItem*>(plan.d_items);
+  p.page_table = d_page_table;
+  p.page_stride_rows = static_cast<int>(page_stride_rows);
+  p.head_stride_rows = static_cast<int>(head_stride_rows);
   p.n_heads = n_heads;
   p.n_kv_heads = n_kv_heads;
   p.scale_log2 = scale_log2;
   prof_begin(PROF_ATTN, stream, plan.algo_bytes);
   VLO_CUDA(launch_pdl(attn_kvappend_kernel, dim3(plan.max_splits, n_kv_heads, plan.n_items), dim3(kAttnThreads),
-                      kAttnSmemBytes, stream, tk, tv, p));
+                      attn_smem_bytes(plan.max_blocks_per_split), stream, tk, tv, p));
   prof_end(stream);
   count_launch();
   if (plan.skip_merge) return 0;

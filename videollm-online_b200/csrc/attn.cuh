@@ -22,14 +22,23 @@ constexpr int kAttnGroups = 2;     // warp groups per CTA, alternate key blocks
 constexpr int kAttnThreads = 32 * (1 + 4 * kAttnGroups);  // 1 producer warp + 8 MMA warps
 constexpr int kAttnSubTile = kAttnBlk * 128;               // 64 keys x 64 dims x 2 B = 8 KB
 constexpr int kAttnStageBytes = 4 * kAttnSubTile;          // K(2 halves) + V(2 halves) = 32 KB
-constexpr int kAttnSmemBytes = kAttnGroups * kAttnStages * kAttnStageBytes + 1024 + 256;
+constexpr int kAttnSmemBase = kAttnGroups * kAttnStages * kAttnStageBytes + 1024 + 256;  // ring + alignment + barriers
+constexpr int kAttnSmemOptIn = 232448;  // 227 KB: the per-block dynamic shared memory limit of sm_90
+// All of a split's page-table entries (4 B each) are staged in shared memory behind the barriers before the grid
+// dependency resolves, so the TMA producer issues every key block without a global load.  A launch sizes that area for
+// the plan's longest split (attn_smem_bytes); the opt-in limit leaves room for kAttnPtMax entries (552 960 keys).
+constexpr int kAttnPtMax = (kAttnSmemOptIn - kAttnSmemBase) / 4;
+inline int attn_smem_bytes(int max_blocks_per_split) { return kAttnSmemBase + 4 * max_blocks_per_split; }
 
+// Key block b (64 keys) of kv head h of an item lives at row page_table[pt0 + b] * page_stride_rows + h * head_stride_rows
+// of the K / V maps (rows in units of head_dim elements).  The engine's page pool has page_stride_rows = n_kv_heads * 64
+// and head_stride_rows = 64; a contiguous [n_kv_heads][stride][128] cache is an identity table with page_stride_rows = 64
+// and head_stride_rows = stride.
 struct AttnItem {
   int q_tok0;          // first token of this chunk in the packed q / out arrays
   int q_count;         // tokens in the chunk; q_count * G <= 64
   int q_pos0;          // absolute position of the chunk's first token (= #keys strictly before it)
-  int kv_row0;         // row (in units of head_dim elements) of key 0 of kv head 0 in the K / V maps
-  int kv_head_stride;  // rows between consecutive kv heads
+  int pt0;             // page-table entry of the sequence's key block 0
   int n_splits;        // splits that own at least one key block
   int blocks_per_split;
   int ws_slot0;        // first workspace row-slot of this item
@@ -40,6 +49,8 @@ struct AttnParams {
   float* ws_o;             // [slots, 128] un-normalised partial outputs
   float* ws_ml;            // [slots, 2]   (row max in raw-score units, row sum)
   const AttnItem* items;
+  const int* page_table;   // page of each 64-key block, per sequence from AttnItem::pt0
+  int page_stride_rows, head_stride_rows;
   int n_heads, n_kv_heads;
   float scale_log2;        // head_dim^-0.5 * log2(e)
 };
@@ -49,7 +60,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
                      const AttnParams p) {
   pdl_trigger();
-  pdl_wait();   // the freshly appended K/V rows and Q come from predecessors
+  // The item table and the page tables were uploaded by the memcpy at the start of the step: they (and this split's
+  // page entries, below) are read before the grid dependency resolves.
   const AttnItem it = p.items[blockIdx.z];
   const int split = blockIdx.x;
   if (split >= it.n_splits) return;
@@ -68,8 +80,10 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kAttnGroups * kAttnStages * kAttnStageBytes);
   uint64_t* empty_bar = full_bar + kAttnGroups * kAttnStages;
+  int* s_pt = reinterpret_cast<int*>(smem + kAttnGroups * kAttnStages * kAttnStageBytes + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int j = threadIdx.x; j < nblk; j += kAttnThreads) s_pt[j] = p.page_table[it.pt0 + blk0 + j];
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
@@ -79,9 +93,10 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
     }
     fence_mbar_init();
   }
+  pdl_wait();   // the freshly appended K/V rows and Q come from predecessors
   __syncthreads();
 
-  const int kv_row_base = it.kv_row0 + kvh * it.kv_head_stride;
+  const int head_row = kvh * p.head_stride_rows;
 
   // MMA-warp state (also declared for the producer warp; unused there)
   float o_acc[16][4];
@@ -107,7 +122,7 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
         mbar_wait(&empty_bar[g * kAttnStages + s], ph ^ 1);
         mbar_arrive_expect_tx(fb, kAttnStageBytes);
         uint8_t* st = smem + (g * kAttnStages + s) * kAttnStageBytes;
-        const int row = kv_row_base + (blk0 + b) * kAttnBlk;
+        const int row = s_pt[b] * p.page_stride_rows + head_row;
         tma_load_2d(st, &tm_k, fb, 0, row, kEvictFirst);
         tma_load_2d(st + kAttnSubTile, &tm_k, fb, 64, row, kEvictFirst);
         tma_load_2d(st + 2 * kAttnSubTile, &tm_v, fb, 0, row, kEvictFirst);

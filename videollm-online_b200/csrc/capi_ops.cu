@@ -3,6 +3,7 @@
 
 #include "common.h"
 #include "gemm.cuh"
+#include "kv_pages.h"
 
 using namespace vlo;
 
@@ -85,33 +86,77 @@ int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, in
   return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
 }
 
+}  // extern "C"
+
+namespace {
+
+size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+
+// Plan one sequence of n_tok queries over kv_len keys and upload the plan into d_ws.  h_identity_pt: also upload an
+// identity page table (the contiguous [n_kv_heads][kv_stride][128] layout, one "page" per 64-key block) behind the
+// plan's workspace and return its device address in *d_pt.  The upload is synchronised: the staging is pageable.
+int op_attn_plan(AttnPlan* plan, float* d_ws, int n_tok, int n_heads, int n_kv_heads, int head_dim, int kv_len,
+                 bool identity_pt, const int** d_pt, cudaStream_t st) {
+  VLO_CHECK(n_tok > 0 && kv_len >= n_tok, "attn: need 0 < n_tok <= kv_len");
+  AttnSeq s{};
+  s.q_tok0 = 0;
+  s.q_len = n_tok;
+  s.kv_len = kv_len;
+  s.pt0 = 0;
+  const size_t plan_stage = attn_stage_bytes(n_tok, 1, n_heads, n_kv_heads);
+  const int nblk = kv_pages_for(kv_len);
+  static thread_local std::vector<uint8_t> stage;
+  stage.resize(plan_stage + sizeof(int) * nblk);
+  if (attn_plan(plan, d_ws, stage.data(), &s, 1, n_tok, n_heads, n_kv_heads, head_dim, st)) return -1;
+  if (identity_pt) {
+    int* h_pt = reinterpret_cast<int*>(stage.data() + plan_stage);
+    for (int b = 0; b < nblk; ++b) h_pt[b] = b;
+    int* pt = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(d_ws) + attn_ws_bytes(n_tok, 1, n_heads, n_kv_heads));
+    VLO_CUDA(cudaMemcpyAsync(pt, h_pt, sizeof(int) * nblk, cudaMemcpyHostToDevice, st));
+    *d_pt = pt;
+  }
+  VLO_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len) {
   (void)head_dim;
-  (void)kv_len;
-  // n_kv_heads is not part of this query: bound it by n_heads (G = 1 is the worst case)
-  return 2 * static_cast<int64_t>(attn_ws_bytes(n_tok, 1, n_heads, n_heads));
+  // n_kv_heads is not part of this query: bound it by n_heads (G = 1 is the worst case); the identity page table of
+  // the contiguous layout follows the plan's workspace
+  return 2 * static_cast<int64_t>(attn_ws_bytes(n_tok, 1, n_heads, n_heads)) +
+         static_cast<int64_t>(align256(sizeof(int) * kv_pages_for(kv_len)));
 }
 
 int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void* d_out, float* d_ws, int n_tok,
                          int n_heads, int n_kv_heads, int head_dim, int kv_len, long long kv_stride,
                          void* cuda_stream) {
-  AttnSeq s{};
-  s.q_tok0 = 0;
-  s.q_len = n_tok;
-  s.kv_len = kv_len;
-  s.kv_row0 = 0;
-  s.kv_head_stride = static_cast<int>(kv_stride);
-  // the staging copy must outlive the async H2D: keep it in a per-thread buffer and sync the copy
-  static thread_local std::vector<uint8_t> stage;
-  stage.resize(attn_stage_bytes(n_tok, 1, n_heads, n_kv_heads));
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   AttnPlan plan{};
-  int rc = attn_plan(&plan, d_ws, stage.data(), &s, 1, n_tok, n_heads, n_kv_heads, head_dim, st);
-  if (rc != 0) return rc;
-  rc = attn_run(plan, d_q, d_k, d_v, static_cast<long long>(n_kv_heads) * kv_stride, d_out, n_heads, n_kv_heads,
-                head_dim, st);
-  if (rc != 0) return rc;
-  VLO_CUDA(cudaStreamSynchronize(st));  // pageable staging buffer: make the copies complete before returning
+  const int* pt = nullptr;
+  if (op_attn_plan(&plan, d_ws, n_tok, n_heads, n_kv_heads, head_dim, kv_len, true, &pt, st)) return -1;
+  if (attn_run(plan, d_q, d_k, d_v, static_cast<long long>(n_kv_heads) * kv_stride, pt, kKvPageTokens, kv_stride, d_out,
+               n_heads, n_kv_heads, head_dim, st))
+    return -1;
+  VLO_CUDA(cudaStreamSynchronize(st));  // the plan lives in a per-thread buffer: finish before it can be reused
+  return 0;
+}
+
+int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
+                               int n_pages, void* d_out, float* d_ws, int n_tok, int n_heads, int n_kv_heads,
+                               int head_dim, int kv_len, void* cuda_stream) {
+  VLO_CHECK(n_pages > 0 && n_kv_heads > 0, "attn_paged: sizes");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  AttnPlan plan{};
+  if (op_attn_plan(&plan, d_ws, n_tok, n_heads, n_kv_heads, head_dim, kv_len, false, nullptr, st)) return -1;
+  const long long page_rows = static_cast<long long>(n_kv_heads) * kKvPageTokens;
+  if (attn_run(plan, d_q, d_k_pool, d_v_pool, n_pages * page_rows, d_page_table, page_rows, kKvPageTokens, d_out, n_heads,
+               n_kv_heads, head_dim, st))
+    return -1;
+  VLO_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -122,25 +167,18 @@ int vlo_op_attn_bench(const void* d_q, const void* d_k, const void* d_v, void* d
                       int n_kv_heads, int head_dim, int kv_len, long long kv_stride, int n_layers,
                       long long layer_stride_rows, int iters, int skip_merge, double* h_algo_bytes, void* cuda_stream) {
   VLO_CHECK(n_layers > 0 && iters > 0 && layer_stride_rows >= static_cast<long long>(n_kv_heads) * kv_stride, "attn_bench: sizes");
-  AttnSeq s{};
-  s.q_tok0 = 0;
-  s.q_len = n_tok;
-  s.kv_len = kv_len;
-  s.kv_row0 = 0;
-  s.kv_head_stride = static_cast<int>(kv_stride);
-  static thread_local std::vector<uint8_t> stage;
-  stage.resize(attn_stage_bytes(n_tok, 1, n_heads, n_kv_heads));
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   AttnPlan plan{};
-  if (attn_plan(&plan, d_ws, stage.data(), &s, 1, n_tok, n_heads, n_kv_heads, head_dim, st)) return -1;
-  VLO_CUDA(cudaStreamSynchronize(st));
+  const int* pt = nullptr;
+  if (op_attn_plan(&plan, d_ws, n_tok, n_heads, n_kv_heads, head_dim, kv_len, true, &pt, st)) return -1;
   plan.skip_merge = skip_merge;
   if (h_algo_bytes) *h_algo_bytes = plan.algo_bytes;
   const size_t lstride = static_cast<size_t>(layer_stride_rows) * head_dim * 2;
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < n_layers; ++l)
       if (attn_run(plan, d_q, static_cast<const uint8_t*>(d_k) + l * lstride, static_cast<const uint8_t*>(d_v) + l * lstride,
-                   static_cast<long long>(n_kv_heads) * kv_stride, d_out, n_heads, n_kv_heads, head_dim, st))
+                   static_cast<long long>(n_kv_heads) * kv_stride, pt, kKvPageTokens, kv_stride, d_out, n_heads,
+                   n_kv_heads, head_dim, st))
         return -1;
   return 0;
 }

@@ -134,8 +134,7 @@ struct AttnSeq {
   int q_tok0;          // first packed token of the sequence
   int q_len;           // new tokens
   int kv_len;          // cache length INCLUDING the new tokens
-  long long kv_row0;   // row of (key 0, kv head 0) in the K / V matrices ([rows, head_dim])
-  int kv_head_stride;  // rows between kv heads
+  int pt0;             // entry of the page table holding the page of key block 0 (ceil(kv_len / 64) entries follow)
 };
 // bytes of scratch attn_launch needs for these sequences (upper bound)
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads);
@@ -146,6 +145,7 @@ struct AttnPlan {
   void* d_items;
   int* d_tok_item;
   int n_items, max_splits, total_tokens;
+  int max_blocks_per_split;  // sizes the page-table staging of the launch
   int blk;            // keys per pipeline block
   int skip_merge;     // measurement only: launch the main kernel without the split-KV merge
   double algo_bytes;  // algorithmic HBM bytes of one attn_run over this plan (K+V rows read, Q read, out written)
@@ -154,9 +154,14 @@ struct AttnPlan {
 // must stay untouched until the copies enqueued on `stream` have run.
 int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, int n_seqs, int total_tokens,
               int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream);
-// d_k / d_v: one layer's K / V matrices [kv_rows, 128] bf16; d_q [T, n_heads, 128]; d_out [T, n_heads*128].
-int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows, void* d_out,
-             int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream);
+// d_k / d_v: one layer's K / V matrices [kv_rows, 128] bf16; key block b of kv head h of a sequence sits at row
+// d_page_table[pt0 + b] * page_stride_rows + h * head_stride_rows (attn.cuh); d_q [T, n_heads, 128]; d_out [T, n_heads*128].
+int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void* d_v, long long kv_rows,
+             const int* d_page_table, long long page_stride_rows, long long head_stride_rows, void* d_out, int n_heads,
+             int n_kv_heads, int head_dim, cudaStream_t stream);
+
+// longest sequence, in 64-key blocks, whose page table one attention CTA can stage (any plan of it then succeeds)
+int attn_max_key_blocks();
 
 // 2D TMA map over a row-major 16-bit matrix [rows, k], box 64 x box_rows, 128-byte swizzle (cached).
 int tmap_2d_sw128(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out);

@@ -123,8 +123,8 @@ struct QkvRopeParams {
   const __nv_bfloat16* cos_tab;
   const __nv_bfloat16* sin_tab;
   const int* tok_pos;      // [T] absolute position of the token in its stream
-  const long long* tok_kvrow;  // [T] cache row of (key 0, kv head 0) of the token's stream
-  int kv_head_stride;      // rows between kv heads
+  const long long* tok_kvrow;  // [T] cache row of (the token's position, kv head 0): its page's row + pos % 64
+  int kv_head_stride;      // rows between kv heads (64 in the page pool)
   __nv_bfloat16* q_out;    // [T, nh, 128]
   __nv_bfloat16* k_cache;  // layer base, rows of 128
   __nv_bfloat16* v_cache;
@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(64) qkv_rope_append_kernel(const QkvRopeParams
   } else {
     const int kvh = (hh - p.n_heads) % p.n_kv_heads;
     __nv_bfloat16* base = (hh < p.n_heads + p.n_kv_heads) ? p.k_cache : p.v_cache;
-    dst = base + (kvrow + static_cast<long long>(kvh) * p.kv_head_stride + pos) * 128;
+    dst = base + (kvrow + static_cast<long long>(kvh) * p.kv_head_stride) * 128;
   }
   dst[d] = __float2bfloat16_rn(x1);
   dst[d + 64] = __float2bfloat16_rn(x2);
@@ -364,17 +364,51 @@ __global__ void __launch_bounds__(1024) decision_kernel(const __nv_bfloat16* log
   }
 }
 
-// KV synthetic fill (bench pre-fill): deterministic finite pseudo-random bf16 in about [-1, 1].
-__global__ void kv_fill_kernel(__nv_bfloat16* base, long long row0, int n_rows, unsigned long long seed) {
-  const long long n = static_cast<long long>(n_rows) * 128;
+// ---------------------------------------------------------------------------------------------
+// KV page-pool copies and fill.  One layer's K or V matrix is a plane of [page][kv_head][64][128] rows (kv_pages.h);
+// planes follow each other at plane_stride elements.  A paged side is addressed through its page table, a
+// contiguous side is [n_kv_heads][ld][128].
+struct KvSide {
+  __nv_bfloat16* base;
+  const int* pt;  // page table, or null: contiguous
+  long long plane_stride;
+  int ld;         // contiguous rows per kv head
+};
+__device__ __forceinline__ long long kv_side_row(const KvSide& s, int n_kv, int h, int pos) {
+  return s.pt ? (static_cast<long long>(s.pt[pos >> 6]) * n_kv + h) * 64 + (pos & 63)
+              : static_cast<long long>(h) * s.ld + pos;
+}
+
+// rows [0, n_tok) of every kv head and plane: src -> dst, 16 bytes per thread.
+// grid = (ceil(n_tok * 16 / 256), n_kv_heads, planes), block = 256.
+__global__ void __launch_bounds__(256) kv_copy_kernel(const KvSide src, const KvSide dst, int n_kv, int n_tok) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(n_tok) * 16) return;
+  const int pos = static_cast<int>(i >> 4), c = static_cast<int>(i & 15), h = blockIdx.y, pl = blockIdx.z;
+  const uint4* s = reinterpret_cast<const uint4*>(src.base + pl * src.plane_stride + kv_side_row(src, n_kv, h, pos) * 128);
+  uint4* d = reinterpret_cast<uint4*>(dst.base + pl * dst.plane_stride + kv_side_row(dst, n_kv, h, pos) * 128);
+  d[c] = s[c];
+}
+
+// KV synthetic fill (bench pre-fill): deterministic finite pseudo-random bf16 in about [-1, 1].  The value of element
+// d of (position pos, kv head h) of plane pl = 2 layer + is_v hashes the LOGICAL index
+// ((sid * n_kv + h) * max_kv_tokens + pos) * 128 + d with seed + pl * 1315423911 + h * 2654435761, wherever its page is.
+// grid = (x, n_kv_heads, planes), block = 256.
+__global__ void __launch_bounds__(256) kv_fill_kernel(const KvSide dst, int n_kv, int n_tok, int sid, int max_kv_tokens,
+                                                      unsigned long long seed) {
+  const int h = blockIdx.y, pl = blockIdx.z;
+  const unsigned long long sd = seed + static_cast<unsigned long long>(pl) * 1315423911ull + h * 2654435761ull;
+  const long long row0 = (static_cast<long long>(sid) * n_kv + h) * max_kv_tokens;
+  const long long n = static_cast<long long>(n_tok) * 128;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * static_cast<unsigned long long>(row0 * 128 + i + 1);
+    unsigned long long z = sd + 0x9E3779B97F4A7C15ull * static_cast<unsigned long long>(row0 * 128 + i + 1);
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
     z ^= z >> 31;
     const float u = static_cast<float>(z >> 40) * (1.0f / 16777216.0f);  // [0,1)
-    base[row0 * 128 + i] = __float2bfloat16_rn(2.f * u - 1.f);
+    const int pos = static_cast<int>(i >> 7);
+    dst.base[pl * dst.plane_stride + kv_side_row(dst, n_kv, h, pos) * 128 + (i & 127)] = __float2bfloat16_rn(2.f * u - 1.f);
   }
 }
 

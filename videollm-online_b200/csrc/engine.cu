@@ -11,6 +11,7 @@
 #include "decoder_kernels.cuh"
 #include "gemm.cuh"
 #include "gemm_wsf.cuh"
+#include "kv_pages.h"
 #include "vit_kernels.cuh"
 #include "vlo_b200.h"
 
@@ -59,7 +60,9 @@ struct vlo_engine {
   // device allocations owned by the engine
   std::vector<void*> allocs;
   int64_t device_bytes = 0;
-  bf16* kv = nullptr;  // [layer][2][stream][kv_head][cap][128]
+  bf16* kv = nullptr;  // [layer][2][page][kv_head][64][128], pages owned through `pool`
+  KvPool pool;
+  int* kv_op_pt = nullptr;  // device page tables of the KV copy / fill calls (two streams' worth)
   std::vector<int> kv_len;
   std::vector<char> stream_open;
 
@@ -70,7 +73,7 @@ struct vlo_engine {
   size_t part_elems = 0;
   int* sk_flags = nullptr;          // stream-K arrival counters of the fused gate|up GEMM (zero between launches)
   uint8_t* attn_ws = nullptr;
-  uint8_t* meta_dev = nullptr;  // tok_pos | tok_kvrow | last_index | first_rows
+  uint8_t* meta_dev = nullptr;  // tok_pos | last_index | first_rows | tok_kvrow | page tables of the step's streams
   size_t meta_bytes = 0;
   DecisionOut* decisions = nullptr;
   // host staging ring (pinned)
@@ -223,13 +226,36 @@ int stage_release(vlo_engine* e, int slot, cudaStream_t st) {
   return 0;
 }
 
-inline bf16* kv_layer_base(vlo_engine* e, int layer, int is_v) {
-  const vlo_config& c = e->cfg;
-  const size_t rows = static_cast<size_t>(c.max_streams) * c.num_kv_heads * c.max_kv_tokens;
-  return e->kv + (static_cast<size_t>(layer) * 2 + is_v) * rows * c.head_dim;
+// step metadata: the page tables follow tok_pos | last_index | first_rows | tok_kvrow
+inline size_t meta_pt_offset(const vlo_config& c) {
+  return align256(sizeof(int) * c.max_step_tokens) * 3 + align256(sizeof(long long) * c.max_step_tokens);
 }
-inline long long kv_rows_per_layer(const vlo_config& c) {
-  return static_cast<long long>(c.max_streams) * c.num_kv_heads * c.max_kv_tokens;
+
+// elements of one layer's K or V matrix
+inline size_t kv_plane_elems(const vlo_engine* e) { return static_cast<size_t>(e->pool.rows_per_layer()) * e->cfg.head_dim; }
+inline bf16* kv_layer_base(vlo_engine* e, int layer, int is_v) {
+  return e->kv + (static_cast<size_t>(layer) * 2 + is_v) * kv_plane_elems(e);
+}
+// the paged side of a KV copy / fill: table of stream `sid` uploaded to d_pt
+inline KvSide kv_paged_side(vlo_engine* e, bf16* plane0, const int* d_pt) {
+  return KvSide{plane0, d_pt, static_cast<long long>(kv_plane_elems(e)), 0};
+}
+
+// Upload the page tables of up to two streams (first n_pages[i] entries each) to e->kv_op_pt through a staging slot.
+int upload_op_tables(vlo_engine* e, int n, const int* sids, const int* n_pages, const int** d_pt, cudaStream_t st) {
+  uint8_t* hs;
+  int slot;
+  if (stage_acquire(e, &hs, &slot)) return -1;
+  int* h = reinterpret_cast<int*>(hs);
+  const int per = kv_pages_for(e->cfg.max_kv_tokens);
+  size_t used = 0;
+  for (int i = 0; i < n; ++i) {
+    std::memcpy(h + static_cast<size_t>(i) * per, e->pool.tables[sids[i]].data(), sizeof(int) * n_pages[i]);
+    d_pt[i] = e->kv_op_pt + static_cast<size_t>(i) * per;
+    used = static_cast<size_t>(i) * per + n_pages[i];
+  }
+  VLO_CUDA(cudaMemcpyAsync(e->kv_op_pt, h, sizeof(int) * used, cudaMemcpyHostToDevice, st));
+  return stage_release(e, slot, st);
 }
 
 // Every entry point that touches the device runs on the engine's GPU whatever the caller's current device is
@@ -256,9 +282,13 @@ int check_stream(vlo_engine* e, int sid) {
 
 extern "C" {
 
-static int engine_init(vlo_engine* e);
+static int engine_init(vlo_engine* e, int64_t kv_pool_tokens);
 
 int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out) {
+  return vlo_engine_create_pooled(cfg, 0, device, out);
+}
+
+int vlo_engine_create_pooled(const vlo_config* cfg, int64_t kv_pool_tokens, int device, vlo_engine** out) {
   VLO_CHECK(cfg != nullptr && out != nullptr, "null argument");
   *out = nullptr;
   int prev_dev = -1;
@@ -271,6 +301,9 @@ int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out) {
   VLO_CHECK(c.hidden_size % 128 == 0 && c.intermediate_size % 128 == 0, "hidden/intermediate must be multiples of 128");
   VLO_CHECK(c.num_heads % c.num_kv_heads == 0, "num_heads % num_kv_heads");
   VLO_CHECK(c.max_streams >= 1 && c.max_kv_tokens >= 64 && c.max_step_tokens >= 1, "capacities");
+  VLO_CHECK(kv_pages_for(c.max_kv_tokens) <= attn_max_key_blocks(),
+            "max_kv_tokens above " + std::to_string(attn_max_key_blocks() * kKvPageTokens) +
+                " (the attention stages a stream's page table in shared memory)");
   VLO_CHECK(c.max_step_tokens <= 128, "max_step_tokens <= 128 (longer inputs are chunked by the host; chunked == one pass)");
   VLO_CHECK(c.vit_layers == 0 || (c.vit_hidden % 128 == 0 && c.vit_hidden / c.vit_heads == 64 && c.vit_mlp % 64 == 0),
             "vision tower: hidden % 64, head_dim == 64");
@@ -287,7 +320,7 @@ int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out) {
   e->n_frame_tokens = (c.frame_token_cls ? 1 : 0) + c.pool_h * c.pool_w;
   e->kv_len.assign(c.max_streams, 0);
   e->stream_open.assign(c.max_streams, 0);
-  const int rc = engine_init(e);
+  const int rc = engine_init(e, kv_pool_tokens);
   if (rc != 0) {   // no half-built engine escapes: free what was allocated, keep the error text
     const std::string msg = last_error();
     vlo_engine_destroy(e);
@@ -299,13 +332,20 @@ int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out) {
   return rc;
 }
 
-static int engine_init(vlo_engine* e) {
+static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   const vlo_config& c = e->cfg;
   const int T = c.max_step_tokens;
   const int H = c.hidden_size;
-  // KV cache, zero-initialised once: attention may touch (masked) rows past kv_len, they must be finite.
-  const size_t kv_elems = static_cast<size_t>(c.num_layers) * 2 * kv_rows_per_layer(c) * c.head_dim;
+  // KV cache: a pool of 64-token pages shared by all streams, zero-initialised once.  Attention reads (masked) rows
+  // past kv_len inside a stream's last page; they must be finite.
+  const int per_stream = kv_pages_for(c.max_kv_tokens);
+  const int64_t pages = kv_pool_tokens > 0 ? (kv_pool_tokens + kKvPageTokens - 1) / kKvPageTokens
+                                           : static_cast<int64_t>(c.max_streams) * per_stream;
+  VLO_CHECK(pages * c.num_kv_heads * kKvPageTokens < (1ll << 31), "KV pool too large for one TMA map per layer");
+  e->pool.init(c.max_streams, c.num_kv_heads, static_cast<int>(pages));
+  const size_t kv_elems = static_cast<size_t>(c.num_layers) * 2 * e->pool.rows_per_layer() * c.head_dim;
   if (dev_alloc_t(e, &e->kv, kv_elems, true)) return -1;
+  if (dev_alloc_t(e, &e->kv_op_pt, static_cast<size_t>(2) * per_stream)) return -1;
   if (dev_alloc_t(e, &e->h, static_cast<size_t>(T) * H)) return -1;
   if (dev_alloc_t(e, &e->xn, static_cast<size_t>(T) * H)) return -1;
   if (dev_alloc_t(e, &e->xn_last, static_cast<size_t>(c.max_streams) * H)) return -1;
@@ -320,7 +360,7 @@ static int engine_init(vlo_engine* e) {
   if (dev_alloc_t(e, &e->sk_flags, 4096, true)) return -1;
   const size_t aws = attn_ws_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads);
   if (dev_alloc(e, reinterpret_cast<void**>(&e->attn_ws), aws, false)) return -1;
-  e->meta_bytes = align256(sizeof(int) * T) * 3 + align256(sizeof(long long) * T);
+  e->meta_bytes = meta_pt_offset(c) + align256(sizeof(int) * std::max(2, c.max_streams) * per_stream);
   if (dev_alloc(e, reinterpret_cast<void**>(&e->meta_dev), e->meta_bytes, false)) return -1;
   e->stage_slot_bytes = align256(e->meta_bytes + attn_stage_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads));
   VLO_CUDA(cudaMallocHost(reinterpret_cast<void**>(&e->stage), e->stage_slot_bytes * kStageSlots));
@@ -457,13 +497,22 @@ int vlo_stream_open(vlo_engine* e, int* stream_id) {
 }
 int vlo_stream_reset(vlo_engine* e, int sid) {
   if (check_stream(e, sid)) return -1;
+  e->pool.resize(sid, 0);
   e->kv_len[sid] = 0;
   return 0;
 }
 int vlo_stream_close(vlo_engine* e, int sid) {
   if (check_stream(e, sid)) return -1;
+  e->pool.resize(sid, 0);
   e->stream_open[sid] = 0;
   e->kv_len[sid] = 0;
+  return 0;
+}
+int vlo_kv_pool_info(vlo_engine* e, int* page_tokens, int64_t* total_pages, int64_t* free_pages) {
+  VLO_CHECK(e != nullptr, "null engine");
+  if (page_tokens) *page_tokens = kKvPageTokens;
+  if (total_pages) *total_pages = e->pool.n_pages;
+  if (free_pages) *free_pages = e->pool.free_pages();
   return 0;
 }
 int vlo_kv_len(vlo_engine* e, int sid, int* out_len) {
@@ -474,6 +523,7 @@ int vlo_kv_len(vlo_engine* e, int sid, int* out_len) {
 int vlo_kv_truncate(vlo_engine* e, int sid, int new_len) {
   if (check_stream(e, sid)) return -1;
   VLO_CHECK(new_len >= 0 && new_len <= e->kv_len[sid], "kv_truncate: new_len must be within [0, kv_len]");
+  e->pool.resize(sid, new_len);
   e->kv_len[sid] = new_len;
   return 0;
 }
@@ -482,32 +532,41 @@ int vlo_kv_fill_synthetic(vlo_engine* e, int sid, int n_tokens, uint64_t seed, v
   if (check_stream(e, sid)) return -1;
   const vlo_config& c = e->cfg;
   VLO_CHECK(n_tokens >= 0 && n_tokens <= c.max_kv_tokens, "kv_fill: n_tokens out of range");
-  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  for (int l = 0; l < c.num_layers; ++l)
-    for (int v = 0; v < 2; ++v)
-      for (int hd = 0; hd < c.num_kv_heads; ++hd) {
-        const long long row0 = (static_cast<long long>(sid) * c.num_kv_heads + hd) * c.max_kv_tokens;
-        if (n_tokens > 0) {
-          kv_fill_kernel<<<std::min(1024, (n_tokens * 128 + 255) / 256), 256, 0, st>>>(
-              kv_layer_base(e, l, v), row0, n_tokens, seed + (static_cast<uint64_t>(l) * 2 + v) * 1315423911ull + hd * 2654435761ull);
-        }
-      }
-  VLO_LAUNCH_CHECK();
+  if (e->pool.resize(sid, n_tokens)) return -1;
   e->kv_len[sid] = n_tokens;
+  if (n_tokens == 0) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const int n_pages = kv_pages_for(n_tokens);
+  const int* d_pt;
+  if (upload_op_tables(e, 1, &sid, &n_pages, &d_pt, st)) return -1;
+  kv_fill_kernel<<<dim3(std::min(64, (n_tokens * 128 + 255) / 256), c.num_kv_heads, 2 * c.num_layers), 256, 0, st>>>(
+      kv_paged_side(e, e->kv, d_pt), c.num_kv_heads, n_tokens, sid, c.max_kv_tokens, seed);
+  VLO_LAUNCH_CHECK();
   return 0;
 }
+
+namespace {
+int launch_kv_copy(const KvSide& src, const KvSide& dst, int n_kv, int n_tok, int planes, cudaStream_t st) {
+  kv_copy_kernel<<<dim3((n_tok * 16 + 255) / 256, n_kv, planes), 256, 0, st>>>(src, dst, n_kv, n_tok);
+  VLO_LAUNCH_CHECK();
+  return 0;
+}
+}  // namespace
+
 int vlo_kv_read(vlo_engine* e, int sid, int layer, int is_v, void* d_out, void* cuda_stream) {
   DevGuard dev_guard(e);
   if (check_stream(e, sid)) return -1;
   const vlo_config& c = e->cfg;
   VLO_CHECK(layer >= 0 && layer < c.num_layers, "layer out of range");
+  VLO_CHECK((reinterpret_cast<uintptr_t>(d_out) & 15) == 0, "kv_read: d_out must be 16-byte aligned");
   const int len = e->kv_len[sid];
   if (len == 0) return 0;
-  const bf16* src = kv_layer_base(e, layer, is_v) + static_cast<size_t>(sid) * c.num_kv_heads * c.max_kv_tokens * c.head_dim;
-  VLO_CUDA(cudaMemcpy2DAsync(d_out, static_cast<size_t>(len) * c.head_dim * 2, src,
-                             static_cast<size_t>(c.max_kv_tokens) * c.head_dim * 2, static_cast<size_t>(len) * c.head_dim * 2,
-                             c.num_kv_heads, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(cuda_stream)));
-  return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const int n_pages = kv_pages_for(len);
+  const int* d_pt;
+  if (upload_op_tables(e, 1, &sid, &n_pages, &d_pt, st)) return -1;
+  return launch_kv_copy(kv_paged_side(e, kv_layer_base(e, layer, is_v), d_pt), KvSide{static_cast<bf16*>(d_out), nullptr, 0, len},
+                        c.num_kv_heads, len, 1, st);
 }
 int vlo_kv_write(vlo_engine* e, int sid, int layer, int is_v, const void* d_in, int n_tokens, void* cuda_stream) {
   DevGuard dev_guard(e);
@@ -515,13 +574,15 @@ int vlo_kv_write(vlo_engine* e, int sid, int layer, int is_v, const void* d_in, 
   const vlo_config& c = e->cfg;
   VLO_CHECK(layer >= 0 && layer < c.num_layers, "layer out of range");
   VLO_CHECK(n_tokens > 0 && n_tokens <= c.max_kv_tokens, "kv_write: n_tokens out of range");
-  bf16* dst = kv_layer_base(e, layer, is_v) + static_cast<size_t>(sid) * c.num_kv_heads * c.max_kv_tokens * c.head_dim;
-  VLO_CUDA(cudaMemcpy2DAsync(dst, static_cast<size_t>(c.max_kv_tokens) * c.head_dim * 2, d_in,
-                             static_cast<size_t>(n_tokens) * c.head_dim * 2, static_cast<size_t>(n_tokens) * c.head_dim * 2,
-                             c.num_kv_heads, cudaMemcpyDeviceToDevice,
-                             static_cast<cudaStream_t>(cuda_stream)));
+  VLO_CHECK((reinterpret_cast<uintptr_t>(d_in) & 15) == 0, "kv_write: d_in must be 16-byte aligned");
+  if (e->pool.resize(sid, n_tokens)) return -1;
   e->kv_len[sid] = n_tokens;
-  return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const int n_pages = kv_pages_for(n_tokens);
+  const int* d_pt;
+  if (upload_op_tables(e, 1, &sid, &n_pages, &d_pt, st)) return -1;
+  return launch_kv_copy(KvSide{static_cast<bf16*>(const_cast<void*>(d_in)), nullptr, 0, n_tokens},
+                        kv_paged_side(e, kv_layer_base(e, layer, is_v), d_pt), c.num_kv_heads, n_tokens, 1, st);
 }
 
 int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, void* cuda_stream) {
@@ -530,19 +591,20 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, vo
   const vlo_config& c = e->cfg;
   VLO_CHECK(src_sid != dst_sid, "kv_copy_prefix: source and destination streams must differ");
   VLO_CHECK(n_tokens >= 0 && n_tokens <= e->kv_len[src_sid], "kv_copy_prefix: n_tokens exceeds the source length");
-  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const size_t per_stream = static_cast<size_t>(c.num_kv_heads) * c.max_kv_tokens * c.head_dim;
-  const size_t pitch = static_cast<size_t>(c.max_kv_tokens) * c.head_dim * sizeof(bf16);
-  if (n_tokens > 0)
-    for (int l = 0; l < c.num_layers; ++l)
-      for (int v = 0; v < 2; ++v) {
-        bf16* base = kv_layer_base(e, l, v);
-        VLO_CUDA(cudaMemcpy2DAsync(base + static_cast<size_t>(dst_sid) * per_stream, pitch, base + static_cast<size_t>(src_sid) * per_stream,
-                                   pitch, static_cast<size_t>(n_tokens) * c.head_dim * sizeof(bf16), c.num_kv_heads,
-                                   cudaMemcpyDeviceToDevice, st));
-      }
+  // the destination's pages are dropped and fresh ones taken: check first, so a short pool changes nothing
+  const int n_pages = kv_pages_for(n_tokens);
+  const int have = static_cast<int>(e->pool.tables[dst_sid].size());
+  if (n_pages > e->pool.free_pages() + have) return e->pool.resize(dst_sid, n_tokens);  // fails with the pool's message
+  e->pool.resize(dst_sid, 0);
+  e->pool.resize(dst_sid, n_tokens);
   e->kv_len[dst_sid] = n_tokens;
-  return 0;
+  if (n_tokens == 0) return 0;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const int sids[2] = {src_sid, dst_sid}, counts[2] = {n_pages, n_pages};
+  const int* d_pt[2];
+  if (upload_op_tables(e, 2, sids, counts, d_pt, st)) return -1;
+  return launch_kv_copy(kv_paged_side(e, e->kv, d_pt[0]), kv_paged_side(e, e->kv, d_pt[1]), c.num_kv_heads, n_tokens,
+                        2 * c.num_layers, st);
 }
 
 // ------------------------------------------------------------------------------ vision
@@ -790,35 +852,60 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     T += h_q_lens[i];
   }
   VLO_CHECK(T <= c.max_step_tokens, "step: total new tokens exceed max_step_tokens");
+  // ---- pages for the new tokens, taken before anything is enqueued; a short pool fails with no stream changed
+  {
+    int need = 0;
+    for (int i = 0; i < n_seqs; ++i) need += e->pool.missing(h_stream_ids[i], e->kv_len[h_stream_ids[i]] + h_q_lens[i]);
+    if (need > e->pool.free_pages())
+      return fail("step: KV page pool exhausted: the step needs " + std::to_string(need) + " more pages of " +
+                  std::to_string(kKvPageTokens) + " tokens, " + std::to_string(e->pool.free_pages()) + " of " +
+                  std::to_string(e->pool.n_pages) + " are free");
+    for (int i = 0; i < n_seqs; ++i) e->pool.resize(h_stream_ids[i], e->kv_len[h_stream_ids[i]] + h_q_lens[i]);
+  }
+  // a failure before the lengths are committed gives the pages back: every table stays ceil(kv_len / 64) long
+  struct PageRollback {
+    vlo_engine* e;
+    int n;
+    const int32_t* sids;
+    bool armed = true;
+    ~PageRollback() {
+      if (armed)
+        for (int i = 0; i < n; ++i) e->pool.resize(sids[i], e->kv_len[sids[i]]);
+    }
+  } rollback{e, n_seqs, h_stream_ids};
 
   // ---- per-step metadata: built on the host, one pinned slot, uploaded once, reused by all layers
   uint8_t* hs;
   int slot;
   if (stage_acquire(e, &hs, &slot)) return -1;
   const size_t o_pos = 0, o_last = align256(sizeof(int) * c.max_step_tokens), o_first = 2 * o_last,
-               o_row = 3 * o_last;
+               o_row = 3 * o_last, o_pt = meta_pt_offset(c);
   int* tok_pos = reinterpret_cast<int*>(hs + o_pos);
   int* last_index = reinterpret_cast<int*>(hs + o_last);
   int* first_rows = reinterpret_cast<int*>(hs + o_first);
   long long* tok_kvrow = reinterpret_cast<long long*>(hs + o_row);
+  int* page_tables = reinterpret_cast<int*>(hs + o_pt);  // ceil(kv_len / 64) entries per sequence, back to back
   std::vector<AttnSeq> seqs(n_seqs);
-  int t = 0;
+  int t = 0, n_pt = 0;
   for (int i = 0; i < n_seqs; ++i) {
     const int sid = h_stream_ids[i], ql = h_q_lens[i], past = e->kv_len[sid];
-    const long long row0 = static_cast<long long>(sid) * c.num_kv_heads * c.max_kv_tokens;
     first_rows[i] = t;
     for (int j = 0; j < ql; ++j) {
       tok_pos[t + j] = past + j;
-      tok_kvrow[t + j] = row0;
+      tok_kvrow[t + j] = e->pool.row(sid, past + j);
       last_index[t + j] = (j == ql - 1) ? i : -1;
     }
-    seqs[i] = AttnSeq{t, ql, past + ql, row0, c.max_kv_tokens};
+    seqs[i] = AttnSeq{t, ql, past + ql, n_pt};
+    const std::vector<int>& tab = e->pool.tables[sid];
+    std::memcpy(page_tables + n_pt, tab.data(), sizeof(int) * tab.size());
+    n_pt += static_cast<int>(tab.size());
     t += ql;
   }
-  VLO_CUDA(cudaMemcpyAsync(e->meta_dev, hs, e->meta_bytes, cudaMemcpyHostToDevice, st));
+  VLO_CUDA(cudaMemcpyAsync(e->meta_dev, hs, o_pt + sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
   const int* d_tok_pos = reinterpret_cast<const int*>(e->meta_dev + o_pos);
   const int* d_last_index = reinterpret_cast<const int*>(e->meta_dev + o_last);
   const long long* d_tok_kvrow = reinterpret_cast<const long long*>(e->meta_dev + o_row);
+  const int* d_page_tables = reinterpret_cast<const int*>(e->meta_dev + o_pt);
   AttnPlan plan{};
   if (attn_plan(&plan, e->attn_ws, hs + e->meta_bytes, seqs.data(), n_seqs, T, c.num_heads, c.num_kv_heads, c.head_dim, st))
     return -1;
@@ -868,7 +955,7 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     p.sin_tab = e->rope_sin;
     p.tok_pos = d_tok_pos;
     p.tok_kvrow = d_tok_kvrow;
-    p.kv_head_stride = c.max_kv_tokens;
+    p.kv_head_stride = KvPool::head_stride_rows();
     p.q_out = e->q;
     p.k_cache = kv_layer_base(e, l, 0);
     p.v_cache = kv_layer_base(e, l, 1);
@@ -876,8 +963,9 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     p.n_kv_heads = c.num_kv_heads;
     VLO_CUDA(launch_pdl(qkv_rope_append_kernel, dim3(T, c.num_heads + 2 * c.num_kv_heads), dim3(64), 0, st, p));
     count_launch();
-    if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), kv_rows_per_layer(c), e->attn_out,
-                 c.num_heads, c.num_kv_heads, c.head_dim, st))
+    if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), e->pool.rows_per_layer(), d_page_tables,
+                 e->pool.page_stride_rows(), KvPool::head_stride_rows(), e->attn_out, c.num_heads, c.num_kv_heads,
+                 c.head_dim, st))
       return -1;
     // ---- o_proj + residual, then post-attention RMSNorm
     if (gemm_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
@@ -898,6 +986,7 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   count_launch();
 
   for (int i = 0; i < n_seqs; ++i) e->kv_len[h_stream_ids[i]] += h_q_lens[i];
+  rollback.armed = false;
   e->last_step_tokens = T;
   return 0;
 }
@@ -924,12 +1013,23 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
     if (check_stream(e, h_stream_ids[i])) return -1;
     const int kv_len = e->kv_len[h_stream_ids[i]];
     VLO_CHECK(kv_len >= n_tok, "bench_attn: need kv_len >= n_tok");
-    seqs[i] = AttnSeq{i * n_tok, n_tok, kv_len, static_cast<long long>(h_stream_ids[i]) * c.num_kv_heads * c.max_kv_tokens,
-                      c.max_kv_tokens};
   }
+  // the streams' page tables go up in the same region and memcpy as a step's
   uint8_t* hs;
   int slot;
   if (stage_acquire(e, &hs, &slot)) return -1;
+  const size_t o_pt = meta_pt_offset(c);
+  int* page_tables = reinterpret_cast<int*>(hs + o_pt);
+  int n_pt = 0;
+  for (int i = 0; i < n_seqs; ++i) {
+    const int sid = h_stream_ids[i];
+    seqs[i] = AttnSeq{i * n_tok, n_tok, e->kv_len[sid], n_pt};
+    const std::vector<int>& tab = e->pool.tables[sid];
+    std::memcpy(page_tables + n_pt, tab.data(), sizeof(int) * tab.size());
+    n_pt += static_cast<int>(tab.size());
+  }
+  VLO_CUDA(cudaMemcpyAsync(e->meta_dev + o_pt, page_tables, sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
+  const int* d_page_tables = reinterpret_cast<const int*>(e->meta_dev + o_pt);
   AttnPlan plan{};
   if (attn_plan(&plan, e->attn_ws, hs + e->meta_bytes, seqs.data(), n_seqs, n_seqs * n_tok, c.num_heads, c.num_kv_heads,
                 c.head_dim, st))
@@ -939,8 +1039,9 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
   if (h_algo_bytes_per_launch) *h_algo_bytes_per_launch = plan.algo_bytes;
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < c.num_layers; ++l)
-      if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), kv_rows_per_layer(c), e->attn_out, c.num_heads,
-                   c.num_kv_heads, c.head_dim, st))
+      if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), e->pool.rows_per_layer(), d_page_tables,
+                   e->pool.page_stride_rows(), KvPool::head_stride_rows(), e->attn_out, c.num_heads, c.num_kv_heads,
+                   c.head_dim, st))
         return -1;
   return 0;
 }

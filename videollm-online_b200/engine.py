@@ -47,7 +47,11 @@ class Decision:
 
 class Engine:
     def __init__(self, cfg: LiveConfig, device: str | torch.device = "cuda:0", *, max_streams: int = 1,
-                 max_kv_tokens: int = 16384, max_step_tokens: int = 128, max_vit_batch: int = 8):
+                 max_kv_tokens: int = 16384, max_step_tokens: int = 128, max_vit_batch: int = 8,
+                 kv_pool_tokens: Optional[int] = None):
+        """kv_pool_tokens: size of the KV page pool all streams share (rounded up to 64-token pages); None reserves
+        max_streams * max_kv_tokens, so every stream can reach max_kv_tokens at once.  A smaller pool over-subscribes:
+        a step that needs more pages than are free raises VloError and leaves every stream as it was."""
         self.lib = _lib.load()
         self.cfg = cfg
         self.device = torch.device(device)
@@ -74,7 +78,8 @@ class Engine:
         self._lock = threading.Lock()
         self._weights: Dict[str, torch.Tensor] = {}
         with torch.cuda.device(self.index):
-            check(self.lib.vlo_engine_create(C.byref(c), self.index, C.byref(self._h)), "vlo_engine_create")
+            check(self.lib.vlo_engine_create_pooled(C.byref(c), int(kv_pool_tokens or 0), self.index, C.byref(self._h)),
+                  "vlo_engine_create_pooled")
         # device scratch for results (decisions, last logits)
         self._dec_dev = torch.zeros(max_streams, DECISION_DTYPE_FIELDS, dtype=torch.int32, device=self.device)
         self._dec_host = torch.zeros(max_streams, DECISION_DTYPE_FIELDS, dtype=torch.int32).pin_memory()
@@ -112,6 +117,12 @@ class Engine:
 
     def device_bytes(self) -> int:
         return int(self.lib.vlo_engine_device_bytes(self._h))
+
+    def kv_pool_info(self) -> Dict[str, int]:
+        """{"page_tokens", "total_pages", "free_pages"} of the shared KV page pool."""
+        pt, total, free = C.c_int(0), C.c_int64(0), C.c_int64(0)
+        check(self.lib.vlo_kv_pool_info(self._h, C.byref(pt), C.byref(total), C.byref(free)), "vlo_kv_pool_info")
+        return {"page_tokens": pt.value, "total_pages": total.value, "free_pages": free.value}
 
     # ------------------------------------------------------------------ streams
     def stream_open(self) -> int:
@@ -230,25 +241,33 @@ class Engine:
         dec_out = torch.empty(n, DECISION_DTYPE_FIELDS, dtype=torch.int32, device=self.device)
         off, done = 0, [0] * n
         starts = [int(sum(q_lens[:i])) for i in range(n)]
-        while any(done[i] < q_lens[i] for i in range(n)):
-            sub_ids, sub_lens, sub_rows, room = [], [], [], cap
-            for i in range(n):
-                left = q_lens[i] - done[i]
-                if left <= 0 or room <= 0:
-                    continue
-                take = min(left, room)
-                sub_ids.append(i)
-                sub_lens.append(take)
-                sub_rows.append(embeds[starts[i] + done[i]: starts[i] + done[i] + take])
-                room -= take
-            lg, dc = self.step([stream_ids[i] for i in sub_ids], sub_lens, torch.cat(sub_rows, 0), interval_id=interval_id,
-                               want_logits=want_logits)
-            for j, i in enumerate(sub_ids):
-                done[i] += sub_lens[j]
-                if done[i] == q_lens[i]:
-                    dec_out[i].copy_(dc[j])
-                    if want_logits:
-                        logits_out[i].copy_(lg[j])
+        kv0 = [self.kv_len(s) for s in stream_ids]
+        try:
+            while any(done[i] < q_lens[i] for i in range(n)):
+                sub_ids, sub_lens, sub_rows, room = [], [], [], cap
+                for i in range(n):
+                    left = q_lens[i] - done[i]
+                    if left <= 0 or room <= 0:
+                        continue
+                    take = min(left, room)
+                    sub_ids.append(i)
+                    sub_lens.append(take)
+                    sub_rows.append(embeds[starts[i] + done[i]: starts[i] + done[i] + take])
+                    room -= take
+                lg, dc = self.step([stream_ids[i] for i in sub_ids], sub_lens, torch.cat(sub_rows, 0),
+                                   interval_id=interval_id, want_logits=want_logits)
+                for j, i in enumerate(sub_ids):
+                    done[i] += sub_lens[j]
+                    if done[i] == q_lens[i]:
+                        dec_out[i].copy_(dc[j])
+                        if want_logits:
+                            logits_out[i].copy_(lg[j])
+        except VloError:
+            # a later piece failed (e.g. on an exhausted KV page pool): undo the earlier pieces, so the call changes
+            # no stream and the caller can retry it whole
+            for s, k in zip(stream_ids, kv0):
+                self.kv_truncate(s, k)
+            raise
         self._dec_dev[:n].copy_(dec_out)
         if want_logits:
             self._logits[:n].copy_(logits_out)

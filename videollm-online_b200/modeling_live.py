@@ -281,9 +281,10 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
                resume_from_checkpoint: str = "", set_vision_inside: bool = False, device: str = "cuda:0",
                synthetic_weights: bool = False, seed: int = 0, max_streams: int = 1, max_kv_tokens: int = 16384,
                max_step_tokens: int = 128, max_vit_batch: int = 8, llm_state=None, vision_state=None,
-               lora_r: int = 128, lora_alpha: int = 256, **kwargs):
+               lora_r: int = 128, lora_alpha: int = 256, kv_pool_tokens: Optional[int] = None, **kwargs):
     """models/modeling_live.py:184-222 for inference: build config + tokenizer, load (or synthesise)
-    weights, merge LoRA, hand everything to the engine."""
+    weights, merge LoRA, hand everything to the engine.  kv_pool_tokens: size of the KV page pool the streams
+    share (None or <= 0: max_streams * max_kv_tokens)."""
     if is_training:
         raise NotImplementedError("the vlo_b200 engine covers the streaming-inference path only")
     cfg = config or llama3_8b_siglip_l()
@@ -293,7 +294,7 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
             setattr(cfg, k, kwargs[k])
     tokenizer = build_live_tokenizer_and_update_config(llm_pretrained or "", cfg)
     engine = Engine(cfg, device, max_streams=max_streams, max_kv_tokens=max_kv_tokens,
-                    max_step_tokens=max_step_tokens, max_vit_batch=max_vit_batch)
+                    max_step_tokens=max_step_tokens, max_vit_batch=max_vit_batch, kv_pool_tokens=kv_pool_tokens)
     if llm_state is not None:
         packed = W.pack_llm_for_engine(cfg, llm_state, engine.device, max_kv_tokens)
         if set_vision_inside:
