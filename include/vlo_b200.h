@@ -173,7 +173,8 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
 int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, int rows_w, int k, void* d_out, int ld_out,
                 const float* d_bias, const float* d_pos, int pos_rows, int bn, void* cuda_stream);
 /* Persistent weight-streaming GEMM (csrc/gemm_ws.cuh): out[t, n] = sum_k X[t,k] W[n,k].  bn = token-tile width
- * (0: smallest of 16/32/64/128 covering rows_x, which must then be <= 128; 64/96/128/192 tile larger rows_x).
+ * (0: the smallest of 16/32/64/128 covering rows_x, with 96 too for bf16, and 128 above 128 rows; 64/96/128/192
+ * tile larger rows_x).
  * mode 0: stream-K over all SMs, fp32 partial planes out[plane][rows_x][rows_w] (the caller zero-fills d_out
  *         and sums the planes; *h_max_planes tells how many planes to provide); d_out == NULL only plans.
  * mode 1: whole tiles, 16-bit out[rows_x][ld_out] = act(acc + bias). */

@@ -18,9 +18,6 @@ namespace vlo {
 static_assert(kKvPageTokens == kAttnBlk, "KV page size must equal the attention key block");
 
 namespace {
-constexpr size_t kAlign = 256;
-size_t align_up(size_t x) { return (x + kAlign - 1) / kAlign * kAlign; }
-
 int max_chunks(int total_tokens, int n_seqs, int G) {
   const int per = std::max(1, 64 / G);
   return total_tokens / per + n_seqs + 1;
@@ -35,14 +32,14 @@ size_t cap_slots_for(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) 
 
 size_t attn_stage_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
   const int G = n_heads / n_kv_heads;
-  return align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens);
+  return align256(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align256(sizeof(int) * total_tokens);
 }
 
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
   const int G = n_heads / n_kv_heads;
   const size_t slots = cap_slots_for(total_tokens, n_seqs, n_heads, n_kv_heads);
-  return align_up(slots * kAttnHD * 4) + align_up(slots * 2 * 4) +
-         align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align_up(sizeof(int) * total_tokens);
+  return align256(slots * kAttnHD * 4) + align256(slots * 2 * 4) +
+         align256(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G)) + align256(sizeof(int) * total_tokens);
 }
 
 int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, int n_seqs, int total_tokens,
@@ -100,11 +97,11 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   // workspace carve-up (same order as attn_ws_bytes)
   uint8_t* w = static_cast<uint8_t*>(d_ws);
   plan->ws_o = reinterpret_cast<float*>(w);
-  w += align_up(cap_slots * kAttnHD * 4);
+  w += align256(cap_slots * kAttnHD * 4);
   plan->ws_ml = reinterpret_cast<float*>(w);
-  w += align_up(cap_slots * 2 * 4);
+  w += align256(cap_slots * 2 * 4);
   plan->d_items = w;
-  w += align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G));
+  w += align256(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G));
   plan->d_tok_item = reinterpret_cast<int*>(w);
   plan->n_items = n_items;
   plan->max_splits = max_splits;
@@ -113,7 +110,7 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
 
   uint8_t* hs = static_cast<uint8_t*>(h_stage);
   std::memcpy(hs, items.data(), sizeof(AttnItem) * n_items);
-  uint8_t* hs2 = hs + align_up(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G));
+  uint8_t* hs2 = hs + align256(sizeof(AttnItem) * max_chunks(total_tokens, n_seqs, G));
   std::memcpy(hs2, tok_item.data(), sizeof(int) * total_tokens);
   VLO_CUDA(cudaMemcpyAsync(plan->d_items, hs, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, stream));
   VLO_CUDA(cudaMemcpyAsync(plan->d_tok_item, hs2, sizeof(int) * total_tokens, cudaMemcpyHostToDevice, stream));

@@ -1,11 +1,44 @@
 // C-ABI: library-level and kernel-level entry points (see include/vlo_b200.h).
 #include "vlo_b200.h"
 
+#include <vector>
+
 #include "common.h"
 #include "gemm.cuh"
 #include "kv_pages.h"
 
 using namespace vlo;
+
+namespace {
+
+// Plan one sequence of n_tok queries over kv_len keys and upload the plan into d_ws.  h_identity_pt: also upload an
+// identity page table (the contiguous [n_kv_heads][kv_stride][128] layout, one "page" per 64-key block) behind the
+// plan's workspace and return its device address in *d_pt.  The upload is synchronised: the staging is pageable.
+int op_attn_plan(AttnPlan* plan, float* d_ws, int n_tok, int n_heads, int n_kv_heads, int head_dim, int kv_len,
+                 bool identity_pt, const int** d_pt, cudaStream_t st) {
+  VLO_CHECK(n_tok > 0 && kv_len >= n_tok, "attn: need 0 < n_tok <= kv_len");
+  AttnSeq s{};
+  s.q_tok0 = 0;
+  s.q_len = n_tok;
+  s.kv_len = kv_len;
+  s.pt0 = 0;
+  const size_t plan_stage = attn_stage_bytes(n_tok, 1, n_heads, n_kv_heads);
+  const int nblk = kv_pages_for(kv_len);
+  static thread_local std::vector<uint8_t> stage;
+  stage.resize(plan_stage + sizeof(int) * nblk);
+  if (attn_plan(plan, d_ws, stage.data(), &s, 1, n_tok, n_heads, n_kv_heads, head_dim, st)) return -1;
+  if (identity_pt) {
+    int* h_pt = reinterpret_cast<int*>(stage.data() + plan_stage);
+    for (int b = 0; b < nblk; ++b) h_pt[b] = b;
+    int* pt = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(d_ws) + attn_ws_bytes(n_tok, 1, n_heads, n_kv_heads));
+    VLO_CUDA(cudaMemcpyAsync(pt, h_pt, sizeof(int) * nblk, cudaMemcpyHostToDevice, st));
+    *d_pt = pt;
+  }
+  VLO_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -45,15 +78,9 @@ int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, 
   c.bias = d_bias;
   c.pos = d_pos;
   c.pos_rows = pos_rows;
-  c.bn = bn;
+  c.bn = bn > 0 ? bn : 128;
   return gemm_launch(c, static_cast<cudaStream_t>(cuda_stream));
 }
-
-}  // extern "C"
-
-#include <vector>
-
-extern "C" {
 
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
@@ -67,61 +94,23 @@ int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d
   c.rows_x = rows_x;
   c.k = k;
   c.out = d_out;
+  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
   c.ld_out = ld_out;
   c.plane_stride = plane_stride;
   c.bias = d_bias;
   c.act = act;
-  int planes = 1;
+  c.n_ctas = n_ctas;
   c.bn = bn;
-  c.weights_hot = rows_x > 128;
-  const int eff_bn = bn > 0 ? bn : (rows_x <= 16 ? 16 : (rows_x <= 32 ? 32 : (rows_x <= 64 ? 64 : 128)));
-  gemm_ws_plan(rows_w, k, mode, n_ctas, &c.sk, &planes, (rows_x + eff_bn - 1) / eff_bn);
-  if (h_max_planes) *h_max_planes = planes;
-  if (d_out == nullptr) return 0;  // planning query only
-  return gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream));
+  GemmWsPlan plan{};
+  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
+  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
+  return rc;
 }
 
 int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
                     const float* d_bias, int act, int n_ctas, void* cuda_stream) {
   return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
 }
-
-}  // extern "C"
-
-namespace {
-
-size_t align256(size_t x) { return (x + 255) / 256 * 256; }
-
-// Plan one sequence of n_tok queries over kv_len keys and upload the plan into d_ws.  h_identity_pt: also upload an
-// identity page table (the contiguous [n_kv_heads][kv_stride][128] layout, one "page" per 64-key block) behind the
-// plan's workspace and return its device address in *d_pt.  The upload is synchronised: the staging is pageable.
-int op_attn_plan(AttnPlan* plan, float* d_ws, int n_tok, int n_heads, int n_kv_heads, int head_dim, int kv_len,
-                 bool identity_pt, const int** d_pt, cudaStream_t st) {
-  VLO_CHECK(n_tok > 0 && kv_len >= n_tok, "attn: need 0 < n_tok <= kv_len");
-  AttnSeq s{};
-  s.q_tok0 = 0;
-  s.q_len = n_tok;
-  s.kv_len = kv_len;
-  s.pt0 = 0;
-  const size_t plan_stage = attn_stage_bytes(n_tok, 1, n_heads, n_kv_heads);
-  const int nblk = kv_pages_for(kv_len);
-  static thread_local std::vector<uint8_t> stage;
-  stage.resize(plan_stage + sizeof(int) * nblk);
-  if (attn_plan(plan, d_ws, stage.data(), &s, 1, n_tok, n_heads, n_kv_heads, head_dim, st)) return -1;
-  if (identity_pt) {
-    int* h_pt = reinterpret_cast<int*>(stage.data() + plan_stage);
-    for (int b = 0; b < nblk; ++b) h_pt[b] = b;
-    int* pt = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(d_ws) + attn_ws_bytes(n_tok, 1, n_heads, n_kv_heads));
-    VLO_CUDA(cudaMemcpyAsync(pt, h_pt, sizeof(int) * nblk, cudaMemcpyHostToDevice, st));
-    *d_pt = pt;
-  }
-  VLO_CUDA(cudaStreamSynchronize(st));
-  return 0;
-}
-
-}  // namespace
-
-extern "C" {
 
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len) {
   (void)head_dim;

@@ -53,6 +53,8 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
+inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+
 int num_sms();  // multiprocessors of the current device (queried once)
 
 // cudaFuncAttributeMaxDynamicSharedMemorySize is a per-device function attribute: set it once per (device, kernel).
@@ -93,41 +95,56 @@ struct GemmCall {
   const float* bias;
   const float* pos;
   int pos_rows;
-  int bn;    // 64 or 128 (0 = 128)
+  int bn;    // 64 or 128 (0: one wave of CTAs if possible, else the less wasted last wave; gemm.cu)
 };
 int gemm_launch(const GemmCall& c, cudaStream_t stream);
 
 // ---- persistent weight-streaming GEMM (gemm_ws.cuh / gemm.cu)
+// How gemm_ws_launch picks the token-tile width when GemmWsCall::bn is 0 (the rules sit next to the instances in gemm.cu)
+enum WsTiling : int {
+  WS_TILE_FIT = 0,             // the smallest instance covering rows_x (one tile up to 128 rows, 128-wide tiles beyond)
+  WS_TILE_TRUNK = 1,           // ViT trunk of 3+ frames: least padding, and in mode 1 the fullest last wave of CTAs
+  WS_TILE_BESIDE_DECODER = 2,  // ViT trunk of 1-2 frames, fp16: 64-token tiles on a 3-stage ring (83 KB), so the CTA
+                               // shares an SM with a decoder weight-streaming CTA
+};
 struct GemmWsCall {
   int fmt;            // 0 fp16, 1 bf16
   int mode;           // 0 stream-K fp32 partial planes, 1 whole tiles + 16-bit epilogue
   const void* w;      // [rows_w, k]
   int rows_w;
-  const void* x;      // [rows_x, k], rows_x <= 128
+  const void* x;      // [rows_x, k]
   int rows_x;
   int k;
-  void* out;
+  void* out;          // null: plan only
+  size_t out_elems;   // mode 0: capacity of out; a plan that needs more planes is rejected before the launch
   int ld_out;
   long long plane_stride;
   const float* bias;
   int act;
-  SkInfo sk;          // from gemm_ws_plan
-  int bn;             // token-tile width (0 = smallest of 16/32/64/128 covering rows_x); 96 / 192 for the ViT
-  int weights_hot;    // 1: weights are re-read by several token tiles (keep them in L2)
-  int small_smem;     // 1 with bn 64, fp16: shallow 3-stage ring (83 KB) so the CTA can share an SM with a decoder weight-streaming CTA
+  int n_ctas;         // <= 0: one CTA per SM
+  int bn;             // token-tile width; 0: chosen by `tiling`
+  int tiling;         // WsTiling
 };
-// decomposition for (rows_w, k): n_ctas <= 0 -> one CTA per SM; max_planes = fp32 planes the partials need
-int gemm_ws_plan(int rows_w, int k, int mode, int n_ctas, SkInfo* sk, int* max_planes, int x_tiles = 1);
-int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream);
+// What a launch decided, for the kernels that fold its partial planes.
+struct GemmWsPlan {
+  SkInfo sk;
+  int bn;             // token-tile width
+  int x_tiles;        // token tiles
+  int planes;         // most fp32 partial planes one tile needs (1 in mode 1)
+};
+// Picks the token tile, plans the stream-K split and launches; out == null only fills *plan.
+int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan = nullptr);
 
 // ---- ViT trunk GEMM, 128-token x 128-feature tiles (gemm_vit.cuh / gemm.cu): fp16 x [rows_x, k], w [rows_w, k] ->
 // fp16 out[rows_x][ld_out] = act(fp16(x w^T + bias)); n_ctas <= 0 -> one CTA per SM
 int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
                     const float* bias, int act, int n_ctas, cudaStream_t stream);
 
-// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu); args struct defined in gemm_wsf.cuh
-struct GemmWsfArgs;
-int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, cudaStream_t stream);
+// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), bf16, one CTA per SM:
+// act[rows_x][rows_w / 2] = SwiGLU(x w^T).  planes (plane_elems floats) take the partials of the non-finisher CTAs,
+// flags (n_flags counters, zero between launches) their arrivals.
+int gemm_wsf_launch(const void* w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
+                    size_t plane_elems, int* flags, int n_flags, cudaStream_t stream);
 
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {

@@ -10,7 +10,6 @@
 #include "common.h"
 #include "decoder_kernels.cuh"
 #include "gemm.cuh"
-#include "gemm_wsf.cuh"
 #include "kv_pages.h"
 #include "vit_kernels.cuh"
 #include "vlo_b200.h"
@@ -20,6 +19,7 @@ using namespace vlo;
 namespace {
 
 constexpr int kStageSlots = 16;
+constexpr int kSkFlags = 4096;  // stream-K arrival counters of the fused gate|up GEMM: one per 128-row weight tile
 
 using bf16 = __nv_bfloat16;
 
@@ -30,8 +30,6 @@ struct VitLayer {
   const float *ln1_w, *ln1_b, *ln2_w, *ln2_b, *qkv_b, *out_b, *fc1_b, *fc2_b;
   const __half *qkv_w, *out_w, *fc1_w, *fc2_w;
 };
-
-size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 
 }  // namespace
 
@@ -71,10 +69,14 @@ struct vlo_engine {
        *logits = nullptr;
   float* part = nullptr;
   size_t part_elems = 0;
-  int* sk_flags = nullptr;          // stream-K arrival counters of the fused gate|up GEMM (zero between launches)
+  int* sk_flags = nullptr;          // kSkFlags counters, zero between launches
   uint8_t* attn_ws = nullptr;
-  uint8_t* meta_dev = nullptr;  // tok_pos | last_index | first_rows | tok_kvrow | page tables of the step's streams
-  size_t meta_bytes = 0;
+  uint8_t* meta_dev = nullptr;  // the step's tables, laid out as `meta` says
+  // Byte offsets of tok_pos | last_index | first_rows | tok_kvrow | page tables in meta_dev and in a staging slot, whose
+  // attention plan starts at `bytes` (set by engine_init).
+  struct {
+    size_t pos, last, first, kvrow, pt, bytes;
+  } meta{};
   DecisionOut* decisions = nullptr;
   // host staging ring (pinned)
   uint8_t* stage = nullptr;
@@ -118,25 +120,32 @@ int lookup(vlo_engine* e, const std::string& name, int64_t expect_elems, const T
   return 0;
 }
 
-// weights [n_out, k] x tokens [T, k] -> stream-K fp32 partial planes in e->part (persistent kernel)
-int gemm_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, SkInfo* sk, cudaStream_t st) {
-  int planes = 1;
-  gemm_ws_plan(n_out, k, 0, 0, sk, &planes);
-  VLO_CHECK(static_cast<size_t>(planes) * T * n_out <= e->part_elems, "stream-K workspace too small");
-  VLO_CHECK(planes <= kFixMaxPlanes, "stream-K produced more partial planes than the fix-up kernels unroll");
+// weights [n_out, k] x tokens [rows, k] -> stream-K fp32 partial planes part[plane][rows][n_out] (persistent kernel),
+// which a fix-up kernel folds.  The fix-up kernels unroll kFixMaxPlanes planes: this is the one check of that limit,
+// made before the fix-up kernel that would read the planes is launched.
+int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int k, float* part, size_t part_elems,
+                 int tiling, GemmWsPlan* plan, cudaStream_t st) {
   GemmWsCall c{};
-  c.fmt = FMT_BF16;
+  c.fmt = fmt;
   c.mode = 0;
   c.w = w;
   c.rows_w = n_out;
   c.x = x;
-  c.rows_x = T;
+  c.rows_x = rows;
   c.k = k;
-  c.out = e->part;
+  c.out = part;
+  c.out_elems = part_elems;
   c.ld_out = n_out;
-  c.plane_stride = static_cast<long long>(T) * n_out;
-  c.sk = *sk;
-  return gemm_ws_launch(c, st);
+  c.plane_stride = static_cast<long long>(rows) * n_out;
+  c.tiling = tiling;
+  if (gemm_ws_launch(c, st, plan)) return -1;
+  VLO_CHECK(plan->planes <= kFixMaxPlanes, "stream-K produced more partial planes than the fix-up kernels unroll");
+  return 0;
+}
+
+// the decoder's partial GEMMs: bf16, the step's T tokens, planes in e->part
+int dec_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, GemmWsPlan* sk, cudaStream_t st) {
+  return gemm_partial(FMT_BF16, w, n_out, x, T, k, e->part, e->part_elems, WS_TILE_FIT, sk, st);
 }
 
 // gate|up GEMM + SwiGLU: the stream-K finisher CTAs apply the fix-up themselves (gemm_wsf.cuh).  A finisher's epilogue
@@ -145,26 +154,12 @@ int gemm_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, 
 // enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB plane round trip of
 // its fix-up; q|k|v, o_proj and down_proj go through gemm_partial and a fix-up kernel (DESIGN.md section 5).
 int gemm_swiglu(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, cudaStream_t st) {
-  GemmWsfArgs a{};
-  int planes = 1;
-  gemm_ws_plan(n_out, k, 0, 0, &a.sk, &planes);
-  VLO_CHECK(static_cast<size_t>(std::max(1, planes - 1)) * T * n_out <= e->part_elems, "stream-K workspace too small");
-  VLO_CHECK((n_out + 127) / 128 <= 4096, "stream-K flag array too small");
-  a.rows_w = n_out;
-  a.rows_x = T;
-  a.k = k;
-  a.planes = e->part;
-  a.plane_stride = static_cast<long long>(T) * n_out;
-  a.flags = e->sk_flags;
-  a.hint_w = kEvictFirst;
-  a.act = e->act;
-  a.I = n_out / 2;
-  return gemm_wsf_launch(a, w, x, st);
+  return gemm_wsf_launch(w, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st);
 }
 
 // whole-tile persistent GEMM with the 16-bit epilogue: out[T, n_out] = act(x W^T + bias)
 int gemm_ws_store16(int fmt, const void* w, int n_out, const void* x, int T, int k, void* out, int ld, const float* bias,
-                    int act, cudaStream_t st) {
+                    int act, cudaStream_t st, int tiling = WS_TILE_FIT) {
   GemmWsCall c{};
   c.fmt = fmt;
   c.mode = 1;
@@ -177,13 +172,13 @@ int gemm_ws_store16(int fmt, const void* w, int n_out, const void* x, int T, int
   c.ld_out = ld;
   c.bias = bias;
   c.act = act;
-  gemm_ws_plan(n_out, k, 1, 0, &c.sk, nullptr);
+  c.tiling = tiling;
   return gemm_ws_launch(c, st);
 }
 
 // one-tile fp16 GEMM with the 16-bit epilogue: out[rows_a, rows_b] = act(a b^T + bias)
 int gemm_store16(const void* a, int rows_a, const void* b, int rows_b, int k, void* out, int ld, const float* bias, int act,
-                 int bn, cudaStream_t st) {
+                 cudaStream_t st) {
   GemmCall c{};
   c.epi = EPI_STORE16;
   c.act = act;
@@ -195,20 +190,7 @@ int gemm_store16(const void* a, int rows_a, const void* b, int rows_b, int k, vo
   c.out = out;
   c.ld_out = ld;
   c.bias = bias;
-  c.bn = bn;
   return gemm_launch(c, st);
-}
-
-// N-tile width for the ViT trunk GEMMs: prefer a single wave of CTAs (one CTA per SM); two waves cost 2x.
-int vit_bn(int rows, int n_out) {
-  const int mt = (rows + 127) / 128;
-  const int t64 = mt * ((n_out + 63) / 64), t128 = mt * ((n_out + 127) / 128);
-  if (t64 <= num_sms()) return 64;     // everything fits in one wave even with the narrow tile
-  if (t128 <= num_sms()) return 128;   // one wave with the wide tile
-  // multi-wave: wide tiles (better operand reuse) unless the narrow ones waste much less of the last wave
-  const double e64 = static_cast<double>(t64) / (((t64 + num_sms() - 1) / num_sms()) * num_sms());
-  const double e128 = static_cast<double>(t128) / (((t128 + num_sms() - 1) / num_sms()) * num_sms());
-  return e64 > e128 + 0.15 ? 64 : 128;
 }
 
 // pinned staging slot, recycled behind a CUDA event
@@ -226,9 +208,18 @@ int stage_release(vlo_engine* e, int slot, cudaStream_t st) {
   return 0;
 }
 
-// step metadata: the page tables follow tok_pos | last_index | first_rows | tok_kvrow
-inline size_t meta_pt_offset(const vlo_config& c) {
-  return align256(sizeof(int) * c.max_step_tokens) * 3 + align256(sizeof(long long) * c.max_step_tokens);
+// Pack the page tables of streams sids[0..n) back to back into the table region of staging slot hs; pt0[i] receives
+// the entry of stream i's first page.  Returns the entries written.
+int stage_page_tables(const vlo_engine* e, uint8_t* hs, int n, const int* sids, int* pt0) {
+  int* dst = reinterpret_cast<int*>(hs + e->meta.pt);
+  int used = 0;
+  for (int i = 0; i < n; ++i) {
+    const std::vector<int>& tab = e->pool.tables[sids[i]];
+    std::memcpy(dst + used, tab.data(), sizeof(int) * tab.size());
+    pt0[i] = used;
+    used += static_cast<int>(tab.size());
+  }
+  return used;
 }
 
 // elements of one layer's K or V matrix
@@ -241,21 +232,24 @@ inline KvSide kv_paged_side(vlo_engine* e, bf16* plane0, const int* d_pt) {
   return KvSide{plane0, d_pt, static_cast<long long>(kv_plane_elems(e)), 0};
 }
 
-// Upload the page tables of up to two streams (first n_pages[i] entries each) to e->kv_op_pt through a staging slot.
-int upload_op_tables(vlo_engine* e, int n, const int* sids, const int* n_pages, const int** d_pt, cudaStream_t st) {
+// Upload the page tables of n <= 2 streams to e->kv_op_pt through a staging slot; d_pt[i] = stream i's table.
+int upload_op_tables(vlo_engine* e, int n, const int* sids, const int** d_pt, cudaStream_t st) {
   uint8_t* hs;
   int slot;
   if (stage_acquire(e, &hs, &slot)) return -1;
-  int* h = reinterpret_cast<int*>(hs);
-  const int per = kv_pages_for(e->cfg.max_kv_tokens);
-  size_t used = 0;
-  for (int i = 0; i < n; ++i) {
-    std::memcpy(h + static_cast<size_t>(i) * per, e->pool.tables[sids[i]].data(), sizeof(int) * n_pages[i]);
-    d_pt[i] = e->kv_op_pt + static_cast<size_t>(i) * per;
-    used = static_cast<size_t>(i) * per + n_pages[i];
-  }
-  VLO_CUDA(cudaMemcpyAsync(e->kv_op_pt, h, sizeof(int) * used, cudaMemcpyHostToDevice, st));
+  int pt0[2];
+  const int used = stage_page_tables(e, hs, n, sids, pt0);
+  for (int i = 0; i < n; ++i) d_pt[i] = e->kv_op_pt + pt0[i];
+  VLO_CUDA(cudaMemcpyAsync(e->kv_op_pt, hs + e->meta.pt, sizeof(int) * used, cudaMemcpyHostToDevice, st));
   return stage_release(e, slot, st);
+}
+
+// attention of decoder layer l over the KV pool, e->q -> e->attn_out, through the page tables staged in meta_dev
+int attn_layer(vlo_engine* e, const AttnPlan& plan, int l, cudaStream_t st) {
+  const vlo_config& c = e->cfg;
+  return attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), e->pool.rows_per_layer(),
+                  reinterpret_cast<const int*>(e->meta_dev + e->meta.pt), e->pool.page_stride_rows(),
+                  KvPool::head_stride_rows(), e->attn_out, c.num_heads, c.num_kv_heads, c.head_dim, st);
 }
 
 // Every entry point that touches the device runs on the engine's GPU whatever the caller's current device is
@@ -357,12 +351,19 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   const int widest = std::max(std::max(e->qkv_width, 2 * c.intermediate_size), H);
   e->part_elems = static_cast<size_t>(8) * T * widest;  // stream-K needs <= kb/floor(U/G) + 2 planes (<= 4 in practice)
   if (dev_alloc_t(e, &e->part, e->part_elems)) return -1;
-  if (dev_alloc_t(e, &e->sk_flags, 4096, true)) return -1;
+  if (dev_alloc_t(e, &e->sk_flags, kSkFlags, true)) return -1;
   const size_t aws = attn_ws_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads);
   if (dev_alloc(e, reinterpret_cast<void**>(&e->attn_ws), aws, false)) return -1;
-  e->meta_bytes = meta_pt_offset(c) + align256(sizeof(int) * std::max(2, c.max_streams) * per_stream);
-  if (dev_alloc(e, reinterpret_cast<void**>(&e->meta_dev), e->meta_bytes, false)) return -1;
-  e->stage_slot_bytes = align256(e->meta_bytes + attn_stage_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads));
+  // the table region also stages the two streams' tables of a KV copy (upload_op_tables)
+  const size_t per_token = align256(sizeof(int) * T);
+  e->meta.pos = 0;
+  e->meta.last = per_token;
+  e->meta.first = 2 * per_token;
+  e->meta.kvrow = 3 * per_token;
+  e->meta.pt = e->meta.kvrow + align256(sizeof(long long) * T);
+  e->meta.bytes = e->meta.pt + align256(sizeof(int) * std::max(2, c.max_streams) * per_stream);
+  if (dev_alloc(e, reinterpret_cast<void**>(&e->meta_dev), e->meta.bytes, false)) return -1;
+  e->stage_slot_bytes = align256(e->meta.bytes + attn_stage_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads));
   VLO_CUDA(cudaMallocHost(reinterpret_cast<void**>(&e->stage), e->stage_slot_bytes * kStageSlots));
   for (int i = 0; i < kStageSlots; ++i) VLO_CUDA(cudaEventCreateWithFlags(&e->stage_events[i], cudaEventDisableTiming));
 
@@ -536,9 +537,8 @@ int vlo_kv_fill_synthetic(vlo_engine* e, int sid, int n_tokens, uint64_t seed, v
   e->kv_len[sid] = n_tokens;
   if (n_tokens == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const int n_pages = kv_pages_for(n_tokens);
   const int* d_pt;
-  if (upload_op_tables(e, 1, &sid, &n_pages, &d_pt, st)) return -1;
+  if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
   kv_fill_kernel<<<dim3(std::min(64, (n_tokens * 128 + 255) / 256), c.num_kv_heads, 2 * c.num_layers), 256, 0, st>>>(
       kv_paged_side(e, e->kv, d_pt), c.num_kv_heads, n_tokens, sid, c.max_kv_tokens, seed);
   VLO_LAUNCH_CHECK();
@@ -562,9 +562,8 @@ int vlo_kv_read(vlo_engine* e, int sid, int layer, int is_v, void* d_out, void* 
   const int len = e->kv_len[sid];
   if (len == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const int n_pages = kv_pages_for(len);
   const int* d_pt;
-  if (upload_op_tables(e, 1, &sid, &n_pages, &d_pt, st)) return -1;
+  if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
   return launch_kv_copy(kv_paged_side(e, kv_layer_base(e, layer, is_v), d_pt), KvSide{static_cast<bf16*>(d_out), nullptr, 0, len},
                         c.num_kv_heads, len, 1, st);
 }
@@ -578,9 +577,8 @@ int vlo_kv_write(vlo_engine* e, int sid, int layer, int is_v, const void* d_in, 
   if (e->pool.resize(sid, n_tokens)) return -1;
   e->kv_len[sid] = n_tokens;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const int n_pages = kv_pages_for(n_tokens);
   const int* d_pt;
-  if (upload_op_tables(e, 1, &sid, &n_pages, &d_pt, st)) return -1;
+  if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
   return launch_kv_copy(KvSide{static_cast<bf16*>(const_cast<void*>(d_in)), nullptr, 0, n_tokens},
                         kv_paged_side(e, kv_layer_base(e, layer, is_v), d_pt), c.num_kv_heads, n_tokens, 1, st);
 }
@@ -600,9 +598,9 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, vo
   e->kv_len[dst_sid] = n_tokens;
   if (n_tokens == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  const int sids[2] = {src_sid, dst_sid}, counts[2] = {n_pages, n_pages};
+  const int sids[2] = {src_sid, dst_sid};
   const int* d_pt[2];
-  if (upload_op_tables(e, 2, sids, counts, d_pt, st)) return -1;
+  if (upload_op_tables(e, 2, sids, d_pt, st)) return -1;
   return launch_kv_copy(kv_paged_side(e, e->kv, d_pt[0]), kv_paged_side(e, e->kv, d_pt[1]), c.num_kv_heads, n_tokens,
                         2 * c.num_layers, st);
 }
@@ -658,7 +656,6 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     g.bias = e->patch_b;
     g.pos = e->pos_emb;
     g.pos_rows = P;
-    g.bn = vit_bn(rows, C);
     if (gemm_launch(g, st)) return -1;
   }
   // ViT attention: mma.sync m16n8k16 over TMA-loaded Q / K / V tiles (vit_kernels.cuh)
@@ -685,72 +682,20 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   // same bits as 64-token swap-AB tiles would; the stream-K planes keep the 64-token decomposition, whose summation
   // order the frame embeddings depend on.
   const bool small = B <= 2;
-  auto pick_bn = [&](int n_out, int mode) {
-    if (small) return 64;
-    const int cands[4] = {64, 96, 128, 192};
-    int best = 64;
-    double best_eff = -1.0;
-    for (int bn : cands) {
-      const int xt = (rows + bn - 1) / bn;
-      const int tiles = ((n_out + 127) / 128) * xt;
-      double eff = static_cast<double>(rows) / (static_cast<double>(xt) * bn);          // padding waste
-      if (mode == 1) eff *= static_cast<double>(tiles) / (((tiles + num_sms() - 1) / num_sms()) * num_sms());  // wave quantisation
-      if (eff >= best_eff - 1e-9) {  // ties -> wider tile (better operand reuse)
-        best_eff = eff;
-        best = bn;
-      }
-    }
-    return best;
-  };
   auto tiles_gemm = [&](const __half* x, const __half* w, int n_out, int k, __half* out, const float* bias, int act) -> int {
     if (small) return gemm_vit_launch(x, rows, w, n_out, k, out, n_out, bias, act, 0, st);
-    GemmWsCall g{};
-    g.fmt = FMT_F16;
-    g.mode = 1;
-    g.w = w;
-    g.rows_w = n_out;
-    g.x = x;
-    g.rows_x = rows;
-    g.k = k;
-    g.out = out;
-    g.ld_out = n_out;
-    g.bias = bias;
-    g.act = act;
-    g.bn = pick_bn(n_out, 1);
-    g.weights_hot = 1;
-    gemm_ws_plan(n_out, k, 1, 0, &g.sk, nullptr, (rows + g.bn - 1) / g.bn);
-    return gemm_ws_launch(g, st);
+    return gemm_ws_store16(FMT_F16, w, n_out, x, rows, k, out, n_out, bias, act, st, WS_TILE_TRUNK);
   };
-  struct SkCall { SkInfo sk; int bn, xt; };
-  auto partial_gemm = [&](const __half* x, const __half* w, int k, SkCall* out) -> int {
-    GemmWsCall g{};
-    g.fmt = FMT_F16;
-    g.mode = 0;
-    g.w = w;
-    g.rows_w = C;
-    g.x = x;
-    g.rows_x = rows;
-    g.k = k;
-    g.out = e->v_part;
-    g.ld_out = C;
-    g.plane_stride = static_cast<long long>(rows) * C;
-    g.bn = pick_bn(C, 0);
-    g.weights_hot = 1;
-    g.small_smem = small ? 1 : 0;
-    int planes = 1;
-    out->bn = g.bn;
-    out->xt = (rows + g.bn - 1) / g.bn;
-    gemm_ws_plan(C, k, 0, 0, &g.sk, &planes, out->xt);
-    VLO_CHECK(planes <= kFixMaxPlanes && static_cast<size_t>(planes) * rows * C <= e->v_part_elems, "ViT stream-K workspace too small");
-    out->sk = g.sk;
-    return gemm_ws_launch(g, st);
+  auto partial_gemm = [&](const __half* x, const __half* w, int k, GemmWsPlan* plan) -> int {
+    return gemm_partial(FMT_F16, w, C, x, rows, k, e->v_part, e->v_part_elems,
+                        small ? WS_TILE_BESIDE_DECODER : WS_TILE_TRUNK, plan, st);
   };
-  auto fix_ln = [&](const SkCall& sc, const float* bias, const float* lw, const float* lb, float* out32) -> int {
+  auto fix_ln = [&](const GemmWsPlan& plan, const float* bias, const float* lw, const float* lb, float* out32) -> int {
     VitFixLnParams p{};
     p.part = e->v_part;
-    p.sk = sc.sk;
-    p.sk_bn = sc.bn;
-    p.sk_xtiles = sc.xt;
+    p.sk = plan.sk;
+    p.sk_bn = plan.bn;
+    p.sk_xtiles = plan.x_tiles;
     p.split_stride = static_cast<long long>(rows) * C;
     p.bias = bias;
     p.h = e->v_h;
@@ -769,17 +714,17 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   count_launch();
   for (int l = 0; l < c.vit_layers; ++l) {
     const VitLayer& v = e->vit[l];
-    SkCall sc{};
+    GemmWsPlan sk{};
     if (tiles_gemm(e->v_xn, v.qkv_w, 3 * C, C, e->v_qkv, v.qkv_b, ACT_NONE)) return -1;
     if (launch_vit_attn()) return -1;
-    if (partial_gemm(e->v_attn, v.out_w, C, &sc)) return -1;
-    if (fix_ln(sc, v.out_b, v.ln2_w, v.ln2_b, nullptr)) return -1;
+    if (partial_gemm(e->v_attn, v.out_w, C, &sk)) return -1;
+    if (fix_ln(sk, v.out_b, v.ln2_w, v.ln2_b, nullptr)) return -1;
     if (tiles_gemm(e->v_xn, v.fc1_w, M, C, e->v_mlp, v.fc1_b, ACT_GELU_TANH)) return -1;
-    if (partial_gemm(e->v_mlp, v.fc2_w, M, &sc)) return -1;
+    if (partial_gemm(e->v_mlp, v.fc2_w, M, &sk)) return -1;
     const bool last = (l == c.vit_layers - 1);
     // the LayerNorm that follows fc2: next block's layer_norm1, or post_layernorm (fp16 copy feeds the MAP
     // head, fp32 copy feeds the pool)
-    if (fix_ln(sc, v.fc2_b, last ? e->post_ln_w : e->vit[l + 1].ln1_w, last ? e->post_ln_b : e->vit[l + 1].ln1_b,
+    if (fix_ln(sk, v.fc2_b, last ? e->post_ln_w : e->vit[l + 1].ln1_w, last ? e->post_ln_b : e->vit[l + 1].ln1_b,
                last ? e->v_ln32 : nullptr))
       return -1;
   }
@@ -794,8 +739,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   }
   if (cls) {
     // MAP head: K/V projection of all tokens, 1-query attention, out-proj, LN, MLP, residual
-    if (gemm_store16(e->v_xn, rows, e->head_kv_w, 2 * C, C, e->v_qkv, 2 * C, e->head_kv_b, ACT_NONE, vit_bn(rows, 2 * C), st))
-      return -1;
+    if (gemm_store16(e->v_xn, rows, e->head_kv_w, 2 * C, C, e->v_qkv, 2 * C, e->head_kv_b, ACT_NONE, st)) return -1;
     probe_attn_kernel<<<dim3(c.vit_heads, B), 128, static_cast<size_t>(P) * sizeof(float), st>>>(e->v_qkv, e->head_q, e->v_pa, P, C, 0.125f);
     VLO_LAUNCH_CHECK();
     VLO_CHECK(B <= 128, "MAP head handles <= 128 frames per call");
@@ -878,15 +822,14 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   uint8_t* hs;
   int slot;
   if (stage_acquire(e, &hs, &slot)) return -1;
-  const size_t o_pos = 0, o_last = align256(sizeof(int) * c.max_step_tokens), o_first = 2 * o_last,
-               o_row = 3 * o_last, o_pt = meta_pt_offset(c);
-  int* tok_pos = reinterpret_cast<int*>(hs + o_pos);
-  int* last_index = reinterpret_cast<int*>(hs + o_last);
-  int* first_rows = reinterpret_cast<int*>(hs + o_first);
-  long long* tok_kvrow = reinterpret_cast<long long*>(hs + o_row);
-  int* page_tables = reinterpret_cast<int*>(hs + o_pt);  // ceil(kv_len / 64) entries per sequence, back to back
+  int* tok_pos = reinterpret_cast<int*>(hs + e->meta.pos);
+  int* last_index = reinterpret_cast<int*>(hs + e->meta.last);
+  int* first_rows = reinterpret_cast<int*>(hs + e->meta.first);
+  long long* tok_kvrow = reinterpret_cast<long long*>(hs + e->meta.kvrow);
+  std::vector<int> pt0(n_seqs);
+  const int n_pt = stage_page_tables(e, hs, n_seqs, h_stream_ids, pt0.data());
   std::vector<AttnSeq> seqs(n_seqs);
-  int t = 0, n_pt = 0;
+  int t = 0;
   for (int i = 0; i < n_seqs; ++i) {
     const int sid = h_stream_ids[i], ql = h_q_lens[i], past = e->kv_len[sid];
     first_rows[i] = t;
@@ -895,19 +838,15 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
       tok_kvrow[t + j] = e->pool.row(sid, past + j);
       last_index[t + j] = (j == ql - 1) ? i : -1;
     }
-    seqs[i] = AttnSeq{t, ql, past + ql, n_pt};
-    const std::vector<int>& tab = e->pool.tables[sid];
-    std::memcpy(page_tables + n_pt, tab.data(), sizeof(int) * tab.size());
-    n_pt += static_cast<int>(tab.size());
+    seqs[i] = AttnSeq{t, ql, past + ql, pt0[i]};
     t += ql;
   }
-  VLO_CUDA(cudaMemcpyAsync(e->meta_dev, hs, o_pt + sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
-  const int* d_tok_pos = reinterpret_cast<const int*>(e->meta_dev + o_pos);
-  const int* d_last_index = reinterpret_cast<const int*>(e->meta_dev + o_last);
-  const long long* d_tok_kvrow = reinterpret_cast<const long long*>(e->meta_dev + o_row);
-  const int* d_page_tables = reinterpret_cast<const int*>(e->meta_dev + o_pt);
+  VLO_CUDA(cudaMemcpyAsync(e->meta_dev, hs, e->meta.pt + sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
+  const int* d_tok_pos = reinterpret_cast<const int*>(e->meta_dev + e->meta.pos);
+  const int* d_last_index = reinterpret_cast<const int*>(e->meta_dev + e->meta.last);
+  const long long* d_tok_kvrow = reinterpret_cast<const long long*>(e->meta_dev + e->meta.kvrow);
   AttnPlan plan{};
-  if (attn_plan(&plan, e->attn_ws, hs + e->meta_bytes, seqs.data(), n_seqs, T, c.num_heads, c.num_kv_heads, c.head_dim, st))
+  if (attn_plan(&plan, e->attn_ws, hs + e->meta.bytes, seqs.data(), n_seqs, T, c.num_heads, c.num_kv_heads, c.head_dim, st))
     return -1;
   if (stage_release(e, slot, st)) return -1;
 
@@ -922,10 +861,10 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
 
   const size_t norm_smem = static_cast<size_t>(H) * sizeof(float);
   // sk == null: no partials (the first layer's input norm)
-  auto resid_norm = [&](const SkInfo* sk, const bf16* w, bool last) -> int {
+  auto resid_norm = [&](const GemmWsPlan* sk, const bf16* w, bool last) -> int {
     ResidNormParams p{};
     p.part = sk ? e->part : nullptr;
-    if (sk) p.sk = *sk;
+    if (sk) p.sk = sk->sk;
     p.split_stride = static_cast<long long>(T) * H;
     p.h = e->h;
     p.w = w;
@@ -943,13 +882,13 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   const int attn_width = c.num_heads * c.head_dim;
   for (int l = 0; l < c.num_layers; ++l) {
     const DecLayer& d = e->dec[l];
-    SkInfo sk{};
+    GemmWsPlan sk{};
     const bool is_last = (l == c.num_layers - 1);
     // ---- q|k|v projection, then RoPE + in-place KV append
-    if (gemm_partial(e, d.qkv, e->qkv_width, e->xn, T, H, &sk, st)) return -1;
+    if (dec_partial(e, d.qkv, e->qkv_width, e->xn, T, H, &sk, st)) return -1;
     QkvRopeParams p{};
     p.part = e->part;
-    p.sk = sk;
+    p.sk = sk.sk;
     p.split_stride = static_cast<long long>(T) * e->qkv_width;
     p.cos_tab = e->rope_cos;
     p.sin_tab = e->rope_sin;
@@ -963,17 +902,14 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     p.n_kv_heads = c.num_kv_heads;
     VLO_CUDA(launch_pdl(qkv_rope_append_kernel, dim3(T, c.num_heads + 2 * c.num_kv_heads), dim3(64), 0, st, p));
     count_launch();
-    if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), e->pool.rows_per_layer(), d_page_tables,
-                 e->pool.page_stride_rows(), KvPool::head_stride_rows(), e->attn_out, c.num_heads, c.num_kv_heads,
-                 c.head_dim, st))
-      return -1;
+    if (attn_layer(e, plan, l, st)) return -1;
     // ---- o_proj + residual, then post-attention RMSNorm
-    if (gemm_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
+    if (dec_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
     if (resid_norm(&sk, d.post_norm, false)) return -1;
     // ---- gate|up + SwiGLU
     if (gemm_swiglu(e, d.gate_up, 2 * c.intermediate_size, e->xn, T, H, st)) return -1;
     // ---- down_proj + residual, then the next RMSNorm (next layer's input norm, or the final norm + last-row compaction)
-    if (gemm_partial(e, d.down, H, e->act, T, c.intermediate_size, &sk, st)) return -1;
+    if (dec_partial(e, d.down, H, e->act, T, c.intermediate_size, &sk, st)) return -1;
     if (resid_norm(&sk, is_last ? e->final_norm : e->dec[l + 1].in_norm, is_last)) return -1;
   }
   // ---- last-position lm_head + on-device decision
@@ -1008,7 +944,6 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
   const vlo_config& c = e->cfg;
   VLO_CHECK(n_seqs > 0 && n_seqs <= c.max_streams && n_tok > 0 && n_seqs * n_tok <= c.max_step_tokens, "bench_attn: sizes");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  std::vector<AttnSeq> seqs(n_seqs);
   for (int i = 0; i < n_seqs; ++i) {
     if (check_stream(e, h_stream_ids[i])) return -1;
     const int kv_len = e->kv_len[h_stream_ids[i]];
@@ -1018,20 +953,13 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
   uint8_t* hs;
   int slot;
   if (stage_acquire(e, &hs, &slot)) return -1;
-  const size_t o_pt = meta_pt_offset(c);
-  int* page_tables = reinterpret_cast<int*>(hs + o_pt);
-  int n_pt = 0;
-  for (int i = 0; i < n_seqs; ++i) {
-    const int sid = h_stream_ids[i];
-    seqs[i] = AttnSeq{i * n_tok, n_tok, e->kv_len[sid], n_pt};
-    const std::vector<int>& tab = e->pool.tables[sid];
-    std::memcpy(page_tables + n_pt, tab.data(), sizeof(int) * tab.size());
-    n_pt += static_cast<int>(tab.size());
-  }
-  VLO_CUDA(cudaMemcpyAsync(e->meta_dev + o_pt, page_tables, sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
-  const int* d_page_tables = reinterpret_cast<const int*>(e->meta_dev + o_pt);
+  std::vector<int> pt0(n_seqs);
+  const int n_pt = stage_page_tables(e, hs, n_seqs, h_stream_ids, pt0.data());
+  std::vector<AttnSeq> seqs(n_seqs);
+  for (int i = 0; i < n_seqs; ++i) seqs[i] = AttnSeq{i * n_tok, n_tok, e->kv_len[h_stream_ids[i]], pt0[i]};
+  VLO_CUDA(cudaMemcpyAsync(e->meta_dev + e->meta.pt, hs + e->meta.pt, sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
   AttnPlan plan{};
-  if (attn_plan(&plan, e->attn_ws, hs + e->meta_bytes, seqs.data(), n_seqs, n_seqs * n_tok, c.num_heads, c.num_kv_heads,
+  if (attn_plan(&plan, e->attn_ws, hs + e->meta.bytes, seqs.data(), n_seqs, n_seqs * n_tok, c.num_heads, c.num_kv_heads,
                 c.head_dim, st))
     return -1;
   if (stage_release(e, slot, st)) return -1;
@@ -1039,10 +967,7 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
   if (h_algo_bytes_per_launch) *h_algo_bytes_per_launch = plan.algo_bytes;
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < c.num_layers; ++l)
-      if (attn_run(plan, e->q, kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), e->pool.rows_per_layer(), d_page_tables,
-                   e->pool.page_stride_rows(), KvPool::head_stride_rows(), e->attn_out, c.num_heads, c.num_kv_heads,
-                   c.head_dim, st))
-        return -1;
+      if (attn_layer(e, plan, l, st)) return -1;
   return 0;
 }
 
@@ -1058,11 +983,11 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < c.num_layers; ++l) {
       const DecLayer& d = e->dec[l];
-      SkInfo sk{};
-      if (gemm_partial(e, d.qkv, e->qkv_width, e->xn, n_tok, H, &sk, st)) return -1;
-      if (gemm_partial(e, d.o, H, e->attn_out, n_tok, A, &sk, st)) return -1;
-      if (gemm_partial(e, d.gate_up, 2 * I, e->xn, n_tok, H, &sk, st)) return -1;
-      if (gemm_partial(e, d.down, H, e->act, n_tok, I, &sk, st)) return -1;
+      GemmWsPlan sk{};
+      if (dec_partial(e, d.qkv, e->qkv_width, e->xn, n_tok, H, &sk, st)) return -1;
+      if (dec_partial(e, d.o, H, e->attn_out, n_tok, A, &sk, st)) return -1;
+      if (dec_partial(e, d.gate_up, 2 * I, e->xn, n_tok, H, &sk, st)) return -1;
+      if (dec_partial(e, d.down, H, e->act, n_tok, I, &sk, st)) return -1;
       if (it == 0)
         bytes += 2.0 * (static_cast<double>(e->qkv_width) * H + static_cast<double>(H) * A + 2.0 * I * H + static_cast<double>(H) * I) +
                  2.0 * n_tok * (2.0 * H + A + I);

@@ -1,6 +1,6 @@
 // Host launchers of the wgmma GEMMs: TMA descriptor construction (driver entry point
 // resolved at run time, so the library loads on a box without libcuda), tile-shape
-// selection and kernel dispatch.
+// selection, stream-K planning and kernel dispatch.
 #include "gemm.cuh"
 #include "gemm_vit.cuh"
 #include "gemm_ws.cuh"
@@ -107,6 +107,18 @@ int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& arg
   return 0;
 }
 
+// N-tile width of the ViT's one-tile GEMMs: prefer a single wave of CTAs (one CTA per SM); two waves cost 2x.
+int vit_bn(int rows, int n_out) {
+  const int mt = (rows + 127) / 128;
+  const int t64 = mt * ((n_out + 63) / 64), t128 = mt * ((n_out + 127) / 128);
+  if (t64 <= num_sms()) return 64;     // everything fits in one wave even with the narrow tile
+  if (t128 <= num_sms()) return 128;   // one wave with the wide tile
+  // multi-wave: wide tiles (better operand reuse) unless the narrow ones waste much less of the last wave
+  const double e64 = static_cast<double>(t64) / (((t64 + num_sms() - 1) / num_sms()) * num_sms());
+  const double e128 = static_cast<double>(t128) / (((t128 + num_sms() - 1) / num_sms()) * num_sms());
+  return e64 > e128 + 0.15 ? 64 : 128;
+}
+
 }  // namespace
 
 int tmap_2d_sw128(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out) {
@@ -116,7 +128,7 @@ int tmap_2d_sw128(const void* ptr, int rows, int k, int box_rows, int fmt, CUten
 int gemm_launch(const GemmCall& c, cudaStream_t stream) {
   VLO_CHECK(c.k > 0 && c.k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(c.rows_a > 0 && c.rows_b > 0, "empty GEMM operand");
-  const int bn = c.bn == 0 ? 128 : c.bn;
+  const int bn = c.bn > 0 ? c.bn : vit_bn(c.rows_a, c.rows_b);
   GemmArgs a{};
   a.rows_a = c.rows_a;
   a.rows_b = c.rows_b;
@@ -171,10 +183,39 @@ int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a,
   count_launch();
   return 0;
 }
-}  // namespace
 
-int gemm_ws_plan(int rows_w, int k, int mode, int n_ctas, SkInfo* sk, int* max_planes, int x_tiles) {
-  const int tiles = ((rows_w + kGemmBM - 1) / kGemmBM) * (x_tiles > 0 ? x_tiles : 1);
+// Token-tile width for rows_x token rows, of both weight-streaming kernels: the smallest instance covering them (a
+// narrower X tile leaves more of the ring to the weight stream: 88 tokens = 8 streams x 11 take the 96-wide instance).
+// fp16 takes 128 above 64 rows; the fused gate|up GEMM is bf16.  Above 128 rows: 128-wide tiles.
+int token_tile(int rows_x, int fmt) {
+  if (rows_x <= 16) return 16;
+  if (rows_x <= 32) return 32;
+  if (rows_x <= 64) return 64;
+  return rows_x <= 96 && fmt == FMT_BF16 ? 96 : 128;
+}
+
+// Token-tile width of the ViT trunk of 3+ frames (many token tiles): the least padding in the last token tile, and in
+// mode 1 also the fullest last wave of CTAs.  Ties go to the wider tile (better operand reuse).
+int trunk_token_tile(int rows, int n_out, int mode) {
+  const int cands[4] = {64, 96, 128, 192};
+  int best = 64;
+  double best_eff = -1.0;
+  for (int bn : cands) {
+    const int xt = (rows + bn - 1) / bn;
+    const int tiles = ((n_out + 127) / 128) * xt;
+    double eff = static_cast<double>(rows) / (static_cast<double>(xt) * bn);          // padding waste
+    if (mode == 1) eff *= static_cast<double>(tiles) / (((tiles + num_sms() - 1) / num_sms()) * num_sms());  // wave quantisation
+    if (eff >= best_eff - 1e-9) {
+      best_eff = eff;
+      best = bn;
+    }
+  }
+  return best;
+}
+
+// Stream-K decomposition of `tiles` output tiles of k / 64 k-blocks over n_ctas CTAs (<= 0: one per SM); in mode 1
+// every CTA owns whole tiles.  Returns the most fp32 partial planes one tile needs.
+int gemm_ws_plan(int tiles, int k, int mode, int n_ctas, SkInfo* sk) {
   const int kb = k / kGemmBK;
   sk->kb = kb;
   sk->U = static_cast<long long>(tiles) * kb;
@@ -185,28 +226,32 @@ int gemm_ws_plan(int rows_w, int k, int mode, int n_ctas, SkInfo* sk, int* max_p
   int mp = 1;
   if (mode == 0)
     for (int t = 0; t < tiles; ++t) mp = std::max(mp, sk_planes(t, *sk));
-  if (max_planes) *max_planes = mp;
-  return 0;
+  return mp;
 }
+}  // namespace
 
-int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
+int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   VLO_CHECK(c.k > 0 && c.k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(c.rows_w > 0 && c.rows_x > 0, "empty GEMM operand");
-  // token-tile width: the smallest instance covering rows_x (a narrower X tile leaves more of the ring to the weight stream:
-  // 88 tokens = 8 streams x 11 take the 96-wide instance)
+  const bool beside = c.tiling == WS_TILE_BESIDE_DECODER;
   const int bn = c.bn > 0 ? c.bn
-                          : (c.rows_x <= 16 ? 16 : (c.rows_x <= 32 ? 32 : (c.rows_x <= 64 ? 64 : ((c.rows_x <= 96 && c.fmt == FMT_BF16) ? 96 : 128))));
+                 : beside ? 64
+                 : c.tiling == WS_TILE_TRUNK ? trunk_token_tile(c.rows_x, c.rows_w, c.mode)
+                 : token_tile(c.rows_x, c.fmt);
+  VLO_CHECK(!beside || (c.fmt == FMT_F16 && bn == 64), "gemm_ws: only the 64-token fp16 instance fits beside a decoder CTA");
   const int x_tiles = (c.rows_x + bn - 1) / bn;
-  VLO_CHECK(c.sk.U == static_cast<long long>((c.rows_w + kGemmBM - 1) / kGemmBM) * x_tiles * (c.k / kGemmBK),
-            "gemm_ws: plan does not match the call (x_tiles / bn)");
   GemmWsArgs a{};
   a.rows_w = c.rows_w;
   a.rows_x = c.rows_x;
   a.k = c.k;
   a.tiles = ((c.rows_w + kGemmBM - 1) / kGemmBM) * x_tiles;
   a.x_tiles = x_tiles;
-  a.hint_w = c.weights_hot ? kEvictNormal : kEvictFirst;
-  a.sk = c.sk;
+  const int planes = gemm_ws_plan(a.tiles, c.k, c.mode, c.n_ctas, &a.sk);
+  if (plan) *plan = GemmWsPlan{a.sk, bn, x_tiles, planes};
+  if (c.out == nullptr) return 0;
+  VLO_CHECK(c.mode != 0 || static_cast<size_t>(planes) * static_cast<size_t>(c.plane_stride) <= c.out_elems,
+            "stream-K workspace too small for " + std::to_string(planes) + " partial planes");
+  a.hint_w = x_tiles > 1 ? kEvictNormal : kEvictFirst;   // weights re-read by several token tiles stay in L2
   a.mode = c.mode;
   a.out = c.out;
   a.ld_out = c.ld_out;
@@ -220,7 +265,7 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream) {
   if (c.fmt == F && bn == N) return launch_ws<F, N>(tw, tx, a, stream);
   // the single-stream decoder GEMM: 6 x 18 KB leaves room on the SM for a co-resident ViT CTA (static_asserts above)
   if (c.fmt == FMT_BF16 && bn == 16) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
-  if (c.fmt == FMT_F16 && c.small_smem && bn == 64) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
+  if (beside) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
   VLO_WS_CASE(FMT_BF16, 32)
   VLO_WS_CASE(FMT_BF16, 64)
   VLO_WS_CASE(FMT_BF16, 96)
@@ -285,15 +330,29 @@ int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& 
 }
 }  // namespace
 
-int gemm_wsf_launch(const GemmWsfArgs& a, const void* w, const void* x, cudaStream_t stream) {
-  VLO_CHECK(a.k > 0 && a.k % kGemmBK == 0, "K must be a positive multiple of 64");
-  VLO_CHECK(a.rows_w > 0 && a.rows_x > 0 && a.rows_x <= 128, "gemm_wsf: 1..128 token rows");
-  VLO_CHECK(a.rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
-  const int bn = a.rows_x <= 16 ? 16 : (a.rows_x <= 32 ? 32 : (a.rows_x <= 64 ? 64 : (a.rows_x <= 96 ? 96 : 128)));
-  VLO_CHECK(a.sk.U == static_cast<long long>((a.rows_w + kGemmBM - 1) / kGemmBM) * (a.k / kGemmBK), "gemm_wsf: plan mismatch");
+int gemm_wsf_launch(const void* w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
+                    size_t plane_elems, int* flags, int n_flags, cudaStream_t stream) {
+  VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
+  VLO_CHECK(rows_w > 0 && rows_x > 0 && rows_x <= 128, "gemm_wsf: 1..128 token rows");
+  VLO_CHECK(rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
+  const int bn = token_tile(rows_x, FMT_BF16);
+  GemmWsfArgs a{};
+  a.rows_w = rows_w;
+  a.rows_x = rows_x;
+  a.k = k;
+  const int n_planes = gemm_ws_plan(rows_w / kGemmBM, k, 0, 0, &a.sk);
+  a.plane_stride = static_cast<long long>(rows_x) * rows_w;
+  VLO_CHECK(static_cast<size_t>(std::max(1, n_planes - 1)) * static_cast<size_t>(a.plane_stride) <= plane_elems,
+            "gemm_wsf: stream-K workspace too small");
+  VLO_CHECK(rows_w / kGemmBM <= n_flags, "gemm_wsf: stream-K flag array too small");
+  a.planes = planes;
+  a.flags = flags;
+  a.hint_w = kEvictFirst;
+  a.act = static_cast<__nv_bfloat16*>(act);
+  a.I = rows_w / 2;
   CUtensorMap tw, tx;
-  if (get_tmap(w, a.rows_w, a.k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
-  if (get_tmap(x, a.rows_x, a.k, bn, FMT_BF16, &tx) != 0) return -1;
+  if (get_tmap(w, rows_w, k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
+  if (get_tmap(x, rows_x, k, bn, FMT_BF16, &tx) != 0) return -1;
   if (bn == 16) return launch_wsf<16>(tw, tx, a, stream);
   if (bn == 32) return launch_wsf<32>(tw, tx, a, stream);
   if (bn == 64) return launch_wsf<64>(tw, tx, a, stream);

@@ -7,7 +7,7 @@
 
 namespace vlo {
 
-// The fix-up kernels unroll their plane loads to this many planes; the launchers reject plans that need more.
+// The fix-up kernels unroll their plane loads to this many planes; the engine rejects plans that need more.
 constexpr int kFixMaxPlanes = 8;
 
 struct SkInfo {
