@@ -200,6 +200,42 @@ int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void
 int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
                                int n_pages, void* d_out, float* d_ws, int n_tok, int n_heads, int n_kv_heads,
                                int head_dim, int kv_len, void* cuda_stream);
+/* The decoder step's fix-up and decision kernels (csrc/decoder_kernels.cuh), launched by the same helpers as vlo_step
+ * (block size, grid, shared memory, PDL).  bf16 tensors unless stated; bf16(.) = round to nearest even.
+ * d_part: fp32 stream-K partial planes [plane][T][width] as vlo_op_gemm_ws mode 0 leaves them (plane_stride T * width)
+ * for the bf16 GEMM of `width` output features over T token rows with this k and n_ctas (<= 0: one CTA per SM).  The
+ * entries take the plan from that GEMM's planning query and read only the sk_planes(tile) planes of each 128-feature
+ * tile (csrc/streamk.h).  They reject T > 128 (one token tile) and plans of more than 8 planes.
+ * Fix-up of feature n of token t: y = bf16(sum_{s < planes(n / 128)} part[s][t][n]), summed in plane order in fp32. */
+/* Residual add + RMSNorm, width = H (a multiple of 4, <= 12288):
+ *   h[t] = bf16(h[t] + y[t])                        (d_part == NULL: no partials, h unchanged)
+ *   xn[t][i] = bf16(w[i] * bf16(h[t][i] * rsqrt(mean_i(h[t][i]^2) + eps)))   (d_xn may be NULL)
+ *   xn_last[last_index[t]] = xn[t] for every t with last_index[t] >= 0      (d_last_index / d_xn_last may be NULL)
+ * Asynchronous. */
+int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
+                         const int32_t* d_last_index, int T, int H, float eps, void* cuda_stream);
+/* q|k|v fix-up + RoPE + KV append, width = (n_heads + 2 n_kv_heads) * 128, head hh = features [128 hh, 128 hh + 128):
+ * heads < n_heads are q, then n_kv_heads k heads, then n_kv_heads v heads.  For d < 64, x1 = y[d], x2 = y[d + 64]:
+ *   q and k: out[d] = bf16(bf16(x1 c) + bf16(-x2 s)), out[d + 64] = bf16(bf16(x2 c) + bf16(x1 s)),
+ *            c = cos[pos][d], s = sin[pos][d] (bf16 tables [n_rope_pos][64]); v: out = y unrotated.
+ *   q heads -> d_q [T, n_heads, 128]; kv head j -> row h_tok_kvrow[t] + j * kv_head_stride of d_k / d_v (rows of 128).
+ * h_tok_pos / h_tok_kvrow: host arrays [T]; every position must lie in [0, n_rope_pos).  Synchronous. */
+int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d_cos, const void* d_sin, int n_rope_pos,
+                           const int32_t* h_tok_pos, const int64_t* h_tok_kvrow, int kv_head_stride, void* d_q, void* d_k,
+                           void* d_v, int T, int n_heads, int n_kv_heads, void* cuda_stream);
+/* Fused gate|up GEMM + SwiGLU (csrc/gemm_wsf.cuh), the decoder's: W [rows_w, k] with rows_w % 128 == 0, 128-row tile j
+ * = 64 gate rows then the matching 64 up rows (features 64 j ..); X [rows_x <= 128, k].  With g, u = bf16 of the fp32
+ * stream-K sums over all SMs,  act[t][64 j + i] = bf16(bf16(g / (1 + exp(-g))) * u),  act [rows_x, rows_w / 2].
+ * d_planes: fp32 scratch of plane_elems floats for the partials; d_flags: n_flags >= rows_w / 128 int32 arrival
+ * counters, zero before the call and zero again when it has run.  Asynchronous. */
+int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
+                       int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream);
+/* Speak / silent decision over bf16 logits [n_rows, vocab] (vocab a multiple of 8, rows 16-byte aligned), one
+ * vlo_decision per row into d_out (device): first-index argmax, max logit, max - second max (a repeated maximum counts
+ * as the second), log-sum-exp, p_interval = bf16(softmax[interval_id]) (0 when interval_id is outside the row), and the
+ * first-index argmax of bf16(softmax) with (argmax_prob_id) and without (argmax_excl_id: that entry set to 0) the
+ * interval id.  Asynchronous. */
+int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream);
 /* Micro-loop of the same attention over n_layers separate K / V matrices (working set > L2), iters passes of back-to-back
  * launches on one plan: what bench tools bracket with ONE CUDA-event pair (per-launch time incl. the PDL overlap of a real
  * step).  skip_merge != 0 launches the main kernel only.  Mirrors vlo_bench_attn without an engine. */

@@ -82,6 +82,11 @@ SIGNATURES = {
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
     "vlo_op_attn_kvappend": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P]),
     "vlo_op_attn_kvappend_paged": (_I, [_P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vlo_op_resid_rmsnorm": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
+    "vlo_op_qkv_rope_append": (_I, [_P, _I, _I, _P, _P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _I, _P, _P, _P,
+                                    _I, _I, _I, _P]),
+    "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
+    "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),
 }
 

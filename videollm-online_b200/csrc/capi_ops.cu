@@ -38,6 +38,33 @@ int op_attn_plan(AttnPlan* plan, float* d_ws, int n_tok, int n_heads, int n_kv_h
   return 0;
 }
 
+// The stream-K plan of the bf16 partial GEMM that produced a fix-up kernel's planes: the planning query of
+// gemm_ws_launch (mode 0) for `width` output features, T token rows, k and n_ctas.
+int op_fix_plan(int width, int T, int k, int n_ctas, SkInfo* sk) {
+  VLO_CHECK(T > 0 && T <= 128, "fix-up kernels: 1..128 token rows (one token tile)");
+  GemmWsCall c{};
+  c.fmt = FMT_BF16;
+  c.mode = 0;
+  c.rows_w = width;
+  c.rows_x = T;
+  c.k = k;
+  c.n_ctas = n_ctas;
+  GemmWsPlan plan{};
+  if (gemm_ws_launch(c, nullptr, &plan)) return -1;
+  VLO_CHECK(plan.planes <= kFixMaxPlanes, "the plan needs " + std::to_string(plan.planes) +
+                                               " partial planes, more than the fix-up kernels unroll");
+  *sk = plan.sk;
+  return 0;
+}
+
+// Device scratch of a synchronous kernel-level entry point, freed on every return path.
+struct OpScratch {
+  void* p = nullptr;
+  ~OpScratch() {
+    if (p) cudaFree(p);
+  }
+};
+
 }  // namespace
 
 extern "C" {
@@ -147,6 +174,55 @@ int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void
     return -1;
   VLO_CUDA(cudaStreamSynchronize(st));
   return 0;
+}
+
+int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
+                         const int32_t* d_last_index, int T, int H, float eps, void* cuda_stream) {
+  // the row is staged in shared memory without an opt-in beyond the default 48 KB
+  VLO_CHECK(T > 0 && H > 0 && H % 4 == 0 && H * sizeof(float) <= 48 * 1024, "resid_rmsnorm: H a multiple of 4, <= 12288");
+  VLO_CHECK(d_last_index == nullptr || d_xn_last != nullptr, "resid_rmsnorm: last_index without xn_last");
+  SkInfo sk{};
+  if (d_part != nullptr && op_fix_plan(H, T, k, n_ctas, &sk)) return -1;
+  return resid_rmsnorm_launch(d_part, &sk, d_h, d_w, d_xn, d_xn_last, d_last_index, T, H, eps,
+                              static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d_cos, const void* d_sin, int n_rope_pos,
+                           const int32_t* h_tok_pos, const int64_t* h_tok_kvrow, int kv_head_stride, void* d_q, void* d_k,
+                           void* d_v, int T, int n_heads, int n_kv_heads, void* cuda_stream) {
+  VLO_CHECK(d_part != nullptr && n_heads > 0 && n_kv_heads > 0 && n_heads % n_kv_heads == 0, "qkv_rope_append: sizes");
+  SkInfo sk{};
+  if (op_fix_plan((n_heads + 2 * n_kv_heads) * 128, T, k, n_ctas, &sk)) return -1;
+  for (int t = 0; t < T; ++t) {
+    VLO_CHECK(h_tok_pos[t] >= 0 && h_tok_pos[t] < n_rope_pos,
+              "qkv_rope_append: position " + std::to_string(h_tok_pos[t]) + " outside the RoPE tables");
+    VLO_CHECK(h_tok_kvrow[t] >= 0, "qkv_rope_append: negative cache row");
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  OpScratch tables;
+  const size_t pos_bytes = align256(sizeof(int) * T);
+  VLO_CUDA(cudaMalloc(&tables.p, pos_bytes + sizeof(long long) * T));
+  int* d_pos = static_cast<int*>(tables.p);
+  long long* d_kvrow = reinterpret_cast<long long*>(static_cast<uint8_t*>(tables.p) + pos_bytes);
+  VLO_CUDA(cudaMemcpyAsync(d_pos, h_tok_pos, sizeof(int) * T, cudaMemcpyHostToDevice, st));
+  VLO_CUDA(cudaMemcpyAsync(d_kvrow, h_tok_kvrow, sizeof(long long) * T, cudaMemcpyHostToDevice, st));
+  if (qkv_rope_launch(d_part, sk, d_cos, d_sin, d_pos, d_kvrow, kv_head_stride, d_q, d_k, d_v, T, n_heads, n_kv_heads, st))
+    return -1;
+  VLO_CUDA(cudaStreamSynchronize(st));  // the tables are freed on return
+  return 0;
+}
+
+int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
+                       int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
+  VLO_CHECK(plane_elems >= 0, "gemm_swiglu: plane_elems");
+  return gemm_wsf_launch(d_w, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags, n_flags,
+                         static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream) {
+  VLO_CHECK(n_rows > 0 && vocab > 0 && vocab % 8 == 0, "decision: rows of a positive multiple of 8 logits");
+  VLO_CHECK((reinterpret_cast<uintptr_t>(d_logits) & 15) == 0, "decision: logits must be 16-byte aligned");
+  return decision_launch(d_logits, n_rows, vocab, interval_id, d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
 /* Back-to-back launches of the KV-append attention over `n_layers` separate K / V matrices (layer l at

@@ -146,6 +146,21 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 int gemm_wsf_launch(const void* w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
                     size_t plane_elems, int* flags, int n_flags, cudaStream_t stream);
 
+// ---- decoder fix-up and decision kernels (decoder_kernels.cuh / engine.cu) -----------
+// bf16 tensors; `part` holds fp32 stream-K planes [plane][T][width] of the plan `sk`, as gemm_ws_launch mode 0 leaves
+// them with plane_stride T * width (null: no partials, resid_rmsnorm only).
+// resid_rmsnorm_kernel: h[T, H] += fix-up, xn[T, H] (may be null) = RMSNorm(h) * w, xn_last[last_index[t]] = xn[t] for
+// last_index[t] >= 0 (both may be null); one CTA per row of min(1024, max(32, H / 4)) threads.
+int resid_rmsnorm_launch(const float* part, const SkInfo* sk, void* h, const void* w, void* xn, void* xn_last,
+                         const int* last_index, int T, int H, float eps, cudaStream_t st);
+// qkv_rope_append_kernel: q[T, n_heads, 128] and K / V rows of the token's position (device tables tok_pos / tok_kvrow)
+// from the fix-up of the q|k|v planes, RoPE from the bf16 [pos][64] cos / sin tables.
+int qkv_rope_launch(const float* part, const SkInfo& sk, const void* cos_tab, const void* sin_tab, const int* tok_pos,
+                    const long long* tok_kvrow, int kv_head_stride, void* q, void* k_cache, void* v_cache, int T,
+                    int n_heads, int n_kv_heads, cudaStream_t st);
+// decision_kernel: one vlo_decision per bf16 logits row [n_rows, vocab].
+int decision_launch(const void* logits, int n_rows, int vocab, int interval_id, void* out, cudaStream_t st);
+
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {
   int q_tok0;          // first packed token of the sequence

@@ -274,6 +274,60 @@ int check_stream(vlo_engine* e, int sid) {
 
 }  // namespace
 
+// ------------------------------------------------------------------------------ decoder fix-up and decision launches
+// The step and the kernel-level entry points (capi_ops.cu) launch these kernels through the helpers below only.
+namespace vlo {
+
+int resid_rmsnorm_launch(const float* part, const SkInfo* sk, void* h, const void* w, void* xn, void* xn_last,
+                         const int* last_index, int T, int H, float eps, cudaStream_t st) {
+  ResidNormParams p{};
+  p.part = part;
+  if (part) p.sk = *sk;
+  p.split_stride = static_cast<long long>(T) * H;
+  p.h = static_cast<bf16*>(h);
+  p.w = static_cast<const bf16*>(w);
+  p.xn = static_cast<bf16*>(xn);
+  p.xn_last = static_cast<bf16*>(xn_last);
+  p.last_index = last_index;
+  p.H = H;
+  p.eps = eps;
+  VLO_CUDA(launch_pdl(resid_rmsnorm_kernel, dim3(T), dim3(std::min(1024, std::max(32, H / 4))),
+                      static_cast<size_t>(H) * sizeof(float), st, p));
+  count_launch();
+  return 0;
+}
+
+int qkv_rope_launch(const float* part, const SkInfo& sk, const void* cos_tab, const void* sin_tab, const int* tok_pos,
+                    const long long* tok_kvrow, int kv_head_stride, void* q, void* k_cache, void* v_cache, int T,
+                    int n_heads, int n_kv_heads, cudaStream_t st) {
+  QkvRopeParams p{};
+  p.part = part;
+  p.sk = sk;
+  p.split_stride = static_cast<long long>(T) * (n_heads + 2 * n_kv_heads) * 128;
+  p.cos_tab = static_cast<const bf16*>(cos_tab);
+  p.sin_tab = static_cast<const bf16*>(sin_tab);
+  p.tok_pos = tok_pos;
+  p.tok_kvrow = tok_kvrow;
+  p.kv_head_stride = kv_head_stride;
+  p.q_out = static_cast<bf16*>(q);
+  p.k_cache = static_cast<bf16*>(k_cache);
+  p.v_cache = static_cast<bf16*>(v_cache);
+  p.n_heads = n_heads;
+  p.n_kv_heads = n_kv_heads;
+  VLO_CUDA(launch_pdl(qkv_rope_append_kernel, dim3(T, n_heads + 2 * n_kv_heads), dim3(64), 0, st, p));
+  count_launch();
+  return 0;
+}
+
+int decision_launch(const void* logits, int n_rows, int vocab, int interval_id, void* out, cudaStream_t st) {
+  VLO_CUDA(launch_pdl(decision_kernel, dim3(n_rows), dim3(1024), 0, st, static_cast<const bf16*>(logits), vocab,
+                      interval_id, static_cast<DecisionOut*>(out)));
+  count_launch();
+  return 0;
+}
+
+}  // namespace vlo
+
 extern "C" {
 
 static int engine_init(vlo_engine* e, int64_t kv_pool_tokens);
@@ -859,23 +913,10 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     count_launch();
   }
 
-  const size_t norm_smem = static_cast<size_t>(H) * sizeof(float);
   // sk == null: no partials (the first layer's input norm)
   auto resid_norm = [&](const GemmWsPlan* sk, const bf16* w, bool last) -> int {
-    ResidNormParams p{};
-    p.part = sk ? e->part : nullptr;
-    if (sk) p.sk = sk->sk;
-    p.split_stride = static_cast<long long>(T) * H;
-    p.h = e->h;
-    p.w = w;
-    p.xn = e->xn;
-    p.xn_last = last ? e->xn_last : nullptr;
-    p.last_index = last ? d_last_index : nullptr;
-    p.H = H;
-    p.eps = c.rms_norm_eps;
-    VLO_CUDA(launch_pdl(resid_rmsnorm_kernel, dim3(T), dim3(std::min(1024, std::max(32, H / 4))), norm_smem, st, p));
-    count_launch();
-    return 0;
+    return resid_rmsnorm_launch(sk ? e->part : nullptr, sk ? &sk->sk : nullptr, e->h, w, e->xn, last ? e->xn_last : nullptr,
+                                last ? d_last_index : nullptr, T, H, c.rms_norm_eps, st);
   };
 
   if (resid_norm(nullptr, e->dec[0].in_norm, false)) return -1;
@@ -886,22 +927,9 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     const bool is_last = (l == c.num_layers - 1);
     // ---- q|k|v projection, then RoPE + in-place KV append
     if (dec_partial(e, d.qkv, e->qkv_width, e->xn, T, H, &sk, st)) return -1;
-    QkvRopeParams p{};
-    p.part = e->part;
-    p.sk = sk.sk;
-    p.split_stride = static_cast<long long>(T) * e->qkv_width;
-    p.cos_tab = e->rope_cos;
-    p.sin_tab = e->rope_sin;
-    p.tok_pos = d_tok_pos;
-    p.tok_kvrow = d_tok_kvrow;
-    p.kv_head_stride = KvPool::head_stride_rows();
-    p.q_out = e->q;
-    p.k_cache = kv_layer_base(e, l, 0);
-    p.v_cache = kv_layer_base(e, l, 1);
-    p.n_heads = c.num_heads;
-    p.n_kv_heads = c.num_kv_heads;
-    VLO_CUDA(launch_pdl(qkv_rope_append_kernel, dim3(T, c.num_heads + 2 * c.num_kv_heads), dim3(64), 0, st, p));
-    count_launch();
+    if (qkv_rope_launch(e->part, sk.sk, e->rope_cos, e->rope_sin, d_tok_pos, d_tok_kvrow, KvPool::head_stride_rows(), e->q,
+                        kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), T, c.num_heads, c.num_kv_heads, st))
+      return -1;
     if (attn_layer(e, plan, l, st)) return -1;
     // ---- o_proj + residual, then post-attention RMSNorm
     if (dec_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
@@ -916,10 +944,9 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   bf16* logits = d_last_logits ? static_cast<bf16*>(d_last_logits) : e->logits;
   if (gemm_ws_store16(FMT_BF16, e->lm_head, c.vocab_size, e->xn_last, n_seqs, H, logits, c.vocab_size, nullptr, ACT_NONE, st))
     return -1;
-  DecisionOut* dec_out = d_decisions ? reinterpret_cast<DecisionOut*>(d_decisions) : e->decisions;
-  VLO_CUDA(launch_pdl(decision_kernel, dim3(n_seqs), dim3(1024), 0, st, static_cast<const bf16*>(logits), c.vocab_size,
-                      interval_id, dec_out));
-  count_launch();
+  if (decision_launch(logits, n_seqs, c.vocab_size, interval_id, d_decisions ? static_cast<void*>(d_decisions) : e->decisions,
+                      st))
+    return -1;
 
   for (int i = 0; i < n_seqs; ++i) e->kv_len[h_stream_ids[i]] += h_q_lens[i];
   rollback.armed = false;
