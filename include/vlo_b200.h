@@ -146,6 +146,20 @@ int vlo_step(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32
 int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_q_lens,
                  const int64_t* d_row_ids, const void* d_embeds, void* d_last_logits, vlo_decision* d_decisions,
                  int interval_id, void* cuda_stream);
+/* Segmented step: several decisions per sequence in one pass, e.g. a backlog of queued frames
+ * [prefix | F1 | interval | F2 | interval | F3 ...] with one decision per frame.
+ *   h_seg_counts[n_seqs] (host): sequence i carries h_seg_counts[i] >= 1 consecutive segments; their lengths follow one
+ *   another in h_seg_lens (host, sum(h_seg_counts) entries, each > 0), and sequence i's q_len is the sum of its own.
+ *   d_seg_logits: bf16 [sum(h_seg_counts), vocab] or NULL; d_decisions: vlo_decision[sum(h_seg_counts)] or NULL; one row
+ *   per segment in order, computed at the segment's last row.
+ * Each segment's attention is planned exactly as a one-sequence step of that segment alone over the keys up to its end
+ * (same work items, split budget and key splits), so a segment computes the bits the same tokens get from a step of
+ * their own on the same cache (decoder GEMM rows do not depend on the other rows of the step).  To take back the
+ * segments after segment j, vlo_kv_truncate the stream to the end of segment j.  Row ids, page taking, pool-exhaustion
+ * rollback and the capacity errors are those of vlo_step_ids, which is this call with one segment per sequence. */
+int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_seg_counts,
+                      const int32_t* h_seg_lens, const int64_t* d_row_ids, const void* d_embeds, void* d_seg_logits,
+                      vlo_decision* d_decisions, int interval_id, void* cuda_stream);
 /* all-position logits for the last vlo_step's tokens (the reference's logits_to_keep=0 behaviour,
  * HF:models/llama/modeling_llama.py:485-487); d_logits bf16 [sum(q_lens), vocab]. Test/compat path. */
 int vlo_last_step_logits(vlo_engine* e, void* d_logits, void* cuda_stream);
@@ -200,6 +214,16 @@ int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void
 int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
                                int n_pages, void* d_out, float* d_ws, int n_tok, int n_heads, int n_kv_heads,
                                int head_dim, int kv_len, void* cuda_stream);
+/* kernel-level: the attention of one segmented sequence over a paged pool, planned and launched as vlo_step_segments
+ * does.  n_tok = sum(h_seg_lens[0..n_segs)) query rows (host array, each > 0) sit at positions kv_len - n_tok ..
+ * kv_len - 1 of d_q [n_tok, n_heads, head_dim]; row r attends causally to keys 0..(its position).  Segment j (rows
+ * o_j .. o_j + len_j - 1, ending at key e_j = kv_len - n_tok + o_j + len_j) gets in d_out exactly the bits
+ * vlo_op_attn_kvappend_paged gives its rows alone with kv_len = e_j on the same pool.  n_segs = 1 is that call.
+ * Keys past a row's position are masked: they may hold any finite values.  Scratch is allocated internally;
+ * synchronous. */
+int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
+                                  int n_pages, void* d_out, int n_segs, const int32_t* h_seg_lens, int n_heads,
+                                  int n_kv_heads, int head_dim, int kv_len, void* cuda_stream);
 /* The decoder step's fix-up and decision kernels (csrc/decoder_kernels.cuh), launched by the same helpers as vlo_step
  * (block size, grid, shared memory, PDL).  bf16 tensors unless stated; bf16(.) = round to nearest even.
  * d_part: fp32 stream-K partial planes [plane][T][width] as vlo_op_gemm_ws mode 0 leaves them (plane_stride T * width)

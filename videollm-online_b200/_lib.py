@@ -72,6 +72,8 @@ SIGNATURES = {
     "vlo_embed_tokens": (_I, [_P, _P, _I, _P, _P]),
     "vlo_step": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _I, _P]),
     "vlo_step_ids": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _P, _I, _P]),
+    "vlo_step_segments": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _P,
+                               _I, _P]),
     "vlo_last_step_logits": (_I, [_P, _P, _P]),
     "vlo_last_step_hidden": (_I, [_P, _P, _P]),
     "vlo_bench_attn": (_I, [_P, _I, C.POINTER(C.c_int32), _I, _I, _I, C.POINTER(C.c_double), _P]),
@@ -82,6 +84,7 @@ SIGNATURES = {
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
     "vlo_op_attn_kvappend": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P]),
     "vlo_op_attn_kvappend_paged": (_I, [_P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "vlo_op_attn_kvappend_segments": (_I, [_P, _P, _P, _P, _I, _P, _I, C.POINTER(C.c_int32), _I, _I, _I, _I, _P]),
     "vlo_op_resid_rmsnorm": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
     "vlo_op_qkv_rope_append": (_I, [_P, _I, _I, _P, _P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _I, _P, _P, _P,
                                     _I, _I, _I, _P]),

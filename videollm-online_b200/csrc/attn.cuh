@@ -55,17 +55,20 @@ struct AttnParams {
   float scale_log2;        // head_dim^-0.5 * log2(e)
 };
 
-// grid = (max_splits, n_kv_heads, n_items); block = kAttnThreads.
-__global__ void __launch_bounds__(kAttnThreads, 1)
-attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
-                     const AttnParams p) {
-  pdl_trigger();
-  // The item table and the page tables were uploaded by the memcpy at the start of the step: they (and this split's
-  // page entries, below) are read before the grid dependency resolves.
-  const AttnItem it = p.items[blockIdx.z];
-  const int split = blockIdx.x;
-  if (split >= it.n_splits) return;
-  const int kvh = blockIdx.y;
+// One CTA of the KV-append attention: item `it`, key split `split`, kv head `kvh`.
+// kCluster = false: attn_kvappend_kernel, the CTA loads its own key blocks.
+// kCluster = true: attn_kvappend_cluster_kernel, one CTA per item of a cluster of items of ONE stream with the same
+//   blocks_per_split, all on the same (split, kv head).  The cluster loads nblk_load >= nblk key blocks (the longest
+//   member's); block b is loaded by CTA b % cs with a TMA multicast into the same ring stage of every CTA, so the cache
+//   crosses HBM -> L2 -> SM once per cluster.  A stage is refilled only when every CTA has released it: each producer,
+//   once its own MMA warps released a stage, arrives on the cluster-release barrier of every CTA, and the loading CTA
+//   waits on its own.  The MMA warps run the same code on the blocks of their own item and only take part in the ring
+//   protocol on the others; a CTA that is not `active` (its item has no block in this split, or a padding rank) writes
+//   nothing.
+template <bool kCluster>
+__device__ __forceinline__ void attn_kvappend_cta(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const AttnParams& p,
+                                                  const AttnItem& it, int split, int kvh, int nblk_load, bool active,
+                                                  uint32_t rank, uint32_t cs) {
   const int G = p.n_heads / p.n_kv_heads;
   const int rows = it.q_count * G;
   const int mt_active = (rows + 15) >> 4;  // MMA warps per group that own real rows
@@ -73,28 +76,32 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
   const int nblk_total = (kv_end + kAttnBlk - 1) / kAttnBlk;
   const int blk0 = split * it.blocks_per_split;
   const int blk1 = min(blk0 + it.blocks_per_split, nblk_total);
-  const int nblk = blk1 - blk0;
+  const int nblk = kCluster ? (active ? blk1 - blk0 : 0) : blk1 - blk0;
+  const int nblk_ld = kCluster ? nblk_load : nblk;  // key blocks that go through this CTA's ring
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kAttnGroups * kAttnStages * kAttnStageBytes);
   uint64_t* empty_bar = full_bar + kAttnGroups * kAttnStages;
+  uint64_t* cl_empty_bar = empty_bar + kAttnGroups * kAttnStages;  // cluster release (kCluster only)
   int* s_pt = reinterpret_cast<int*>(smem + kAttnGroups * kAttnStages * kAttnStageBytes + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int j = threadIdx.x; j < nblk; j += kAttnThreads) s_pt[j] = p.page_table[it.pt0 + blk0 + j];
+  for (int j = threadIdx.x; j < nblk_ld; j += kAttnThreads) s_pt[j] = p.page_table[it.pt0 + blk0 + j];
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
     for (int i = 0; i < kAttnGroups * kAttnStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], mt_active);
+      if (kCluster) mbar_init(&cl_empty_bar[i], cs);
     }
     fence_mbar_init();
   }
   pdl_wait();   // the freshly appended K/V rows and Q come from predecessors
   __syncthreads();
+  if (kCluster) cluster_sync();  // every CTA's barriers are initialised before any multicast or remote arrive
 
   const int head_row = kvh * p.head_stride_rows;
 
@@ -113,20 +120,33 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
   if (warp == 0) {
     if (lane == 0) {
       // ---------------------------------------------------------- TMA producer
-      for (int b = 0; b < nblk; ++b) {
+      for (int b = 0; b < nblk_ld; ++b) {
         const int g = b & 1;
         const int i = b >> 1;
         const int s = i % kAttnStages;
         const uint32_t ph = (i / kAttnStages) & 1;
         uint64_t* fb = &full_bar[g * kAttnStages + s];
         mbar_wait(&empty_bar[g * kAttnStages + s], ph ^ 1);
-        mbar_arrive_expect_tx(fb, kAttnStageBytes);
+        if (kCluster && i >= kAttnStages)  // this CTA released the stage's previous block: tell every CTA of the cluster
+          for (uint32_t r = 0; r < cs; ++r) mbar_arrive_cluster(&cl_empty_bar[g * kAttnStages + s], r);
+        mbar_arrive_expect_tx(fb, kAttnStageBytes);  // cluster: peers' copies may land before this, the phase waits for it
         uint8_t* st = smem + (g * kAttnStages + s) * kAttnStageBytes;
         const int row = s_pt[b] * p.page_stride_rows + head_row;
-        tma_load_2d(st, &tm_k, fb, 0, row, kEvictFirst);
-        tma_load_2d(st + kAttnSubTile, &tm_k, fb, 64, row, kEvictFirst);
-        tma_load_2d(st + 2 * kAttnSubTile, &tm_v, fb, 0, row, kEvictFirst);
-        tma_load_2d(st + 3 * kAttnSubTile, &tm_v, fb, 64, row, kEvictFirst);
+        if (kCluster) {
+          if (static_cast<uint32_t>(b) % cs == rank) {
+            mbar_wait(&cl_empty_bar[g * kAttnStages + s], ph ^ 1);  // every CTA released the stage
+            const uint16_t mask = static_cast<uint16_t>((1u << cs) - 1);
+            tma_load_2d_multicast(st, &tm_k, fb, 0, row, mask, kEvictFirst);
+            tma_load_2d_multicast(st + kAttnSubTile, &tm_k, fb, 64, row, mask, kEvictFirst);
+            tma_load_2d_multicast(st + 2 * kAttnSubTile, &tm_v, fb, 0, row, mask, kEvictFirst);
+            tma_load_2d_multicast(st + 3 * kAttnSubTile, &tm_v, fb, 64, row, mask, kEvictFirst);
+          }
+        } else {
+          tma_load_2d(st, &tm_k, fb, 0, row, kEvictFirst);
+          tma_load_2d(st + kAttnSubTile, &tm_k, fb, 64, row, kEvictFirst);
+          tma_load_2d(st + 2 * kAttnSubTile, &tm_v, fb, 0, row, kEvictFirst);
+          tma_load_2d(st + 3 * kAttnSubTile, &tm_v, fb, 64, row, kEvictFirst);
+        }
       }
     }
   } else if (mt < mt_active) {
@@ -156,11 +176,16 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
     const int lim1 = r1 < rows ? it.q_pos0 + r1 / G : -1;
     const float c = p.scale_log2;
 
-    for (int b = grp; b < nblk; b += kAttnGroups) {
+    for (int b = grp; b < nblk_ld; b += kAttnGroups) {
       const int i = b >> 1;
       const int s = i % kAttnStages;
       const uint32_t ph = (i / kAttnStages) & 1;
       mbar_wait(&full_bar[grp * kAttnStages + s], ph);
+      if (kCluster && b >= nblk) {  // a block of a longer member of the cluster: release it untouched
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[grp * kAttnStages + s]);
+        continue;
+      }
       const uint32_t st = smem_u32(smem + (grp * kAttnStages + s) * kAttnStageBytes);
       const int key0 = (blk0 + b) * kAttnBlk;
 
@@ -260,6 +285,7 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
 
   // ---- merge the two warp groups through shared memory (pipeline buffers are idle now)
   __syncthreads();
+  if (kCluster && !active) return;  // the caller's cluster_sync follows
   float* xo = reinterpret_cast<float*>(smem);            // [4 warps][16 rows][128]
   float* xml = xo + 4 * 16 * kAttnHD;                     // [4 warps][16 rows][2]
   if (warp > 0 && mt < mt_active && grp == 1) {
@@ -312,6 +338,52 @@ attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_cons
       }
     }
   }
+}
+
+
+// grid = (max_splits, n_kv_heads, n_items); block = kAttnThreads.
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_kvappend_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
+                     const AttnParams p) {
+  pdl_trigger();
+  // The item table and the page tables were uploaded by the memcpy at the start of the step: they (and this split's
+  // page entries, below) are read before the grid dependency resolves.
+  const AttnItem it = p.items[blockIdx.z];
+  const int split = blockIdx.x;
+  if (split >= it.n_splits) return;
+  attn_kvappend_cta<false>(tm_k, tm_v, p, it, split, blockIdx.y, 0, true, 0, 1);
+}
+
+constexpr int kAttnClusterMax = 8;  // portable cluster size
+// members of one cluster: item indices, -1 for the padding ranks of a cluster smaller than the launch's cluster size
+struct AttnCluster {
+  int item[kAttnClusterMax];
+};
+
+// grid = (cs * n_clusters, max_splits, n_kv_heads), cluster = (cs, 1, 1); block = kAttnThreads.
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_kvappend_cluster_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
+                             const AttnParams p, const AttnCluster* clusters) {
+  pdl_trigger();
+  const uint32_t cs = cluster_nctarank();
+  const uint32_t rank = cluster_ctarank();
+  const AttnCluster& cl = clusters[blockIdx.x / cs];
+  const int split = blockIdx.y;
+  // blocks the cluster loads in this split: the longest member's (all members share blocks_per_split)
+  int nblk_load = 0;
+  for (uint32_t r = 0; r < cs; ++r) {
+    const int m = cl.item[r];
+    if (m < 0) continue;
+    const AttnItem& im = p.items[m];
+    if (split >= im.n_splits) continue;
+    const int nb = (im.q_pos0 + im.q_count + kAttnBlk - 1) / kAttnBlk;
+    nblk_load = max(nblk_load, min(im.blocks_per_split, nb - split * im.blocks_per_split));
+  }
+  if (nblk_load == 0) return;  // no member has this split: the whole cluster leaves together
+  const int own = cl.item[rank];
+  const AttnItem it = p.items[own >= 0 ? own : cl.item[0]];
+  attn_kvappend_cta<true>(tm_k, tm_v, p, it, split, blockIdx.z, nblk_load, own >= 0 && split < it.n_splits, rank, cs);
+  cluster_sync();  // no CTA leaves while another may still arrive on its barriers
 }
 
 // out[token, head, :] = sum_s O_s * 2^((m_s - M) c) / sum_s l_s * 2^((m_s - M) c)

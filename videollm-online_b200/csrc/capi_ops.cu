@@ -14,14 +14,17 @@ namespace {
 // Plan one sequence of n_tok queries over kv_len keys and upload the plan into d_ws.  h_identity_pt: also upload an
 // identity page table (the contiguous [n_kv_heads][kv_stride][128] layout, one "page" per 64-key block) behind the
 // plan's workspace and return its device address in *d_pt.  The upload is synchronised: the staging is pageable.
-int op_attn_plan(AttnPlan* plan, float* d_ws, int n_tok, int n_heads, int n_kv_heads, int head_dim, int kv_len,
-                 bool identity_pt, const int** d_pt, cudaStream_t st) {
+// n_segs > 1: the n_tok rows are segments of h_seg_lens[] rows, planned as by a segmented decoder step.
+int op_attn_plan(AttnPlan* plan, void* d_ws, int n_tok, int n_heads, int n_kv_heads, int head_dim, int kv_len,
+                 bool identity_pt, const int** d_pt, cudaStream_t st, int n_segs = 0, const int* h_seg_lens = nullptr) {
   VLO_CHECK(n_tok > 0 && kv_len >= n_tok, "attn: need 0 < n_tok <= kv_len");
   AttnSeq s{};
   s.q_tok0 = 0;
   s.q_len = n_tok;
   s.kv_len = kv_len;
   s.pt0 = 0;
+  s.n_segs = n_segs;
+  s.seg_lens = h_seg_lens;
   const size_t plan_stage = attn_stage_bytes(n_tok, 1, n_heads, n_kv_heads);
   const int nblk = kv_pages_for(kv_len);
   static thread_local std::vector<uint8_t> stage;
@@ -173,6 +176,30 @@ int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void
                n_kv_heads, head_dim, st))
     return -1;
   VLO_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
+                                  int n_pages, void* d_out, int n_segs, const int32_t* h_seg_lens, int n_heads,
+                                  int n_kv_heads, int head_dim, int kv_len, void* cuda_stream) {
+  VLO_CHECK(n_pages > 0 && n_kv_heads > 0 && n_heads > 0 && n_heads % n_kv_heads == 0, "attn_segments: sizes");
+  VLO_CHECK(n_segs > 0 && h_seg_lens != nullptr, "attn_segments: need at least one segment");
+  int n_tok = 0;
+  for (int j = 0; j < n_segs; ++j) {
+    VLO_CHECK(h_seg_lens[j] > 0, "attn_segments: segment lengths must be positive");
+    n_tok += h_seg_lens[j];
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  OpScratch ws;  // sized for the plan's segments: the caller's query of vlo_op_attn_ws_bytes does not know them
+  VLO_CUDA(cudaMalloc(&ws.p, attn_ws_bytes(n_tok, 1, n_heads, n_kv_heads)));
+  AttnPlan plan{};
+  if (op_attn_plan(&plan, ws.p, n_tok, n_heads, n_kv_heads, head_dim, kv_len, false, nullptr, st, n_segs, h_seg_lens))
+    return -1;
+  const long long page_rows = static_cast<long long>(n_kv_heads) * kKvPageTokens;
+  if (attn_run(plan, d_q, d_k_pool, d_v_pool, n_pages * page_rows, d_page_table, page_rows, kKvPageTokens, d_out, n_heads,
+               n_kv_heads, head_dim, st))
+    return -1;
+  VLO_CUDA(cudaStreamSynchronize(st));  // the workspace is freed on return
   return 0;
 }
 

@@ -167,6 +167,10 @@ struct AttnSeq {
   int q_len;           // new tokens
   int kv_len;          // cache length INCLUDING the new tokens
   int pt0;             // entry of the page table holding the page of key block 0 (ceil(kv_len / 64) entries follow)
+  // > 1: the q_len rows are n_segs consecutive segments of seg_lens[j] rows (host array), each planned exactly as a
+  // one-sequence step of that segment alone over the keys up to its end (attn_plan); 0 or 1: one segment
+  int n_segs;
+  const int* seg_lens;
 };
 // bytes of scratch attn_launch needs for these sequences (upper bound)
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads);
@@ -179,6 +183,11 @@ struct AttnPlan {
   int n_items, max_splits, total_tokens;
   int max_blocks_per_split;  // sizes the page-table staging of the launch
   int blk;            // keys per pipeline block
+  // Items [n_plain, n_items) belong to clusters (attn_kvappend_cluster_kernel): n_clusters tables of cluster_size
+  // members at d_clusters, max_cluster_splits splits.  n_plain == n_items when no segmented sequence has two items of
+  // the same split grid.
+  int n_plain, n_clusters, cluster_size, max_cluster_splits;
+  void* d_clusters;
   int skip_merge;     // measurement only: launch the main kernel without the split-KV merge
   double algo_bytes;  // algorithmic HBM bytes of one attn_run over this plan (K+V rows read, Q read, out written)
 };

@@ -396,12 +396,14 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   if (dev_alloc_t(e, &e->kv_op_pt, static_cast<size_t>(2) * per_stream)) return -1;
   if (dev_alloc_t(e, &e->h, static_cast<size_t>(T) * H)) return -1;
   if (dev_alloc_t(e, &e->xn, static_cast<size_t>(T) * H)) return -1;
-  if (dev_alloc_t(e, &e->xn_last, static_cast<size_t>(c.max_streams) * H)) return -1;
+  // decision rows: one per sequence, or one per segment of a segmented step (each segment holds >= 1 of the T tokens)
+  const int rows = std::max(c.max_streams, T);
+  if (dev_alloc_t(e, &e->xn_last, static_cast<size_t>(rows) * H)) return -1;
   if (dev_alloc_t(e, &e->q, static_cast<size_t>(T) * c.num_heads * c.head_dim)) return -1;
   if (dev_alloc_t(e, &e->attn_out, static_cast<size_t>(T) * c.num_heads * c.head_dim)) return -1;
   if (dev_alloc_t(e, &e->act, static_cast<size_t>(T) * c.intermediate_size)) return -1;
-  if (dev_alloc_t(e, &e->logits, static_cast<size_t>(c.max_streams) * c.vocab_size)) return -1;
-  if (dev_alloc_t(e, &e->decisions, static_cast<size_t>(c.max_streams))) return -1;
+  if (dev_alloc_t(e, &e->logits, static_cast<size_t>(rows) * c.vocab_size)) return -1;
+  if (dev_alloc_t(e, &e->decisions, static_cast<size_t>(rows))) return -1;
   const int widest = std::max(std::max(e->qkv_width, 2 * c.intermediate_size), H);
   e->part_elems = static_cast<size_t>(8) * T * widest;  // stream-K needs <= kb/floor(U/G) + 2 planes (<= 4 in practice)
   if (dev_alloc_t(e, &e->part, e->part_elems)) return -1;
@@ -831,25 +833,40 @@ int vlo_embed_tokens(vlo_engine* e, const int64_t* d_ids, int n, void* d_out, vo
   return 0;
 }
 
-int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_q_lens,
-                 const int64_t* d_row_ids, const void* d_embeds, void* d_last_logits, vlo_decision* d_decisions,
-                 int interval_id, void* cuda_stream) {
+namespace {
+
+// The decoder step.  Sequence i carries h_seg_counts[i] consecutive segments (h_seg_counts == NULL: one each) whose
+// lengths follow one another in h_seg_lens; one lm_head row and one decision per segment, read at its last row.
+int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_seg_counts,
+                  const int32_t* h_seg_lens, const int64_t* d_row_ids, const void* d_embeds, void* d_last_logits,
+                  vlo_decision* d_decisions, int interval_id, cudaStream_t st) {
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
   const vlo_config& c = e->cfg;
   VLO_CHECK(n_seqs > 0 && n_seqs <= c.max_streams, "step: n_seqs out of range");
-  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  VLO_CHECK(h_stream_ids != nullptr && h_seg_lens != nullptr, "step: null argument");
   const int H = c.hidden_size;
-  int T = 0;
+  int T = 0, n_rows = 0;
+  std::vector<int> q_lens(n_seqs), seg0(n_seqs);  // seg0[i]: index of sequence i's first segment
   for (int i = 0; i < n_seqs; ++i) {
     if (check_stream(e, h_stream_ids[i])) return -1;
     for (int j = 0; j < i; ++j) VLO_CHECK(h_stream_ids[j] != h_stream_ids[i], "step: a stream appears twice in one batch");
-    VLO_CHECK(h_q_lens[i] > 0, "step: q_len must be positive");
-    VLO_CHECK(e->kv_len[h_stream_ids[i]] + h_q_lens[i] <= c.max_kv_tokens,
+    const int n_segs = h_seg_counts ? h_seg_counts[i] : 1;
+    VLO_CHECK(n_segs > 0, "step: a sequence needs at least one segment");
+    seg0[i] = n_rows;
+    for (int j = 0; j < n_segs; ++j) {
+      const int32_t q_len = h_seg_lens[n_rows + j];
+      VLO_CHECK(q_len > 0, "step: q_len and segment lengths must be positive");
+      q_lens[i] += q_len;
+    }
+    n_rows += n_segs;
+    VLO_CHECK(e->kv_len[h_stream_ids[i]] + q_lens[i] <= c.max_kv_tokens,
               "step: KV cache capacity exceeded for stream " + std::to_string(h_stream_ids[i]));
-    T += h_q_lens[i];
+    T += q_lens[i];
   }
+  // every segment holds at least one token, so the n_rows <= T decision rows fit the buffers sized in engine_init
   VLO_CHECK(T <= c.max_step_tokens, "step: total new tokens exceed max_step_tokens");
+  const int32_t* h_q_lens = q_lens.data();
   // ---- pages for the new tokens, taken before anything is enqueued; a short pool fails with no stream changed
   {
     int need = 0;
@@ -886,13 +903,18 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   int t = 0;
   for (int i = 0; i < n_seqs; ++i) {
     const int sid = h_stream_ids[i], ql = h_q_lens[i], past = e->kv_len[sid];
+    const int n_segs = h_seg_counts ? h_seg_counts[i] : 1;
     first_rows[i] = t;
     for (int j = 0; j < ql; ++j) {
       tok_pos[t + j] = past + j;
       tok_kvrow[t + j] = e->pool.row(sid, past + j);
-      last_index[t + j] = (j == ql - 1) ? i : -1;
+      last_index[t + j] = -1;
     }
-    seqs[i] = AttnSeq{t, ql, past + ql, pt0[i]};
+    for (int s = 0, end = 0; s < n_segs; ++s) {  // the decision row of each segment sits at its last token
+      end += h_seg_lens[seg0[i] + s];
+      last_index[t + end - 1] = seg0[i] + s;
+    }
+    seqs[i] = AttnSeq{t, ql, past + ql, pt0[i], n_segs, h_seg_lens + seg0[i]};
     t += ql;
   }
   VLO_CUDA(cudaMemcpyAsync(e->meta_dev, hs, e->meta.pt + sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
@@ -940,11 +962,11 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
     if (dec_partial(e, d.down, H, e->act, T, c.intermediate_size, &sk, st)) return -1;
     if (resid_norm(&sk, is_last ? e->final_norm : e->dec[l + 1].in_norm, is_last)) return -1;
   }
-  // ---- last-position lm_head + on-device decision
+  // ---- last-position lm_head + on-device decision (one row per segment)
   bf16* logits = d_last_logits ? static_cast<bf16*>(d_last_logits) : e->logits;
-  if (gemm_ws_store16(FMT_BF16, e->lm_head, c.vocab_size, e->xn_last, n_seqs, H, logits, c.vocab_size, nullptr, ACT_NONE, st))
+  if (gemm_ws_store16(FMT_BF16, e->lm_head, c.vocab_size, e->xn_last, n_rows, H, logits, c.vocab_size, nullptr, ACT_NONE, st))
     return -1;
-  if (decision_launch(logits, n_seqs, c.vocab_size, interval_id, d_decisions ? static_cast<void*>(d_decisions) : e->decisions,
+  if (decision_launch(logits, n_rows, c.vocab_size, interval_id, d_decisions ? static_cast<void*>(d_decisions) : e->decisions,
                       st))
     return -1;
 
@@ -952,6 +974,23 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
   rollback.armed = false;
   e->last_step_tokens = T;
   return 0;
+}
+
+}  // namespace
+
+int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_q_lens,
+                 const int64_t* d_row_ids, const void* d_embeds, void* d_last_logits, vlo_decision* d_decisions,
+                 int interval_id, void* cuda_stream) {
+  return step_segments(e, n_seqs, h_stream_ids, nullptr, h_q_lens, d_row_ids, d_embeds, d_last_logits, d_decisions,
+                       interval_id, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_seg_counts,
+                      const int32_t* h_seg_lens, const int64_t* d_row_ids, const void* d_embeds, void* d_seg_logits,
+                      vlo_decision* d_decisions, int interval_id, void* cuda_stream) {
+  VLO_CHECK(h_seg_counts != nullptr, "step_segments: null h_seg_counts");
+  return step_segments(e, n_seqs, h_stream_ids, h_seg_counts, h_seg_lens, d_row_ids, d_embeds, d_seg_logits, d_decisions,
+                       interval_id, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_step(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_q_lens, const void* d_embeds,

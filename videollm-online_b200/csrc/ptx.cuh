@@ -115,6 +115,43 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
+// The same box written at the same shared-memory offset of every CTA of the cluster in cta_mask; each destination's
+// mbarrier at bar's offset receives the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0, int32_t c1,
+                                                      uint16_t cta_mask, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(hint)
+      : "memory");
+}
+
+// ------------------------------------------------------------------ clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_nctarank;\n" : "=r"(r));
+  return r;
+}
+// all threads of all CTAs of the cluster; release / acquire order shared-memory writes (barrier init) across CTAs
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+}
+// arrive on the mbarrier at bar's offset in the shared memory of CTA `rank` of this cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)),
+      "r"(rank)
+      : "memory");
+}
+
 // ---------------------------------------------- programmatic dependent launch (PDL)
 // A kernel launched with the programmatic-stream-serialization attribute may start while its
 // predecessor in the stream is still running; it must execute pdl_wait() before touching anything the

@@ -80,10 +80,11 @@ class Engine:
         with torch.cuda.device(self.index):
             check(self.lib.vlo_engine_create_pooled(C.byref(c), int(kv_pool_tokens or 0), self.index, C.byref(self._h)),
                   "vlo_engine_create_pooled")
-        # device scratch for results (decisions, last logits)
-        self._dec_dev = torch.zeros(max_streams, DECISION_DTYPE_FIELDS, dtype=torch.int32, device=self.device)
-        self._dec_host = torch.zeros(max_streams, DECISION_DTYPE_FIELDS, dtype=torch.int32).pin_memory()
-        self._logits = torch.zeros(max_streams, cfg.vocab_size, dtype=torch.bfloat16, device=self.device)
+        # device scratch for results (decisions, last logits): one row per sequence, or per segment of a segmented step
+        rows = max(max_streams, max_step_tokens)
+        self._dec_dev = torch.zeros(rows, DECISION_DTYPE_FIELDS, dtype=torch.int32, device=self.device)
+        self._dec_host = torch.zeros(rows, DECISION_DTYPE_FIELDS, dtype=torch.int32).pin_memory()
+        self._logits = torch.zeros(rows, cfg.vocab_size, dtype=torch.bfloat16, device=self.device)
 
     # ------------------------------------------------------------------ life cycle
     def close(self):
@@ -202,31 +203,61 @@ class Engine:
 
     def step(self, stream_ids: Sequence[int], q_lens: Sequence[int], embeds: torch.Tensor, *,
              row_ids: Optional[torch.Tensor] = None, interval_id: Optional[int] = None,
-             want_logits: bool = True):
+             want_logits: bool = True, segments: Optional[Sequence[Sequence[int]]] = None):
         """KV-append forward of a ragged batch.  `row_ids` (int64 [sum q_lens], optional): id >= 0 -> the row is the
         embedding of that token (gathered on the device), id < 0 -> the row of `embeds` is used as is.  Returns (logits [n_seqs, V] bf16 view or None, decisions
-        device tensor int32 [n_seqs, 8]).  Nothing is synchronised; call `read_decisions` for host values."""
+        device tensor int32 [n_seqs, 8]).  Nothing is synchronised; call `read_decisions` for host values.
+
+        `segments` (optional): per sequence, the lengths of the consecutive segments its q_len rows are made of (they
+        must add up to q_lens[i]).  Then there is one logits row and one decision per segment, in order, read at the
+        segment's last row ([n_segments, V] / [n_segments, 8]), and every segment computes the bits the same rows get
+        from a step of their own (vlo_step_segments).  A segmented step longer than max_step_tokens is an error."""
         n = len(stream_ids)
         T = int(sum(q_lens))
         embeds = embeds.contiguous()
+        if segments is not None:
+            return self._step_segments(stream_ids, q_lens, segments, embeds, row_ids, interval_id, want_logits)
         if T > self.max_step_tokens:
             return self._step_chunked(stream_ids, q_lens, embeds, row_ids, interval_id, want_logits)
-        if embeds.dtype != torch.bfloat16 or embeds.device != self.device or embeds.numel() != T * self.cfg.hidden_size:
-            raise VloError(f"step: embeds must be bf16 [{T},{self.cfg.hidden_size}] on {self.device}")
+        iid, pid = self._step_inputs(T, embeds, row_ids, interval_id)
         sid = (C.c_int32 * n)(*stream_ids)
         ql = (C.c_int32 * n)(*q_lens)
+        logits = self._logits[:n] if want_logits else None
+        check(self.lib.vlo_step_ids(self._h, n, sid, ql, _ptr(pid), _ptr(embeds), _ptr(logits), _ptr(self._dec_dev), iid,
+                                    self._stream()), "vlo_step")
+        return logits, self._dec_dev[:n]
+
+    def _step_inputs(self, T, embeds, row_ids, interval_id):
+        """(interval id, device row ids or None) of a step over T packed rows, after checking the inputs"""
+        if embeds.dtype != torch.bfloat16 or embeds.device != self.device or embeds.numel() != T * self.cfg.hidden_size:
+            raise VloError(f"step: embeds must be bf16 [{T},{self.cfg.hidden_size}] on {self.device}")
         iid = self.cfg.frame_token_interval_id if interval_id is None else interval_id
         if iid is None:
             iid = -1
-        logits = self._logits[:n] if want_logits else None
         pid = None
         if row_ids is not None:
             pid = row_ids.to(device=self.device, dtype=torch.int64).contiguous().view(-1)
             if pid.numel() != T:
                 raise VloError(f"step: row_ids must have one entry per packed row ({T}), got {pid.numel()}")
-        check(self.lib.vlo_step_ids(self._h, n, sid, ql, _ptr(pid), _ptr(embeds), _ptr(logits), _ptr(self._dec_dev), iid,
-                                    self._stream()), "vlo_step")
-        return logits, self._dec_dev[:n]
+        return iid, pid
+
+    def _step_segments(self, stream_ids, q_lens, segments, embeds, row_ids, interval_id, want_logits):
+        n, T = len(stream_ids), int(sum(q_lens))
+        if len(segments) != n or any(sum(s) != q for s, q in zip(segments, q_lens)):
+            raise VloError("step: segments must give each sequence segment lengths that add up to its q_len")
+        if T > self.max_step_tokens:
+            raise VloError(f"step: a segmented step of {T} tokens exceeds max_step_tokens ({self.max_step_tokens}); "
+                           "segmented steps are not chunked")
+        iid, pid = self._step_inputs(T, embeds, row_ids, interval_id)
+        lens = [int(x) for s in segments for x in s]
+        n_rows = len(lens)
+        sid = (C.c_int32 * n)(*stream_ids)
+        counts = (C.c_int32 * n)(*[len(s) for s in segments])
+        sl = (C.c_int32 * n_rows)(*lens)
+        logits = self._logits[:n_rows] if want_logits else None
+        check(self.lib.vlo_step_segments(self._h, n, sid, counts, sl, _ptr(pid), _ptr(embeds), _ptr(logits),
+                                         _ptr(self._dec_dev), iid, self._stream()), "vlo_step_segments")
+        return logits, self._dec_dev[:n_rows]
 
     def _step_chunked(self, stream_ids, q_lens, embeds, row_ids, interval_id, want_logits):
         """Inputs longer than max_step_tokens (the first frame's system prompt, long queries): feed the KV-append

@@ -7,11 +7,15 @@ demo/cli.py and demo/app.py can drive it unchanged.  Differences, all behind the
   * the speak/silent decision and the greedy argmax are computed on the device; one 32-byte read-back
     per frame / generated token replaces the reference's two tensor-`if` syncs (demo/inference.py:77,80);
   * the steady-state frame step feeds [interval-token id | 10 frame embeddings] and lets the engine gather
-    the token row, so no separate embedding launch or torch.cat is needed.
+    the token row, so no separate embedding launch or torch.cat is needed;
+  * queued frames (a clip processed faster than real time, a seek, a stalled feed) go through one segmented step
+    [prefix | F1 | interval | F2 | ...] with one decision per frame, the same bits as one step per frame; where a
+    frame speaks or a query is due the stream is cut back to that frame and the rest is queued again.
 """
 from __future__ import annotations
 
 import collections
+import itertools
 import logging
 import threading
 from dataclasses import asdict
@@ -174,23 +178,48 @@ class LiveInfer:
             return self._forward_locked(ids, frame_embeds)
 
     def _forward_locked(self, ids: torch.Tensor, frame_embeds: torch.Tensor = None):
+        self._enqueue_step(ids, [] if frame_embeds is None else [frame_embeds])
+        return self._consume(self.model.engine.read_decisions(1)[0])
+
+    def _consume(self, dec):
+        """a decision the session acts on: the test seam sees it and it counts as one call"""
+        if self.decision_hook is not None:
+            dec = self.decision_hook(dec, self._n_calls)
+        self._n_calls += 1
+        return dec
+
+    def _enqueue_step(self, ids: torch.Tensor, frames):
+        """Enqueue one KV-append step over [embed(ids) ; frames[0] ; interval id ; frames[1] ; interval id ; ...].
+        With more than one frame every frame is a segment with its own decision (the step is the same arithmetic as
+        one step per frame, each fed the interval id of a silent predecessor).  Returns the segment lengths."""
         eng = self.model.engine
         id_list = [int(x) for x in ids.reshape(-1).tolist()]
         n_ids = len(id_list)
-        n_fr = 0 if frame_embeds is None else frame_embeds.shape[0]
+        n_frs = tuple(f.shape[0] for f in frames)
+        n_fr = sum(n_frs) + len(frames) - 1 if frames else 0   # rows after the prefix ids
         T = n_ids + n_fr
+        segs = [n_ids + n_frs[0]] + [1 + n for n in n_frs[1:]] if frames else [T]
         # pre-allocated step buffers: no per-step torch.empty / torch.cat / pageable H2D on the hot path
         if T > self._packed.shape[0]:
             self._alloc_step_buffers(2 * T)
         packed = self._packed[:T]
-        if n_fr:
-            packed[n_ids:] = frame_embeds.view(-1, self.hidden_size)
-        key = (tuple(id_list), n_fr)
+        o = n_ids
+        for j, f in enumerate(frames):
+            o += j > 0          # the interval id row, gathered on the device
+            packed[o:o + f.shape[0]] = f.view(-1, self.hidden_size)
+            o += f.shape[0]
+        key = (tuple(id_list), n_frs)
         row_ids = self._row_ids_cache.get(key) if n_fr else None   # steady state: [interval id | 10 frame rows]
         if row_ids is None:
             host = self._row_ids_host[:T]
             host[:n_ids] = torch.tensor(id_list, dtype=torch.int64)
             host[n_ids:] = -1
+            o = n_ids
+            for j, n in enumerate(n_frs):
+                if j:
+                    host[o] = self.frame_token_interval_id
+                    o += 1
+                o += n
             if n_fr:    # frame steps repeat (same prefix ids): keep their device copy
                 row_ids = host.to(self.device, non_blocking=True)
                 if len(self._row_ids_cache) < 64:
@@ -203,7 +232,8 @@ class LiveInfer:
         if self._want_prefetch is not None:
             pre = torch.cuda.Event()
             pre.record(main)
-        eng.step([self._kv.stream_id], [T], packed, row_ids=row_ids)   # token rows gathered on the device
+        eng.step([self._kv.stream_id], [T], packed, row_ids=row_ids,   # token rows gathered on the device
+                 segments=[segs] if len(frames) > 1 else None)
         self.past_key_values = self._kv
         if pre is not None:
             # encode-ahead of the next frame, enqueued AFTER the step's launches (the host is the critical path right
@@ -218,11 +248,7 @@ class LiveInfer:
             for k, e in zip(range(nxt, stop), pe):
                 self._prefetched[k] = (e, ev)
             self._prefetch_event = ev
-        dec = eng.read_decisions(1)[0]
-        if self.decision_hook is not None:
-            dec = self.decision_hook(dec, self._n_calls)
-        self._n_calls += 1
-        return dec
+        return segs
 
     def _call_for_response(self, video_time, query):
         if query is not None:
@@ -252,11 +278,17 @@ class LiveInfer:
             if self.query_queue and self.frame_embeds_queue[0][0] > self.query_queue[0][0]:
                 video_time, query = self.query_queue.popleft()
                 return video_time, query
-            video_time, frame_embeds = self.frame_embeds_queue.popleft()
             if not self.past_key_values:
                 self.last_ids = self._start_ids
             elif int(self.last_ids.reshape(-1)[-1]) == self.eos_token_id and self.last_ids.numel() == 1:
                 self.last_ids = torch.cat([self.last_ids.reshape(1, -1), self._added_stream_prompt_ids], dim=1)
+            n = self._backlog_run()
+            if n > 1:
+                video_time, query, answered = self._stream_backlog(n)
+                if answered:
+                    return video_time, query
+                continue
+            video_time, frame_embeds = self.frame_embeds_queue.popleft()
             dec = self._forward(self.last_ids, frame_embeds)
             # 2. a query due at this frame's time is answered right after the frame
             if self.query_queue and video_time >= self.query_queue[0][0]:
@@ -268,6 +300,63 @@ class LiveInfer:
             if next_id != self.frame_token_interval_id:
                 return video_time, None
         return None, None
+
+    def _backlog_run(self) -> int:
+        """Queued frames (from the head) that one segmented step can take: the loop above would step them one after
+        another, each fed the interval id of a silent predecessor, without a query in between.  So the run stops
+        before a frame that rule 1 would precede, after a frame that rule 2 answers, and at max_step_tokens."""
+        iid, q = self.frame_token_interval_id, self.frame_embeds_queue
+        if iid is None or len(q) < 2:
+            return 1
+        due = self.query_queue[0][0] if self.query_queue else None
+        room = self.model.engine.max_step_tokens - self.last_ids.numel() - q[0][1].shape[0]
+        n, prev = 1, q[0][0]
+        # input_video_stream appends to the queue from another thread under the same lock: a deque may not change
+        # while it is iterated (only this thread pops, so the n frames counted here stay at the head)
+        with self._lock:
+            for video_time, frame_embeds in itertools.islice(q, 1, None):
+                if due is not None and (prev >= due or video_time > due):   # rule 2 after the previous frame / rule 1 before this one
+                    break
+                room -= 1 + frame_embeds.shape[0]
+                if room < 0:
+                    break
+                n, prev = n + 1, video_time
+        return n
+
+    def _stream_backlog(self, n: int):
+        """Step the first n queued frames as one segmented step, then act on their decisions in order exactly as the
+        loop above acts on one frame's.  Where that loop would stop (a frame speaks, or a query is due) the stream is
+        cut back to the end of that frame and the later frames go back to the head of the queue.
+        Returns (video_time, query, stop): stop is False when every frame was silent."""
+        with self._lock:
+            frames = [self.frame_embeds_queue.popleft() for _ in range(n)]
+            eng, sid = self.model.engine, self._kv.stream_id
+            kv0 = eng.kv_len(sid)
+            segs = self._enqueue_step(self.last_ids, [f for _, f in frames])
+            decs = eng.read_decisions(n)
+
+            def take_back(j):   # keep frames [0, j)
+                if j < n:
+                    eng.kv_truncate(sid, kv0 + sum(segs[:j]))
+                    self.frame_embeds_queue.extendleft(reversed(frames[j:]))
+
+            for j, (video_time, _) in enumerate(frames):
+                # 1. a query that is due before this frame is answered first
+                if j and self.query_queue and video_time > self.query_queue[0][0]:
+                    take_back(j)
+                    return (*self.query_queue.popleft(), True)
+                dec = self._consume(decs[j])
+                # 2. a query due at this frame's time is answered right after the frame
+                if self.query_queue and video_time >= self.query_queue[0][0]:
+                    take_back(j + 1)
+                    return (*self.query_queue.popleft(), True)
+                # 3. speak/silent
+                next_id = dec.next_id(self.frame_token_interval_id, self.frame_token_interval_threshold)
+                self.last_ids = torch.tensor([[next_id]], dtype=torch.long)
+                if next_id != self.frame_token_interval_id:
+                    take_back(j + 1)
+                    return video_time, None, True
+            return None, None, False
 
     def __call__(self):
         while not self.frame_embeds_queue:
