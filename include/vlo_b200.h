@@ -224,6 +224,12 @@ int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void
 int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
                                   int n_pages, void* d_out, int n_segs, const int32_t* h_seg_lens, int n_heads,
                                   int n_kv_heads, int head_dim, int kv_len, void* cuda_stream);
+/* The attention plan vlo_op_attn_kvappend_segments (and vlo_step_segments, for one sequence) makes for these segments,
+ * without launching anything: h_counts[0..4) = work items, 2-CTA clusters, packs (runs of consecutive one-token
+ * segments one CTA per (split, kv head) computes in one pass over the cache) and the items inside packs.  Queries the
+ * current device's SM count. */
+int vlo_op_attn_plan_counts(int n_segs, const int32_t* h_seg_lens, int n_heads, int n_kv_heads, int head_dim, int kv_len,
+                            int32_t* h_counts);
 /* The decoder step's fix-up and decision kernels (csrc/decoder_kernels.cuh), launched by the same helpers as vlo_step
  * (block size, grid, shared memory, PDL).  bf16 tensors unless stated; bf16(.) = round to nearest even.
  * d_part: fp32 stream-K partial planes [plane][T][width] as vlo_op_gemm_ws mode 0 leaves them (plane_stride T * width)

@@ -42,7 +42,7 @@ size_t attn_stage_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_head
   (void)n_seqs;
   const int G = n_heads / n_kv_heads;
   return align256(sizeof(AttnItem) * max_items(total_tokens, G)) + align256(sizeof(int) * total_tokens) +
-         align256(sizeof(AttnCluster) * max_items(total_tokens, G));
+         align256(sizeof(AttnCluster) * max_items(total_tokens, G)) + align256(sizeof(AttnPack) * max_items(total_tokens, G));
 }
 
 size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) {
@@ -50,7 +50,7 @@ size_t attn_ws_bytes(int total_tokens, int n_seqs, int n_heads, int n_kv_heads) 
   const size_t slots = cap_slots_for(total_tokens, n_seqs, n_heads, n_kv_heads);
   return align256(slots * kAttnHD * 4) + align256(slots * 2 * 4) +
          align256(sizeof(AttnItem) * max_items(total_tokens, G)) + align256(sizeof(int) * total_tokens) +
-         align256(sizeof(AttnCluster) * max_items(total_tokens, G));
+         align256(sizeof(AttnCluster) * max_items(total_tokens, G)) + align256(sizeof(AttnPack) * max_items(total_tokens, G));
 }
 
 int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, int n_seqs, int total_tokens,
@@ -66,6 +66,7 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   std::vector<AttnItem> items;
   std::vector<int> item_want;  // split budget of each item; 0 = the budget shared by single-segment sequences
   std::vector<int> item_seq;   // segmented sequence of each item, -1 for a single-segment sequence
+  std::vector<char> item_one;  // the item is a one-token segment of a segmented sequence
   std::vector<int> tok_item(total_tokens, 0);
   // rows [q_tok0, q_tok0 + q_len) at positions kv_end - q_len .. kv_end - 1, chunked from the first row
   auto chunk = [&](int q_tok0, int q_len, int kv_end, int pt0, int want, int seq) {
@@ -79,6 +80,7 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
       items.push_back(it);
       item_want.push_back(want);
       item_seq.push_back(seq);
+      item_one.push_back(seq >= 0 && q_len == 1);
     }
   };
   int n_shared = 0;
@@ -134,6 +136,24 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   VLO_CHECK(slots <= cap_slots, "attention workspace plan overflow");
   VLO_CHECK(n_items <= max_items(total_tokens, G), "too many attention work items");
 
+  // Packs: runs of 2 .. per consecutive one-token segments of a sequence whose solo items share the split grid (a run
+  // is cut where n_splits or blocks_per_split change) go to attn_kvappend_packed_kernel, one CTA per (split, kv head)
+  // for the whole run.  Packed items move behind all others, in order.
+  std::vector<AttnPack> packs;
+  std::vector<int> in_pack(n_items, 0);
+  for (int i = 0; i < n_items;) {
+    int j = i + 1;
+    if (item_one[i])
+      while (j < n_items && j - i < per && item_one[j] && item_seq[j] == item_seq[i] &&
+             items[j].n_splits == items[i].n_splits && items[j].blocks_per_split == items[i].blocks_per_split)
+        ++j;
+    if (j - i >= 2) {
+      packs.push_back(AttnPack{i, j - i});
+      for (int k = i; k < j; ++k) in_pack[k] = 1;
+    }
+    i = j;
+  }
+
   // Clusters: the items of one segmented sequence with the same blocks_per_split read the same key blocks of the same
   // pages, so attn_kvappend_cluster_kernel loads each block once for up to kAttnClusterMax of them.  Clustered items
   // move behind the others (the item order changes no result); groups of one stay with attn_kvappend_kernel.
@@ -141,7 +161,7 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   for (int s = 0; s < n_seqs; ++s) {
     std::vector<std::pair<int, std::vector<int>>> by_bps;
     for (int i = 0; i < n_items; ++i) {
-      if (item_seq[i] != s) continue;
+      if (item_seq[i] != s || in_pack[i]) continue;
       auto g = std::find_if(by_bps.begin(), by_bps.end(), [&](const auto& x) { return x.first == items[i].blocks_per_split; });
       if (g == by_bps.end()) by_bps.push_back({items[i].blocks_per_split, {i}});
       else g->second.push_back(i);
@@ -165,15 +185,20 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
     for (int i : g) in_cluster[i] = 1;
   }
   for (int i = 0; i < n_items; ++i)
-    if (!in_cluster[i]) order.push_back(i);
+    if (!in_cluster[i] && !in_pack[i]) order.push_back(i);
   const int n_plain = static_cast<int>(order.size());
-  int max_cluster_splits = 1;
+  int max_cluster_splits = 1, max_pack_splits = 1;
   for (int i = 0; i < n_items; ++i)
     if (in_cluster[i]) {
       order.push_back(i);
       max_cluster_splits = std::max(max_cluster_splits, items[i].n_splits);
     }
-  if (!clusters.empty()) {
+  for (int i = 0; i < n_items; ++i)
+    if (in_pack[i]) {
+      order.push_back(i);
+      max_pack_splits = std::max(max_pack_splits, items[i].n_splits);
+    }
+  if (!clusters.empty() || !packs.empty()) {
     std::vector<int> pos(n_items);
     std::vector<AttnItem> reordered(n_items);
     for (int j = 0; j < n_items; ++j) {
@@ -185,11 +210,20 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
     for (AttnCluster& cl : clusters)
       for (int r = 0; r < kAttnClusterMax; ++r)
         if (cl.item[r] >= 0) cl.item[r] = pos[cl.item[r]];
+    for (AttnPack& pk : packs) pk.item0 = pos[pk.item0];  // a run's items stay consecutive and in order
   }
   plan->n_plain = n_plain;
   plan->n_clusters = static_cast<int>(clusters.size());
   plan->cluster_size = cs;
   plan->max_cluster_splits = max_cluster_splits;
+  plan->n_packs = static_cast<int>(packs.size());
+  plan->n_packed_items = static_cast<int>(std::count(in_pack.begin(), in_pack.end(), 1));
+  plan->max_pack_splits = max_pack_splits;
+  plan->n_items = n_items;
+  plan->max_splits = max_splits;
+  plan->max_blocks_per_split = max_bps;
+  plan->total_tokens = total_tokens;
+  if (d_ws == nullptr) return 0;
 
   // workspace carve-up (same order as attn_ws_bytes)
   uint8_t* w = static_cast<uint8_t*>(d_ws);
@@ -202,10 +236,8 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   plan->d_tok_item = reinterpret_cast<int*>(w);
   w += align256(sizeof(int) * total_tokens);
   plan->d_clusters = w;
-  plan->n_items = n_items;
-  plan->max_splits = max_splits;
-  plan->max_blocks_per_split = max_bps;
-  plan->total_tokens = total_tokens;
+  w += align256(sizeof(AttnCluster) * max_items(total_tokens, G));
+  plan->d_packs = w;
 
   uint8_t* hs = static_cast<uint8_t*>(h_stage);
   std::memcpy(hs, items.data(), sizeof(AttnItem) * n_items);
@@ -213,10 +245,15 @@ int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, in
   std::memcpy(hs2, tok_item.data(), sizeof(int) * total_tokens);
   VLO_CUDA(cudaMemcpyAsync(plan->d_items, hs, sizeof(AttnItem) * n_items, cudaMemcpyHostToDevice, stream));
   VLO_CUDA(cudaMemcpyAsync(plan->d_tok_item, hs2, sizeof(int) * total_tokens, cudaMemcpyHostToDevice, stream));
+  uint8_t* hs3 = hs2 + align256(sizeof(int) * total_tokens);
   if (!clusters.empty()) {
-    uint8_t* hs3 = hs2 + align256(sizeof(int) * total_tokens);
     std::memcpy(hs3, clusters.data(), sizeof(AttnCluster) * clusters.size());
     VLO_CUDA(cudaMemcpyAsync(plan->d_clusters, hs3, sizeof(AttnCluster) * clusters.size(), cudaMemcpyHostToDevice, stream));
+  }
+  if (!packs.empty()) {
+    uint8_t* hs4 = hs3 + align256(sizeof(AttnCluster) * max_items(total_tokens, G));
+    std::memcpy(hs4, packs.data(), sizeof(AttnPack) * packs.size());
+    VLO_CUDA(cudaMemcpyAsync(plan->d_packs, hs4, sizeof(AttnPack) * packs.size(), cudaMemcpyHostToDevice, stream));
   }
   return 0;
 }
@@ -291,7 +328,8 @@ int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void*
   p.scale_log2 = scale_log2;
   const size_t smem = attn_smem_bytes(plan.max_blocks_per_split);
   const bool clustered = plan.n_clusters > 0 && cluster_launch_fits(plan.cluster_size, smem);
-  const int n_plain = clustered ? plan.n_plain : plan.n_items;  // without clusters every item runs alone
+  // without clusters every item but the packed ones runs alone
+  const int n_plain = clustered ? plan.n_plain : plan.n_items - plan.n_packed_items;
   prof_begin(PROF_ATTN, stream, plan.algo_bytes);
   if (n_plain > 0) {
     VLO_CUDA(launch_pdl(attn_kvappend_kernel, dim3(plan.max_splits, n_kv_heads, n_plain), dim3(kAttnThreads), smem, stream,
@@ -316,6 +354,12 @@ int attn_run(const AttnPlan& plan, const void* d_q, const void* d_k, const void*
     cfg.numAttrs = pdl_enabled() ? 2 : 1;
     VLO_CUDA(cudaLaunchKernelEx(&cfg, attn_kvappend_cluster_kernel, tk, tv, p,
                                 static_cast<const AttnCluster*>(plan.d_clusters)));
+    count_launch();
+  }
+  if (plan.n_packs > 0) {
+    if (ensure_max_smem(reinterpret_cast<const void*>(attn_kvappend_packed_kernel), kAttnSmemOptIn)) return -1;
+    VLO_CUDA(launch_pdl(attn_kvappend_packed_kernel, dim3(plan.max_pack_splits, n_kv_heads, plan.n_packs),
+                        dim3(kAttnThreads), smem, stream, tk, tv, p, static_cast<const AttnPack*>(plan.d_packs)));
     count_launch();
   }
   prof_end(stream);

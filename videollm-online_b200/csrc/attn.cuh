@@ -65,10 +65,15 @@ struct AttnParams {
 //   waits on its own.  The MMA warps run the same code on the blocks of their own item and only take part in the ring
 //   protocol on the others; a CTA that is not `active` (its item has no block in this split, or a padding rank) writes
 //   nothing.
-template <bool kCluster>
+// kPacked = true: attn_kvappend_packed_kernel, `it` spans a run of it.q_count consecutive one-token segments whose items
+//   are p.items[item0 ..] and share n_splits and blocks_per_split.  Row r is token r / G of the run, as in a multi-token
+//   item, and it produces the bits of its own segment's item: it skips the key blocks past its own position (its solo
+//   item has none of them; a fully masked block is not a no-op, the rescale FMA need not be exactly 1), and it writes
+//   its partial to that item's slots.
+template <bool kCluster, bool kPacked = false>
 __device__ __forceinline__ void attn_kvappend_cta(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const AttnParams& p,
                                                   const AttnItem& it, int split, int kvh, int nblk_load, bool active,
-                                                  uint32_t rank, uint32_t cs) {
+                                                  uint32_t rank, uint32_t cs, int item0 = 0) {
   const int G = p.n_heads / p.n_kv_heads;
   const int rows = it.q_count * G;
   const int mt_active = (rows + 15) >> 4;  // MMA warps per group that own real rows
@@ -236,7 +241,10 @@ __device__ __forceinline__ void attn_kvappend_cta(const CUtensorMap& tm_k, const
       const float mn0 = fmaxf(m_run[0], mx0), mn1 = fmaxf(m_run[1], mx1);
       const float me0 = (mn0 == -INFINITY) ? 0.f : mn0 * c;
       const float me1 = (mn1 == -INFINITY) ? 0.f : mn1 * c;
-      const float al0 = exp2f(m_run[0] * c - me0), al1 = exp2f(m_run[1] * c - me1);
+      // kPacked: a row past its own last block keeps (m, l, O): its scores are all -inf, so m stays, its P row is 0,
+      // and the rescale is selected to exactly 1 instead of computed
+      const bool in0 = !kPacked || key0 <= lim0, in1 = !kPacked || key0 <= lim1;
+      const float al0 = in0 ? exp2f(m_run[0] * c - me0) : 1.f, al1 = in1 ? exp2f(m_run[1] * c - me1) : 1.f;
       m_run[0] = mn0;
       m_run[1] = mn1;
       float ps0 = 0.f, ps1 = 0.f;
@@ -250,8 +258,9 @@ __device__ __forceinline__ void attn_kvappend_cta(const CUtensorMap& tm_k, const
         pf[nt >> 1][(nt & 1) * 2 + 0] = pack_bf16(p0, p1);
         pf[nt >> 1][(nt & 1) * 2 + 1] = pack_bf16(p2, p3);
       }
-      l_run[0] = l_run[0] * al0 + ps0;
-      l_run[1] = l_run[1] * al1 + ps1;
+      // explicit FMAs (the fusion attn_kvappend_kernel gets): see the warp-group merge below
+      l_run[0] = __fmaf_rn(l_run[0], al0, ps0);
+      l_run[1] = __fmaf_rn(l_run[1], al1, ps1);
 #pragma unroll
       for (int nd = 0; nd < 16; ++nd) {
         o_acc[nd][0] *= al0;
@@ -312,29 +321,45 @@ __device__ __forceinline__ void attn_kvappend_cta(const CUtensorMap& tm_k, const
     const float me0 = (mn0 == -INFINITY) ? 0.f : mn0 * c, me1 = (mn1 == -INFINITY) ? 0.f : mn1 * c;
     const float a0 = exp2f(m_run[0] * c - me0), b0 = exp2f(om0 * c - me0);
     const float a1 = exp2f(m_run[1] * c - me1), b1 = exp2f(om1 * c - me1);
-    const float l0 = l_run[0] * a0 + ol0 * b0, l1 = l_run[1] * a1 + ol1 * b1;
+    // Rounding spelled out: attn_kvappend_kernel computes the first eight rows of an m-tile (r0) without an FMA and the
+    // second eight (r1) with one, as the compiler fused them there.  A packed row must take the form its own one-token
+    // item uses: with G <= 8 that item's rows are all r0 rows.
+    const float l0 = __fadd_rn(__fmul_rn(l_run[0], a0), __fmul_rn(ol0, b0));
+    const float l1 = kPacked && G <= 8 ? __fadd_rn(__fmul_rn(l_run[1], a1), __fmul_rn(ol1, b1))
+                                       : __fmaf_rn(l_run[1], a1, __fmul_rn(ol1, b1));
     const int r0 = mt * 16 + g8, r1 = r0 + 8;
     const size_t slot_base = static_cast<size_t>(it.ws_slot0) +
                              (static_cast<size_t>(kvh) * it.n_splits + split) * rows;
+    // kPacked: row r is row r % G of the one-token item item0 + r / G (G rows per item, the run's n_splits)
+    auto packed_slot = [&](int r) {
+      const int G = p.n_heads / p.n_kv_heads;
+      return static_cast<size_t>(p.items[item0 + r / G].ws_slot0) +
+             (static_cast<size_t>(kvh) * it.n_splits + split) * G + r % G;
+    };
+    size_t pslot0 = 0, pslot1 = 0;
+    if constexpr (kPacked) {
+      if (r0 < rows) pslot0 = packed_slot(r0);
+      if (r1 < rows) pslot1 = packed_slot(r1);
+    }
 #pragma unroll
     for (int nd = 0; nd < 16; ++nd) {
       const float2 x0 = *reinterpret_cast<const float2*>(wo + g8 * kAttnHD + nd * 8 + q4 * 2);
       const float2 x1 = *reinterpret_cast<const float2*>(wo + (g8 + 8) * kAttnHD + nd * 8 + q4 * 2);
       if (r0 < rows)
-        *reinterpret_cast<float2*>(p.ws_o + (slot_base + r0) * kAttnHD + nd * 8 + q4 * 2) =
+        *reinterpret_cast<float2*>(p.ws_o + (kPacked ? pslot0 : slot_base + r0) * kAttnHD + nd * 8 + q4 * 2) =
             make_float2(o_acc[nd][0] * a0 + x0.x * b0, o_acc[nd][1] * a0 + x0.y * b0);
       if (r1 < rows)
-        *reinterpret_cast<float2*>(p.ws_o + (slot_base + r1) * kAttnHD + nd * 8 + q4 * 2) =
+        *reinterpret_cast<float2*>(p.ws_o + (kPacked ? pslot1 : slot_base + r1) * kAttnHD + nd * 8 + q4 * 2) =
             make_float2(o_acc[nd][2] * a1 + x1.x * b1, o_acc[nd][3] * a1 + x1.y * b1);
     }
     if (q4 == 0) {
       if (r0 < rows) {
-        p.ws_ml[(slot_base + r0) * 2] = mn0;
-        p.ws_ml[(slot_base + r0) * 2 + 1] = l0;
+        p.ws_ml[(kPacked ? pslot0 : slot_base + r0) * 2] = mn0;
+        p.ws_ml[(kPacked ? pslot0 : slot_base + r0) * 2 + 1] = l0;
       }
       if (r1 < rows) {
-        p.ws_ml[(slot_base + r1) * 2] = mn1;
-        p.ws_ml[(slot_base + r1) * 2 + 1] = l1;
+        p.ws_ml[(kPacked ? pslot1 : slot_base + r1) * 2] = mn1;
+        p.ws_ml[(kPacked ? pslot1 : slot_base + r1) * 2 + 1] = l1;
       }
     }
   }
@@ -384,6 +409,27 @@ attn_kvappend_cluster_kernel(const __grid_constant__ CUtensorMap tm_k, const __g
   const AttnItem it = p.items[own >= 0 ? own : cl.item[0]];
   attn_kvappend_cta<true>(tm_k, tm_v, p, it, split, blockIdx.z, nblk_load, own >= 0 && split < it.n_splits, rank, cs);
   cluster_sync();  // no CTA leaves while another may still arrive on its barriers
+}
+
+// A run of `count` (2 .. 64 / G) consecutive one-token segments of one sequence: items item0 .. item0 + count - 1, in
+// order, all with the same n_splits and blocks_per_split.
+struct AttnPack {
+  int item0, count;
+};
+
+// grid = (max_pack_splits, n_kv_heads, n_packs); block = kAttnThreads.  One CTA per (split, kv head) reads the run's key
+// blocks once for all of its segments; every row gets the bits of its segment's item run by attn_kvappend_kernel.
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_kvappend_packed_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
+                            const AttnParams p, const AttnPack* packs) {
+  pdl_trigger();
+  // the pack, item and page tables come from the memcpy at the start of the step: readable before the wait
+  const AttnPack pk = packs[blockIdx.z];
+  AttnItem it = p.items[pk.item0];
+  const int split = blockIdx.x;
+  if (split >= it.n_splits) return;
+  it.q_count = pk.count;  // rows of the run: token t at q_tok0 + t, position q_pos0 + t
+  attn_kvappend_cta<false, true>(tm_k, tm_v, p, it, split, blockIdx.y, 0, true, 0, 1, pk.item0);
 }
 
 // out[token, head, :] = sum_s O_s * 2^((m_s - M) c) / sum_s l_s * 2^((m_s - M) c)

@@ -203,6 +203,25 @@ int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const v
   return 0;
 }
 
+int vlo_op_attn_plan_counts(int n_segs, const int32_t* h_seg_lens, int n_heads, int n_kv_heads, int head_dim, int kv_len,
+                            int32_t* h_counts) {
+  VLO_CHECK(n_kv_heads > 0 && n_heads > 0 && n_heads % n_kv_heads == 0, "attn_plan_counts: sizes");
+  VLO_CHECK(n_segs > 0 && h_seg_lens != nullptr && h_counts != nullptr, "attn_plan_counts: null argument");
+  int n_tok = 0;
+  for (int j = 0; j < n_segs; ++j) {
+    VLO_CHECK(h_seg_lens[j] > 0, "attn_plan_counts: segment lengths must be positive");
+    n_tok += h_seg_lens[j];
+  }
+  AttnSeq s{0, n_tok, kv_len, 0, n_segs, h_seg_lens};
+  AttnPlan plan{};
+  if (attn_plan(&plan, nullptr, nullptr, &s, 1, n_tok, n_heads, n_kv_heads, head_dim, nullptr)) return -1;
+  h_counts[0] = plan.n_items;
+  h_counts[1] = plan.n_clusters;
+  h_counts[2] = plan.n_packs;
+  h_counts[3] = plan.n_packed_items;
+  return 0;
+}
+
 int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
                          const int32_t* d_last_index, int T, int H, float eps, void* cuda_stream) {
   // the row is staged in shared memory without an opt-in beyond the default 48 KB

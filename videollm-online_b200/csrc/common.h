@@ -188,11 +188,16 @@ struct AttnPlan {
   // the same split grid.
   int n_plain, n_clusters, cluster_size, max_cluster_splits;
   void* d_clusters;
+  // The last n_packed_items items belong to n_packs runs of one-token segments (attn_kvappend_packed_kernel, tables at
+  // d_packs, max_pack_splits splits); 0 when no sequence has two consecutive one-token segments of one split grid.
+  int n_packs, n_packed_items, max_pack_splits;
+  void* d_packs;
   int skip_merge;     // measurement only: launch the main kernel without the split-KV merge
   double algo_bytes;  // algorithmic HBM bytes of one attn_run over this plan (K+V rows read, Q read, out written)
 };
 // Build the work-item plan on the host and enqueue its upload.  h_stage (>= attn_stage_bytes())
-// must stay untouched until the copies enqueued on `stream` have run.
+// must stay untouched until the copies enqueued on `stream` have run.  d_ws == null: plan only (the counts of *plan),
+// nothing staged or uploaded.
 int attn_plan(AttnPlan* plan, void* d_ws, void* h_stage, const AttnSeq* seqs, int n_seqs, int total_tokens,
               int n_heads, int n_kv_heads, int head_dim, cudaStream_t stream);
 // d_k / d_v: one layer's K / V matrices [kv_rows, 128] bf16; key block b of kv head h of a sequence sits at row

@@ -24,6 +24,7 @@ import torch
 
 from .config import LiveArguments, parse_args
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
+from .speculative import SEP, NgramDrafter, greedy_generate
 
 logger = logging.getLogger("liveinfer")
 
@@ -62,6 +63,10 @@ class LiveInfer:
         # test seam: decision_hook(decision, call_index) -> decision lets a test script the model's choices
         # (random weights never emit the "]\\n" / EOS protocol ids); None in production.
         self.decision_hook = None
+        # drafts for responses: prompt lookup over the session's ids (speculative.py), mirrored with the stream's KV.
+        # A test may substitute its own (sync / extend / propose); None answers one token per step.  Either way the
+        # response ids, the decisions the hook sees and the cache are those of one token per step.
+        self.drafter = NgramDrafter()
         self._n_calls = 0
         # encode-ahead: with a loaded clip the ViT + connector of the NEXT frame run on a side CUDA stream while the
         # decoder works on the current one (same per-frame arithmetic; a live stream delivers the next frame
@@ -106,6 +111,8 @@ class LiveInfer:
         self.video_tensor = None
         self.last_ids = torch.tensor([[]], dtype=torch.long)
         self._kv.engine.stream_reset(self._kv.stream_id)
+        if self.drafter is not None:
+            self.drafter.sync(0)
         self.past_key_values = None
         self._drop_prefetch()
 
@@ -188,17 +195,18 @@ class LiveInfer:
         self._n_calls += 1
         return dec
 
-    def _enqueue_step(self, ids: torch.Tensor, frames):
+    def _enqueue_step(self, ids: torch.Tensor, frames, n_drafts: int = 0):
         """Enqueue one KV-append step over [embed(ids) ; frames[0] ; interval id ; frames[1] ; interval id ; ...].
         With more than one frame every frame is a segment with its own decision (the step is the same arithmetic as
-        one step per frame, each fed the interval id of a silent predecessor).  Returns the segment lengths."""
+        one step per frame, each fed the interval id of a silent predecessor).  n_drafts (no frames): the last n_drafts
+        ids are one-token segments, each with its own decision.  Returns the segment lengths."""
         eng = self.model.engine
         id_list = [int(x) for x in ids.reshape(-1).tolist()]
         n_ids = len(id_list)
         n_frs = tuple(f.shape[0] for f in frames)
         n_fr = sum(n_frs) + len(frames) - 1 if frames else 0   # rows after the prefix ids
         T = n_ids + n_fr
-        segs = [n_ids + n_frs[0]] + [1 + n for n in n_frs[1:]] if frames else [T]
+        segs = [n_ids + n_frs[0]] + [1 + n for n in n_frs[1:]] if frames else [T - n_drafts] + [1] * n_drafts
         # pre-allocated step buffers: no per-step torch.empty / torch.cat / pageable H2D on the hot path
         if T > self._packed.shape[0]:
             self._alloc_step_buffers(2 * T)
@@ -233,8 +241,14 @@ class LiveInfer:
             pre = torch.cuda.Event()
             pre.record(main)
         eng.step([self._kv.stream_id], [T], packed, row_ids=row_ids,   # token rows gathered on the device
-                 segments=[segs] if len(frames) > 1 else None)
+                 segments=[segs] if len(segs) > 1 else None)
         self.past_key_values = self._kv
+        if frames and self.drafter is not None:   # frame rows enter the drafter's history as separators
+            hist = list(id_list)
+            for j, n in enumerate(n_frs):
+                hist += ([self.frame_token_interval_id] if j else []) + [SEP] * n
+            self.drafter.sync(eng.kv_len(self._kv.stream_id) - T)
+            self.drafter.extend(hist)
         if pre is not None:
             # encode-ahead of the next frame, enqueued AFTER the step's launches (the host is the critical path right
             # after a decision read-back) but ordered only behind what preceded the step: it runs concurrently with it
@@ -256,15 +270,16 @@ class LiveInfer:
         else:
             assert int(self.last_ids) == self.stream_end_id, f'{self.last_ids} != {self.stream_end_id}'  # "]\n" closes the frame list
             self.last_ids = self._added_stream_generation_ids
-        ids = self.last_ids
-        n = 0
-        for i in range(self.inplace_output_ids.size(1)):  # fast_greedy_generate, models/modeling_live.py:173-182
-            new_id = self._forward(ids).argmax_id
-            self.inplace_output_ids[0, i] = new_id
-            n = i + 1
-            if new_id == self.eos_token_id:
-                break
-            ids = torch.tensor([[new_id]], dtype=torch.long)
+        ids = [int(x) for x in self.last_ids.reshape(-1).tolist()]
+
+        def step(pending, drafts):
+            with self._lock:
+                self._enqueue_step(torch.tensor(pending + drafts, dtype=torch.long), [], n_drafts=len(drafts))
+        # fast_greedy_generate (models/modeling_live.py:173-182), verifying drafts from the session's history
+        out = greedy_generate(self.model.engine, self._kv.stream_id, step, len(ids), self.inplace_output_ids.size(1),
+                              self.eos_token_id, first_ids=ids, drafter=self.drafter, consume=self._consume)
+        n = len(out)
+        self.inplace_output_ids[0, :n] = torch.tensor(out, dtype=torch.long)
         output_ids = self.inplace_output_ids[:, :n]
         self.last_ids = output_ids[:, -1:].clone()
         if query:
@@ -338,6 +353,8 @@ class LiveInfer:
             def take_back(j):   # keep frames [0, j)
                 if j < n:
                     eng.kv_truncate(sid, kv0 + sum(segs[:j]))
+                    if self.drafter is not None:
+                        self.drafter.sync(kv0 + sum(segs[:j]))
                     self.frame_embeds_queue.extendleft(reversed(frames[j:]))
 
             for j, (video_time, _) in enumerate(frames):

@@ -247,34 +247,48 @@ class LiveLlamaForCausalLM:
                 raise VloError("model(...) is the reference's batch-1 API; use engine.step for ragged batches")
             inputs_embeds = inputs_embeds[0]
         if past_key_values is None:
-            if self._default_stream is None:
-                self._default_stream = self.engine.stream_open()
-            else:
-                self.engine.stream_reset(self._default_stream)
-            past_key_values = StreamKV(self.engine, self._default_stream)
+            past_key_values = self._fresh_default_stream()
         q = inputs_embeds.shape[0]
         logits, dec = self.engine.step([past_key_values.stream_id], [q], inputs_embeds.to(torch.bfloat16))
         return LiveOutput(logits=logits.view(1, 1, -1), past_key_values=past_key_values, decisions=dec)
 
     forward = __call__
 
+    def _fresh_default_stream(self) -> StreamKV:
+        """the stream of a call without past_key_values: opened once, emptied on every such call"""
+        if self._default_stream is None:
+            self._default_stream = self.engine.stream_open()
+        else:
+            self.engine.stream_reset(self._default_stream)
+        return StreamKV(self.engine, self._default_stream)
+
 
 def fast_greedy_generate(*, model: LiveLlamaForCausalLM, inputs_embeds: torch.Tensor, past_key_values: StreamKV,
                          eos_token_id: int, inplace_output_ids: torch.Tensor):
     """models/modeling_live.py:173-182: greedy AR until EOS or the buffer is full.  The argmax is taken
-    on the device; one 32-byte read-back per token replaces the reference's tensor `if` sync."""
+    on the device; one 32-byte read-back per step replaces the reference's tensor `if` sync.  Ids the response
+    has already produced serve as drafts (speculative.py): a step verifies several of them at once, and the ids and
+    the cache are those of one token per step."""
+    from .speculative import NgramDrafter, greedy_generate
     eng = model.engine
-    n = 0
-    for i in range(inplace_output_ids.size(1)):
-        out = model(inputs_embeds=inputs_embeds, past_key_values=past_key_values, use_cache=True)
-        past_key_values = out.past_key_values
-        new_id = eng.read_decisions(1)[0].argmax_id
-        inplace_output_ids[:, i] = new_id
-        n = i + 1
-        if new_id == eos_token_id:
-            break
-        inputs_embeds = model.get_input_embeddings()(torch.tensor([[new_id]], device=eng.device))
-    return inplace_output_ids[:, :n], past_key_values
+    if past_key_values is None:
+        past_key_values = model._fresh_default_stream()
+    sid = past_key_values.stream_id
+    zeros = torch.zeros(eng.max_step_tokens, model.config.hidden_size, dtype=torch.bfloat16, device=eng.device)
+
+    def step(ids, drafts):
+        if ids is None:   # the caller's embeddings
+            model(inputs_embeds=inputs_embeds, past_key_values=past_key_values, use_cache=True)
+            return
+        rows = ids + drafts
+        eng.step([sid], [len(rows)], zeros[:len(rows)], row_ids=torch.tensor(rows, dtype=torch.int64),
+                 segments=[[len(ids)] + [1] * len(drafts)] if drafts else None)
+
+    n_first = inputs_embeds.reshape(-1, model.config.hidden_size).shape[0]
+    ids = greedy_generate(eng, sid, step, n_first, inplace_output_ids.size(1), eos_token_id, drafter=NgramDrafter(),
+                          base=eng.kv_len(sid))
+    inplace_output_ids[:, :len(ids)] = torch.tensor(ids, dtype=inplace_output_ids.dtype)
+    return inplace_output_ids[:, :len(ids)], past_key_values
 
 
 def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None, llm_pretrained: str = None,
