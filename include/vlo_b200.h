@@ -114,6 +114,25 @@ int vlo_kv_fill_synthetic(vlo_engine* e, int stream_id, int n_tokens, uint64_t s
  * 16-byte aligned (the copy moves 16 bytes per thread) */
 int vlo_kv_read(vlo_engine* e, int stream_id, int layer, int is_v, void* d_out, void* cuda_stream);
 int vlo_kv_write(vlo_engine* e, int stream_id, int layer, int is_v, const void* d_in, int n_tokens, void* cuda_stream);
+/* Host images of a stream's cache, so an idle session can give its pages (and stream slot) back and resume later.
+ * Image layout: [page j][layer][K|V][kv_head][64][128] bf16, pages in page-table order; page_bytes = n_kv_heads * 64 *
+ * 128 * 2 (131 072 B for Llama-3-8B).  vlo_kv_image_bytes = ceil(n_tokens / 64) * 2 * num_layers * page_bytes.
+ * The last page of an image also carries that page's rows past n_tokens: stale but finite pool rows, so the pool's
+ * finiteness invariant (csrc/kv_pages.h) survives a round trip.
+ * vlo_kv_swap_out: enqueues on cuda_stream one cudaMemcpy2DAsync per page (2 * num_layers rows of page_bytes at the
+ * pool's plane stride; copy engines only, no kernel) into h_dst (pinned host memory of >= vlo_kv_image_bytes(kv_len)
+ * bytes), then empties the stream: kv_len 0, pages released, slot still open.  The caller orders the copies after the
+ * steps that wrote the stream (usual stream / event rules) and reads h_dst after them.
+ * vlo_kv_swap_in: the stream must be open and empty; takes ceil(n_tokens / 64) pages (or fails with "KV page pool
+ * exhausted" and changes nothing), enqueues the host-to-device copies from h_src (pinned) on cuda_stream and sets
+ * kv_len = n_tokens.
+ * Page reuse is ordered by the engine: pages released by a swap-out stay gated by an event recorded after its copies,
+ * and any later call that takes such a page (a step, vlo_kv_write, vlo_kv_copy_prefix, vlo_kv_fill_synthetic,
+ * vlo_kv_swap_in) makes its own cuda_stream wait on that event (cudaStreamWaitEvent; no host synchronisation).  Gated
+ * pages count as free in vlo_kv_pool_info. */
+int64_t vlo_kv_image_bytes(vlo_engine* e, int n_tokens);
+int vlo_kv_swap_out(vlo_engine* e, int stream_id, void* h_dst, int64_t bytes, void* cuda_stream);
+int vlo_kv_swap_in(vlo_engine* e, int stream_id, const void* h_src, int n_tokens, void* cuda_stream);
 
 /* ------------------------------------------------------------------ hot path
  * vlo_vit_encode replaces LiveMixin.visual_embed (models/modeling_live.py:21-27) =

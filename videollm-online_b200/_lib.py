@@ -67,6 +67,9 @@ SIGNATURES = {
     "vlo_kv_fill_synthetic": (_I, [_P, _I, _I, C.c_uint64, _P]),
     "vlo_kv_read": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_kv_write": (_I, [_P, _I, _I, _I, _P, _I, _P]),
+    "vlo_kv_image_bytes": (C.c_int64, [_P, _I]),
+    "vlo_kv_swap_out": (_I, [_P, _I, _P, C.c_int64, _P]),
+    "vlo_kv_swap_in": (_I, [_P, _I, _P, _I, _P]),
     "vlo_vit_encode": (_I, [_P, _P, _I, _P, _P, _P]),
     "vlo_connector": (_I, [_P, _P, _I, _P, _P]),
     "vlo_embed_tokens": (_I, [_P, _P, _I, _P, _P]),

@@ -63,6 +63,18 @@ struct vlo_engine {
   int* kv_op_pt = nullptr;  // device page tables of the KV copy / fill calls (two streams' worth)
   std::vector<int> kv_len;
   std::vector<char> stream_open;
+  // Pages released by vlo_kv_swap_out sit on the free list while the swap-out's device-to-host copies may still read
+  // them: page_gate[p] is the gate (an event recorded after those copies) page p waits for, or -1.  A call that takes a
+  // gated page makes its stream wait on the event; a gate whose event has completed releases its pages for good.
+  struct KvGate {
+    cudaEvent_t ev = nullptr;
+    std::vector<int> pages;
+    bool live = false;
+  };
+  std::vector<KvGate> gates;
+  std::vector<int> page_gate;
+  int live_gates = 0;
+  size_t max_pitch = 0;  // cudaDevAttrMaxPitch: the plane stride of a swap's 2D copies must not exceed it
 
   // decoder workspaces
   bf16 *h = nullptr, *xn = nullptr, *xn_last = nullptr, *q = nullptr, *attn_out = nullptr, *act = nullptr,
@@ -272,6 +284,47 @@ int check_stream(vlo_engine* e, int sid) {
   return 0;
 }
 
+// Release the gates whose swap-out copies have completed: their pages are ordinary free (or taken) pages again.
+int retire_gates(vlo_engine* e) {
+  for (size_t g = 0; g < e->gates.size() && e->live_gates > 0; ++g) {
+    vlo_engine::KvGate& gate = e->gates[g];
+    if (!gate.live) continue;
+    const cudaError_t q = cudaEventQuery(gate.ev);
+    if (q == cudaErrorNotReady) continue;
+    VLO_CUDA(q);
+    for (int p : gate.pages)
+      if (e->page_gate[p] == static_cast<int>(g)) e->page_gate[p] = -1;
+    gate.pages.clear();
+    gate.live = false;
+    --e->live_gates;
+  }
+  return 0;
+}
+
+// Stream st is about to write the pages stream sid holds from table entry `from` on (just taken from the pool): make
+// it wait for the swap-out copies that may still read any of them.  No gate alive: nothing is enqueued.
+int wait_taken_pages(vlo_engine* e, int sid, size_t from, cudaStream_t st) {
+  if (e->live_gates == 0) return 0;
+  if (retire_gates(e)) return -1;
+  const std::vector<int>& tab = e->pool.tables[sid];
+  std::vector<char> waited(e->gates.size(), 0);
+  for (size_t j = from; j < tab.size(); ++j) {
+    const int g = e->page_gate[tab[j]];
+    if (g < 0 || waited[g]) continue;
+    VLO_CUDA(cudaStreamWaitEvent(st, e->gates[g].ev, 0));
+    waited[g] = 1;
+  }
+  return 0;
+}
+
+// pages stream sid holds: the table entry of the first page a call that grows the stream takes
+inline size_t table_size(const vlo_engine* e, int sid) { return e->pool.tables[sid].size(); }
+
+// bytes of one page in one layer's K or V matrix
+inline size_t kv_page_bytes(const vlo_engine* e) {
+  return static_cast<size_t>(e->pool.page_stride_rows()) * e->cfg.head_dim * sizeof(bf16);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------ decoder fix-up and decision launches
@@ -391,6 +444,10 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
                                            : static_cast<int64_t>(c.max_streams) * per_stream;
   VLO_CHECK(pages * c.num_kv_heads * kKvPageTokens < (1ll << 31), "KV pool too large for one TMA map per layer");
   e->pool.init(c.max_streams, c.num_kv_heads, static_cast<int>(pages));
+  e->page_gate.assign(static_cast<size_t>(pages), -1);
+  int max_pitch = 0;
+  VLO_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, e->device));
+  e->max_pitch = static_cast<size_t>(max_pitch);
   const size_t kv_elems = static_cast<size_t>(c.num_layers) * 2 * e->pool.rows_per_layer() * c.head_dim;
   if (dev_alloc_t(e, &e->kv, kv_elems, true)) return -1;
   if (dev_alloc_t(e, &e->kv_op_pt, static_cast<size_t>(2) * per_stream)) return -1;
@@ -459,6 +516,8 @@ int vlo_engine_destroy(vlo_engine* e) {
   if (e->stage) cudaFreeHost(e->stage);
   for (int i = 0; i < kStageSlots; ++i)
     if (e->stage_events[i]) cudaEventDestroy(e->stage_events[i]);
+  for (auto& g : e->gates)
+    if (g.ev) cudaEventDestroy(g.ev);
   delete e;
   return 0;
 }
@@ -589,10 +648,12 @@ int vlo_kv_fill_synthetic(vlo_engine* e, int sid, int n_tokens, uint64_t seed, v
   if (check_stream(e, sid)) return -1;
   const vlo_config& c = e->cfg;
   VLO_CHECK(n_tokens >= 0 && n_tokens <= c.max_kv_tokens, "kv_fill: n_tokens out of range");
+  const size_t had = table_size(e, sid);
   if (e->pool.resize(sid, n_tokens)) return -1;
   e->kv_len[sid] = n_tokens;
   if (n_tokens == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  if (wait_taken_pages(e, sid, had, st)) return -1;
   const int* d_pt;
   if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
   kv_fill_kernel<<<dim3(std::min(64, (n_tokens * 128 + 255) / 256), c.num_kv_heads, 2 * c.num_layers), 256, 0, st>>>(
@@ -630,9 +691,11 @@ int vlo_kv_write(vlo_engine* e, int sid, int layer, int is_v, const void* d_in, 
   VLO_CHECK(layer >= 0 && layer < c.num_layers, "layer out of range");
   VLO_CHECK(n_tokens > 0 && n_tokens <= c.max_kv_tokens, "kv_write: n_tokens out of range");
   VLO_CHECK((reinterpret_cast<uintptr_t>(d_in) & 15) == 0, "kv_write: d_in must be 16-byte aligned");
+  const size_t had = table_size(e, sid);
   if (e->pool.resize(sid, n_tokens)) return -1;
   e->kv_len[sid] = n_tokens;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  if (wait_taken_pages(e, sid, had, st)) return -1;
   const int* d_pt;
   if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
   return launch_kv_copy(KvSide{static_cast<bf16*>(const_cast<void*>(d_in)), nullptr, 0, n_tokens},
@@ -654,11 +717,93 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, vo
   e->kv_len[dst_sid] = n_tokens;
   if (n_tokens == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  if (wait_taken_pages(e, dst_sid, 0, st)) return -1;
   const int sids[2] = {src_sid, dst_sid};
   const int* d_pt[2];
   if (upload_op_tables(e, 2, sids, d_pt, st)) return -1;
   return launch_kv_copy(kv_paged_side(e, e->kv, d_pt[0]), kv_paged_side(e, e->kv, d_pt[1]), c.num_kv_heads, n_tokens,
                         2 * c.num_layers, st);
+}
+
+// ------------------------------------------------------------------------------ host images of a stream's cache
+// One cudaMemcpy2DAsync per page moves the page's 2L planes (K and V of every layer, each at the plane stride of the
+// pool) to or from `kv_page_bytes x 2L` contiguous host bytes: copy engines only, no SM is taken from other streams.
+namespace {
+int swap_copies(vlo_engine* e, int sid, uint8_t* h, bool to_host, cudaStream_t st) {
+  const size_t pb = kv_page_bytes(e), pitch = kv_plane_elems(e) * sizeof(bf16);
+  const size_t planes = static_cast<size_t>(2) * e->cfg.num_layers;
+  VLO_CHECK(pitch <= e->max_pitch, "kv swap: the pool's plane stride (" + std::to_string(pitch) +
+                                       " B) exceeds the device's maximum copy pitch");
+  const std::vector<int>& tab = e->pool.tables[sid];
+  for (size_t j = 0; j < tab.size(); ++j) {
+    uint8_t* dev = reinterpret_cast<uint8_t*>(e->kv) + static_cast<size_t>(tab[j]) * pb;
+    uint8_t* host = h + j * planes * pb;
+    if (to_host)
+      VLO_CUDA(cudaMemcpy2DAsync(host, pb, dev, pitch, pb, planes, cudaMemcpyDeviceToHost, st));
+    else
+      VLO_CUDA(cudaMemcpy2DAsync(dev, pitch, host, pb, pb, planes, cudaMemcpyHostToDevice, st));
+  }
+  return 0;
+}
+
+int check_pinned(const void* h, const char* what) {
+  cudaPointerAttributes a{};
+  VLO_CUDA(cudaPointerGetAttributes(&a, h));
+  VLO_CHECK(a.type == cudaMemoryTypeHost, std::string(what) + ": the host image must be pinned (page-locked) memory");
+  return 0;
+}
+}  // namespace
+
+int64_t vlo_kv_image_bytes(vlo_engine* e, int n_tokens) {
+  if (e == nullptr || n_tokens < 0) return -1;
+  return static_cast<int64_t>(kv_pages_for(n_tokens)) * 2 * e->cfg.num_layers * static_cast<int64_t>(kv_page_bytes(e));
+}
+
+int vlo_kv_swap_out(vlo_engine* e, int sid, void* h_dst, int64_t bytes, void* cuda_stream) {
+  DevGuard dev_guard(e);
+  if (check_stream(e, sid)) return -1;
+  const int n = e->kv_len[sid];
+  if (n == 0) return 0;
+  VLO_CHECK(h_dst != nullptr && bytes >= vlo_kv_image_bytes(e, n),
+            "kv_swap_out: the host image needs " + std::to_string(vlo_kv_image_bytes(e, n)) + " bytes");
+  if (check_pinned(h_dst, "kv_swap_out")) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  if (swap_copies(e, sid, static_cast<uint8_t*>(h_dst), true, st)) return -1;
+  if (retire_gates(e)) return -1;
+  size_t g = 0;
+  while (g < e->gates.size() && e->gates[g].live) ++g;
+  if (g == e->gates.size()) {
+    e->gates.emplace_back();
+    VLO_CUDA(cudaEventCreateWithFlags(&e->gates[g].ev, cudaEventDisableTiming));
+  }
+  vlo_engine::KvGate& gate = e->gates[g];
+  VLO_CUDA(cudaEventRecord(gate.ev, st));
+  gate.pages = e->pool.tables[sid];
+  gate.live = true;
+  ++e->live_gates;
+  for (int p : gate.pages) e->page_gate[p] = static_cast<int>(g);
+  e->pool.resize(sid, 0);
+  e->kv_len[sid] = 0;
+  return 0;
+}
+
+int vlo_kv_swap_in(vlo_engine* e, int sid, const void* h_src, int n_tokens, void* cuda_stream) {
+  DevGuard dev_guard(e);
+  if (check_stream(e, sid)) return -1;
+  VLO_CHECK(e->kv_len[sid] == 0, "kv_swap_in: the stream must be empty (kv_len " + std::to_string(e->kv_len[sid]) + ")");
+  VLO_CHECK(n_tokens >= 0 && n_tokens <= e->cfg.max_kv_tokens, "kv_swap_in: n_tokens out of range");
+  if (n_tokens == 0) return 0;
+  VLO_CHECK(h_src != nullptr, "kv_swap_in: null host image");
+  if (check_pinned(h_src, "kv_swap_in")) return -1;
+  if (e->pool.resize(sid, n_tokens)) return -1;  // fails with the pool's message, nothing taken
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  if (wait_taken_pages(e, sid, 0, st) ||
+      swap_copies(e, sid, static_cast<uint8_t*>(const_cast<void*>(h_src)), false, st)) {
+    e->pool.resize(sid, 0);
+    return -1;
+  }
+  e->kv_len[sid] = n_tokens;
+  return 0;
 }
 
 // ------------------------------------------------------------------------------ vision
@@ -875,7 +1020,14 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
       return fail("step: KV page pool exhausted: the step needs " + std::to_string(need) + " more pages of " +
                   std::to_string(kKvPageTokens) + " tokens, " + std::to_string(e->pool.free_pages()) + " of " +
                   std::to_string(e->pool.n_pages) + " are free");
-    for (int i = 0; i < n_seqs; ++i) e->pool.resize(h_stream_ids[i], e->kv_len[h_stream_ids[i]] + h_q_lens[i]);
+    for (int i = 0; i < n_seqs; ++i) {
+      const size_t had = table_size(e, h_stream_ids[i]);
+      e->pool.resize(h_stream_ids[i], e->kv_len[h_stream_ids[i]] + h_q_lens[i]);
+      if (wait_taken_pages(e, h_stream_ids[i], had, st)) {
+        for (int j = 0; j <= i; ++j) e->pool.resize(h_stream_ids[j], e->kv_len[h_stream_ids[j]]);
+        return -1;
+      }
+    }
   }
   // a failure before the lengths are committed gives the pages back: every table stays ceil(kv_len / 64) long
   struct PageRollback {

@@ -6,7 +6,8 @@
 //
 // The host owns the free list and the page tables.  A page handed out may hold stale rows from an earlier owner; they
 // are finite (the pool is zero-filled once, and only finite K / V rows are ever written), which is what a masked key of
-// the attention needs (it contributes 0 x V).
+// the attention needs (it contributes 0 x V).  A host image of a stream (vlo_kv_swap_out / vlo_kv_swap_in) moves
+// whole pages, so a swapped-in last page carries the rows past kv_len that it had in the pool: finite as well.
 #pragma once
 #include <algorithm>
 #include <string>

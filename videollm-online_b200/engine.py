@@ -45,6 +45,38 @@ class Decision:
         return self.argmax_prob_id
 
 
+class KvImage:
+    """A stream's KV cache in pinned host memory (`Engine.kv_swap_out`), to be given back with `Engine.kv_swap_in`.
+
+    `data`: uint8 [vlo_kv_image_bytes(n_tokens)], laid out [page][layer][K|V][kv_head][64][head_dim] bf16.  `layout`:
+    (num_layers, num_kv_heads, head_dim, page_tokens), the config fields that layout depends on.  `event`: recorded
+    after the copy that fills (or last read) `data`; None once the image is complete on the host.  An image survives
+    torch.save / torch.load (the copy is waited for when it is saved, and the data pinned again when it is loaded)."""
+
+    def __init__(self, data: torch.Tensor, n_tokens: int, layout: tuple, event: Optional[torch.cuda.Event] = None):
+        self.data, self.n_tokens, self.layout, self.event = data, int(n_tokens), tuple(layout), event
+
+    def synchronize(self) -> "KvImage":
+        """Wait for the copy into `data`; it may then be read on the host."""
+        if self.event is not None:
+            self.event.synchronize()
+            self.event = None
+        return self
+
+    def __getstate__(self):
+        self.synchronize()
+        return {"data": self.data.cpu(), "n_tokens": self.n_tokens, "layout": list(self.layout)}
+
+    def __setstate__(self, st):
+        data = st["data"]
+        if torch.cuda.is_available() and not data.is_pinned():
+            data = data.pin_memory()
+        self.data, self.n_tokens, self.layout, self.event = data, int(st["n_tokens"]), tuple(st["layout"]), None
+
+
+torch.serialization.add_safe_globals([KvImage])
+
+
 class Engine:
     def __init__(self, cfg: LiveConfig, device: str | torch.device = "cuda:0", *, max_streams: int = 1,
                  max_kv_tokens: int = 16384, max_step_tokens: int = 128, max_vit_batch: int = 8,
@@ -85,6 +117,9 @@ class Engine:
         self._dec_dev = torch.zeros(rows, DECISION_DTYPE_FIELDS, dtype=torch.int32, device=self.device)
         self._dec_host = torch.zeros(rows, DECISION_DTYPE_FIELDS, dtype=torch.int32).pin_memory()
         self._logits = torch.zeros(rows, cfg.vocab_size, dtype=torch.bfloat16, device=self.device)
+        # pinned image buffers a swap copy may still write or read: kept alive until their event has completed, so the
+        # caching host allocator cannot hand them to someone else under a copy
+        self._swap_inflight: List[tuple] = []
 
     # ------------------------------------------------------------------ life cycle
     def close(self):
@@ -161,6 +196,60 @@ class Engine:
         rows = rows.to(device=self.device, dtype=torch.bfloat16).contiguous()
         assert rows.shape[0] == self.cfg.num_key_value_heads and rows.shape[2] == self.cfg.head_dim
         check(self.lib.vlo_kv_write(self._h, sid, layer, int(is_v), _ptr(rows), rows.shape[1], self._stream()), "vlo_kv_write")
+
+    # ------------------------------------------------------------------ host images (swap)
+    def kv_layout(self) -> tuple:
+        """(num_layers, num_kv_heads, head_dim, page_tokens): what the layout of a KvImage depends on"""
+        c = self.cfg
+        return (c.num_hidden_layers, c.num_key_value_heads, c.head_dim, self.kv_pool_info()["page_tokens"])
+
+    def kv_image_bytes(self, n_tokens: int) -> int:
+        return int(self.lib.vlo_kv_image_bytes(self._h, int(n_tokens)))
+
+    def _swap_prune(self):
+        self._swap_inflight = [(d, e) for d, e in self._swap_inflight if not e.query()]
+
+    def _swap_hold(self, data: torch.Tensor, ev: torch.cuda.Event):
+        self._swap_prune()
+        self._swap_inflight.append((data, ev))
+
+    def kv_swap_out(self, sid: int) -> KvImage:
+        """Copy stream `sid`'s cache to pinned host memory on the current CUDA stream and empty the stream (its pages go
+        back to the pool, its slot stays open).  Nothing is synchronised: the image's event marks the copy's end, and
+        the engine orders every later use of the released pages behind it."""
+        n = self.kv_len(sid)
+        nbytes = self.kv_image_bytes(n)
+        self._swap_prune()   # buffers whose copies have ended may be reused by this allocation
+        data = torch.empty(nbytes, dtype=torch.uint8, pin_memory=True)
+        check(self.lib.vlo_kv_swap_out(self._h, sid, _ptr(data) if nbytes else None, nbytes, self._stream()),
+              "vlo_kv_swap_out")
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.device))
+        self._swap_hold(data, ev)
+        return KvImage(data, n, self.kv_layout(), ev)
+
+    def kv_swap_in(self, sid: int, image: KvImage):
+        """Fill the empty stream `sid` from `image` (current CUDA stream, ordered after the image's own copy).  Fails,
+        changing nothing, on a short pool ("KV page pool exhausted"), a non-empty stream, an image of another layout or
+        of the wrong size."""
+        if tuple(image.layout) != self.kv_layout():
+            raise VloError(f"kv_swap_in: the image's layout {tuple(image.layout)} (layers, kv heads, head_dim, page "
+                           f"tokens) differs from this engine's {self.kv_layout()}")
+        want = self.kv_image_bytes(image.n_tokens)
+        data = image.data
+        if data.dtype != torch.uint8 or data.device.type != "cpu" or data.numel() != want:
+            raise VloError(f"kv_swap_in: an image of {image.n_tokens} tokens is {want} bytes of host uint8, got "
+                           f"{data.numel() * data.element_size()} bytes ({data.dtype}, {data.device})")
+        if not data.is_pinned():
+            data = image.data = data.pin_memory()
+        main = torch.cuda.current_stream(self.device)
+        if image.event is not None:
+            main.wait_event(image.event)
+        check(self.lib.vlo_kv_swap_in(self._h, sid, _ptr(data) if want else None, image.n_tokens, self._stream()),
+              "vlo_kv_swap_in")
+        ev = torch.cuda.Event()
+        ev.record(main)
+        self._swap_hold(data, ev)
 
     # ------------------------------------------------------------------ hot path
     def vit_encode(self, frames_u8: torch.Tensor, *, return_vit_tokens: bool = False, connector: bool = True):

@@ -18,15 +18,36 @@ import collections
 import itertools
 import logging
 import threading
-from dataclasses import asdict
+from dataclasses import asdict, dataclass
+from typing import Optional
 
 import torch
 
 from .config import LiveArguments, parse_args
+from .engine import KvImage
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
 from .speculative import SEP, NgramDrafter, greedy_generate
 
 logger = logging.getLogger("liveinfer")
+
+
+@dataclass
+class SessionState:
+    """Everything `LiveInfer.__call__` depends on, as `suspend()` returns it: the KV cache as a host image and the
+    session's host state, with the queued frame embeddings on the host.  Not the video: load it again after resuming.
+    Survives torch.save / torch.load."""
+    kv: KvImage
+    last_ids: torch.Tensor
+    video_time: float
+    last_frame_idx: int
+    query_queue: list            # [(video_time, query)]
+    frame_embeds_queue: list     # [(video_time, bf16 [frame_num_tokens, hidden] on the host)]
+    drafter_ids: Optional[list]  # the NgramDrafter's history (SEP for frame rows), None without one
+    n_calls: int
+    started: bool                # past_key_values was set: a step ran since the last reset
+
+
+torch.serialization.add_safe_globals([SessionState])
 
 
 class LiveInfer:
@@ -115,6 +136,46 @@ class LiveInfer:
             self.drafter.sync(0)
         self.past_key_values = None
         self._drop_prefetch()
+
+    def suspend(self) -> SessionState:
+        """Move the session out of the engine: its KV cache to a pinned host image (its pages go back to the pool) and
+        its queued frames to the host.  The session is then reset and its video dropped; `resume(state)` continues it
+        exactly where it stopped, here or in another process whose model has the same config."""
+        with self._lock:
+            self._drop_prefetch()   # encoded-ahead frames are dropped as reset() drops them
+            frames = [(t, f.to("cpu")) for t, f in self.frame_embeds_queue]   # before the cache copy: this one syncs
+            state = SessionState(
+                kv=self._kv.engine.kv_swap_out(self._kv.stream_id), last_ids=self.last_ids.clone(),
+                video_time=self.video_time, last_frame_idx=self.last_frame_idx, query_queue=list(self.query_queue),
+                frame_embeds_queue=frames,
+                drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
+                n_calls=self._n_calls, started=self.past_key_values is not None)
+            self.reset()
+            return state
+
+    def resume(self, state: SessionState):
+        """Continue a session `suspend()` returned: the cache is copied back into this session's (emptied) stream and
+        every queue and counter `__call__` reads is restored.  The video is not part of the state: load it again
+        (before or after resuming).  Raises VloError if the pool is short or the image belongs to another config; the
+        session's stream is then empty and the rest of the session unchanged."""
+        with self._lock:
+            self._drop_prefetch()
+            eng = self._kv.engine
+            eng.stream_reset(self._kv.stream_id)
+            eng.kv_swap_in(self._kv.stream_id, state.kv)
+            dev = self.device
+            self.last_ids = state.last_ids.clone()
+            self.video_time, self.last_frame_idx = state.video_time, state.last_frame_idx
+            self.query_queue = collections.deque(state.query_queue)
+            self.frame_embeds_queue = collections.deque((t, f.to(dev, torch.bfloat16)) for t, f in state.frame_embeds_queue)
+            if self.drafter is not None:
+                self.drafter.sync(0)
+                if state.drafter_ids is not None and isinstance(self.drafter, NgramDrafter):
+                    self.drafter.extend(state.drafter_ids)
+                else:
+                    self.drafter.sync(state.kv.n_tokens)
+            self._n_calls = state.n_calls
+            self.past_key_values = self._kv if state.started else None
 
     def load_video(self, video_path_or_tensor, keep_on_host: bool = False):
         """Reference: read_video(...)[0].to('cuda') (demo/inference.py:111-115).  Accepts a uint8

@@ -12,6 +12,11 @@ side CUDA stream right after the ragged step of the tick has been enqueued, so t
 of the HBM-bound decoder step of tick i.  Only that regime pays: the engine's small-batch ViT configuration shares an
 SM with a decoder weight-streaming CTA, whereas a batch-8 ViT time-slices the SMs with the persistent decoder kernels
 (measured 8 streams: 616 frames/s with the ViT in line, 534 with it on the side stream).
+
+More sessions than the engine holds: a session without work (no pending frame, not responding) may be swapped out to
+a pinned host image (`Engine.kv_swap_out`), and then holds neither KV pages nor a stream slot.  Before each tick every
+session with work is made resident again if it fits (`StreamScheduler._make_room`); the policy is fixed and
+deterministic.
 """
 from __future__ import annotations
 
@@ -20,6 +25,8 @@ from typing import Callable, Deque, List, Optional, Tuple
 
 import torch
 
+from ._lib import VloError
+from .engine import KvImage
 from .modeling_live import LiveLlamaForCausalLM
 
 
@@ -29,13 +36,30 @@ class StreamSession:
 
     def __init__(self, sched: "StreamScheduler", index: int):
         self.sched, self.index = sched, index
-        self.stream_id = sched.model.engine.stream_open()
+        # swapped out (stream_id None): the cache lives in `image` (None: empty) and the session holds no engine stream
+        self.image: Optional[KvImage] = None
+        self.last_step = -1   # tick of the session's last step (least recently stepped is swapped out first)
+        try:
+            self.stream_id: Optional[int] = sched.model.engine.stream_open()
+        except VloError:      # more sessions than stream slots: this one starts swapped out
+            self.stream_id = None
         self.frame_fps = sched.frame_fps
         self.threshold = 0.725
         self.reset()
 
+    @property
+    def resident(self) -> bool:
+        return self.stream_id is not None
+
+    def kv_tokens(self) -> int:
+        if self.resident:
+            return self.sched.model.engine.kv_len(self.stream_id)
+        return self.image.n_tokens if self.image is not None else 0
+
     def reset(self):
-        self.sched.model.engine.stream_reset(self.stream_id)
+        if self.resident:
+            self.sched.model.engine.stream_reset(self.stream_id)
+        self.image = None
         getattr(self.sched, "_ahead", {}).pop(self.index, None)   # an encoded-ahead frame of the old clip
         self.query_queue: Deque[Tuple[float, str]] = collections.deque()
         self.pending_frames: Deque[Tuple[float, int]] = collections.deque()   # (video_time, frame index)
@@ -146,6 +170,7 @@ class StreamScheduler:
         self.start_ids = tk.apply_chat_template([{'role': 'system', 'content': system_prompt}], add_stream_prompt=True)
         self.stream_prompt_ids = tk.apply_chat_template([{}], add_stream_prompt=True)
         self.stream_generation_ids = tk.apply_chat_template([{}], add_stream_generation_prompt=True)
+        self.swaps_out = self.swaps_in = 0
         self.sessions = [StreamSession(self, i) for i in range(n_streams)]
         self.ticks = 0
         self.frames_done = 0
@@ -168,8 +193,9 @@ class StreamScheduler:
         if not plans:
             return 0
         batch, used = [], 0
+        busy = {s.index for s in active}
         for p in plans:
-            if batch and used + p[3] > budget:
+            if (batch and used + p[3] > budget) or not self._make_room(p[0], p[3], batch, busy):
                 # not in this tick: undo the plan (frame / response prompt stays pending)
                 s, ids, fidx, n = p
                 if s._op and s._op[0] == "frame":
@@ -219,9 +245,64 @@ class StreamScheduler:
             self._launch_encode_ahead(pre)        # enqueued after the step's launches, runs concurrently with it
         decs = eng.read_decisions(len(batch))
         for (s, *_), d in zip(batch, decs):
+            s.last_step = self.ticks
             s.advance(d)
         self.ticks += 1
         return len(batch)
+
+    # -- swapping: a session without work may give its pages and stream slot back (host image) and take them again later
+    def _make_room(self, s: StreamSession, n: int, batch, busy) -> bool:
+        """Make session `s` resident with room for n more tokens, next to the sessions already in `batch`.  Resident
+        sessions outside the batch are swapped out for it: first those without work (not in `busy`), then, only while
+        the batch is still empty (so that every tick steps someone), those whose turn is later; least recently stepped
+        first, lowest index on a tie.  False: `s` waits for a later tick.  Raises if `s` alone cannot fit in an empty
+        pool."""
+        eng = self.model.engine
+        info = eng.kv_pool_info()
+        page, total = info["page_tokens"], info["total_pages"]
+        pages = lambda t: -(-t // page)
+        kv = s.kv_tokens()
+        if pages(kv + n) > total:
+            raise VloError(f"session {s.index}: {kv + n} tokens need {pages(kv + n)} KV pages, the pool has {total}")
+        # pages the sessions already in the batch take in this step
+        reserved = sum(pages(q.kv_tokens() + m) - pages(q.kv_tokens()) for q, _, _, m in batch)
+        need = pages(kv + n) - (pages(kv) if s.resident else 0)
+        keep = {q.index for q, *_ in batch} | {s.index}
+
+        def evict() -> bool:
+            cands = [q for q in self.sessions if q.resident and q.index not in keep
+                     and (q.index not in busy or not batch)]
+            if not cands:
+                return False
+            self._swap_out(min(cands, key=lambda q: (q.index in busy, q.last_step, q.index)))
+            return True
+
+        while eng.kv_pool_info()["free_pages"] - reserved < need:
+            if not evict():
+                return False
+        while not s.resident:
+            try:
+                sid = eng.stream_open()
+            except VloError:      # no free stream slot
+                if not evict():
+                    return False
+                continue
+            if s.image is not None:
+                try:
+                    eng.kv_swap_in(sid, s.image)
+                except VloError:
+                    eng.stream_close(sid)
+                    raise
+            s.stream_id, s.image = sid, None
+            self.swaps_in += 1
+        return True
+
+    def _swap_out(self, s: StreamSession):
+        eng = self.model.engine
+        img = eng.kv_swap_out(s.stream_id)
+        eng.stream_close(s.stream_id)
+        s.stream_id, s.image = None, (img if img.n_tokens else None)
+        self.swaps_out += 1
 
     def _launch_encode_ahead(self, after: "torch.cuda.Event"):
         """One batched ViT on the side stream over every stream's next pending frame that is not encoded yet."""
