@@ -179,6 +179,42 @@ int vlo_step_ids(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const i
 int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_seg_counts,
                       const int32_t* h_seg_lens, const int64_t* d_row_ids, const void* d_embeds, void* d_seg_logits,
                       vlo_decision* d_decisions, int interval_id, void* cuda_stream);
+/* ------------------------------------------------------------------ response sampling
+ * Replaces the logits processors HF's `generate(do_sample=True, ...)` runs per token (HF:generation/utils.py
+ * GenerationMixin._get_logits_processor): RepetitionPenaltyLogitsProcessor, TemperatureLogitsWarper, TopKLogitsWarper,
+ * TopPLogitsWarper, then a draw.  One vlo_sample_row per logits row; the kernel (csrc/sampling.cuh, sample_kernel)
+ * applies, in fp32 on the bf16 logits and in this order:
+ *   repetition penalty  l = l < 0 ? l * p : l / p for each distinct id of penalty_ids[offset, offset + count) (ids
+ *                       outside [0, vocab) are ignored; p = 1: off);
+ *   temperature         l = l / temperature;
+ *   top-k               keep l >= the k-th largest l (ties kept; 0 or >= vocab: off);
+ *   top-p               keep id i iff the softmax mass of the ids with a strictly larger probability is < top_p (>= 1:
+ *                       off), over the top-k survivors.  A tie group straddling the boundary is kept whole (HF keeps
+ *                       the part its sort puts first); the maximum is always kept;
+ *   draw                id = first-index argmax over the kept i of l_i - log(-log(u_i)).
+ * Noise layout (Philox4x32-10, 10 rounds, Random123 / curand constants): key = (seed & 0xffffffff, seed >> 32),
+ *   counter = (i / 4, position, 0, 0) for vocab id i; word i % 4 of the output (x, y, z, w order) is x_i, and
+ *   u_i = ((x_i >> 8) + 0.5) * 2^-24.  `position` is the stream position (KV row) of the token whose logits the row
+ *   holds, so a row's id is a pure function of (logits, parameters): the same with any other rows in the launch, in
+ *   a segmented verify step or in a one-token step, and in any run.
+ * temperature 0: the row is not sampled (its id is -1). */
+typedef struct vlo_sample_row {
+  uint64_t seed;
+  int32_t position;
+  float temperature;         /* > 0; 0: skip the row */
+  int32_t top_k;             /* 0: off */
+  float top_p;               /* (0, 1); >= 1: off */
+  float repetition_penalty;  /* > 0; 1: off */
+  int32_t penalty_offset, penalty_count;  /* the row's ids in the call's penalty list (rows may share or overlap) */
+  int32_t reserved;
+} vlo_sample_row;
+/* One id per row of d_logits (bf16 [n_rows, vocab], 16-byte aligned) into d_out_ids (device int32 [n_rows]), on
+ * cuda_stream after the work before it (e.g. the vlo_step that wrote the logits).  n_rows <= max(max_streams,
+ * max_step_tokens); n_penalty_ids <= 65 536.  The rows and the penalty ids (host arrays) go up through the engine's
+ * pinned staging ring in one asynchronous copy: no host synchronisation. */
+int vlo_sample(vlo_engine* e, const void* d_logits, int n_rows, const vlo_sample_row* h_rows, const int32_t* h_penalty_ids,
+               int n_penalty_ids, int32_t* d_out_ids, void* cuda_stream);
+
 /* all-position logits for the last vlo_step's tokens (the reference's logits_to_keep=0 behaviour,
  * HF:models/llama/modeling_llama.py:485-487); d_logits bf16 [sum(q_lens), vocab]. Test/compat path. */
 int vlo_last_step_logits(vlo_engine* e, void* d_logits, void* cuda_stream);
@@ -285,6 +321,12 @@ int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x,
  * first-index argmax of bf16(softmax) with (argmax_prob_id) and without (argmax_excl_id: that entry set to 0) the
  * interval id.  Asynchronous. */
 int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream);
+/* The sampling kernel of vlo_sample without an engine (any vocab % 8 == 0).  d_info (device, may be NULL): per row
+ * {int32 kept count, float top-k threshold, float top-p threshold, int32 0}: an id is kept iff its l (after penalty and
+ * temperature) is >= both thresholds (-inf: that filter is off).  Parameters are uploaded from pageable memory;
+ * synchronous. */
+int vlo_op_sample(const void* d_logits, int n_rows, int vocab, const vlo_sample_row* h_rows, const int32_t* h_penalty_ids,
+                  int n_penalty_ids, int32_t* d_out_ids, void* d_info, void* cuda_stream);
 /* Micro-loop of the same attention over n_layers separate K / V matrices (working set > L2), iters passes of back-to-back
  * launches on one plan: what bench tools bracket with ONE CUDA-event pair (per-launch time incl. the PDL overlap of a real
  * step).  skip_merge != 0 launches the main kernel only.  Mirrors vlo_bench_attn without an engine. */

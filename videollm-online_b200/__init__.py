@@ -3,10 +3,10 @@
 The directory is named `videollm-online_b200/`; import it as `videollm_online_b200` via the
 repo-root bootstrap (`import vlo_bootstrap`), which registers this package under that name.
 """
-from .config import LiveArguments, LiveConfig, llama3_8b_siglip_l, parse_args, tiny_config
+from .config import LiveArguments, LiveConfig, SamplingConfig, llama3_8b_siglip_l, parse_args, tiny_config
 from ._lib import VloError
 
-__all__ = ["LiveArguments", "LiveConfig", "llama3_8b_siglip_l", "parse_args", "tiny_config", "VloError",
+__all__ = ["LiveArguments", "LiveConfig", "SamplingConfig", "llama3_8b_siglip_l", "parse_args", "tiny_config", "VloError",
            "build_model_and_tokenizer", "fast_greedy_generate", "LiveInfer", "Engine"]
 
 

@@ -40,6 +40,14 @@ class VloDecision(C.Structure):
     ]
 
 
+class VloSampleRow(C.Structure):
+    _fields_ = [
+        ("seed", C.c_uint64), ("position", C.c_int32), ("temperature", C.c_float), ("top_k", C.c_int32),
+        ("top_p", C.c_float), ("repetition_penalty", C.c_float), ("penalty_offset", C.c_int32),
+        ("penalty_count", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _LL = C.c_longlong
@@ -77,6 +85,7 @@ SIGNATURES = {
     "vlo_step_ids": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _P, _I, _P]),
     "vlo_step_segments": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _P,
                                _I, _P]),
+    "vlo_sample": (_I, [_P, _P, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P]),
     "vlo_last_step_logits": (_I, [_P, _P, _P]),
     "vlo_last_step_hidden": (_I, [_P, _P, _P]),
     "vlo_bench_attn": (_I, [_P, _I, C.POINTER(C.c_int32), _I, _I, _I, C.POINTER(C.c_double), _P]),
@@ -94,6 +103,7 @@ SIGNATURES = {
                                     _I, _I, _I, _P]),
     "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),
+    "vlo_op_sample": (_I, [_P, _I, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),
 }
 

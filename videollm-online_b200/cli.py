@@ -1,6 +1,9 @@
 """Headless driver + FPS measurement: the engine-backed counterpart of demo/cli.py:12-50.
 
     python -m videollm_online_b200.cli --synthetic_weights true [--frames 100] [--video clip.mp4] [--whole_video]
+        [--do_sample --temperature 0.6 --top_p 0.9 --top_k 50 --repetition_penalty 1.1 --sample_seed 0]
+
+Responses are greedy unless --do_sample is given (SamplingConfig; --seed stays the synthetic weights' seed).
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

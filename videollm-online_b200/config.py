@@ -10,6 +10,7 @@ from __future__ import annotations
 
 import argparse
 import dataclasses
+import math
 from dataclasses import dataclass, field
 from typing import List, Optional
 
@@ -91,6 +92,44 @@ def tiny_config(**over) -> LiveConfig:
 
 
 @dataclass
+class SamplingConfig:
+    """How response tokens are picked, with the names and defaults of HF's GenerationConfig.  do_sample False: greedy
+    (the argmax, what every response is without a config).  do_sample True: each token is drawn on the device
+    (include/vlo_b200.h, vlo_sample) after the repetition penalty over the response's prompt ids and the ids generated
+    so far, the temperature, top-k (0: off) and top-p (1: off).  The noise is a function of (seed, KV position), so a
+    response is reproducible from the seed and its ids do not depend on drafts, batching or a suspend / resume."""
+    do_sample: bool = False
+    temperature: float = 1.0
+    top_k: int = 50
+    top_p: float = 1.0
+    repetition_penalty: float = 1.0
+    seed: int = 0
+
+    def __post_init__(self):
+        if not (math.isfinite(self.temperature) and self.temperature > 0):
+            raise ValueError(f"temperature must be finite and > 0, got {self.temperature}")
+        if isinstance(self.top_k, bool) or not isinstance(self.top_k, int) or self.top_k < 0:
+            raise ValueError(f"top_k must be an int >= 0 (0: off), got {self.top_k!r}")
+        if not (0 < self.top_p <= 1):
+            raise ValueError(f"top_p must lie in (0, 1], got {self.top_p}")
+        if not (math.isfinite(self.repetition_penalty) and self.repetition_penalty > 0):
+            raise ValueError(f"repetition_penalty must be finite and > 0, got {self.repetition_penalty}")
+        if isinstance(self.seed, bool) or not isinstance(self.seed, int) or not 0 <= self.seed < 1 << 64:
+            raise ValueError(f"seed must be an int in [0, 2^64), got {self.seed!r}")
+        if not self.do_sample and self.repetition_penalty != 1.0:
+            raise ValueError("repetition_penalty applies to sampled responses: set do_sample=True (greedy responses "
+                             "take the plain argmax)")
+
+    @classmethod
+    def from_args(cls, args: "LiveArguments") -> Optional["SamplingConfig"]:
+        """The config the --do_sample / --temperature / --top_k / --top_p / --repetition_penalty / --sample_seed flags
+        ask for; None (greedy) without --do_sample."""
+        cfg = cls(do_sample=args.do_sample, temperature=args.temperature, top_k=args.top_k, top_p=args.top_p,
+                  repetition_penalty=args.repetition_penalty, seed=args.sample_seed)
+        return cfg if cfg.do_sample else None
+
+
+@dataclass
 class LiveArguments:
     """Flag surface of `models.parse_args()` that the inference path reads
     (models/arguments_live.py:5-28,40-47; demo/inference.py:14-35)."""
@@ -115,7 +154,14 @@ class LiveArguments:
     max_streams: int = 1
     kv_pool_tokens: int = 0  # KV page pool shared by the streams, tokens; 0: max_streams x the per-stream cap
     synthetic_weights: bool = False
-    seed: int = 0
+    seed: int = 0            # of the synthetic weights
+    # response sampling (SamplingConfig; HF GenerationConfig names, sample_seed = its seed); greedy without --do_sample
+    do_sample: bool = False
+    temperature: float = 1.0
+    top_k: int = 50
+    top_p: float = 1.0
+    repetition_penalty: float = 1.0
+    sample_seed: int = 0
 
 
 def _apply_version(args: LiveArguments) -> LiveArguments:
@@ -140,7 +186,9 @@ def parse_args(argv=None) -> LiveArguments:
         if f.name in ("frame_token_pooled",):
             p.add_argument(f"--{f.name}", type=int, nargs="+", default=None)
         elif f.type in ("bool", "Optional[bool]") or isinstance(f.default, bool):
-            p.add_argument(f"--{f.name}", type=lambda s: s.lower() in ("1", "true", "yes"), default=f.default)
+            # `--flag true|false`, or `--flag` alone for true
+            p.add_argument(f"--{f.name}", type=lambda s: s.lower() in ("1", "true", "yes"), nargs="?", const=True,
+                           default=f.default)
         elif isinstance(f.default, int):
             p.add_argument(f"--{f.name}", type=int, default=f.default)
         elif isinstance(f.default, float):

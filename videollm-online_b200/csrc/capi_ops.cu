@@ -271,6 +271,29 @@ int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id
   return decision_launch(d_logits, n_rows, vocab, interval_id, d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
+int vlo_op_sample(const void* d_logits, int n_rows, int vocab, const vlo_sample_row* h_rows, const int32_t* h_penalty_ids,
+                  int n_penalty_ids, int32_t* d_out_ids, void* d_info, void* cuda_stream) {
+  VLO_CHECK(n_rows > 0 && vocab > 0 && vocab % 8 == 0, "sample: rows of a positive multiple of 8 logits");
+  VLO_CHECK(d_logits != nullptr && d_out_ids != nullptr, "sample: null argument");
+  VLO_CHECK((reinterpret_cast<uintptr_t>(d_logits) & 15) == 0, "sample: logits must be 16-byte aligned");
+  VLO_CHECK(n_penalty_ids >= 0 && (n_penalty_ids == 0 || h_penalty_ids != nullptr), "sample: penalty ids");
+  if (sample_check_rows(h_rows, n_rows, n_penalty_ids)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  const size_t rows_bytes = align256(sizeof(vlo_sample_row) * n_rows);
+  uint8_t* d_par = nullptr;
+  VLO_CUDA(cudaMalloc(&d_par, rows_bytes + sizeof(int32_t) * (n_penalty_ids + 1)));
+  int rc = cudaMemcpy(d_par, h_rows, sizeof(vlo_sample_row) * n_rows, cudaMemcpyHostToDevice) != cudaSuccess ||
+           (n_penalty_ids && cudaMemcpy(d_par + rows_bytes, h_penalty_ids, sizeof(int32_t) * n_penalty_ids,
+                                        cudaMemcpyHostToDevice) != cudaSuccess)
+               ? fail("sample: parameter upload failed")
+               : 0;
+  if (rc == 0) rc = sample_launch(d_logits, n_rows, vocab, d_par, reinterpret_cast<const int*>(d_par + rows_bytes),
+                                  d_out_ids, d_info, st);
+  if (rc == 0 && cudaStreamSynchronize(st) != cudaSuccess) rc = fail("sample: kernel failed");
+  cudaFree(d_par);
+  return rc;
+}
+
 /* Back-to-back launches of the KV-append attention over `n_layers` separate K / V matrices (layer l at
  * d_k + l * layer_stride_rows * head_dim elements), `iters` passes: the micro-loop of vlo_bench_attn without an engine
  * (bench tools time it with one CUDA-event pair).  The plan is built and uploaded once, as in a decoder step. */

@@ -161,6 +161,15 @@ int qkv_rope_launch(const float* part, const SkInfo& sk, const void* cos_tab, co
 // decision_kernel: one vlo_decision per bf16 logits row [n_rows, vocab].
 int decision_launch(const void* logits, int n_rows, int vocab, int interval_id, void* out, cudaStream_t st);
 
+// ---- response sampling (sampling.cuh / engine.cu) -------------------------------------
+// The parameters of n rows of a vlo_sample / vlo_op_sample call (vlo_sample_row, include/vlo_b200.h) over n_ids penalty
+// ids: 0 when every row is valid, else -1 with the message set.
+int sample_check_rows(const void* h_rows, int n_rows, int n_ids);
+// sample_kernel: one id per bf16 logits row [n_rows, vocab] (vocab % 8 == 0, 16-byte aligned rows); rows / penalty_ids /
+// info are device arrays (info may be null).
+int sample_launch(const void* logits, int n_rows, int vocab, const void* rows, const int* penalty_ids, int* out_ids,
+                  void* info, cudaStream_t st);
+
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {
   int q_tok0;          // first packed token of the sequence

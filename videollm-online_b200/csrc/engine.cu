@@ -11,14 +11,18 @@
 #include "decoder_kernels.cuh"
 #include "gemm.cuh"
 #include "kv_pages.h"
+#include "sampling.cuh"
 #include "vit_kernels.cuh"
 #include "vlo_b200.h"
 
 using namespace vlo;
 
+static_assert(sizeof(vlo_sample_row) == sizeof(SampleRow), "vlo_sample_row and SampleRow must match");
+
 namespace {
 
 constexpr int kStageSlots = 16;
+constexpr int kSamplePenaltyIds = 65536;  // penalty ids one vlo_sample call may pass
 constexpr int kSkFlags = 4096;  // stream-K arrival counters of the fused gate|up GEMM: one per 128-row weight tile
 
 using bf16 = __nv_bfloat16;
@@ -90,6 +94,11 @@ struct vlo_engine {
     size_t pos, last, first, kvrow, pt, bytes;
   } meta{};
   DecisionOut* decisions = nullptr;
+  // vlo_sample parameters: sample_rows rows, then (at sample_ids) up to kSamplePenaltyIds penalty ids; the same layout
+  // sits at byte sample_stage of every staging slot
+  uint8_t* sample_dev = nullptr;
+  int sample_rows = 0;
+  size_t sample_ids = 0, sample_stage = 0;
   // host staging ring (pinned)
   uint8_t* stage = nullptr;
   size_t stage_slot_bytes = 0;
@@ -379,6 +388,35 @@ int decision_launch(const void* logits, int n_rows, int vocab, int interval_id, 
   return 0;
 }
 
+int sample_check_rows(const void* h_rows, int n_rows, int n_ids) {
+  VLO_CHECK(h_rows != nullptr, "sample: null rows");
+  const SampleRow* rows = static_cast<const SampleRow*>(h_rows);
+  for (int i = 0; i < n_rows; ++i) {
+    const SampleRow& r = rows[i];
+    const std::string at = "sample: row " + std::to_string(i) + ": ";
+    VLO_CHECK(r.temperature >= 0.f && r.temperature <= 3.4e38f, at + "temperature must be finite and >= 0 (0: not sampled)");
+    if (r.temperature == 0.f) continue;  // a skipped row: nothing else of it is read
+    VLO_CHECK(r.top_k >= 0, at + "top_k must be >= 0 (0: off)");
+    VLO_CHECK(r.top_p > 0.f, at + "top_p must be > 0 (>= 1: off)");
+    VLO_CHECK(r.repetition_penalty > 0.f && r.repetition_penalty <= 3.4e38f, at + "repetition_penalty must be finite and > 0");
+    VLO_CHECK(r.penalty_offset >= 0 && r.penalty_count >= 0 &&
+                  static_cast<long long>(r.penalty_offset) + r.penalty_count <= n_ids,
+              at + "penalty ids [offset, offset + count) must lie in the call's list");
+  }
+  return 0;
+}
+
+int sample_launch(const void* logits, int n_rows, int vocab, const void* rows, const int* penalty_ids, int* out_ids,
+                  void* info, cudaStream_t st) {
+  const int smem = static_cast<int>(sizeof(uint32_t)) * ((vocab + 31) / 32);
+  if (smem + sizeof(SampleShared) > 48 * 1024 && ensure_max_smem(reinterpret_cast<const void*>(sample_kernel), smem))
+    return -1;
+  VLO_CUDA(launch_pdl(sample_kernel, dim3(n_rows), dim3(kSampleThreads), smem, st, static_cast<const bf16*>(logits), vocab,
+                      static_cast<const SampleRow*>(rows), penalty_ids, out_ids, static_cast<SampleInfo*>(info)));
+  count_launch();
+  return 0;
+}
+
 }  // namespace vlo
 
 extern "C" {
@@ -476,7 +514,12 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   e->meta.pt = e->meta.kvrow + align256(sizeof(long long) * T);
   e->meta.bytes = e->meta.pt + align256(sizeof(int) * std::max(2, c.max_streams) * per_stream);
   if (dev_alloc(e, reinterpret_cast<void**>(&e->meta_dev), e->meta.bytes, false)) return -1;
-  e->stage_slot_bytes = align256(e->meta.bytes + attn_stage_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads));
+  e->sample_rows = rows;
+  e->sample_ids = align256(sizeof(SampleRow) * rows);
+  const size_t sample_bytes = e->sample_ids + sizeof(int) * kSamplePenaltyIds;
+  if (dev_alloc(e, reinterpret_cast<void**>(&e->sample_dev), sample_bytes, false)) return -1;
+  e->sample_stage = align256(e->meta.bytes + attn_stage_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads));
+  e->stage_slot_bytes = align256(e->sample_stage + sample_bytes);
   VLO_CUDA(cudaMallocHost(reinterpret_cast<void**>(&e->stage), e->stage_slot_bytes * kStageSlots));
   for (int i = 0; i < kStageSlots; ++i) VLO_CUDA(cudaEventCreateWithFlags(&e->stage_events[i], cudaEventDisableTiming));
 
@@ -1149,6 +1192,31 @@ int vlo_step(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32
              void* d_last_logits, vlo_decision* d_decisions, int interval_id, void* cuda_stream) {
   return vlo_step_ids(e, n_seqs, h_stream_ids, h_q_lens, nullptr, d_embeds, d_last_logits, d_decisions, interval_id,
                       cuda_stream);
+}
+
+int vlo_sample(vlo_engine* e, const void* d_logits, int n_rows, const vlo_sample_row* h_rows, const int32_t* h_penalty_ids,
+               int n_penalty_ids, int32_t* d_out_ids, void* cuda_stream) {
+  DevGuard dev_guard(e);
+  VLO_CHECK(e != nullptr && d_logits != nullptr && d_out_ids != nullptr, "sample: null argument");
+  VLO_CHECK(n_rows > 0 && n_rows <= e->sample_rows,
+            "sample: n_rows must lie in [1, max(max_streams, max_step_tokens)] = [1, " + std::to_string(e->sample_rows) + "]");
+  VLO_CHECK(n_penalty_ids >= 0 && n_penalty_ids <= kSamplePenaltyIds,
+            "sample: at most " + std::to_string(kSamplePenaltyIds) + " penalty ids per call");
+  VLO_CHECK(n_penalty_ids == 0 || h_penalty_ids != nullptr, "sample: null penalty ids");
+  VLO_CHECK((reinterpret_cast<uintptr_t>(d_logits) & 15) == 0, "sample: logits must be 16-byte aligned");
+  if (sample_check_rows(h_rows, n_rows, n_penalty_ids)) return -1;
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  // parameters and ids through one pinned slot, one upload
+  uint8_t* hs;
+  int slot;
+  if (stage_acquire(e, &hs, &slot)) return -1;
+  std::memcpy(hs + e->sample_stage, h_rows, sizeof(SampleRow) * n_rows);
+  if (n_penalty_ids) std::memcpy(hs + e->sample_stage + e->sample_ids, h_penalty_ids, sizeof(int) * n_penalty_ids);
+  VLO_CUDA(cudaMemcpyAsync(e->sample_dev, hs + e->sample_stage, e->sample_ids + sizeof(int) * n_penalty_ids,
+                           cudaMemcpyHostToDevice, st));
+  if (stage_release(e, slot, st)) return -1;
+  return sample_launch(d_logits, n_rows, e->cfg.vocab_size, e->sample_dev,
+                       reinterpret_cast<const int*>(e->sample_dev + e->sample_ids), d_out_ids, nullptr, st);
 }
 
 // ------------------------------------------------------------------------------ kernel-class micro loops

@@ -7,12 +7,13 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
+from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence
 
 import torch
 
 from . import _lib
-from ._lib import VloConfig, VloDecision, VloError, check
+from ._lib import VloConfig, VloDecision, VloError, VloSampleRow, check
 from .config import LiveConfig
 
 DECISION_DTYPE_FIELDS = 8  # 8 x 4 bytes
@@ -23,10 +24,12 @@ def _ptr(t: Optional[torch.Tensor]):
 
 
 class Decision:
-    """Host copy of one `vlo_decision`."""
-    __slots__ = ("argmax_id", "argmax_excl_id", "p_interval", "max_logit", "top2_margin", "lse", "argmax_prob_id")
+    """Host copy of one `vlo_decision`, plus the id `Engine.step(..., sample=...)` drew for its row (None: not
+    sampled)."""
+    __slots__ = ("argmax_id", "argmax_excl_id", "p_interval", "max_logit", "top2_margin", "lse", "argmax_prob_id",
+                 "sampled_id")
 
-    def __init__(self, row_i32: torch.Tensor, row_f32: torch.Tensor):
+    def __init__(self, row_i32: torch.Tensor, row_f32: torch.Tensor, sampled_id: Optional[int] = None):
         self.argmax_id = int(row_i32[0])
         self.argmax_excl_id = int(row_i32[1])
         self.p_interval = float(row_f32[2])
@@ -34,6 +37,7 @@ class Decision:
         self.top2_margin = float(row_f32[4])
         self.lse = float(row_f32[5])
         self.argmax_prob_id = int(row_i32[6])
+        self.sampled_id = sampled_id
 
     def next_id(self, interval_id: int, threshold: float) -> int:
         """The reference's rule (demo/inference.py:76-79) on bf16 probabilities: if p(interval) < threshold the
@@ -77,6 +81,23 @@ class KvImage:
 torch.serialization.add_safe_globals([KvImage])
 
 
+@dataclass
+class SampleRow:
+    """What `Engine.step(..., sample=...)` draws one decision row's id with (vlo_sample_row, include/vlo_b200.h).
+
+    position: the KV position of the token whose logits the row holds (the noise depends on it and on the seed only).
+    The repetition penalty applies to the first n_penalty ids of penalty_ids (None: all of them); rows of one step
+    that pass the same list object share its upload, so the rows of a verify step can use one growing list."""
+    seed: int
+    position: int
+    temperature: float = 1.0
+    top_k: int = 0
+    top_p: float = 1.0
+    repetition_penalty: float = 1.0
+    penalty_ids: Sequence[int] = ()
+    n_penalty: Optional[int] = None
+
+
 class Engine:
     def __init__(self, cfg: LiveConfig, device: str | torch.device = "cuda:0", *, max_streams: int = 1,
                  max_kv_tokens: int = 16384, max_step_tokens: int = 128, max_vit_batch: int = 8,
@@ -113,9 +134,14 @@ class Engine:
             check(self.lib.vlo_engine_create_pooled(C.byref(c), int(kv_pool_tokens or 0), self.index, C.byref(self._h)),
                   "vlo_engine_create_pooled")
         # device scratch for results (decisions, last logits): one row per sequence, or per segment of a segmented step
+        # and the sampled ids right behind the decisions, so that one copy brings both back
         rows = max(max_streams, max_step_tokens)
-        self._dec_dev = torch.zeros(rows, DECISION_DTYPE_FIELDS, dtype=torch.int32, device=self.device)
-        self._dec_host = torch.zeros(rows, DECISION_DTYPE_FIELDS, dtype=torch.int32).pin_memory()
+        self._res_dev = torch.zeros(rows * (DECISION_DTYPE_FIELDS + 1), dtype=torch.int32, device=self.device)
+        self._res_host = torch.zeros(rows * (DECISION_DTYPE_FIELDS + 1), dtype=torch.int32).pin_memory()
+        self._dec_dev = self._res_dev[:rows * DECISION_DTYPE_FIELDS].view(rows, DECISION_DTYPE_FIELDS)
+        self._dec_host = self._res_host[:rows * DECISION_DTYPE_FIELDS].view(rows, DECISION_DTYPE_FIELDS)
+        self._ids_dev = self._res_dev[rows * DECISION_DTYPE_FIELDS:]
+        self._sampled: Optional[List[bool]] = None   # rows of the last step that were sampled (None: no sampling)
         self._logits = torch.zeros(rows, cfg.vocab_size, dtype=torch.bfloat16, device=self.device)
         # pinned image buffers a swap copy may still write or read: kept alive until their event has completed, so the
         # caching host allocator cannot hand them to someone else under a copy
@@ -292,7 +318,8 @@ class Engine:
 
     def step(self, stream_ids: Sequence[int], q_lens: Sequence[int], embeds: torch.Tensor, *,
              row_ids: Optional[torch.Tensor] = None, interval_id: Optional[int] = None,
-             want_logits: bool = True, segments: Optional[Sequence[Sequence[int]]] = None):
+             want_logits: bool = True, segments: Optional[Sequence[Sequence[int]]] = None,
+             sample: Optional[Sequence[Optional[SampleRow]]] = None):
         """KV-append forward of a ragged batch.  `row_ids` (int64 [sum q_lens], optional): id >= 0 -> the row is the
         embedding of that token (gathered on the device), id < 0 -> the row of `embeds` is used as is.  Returns (logits [n_seqs, V] bf16 view or None, decisions
         device tensor int32 [n_seqs, 8]).  Nothing is synchronised; call `read_decisions` for host values.
@@ -300,7 +327,45 @@ class Engine:
         `segments` (optional): per sequence, the lengths of the consecutive segments its q_len rows are made of (they
         must add up to q_lens[i]).  Then there is one logits row and one decision per segment, in order, read at the
         segment's last row ([n_segments, V] / [n_segments, 8]), and every segment computes the bits the same rows get
-        from a step of their own (vlo_step_segments).  A segmented step longer than max_step_tokens is an error."""
+        from a step of their own (vlo_step_segments).  A segmented step longer than max_step_tokens is an error.
+
+        `sample` (optional): one SampleRow or None per decision row.  The step then keeps its logits and enqueues
+        vlo_sample over them; `read_decisions` returns the drawn ids as `Decision.sampled_id` (None for rows given
+        None).  Without it the step runs exactly as before."""
+        self._sampled = None
+        if sample is None:
+            return self._step(stream_ids, q_lens, embeds, row_ids, interval_id, want_logits, segments)
+        logits, dec = self._step(stream_ids, q_lens, embeds, row_ids, interval_id, True, segments)
+        self._sample(logits, sample)
+        return logits, dec
+
+    def _sample(self, logits: torch.Tensor, sample: Sequence[Optional[SampleRow]]):
+        if len(sample) != logits.shape[0]:
+            raise VloError(f"step: sample needs one entry per decision row ({logits.shape[0]}), got {len(sample)}")
+        m = max((i + 1 for i, r in enumerate(sample) if r is not None), default=0)
+        if m:
+            rows = (VloSampleRow * m)()
+            ids: List[int] = []
+            at: Dict[int, int] = {}     # id(penalty list) -> its offset in `ids`
+            for c, r in zip(rows, sample[:m]):
+                if r is None:           # temperature 0: the kernel skips the row
+                    continue
+                c.seed, c.position, c.temperature = r.seed, r.position, r.temperature
+                c.top_k, c.top_p, c.repetition_penalty = r.top_k, r.top_p, r.repetition_penalty
+                if r.repetition_penalty != 1.0:
+                    n_pen = len(r.penalty_ids) if r.n_penalty is None else r.n_penalty
+                    if not 0 <= n_pen <= len(r.penalty_ids):
+                        raise VloError(f"step: n_penalty {n_pen} outside the row's {len(r.penalty_ids)} penalty ids")
+                    if id(r.penalty_ids) not in at:
+                        at[id(r.penalty_ids)] = len(ids)
+                        ids.extend(r.penalty_ids)
+                    c.penalty_offset, c.penalty_count = at[id(r.penalty_ids)], n_pen
+            pen = torch.tensor(ids, dtype=torch.int32) if ids else None
+            check(self.lib.vlo_sample(self._h, _ptr(logits), m, rows, _ptr(pen), len(ids), _ptr(self._ids_dev),
+                                      self._stream()), "vlo_sample")
+        self._sampled = [r is not None for r in sample]
+
+    def _step(self, stream_ids, q_lens, embeds, row_ids, interval_id, want_logits, segments):
         n = len(stream_ids)
         T = int(sum(q_lens))
         embeds = embeds.contiguous()
@@ -394,11 +459,20 @@ class Engine:
         return (self._logits[:n] if want_logits else None), self._dec_dev[:n]
 
     def read_decisions(self, n: int) -> List[Decision]:
-        """One small D2H copy + sync: the only host<->device sync of a frame step."""
-        self._dec_host[:n].copy_(self._dec_dev[:n], non_blocking=True)
-        torch.cuda.current_stream(self.device).synchronize()
+        """One small D2H copy + sync: the only host<->device sync of a frame step.  After a sampling step the same copy
+        also carries the sampled ids, which sit behind the decision rows."""
         f32 = self._dec_host.view(torch.float32)
-        return [Decision(self._dec_host[i], f32[i]) for i in range(n)]
+        if self._sampled is None:
+            self._dec_host[:n].copy_(self._dec_dev[:n], non_blocking=True)
+            torch.cuda.current_stream(self.device).synchronize()
+            return [Decision(self._dec_host[i], f32[i]) for i in range(n)]
+        end = self._dec_dev.numel() + n
+        self._res_host[:end].copy_(self._res_dev[:end], non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
+        ids = self._res_host[self._dec_dev.numel():end].tolist()
+        sampled = self._sampled
+        return [Decision(self._dec_host[i], f32[i], ids[i] if i < len(sampled) and sampled[i] else None)
+                for i in range(n)]
 
     def last_step_logits(self, n_tokens: int) -> torch.Tensor:
         out = torch.empty(n_tokens, self.cfg.vocab_size, dtype=torch.bfloat16, device=self.device)

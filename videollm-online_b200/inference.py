@@ -23,10 +23,10 @@ from typing import Optional
 
 import torch
 
-from .config import LiveArguments, parse_args
+from .config import LiveArguments, SamplingConfig, parse_args
 from .engine import KvImage
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
-from .speculative import SEP, NgramDrafter, greedy_generate
+from .speculative import SEP, NgramDrafter, generate_ids
 
 logger = logging.getLogger("liveinfer")
 
@@ -45,9 +45,10 @@ class SessionState:
     drafter_ids: Optional[list]  # the NgramDrafter's history (SEP for frame rows), None without one
     n_calls: int
     started: bool                # past_key_values was set: a step ran since the last reset
+    sampling: Optional[SamplingConfig] = None   # LiveInfer.sampling (None: greedy responses)
 
 
-torch.serialization.add_safe_globals([SessionState])
+torch.serialization.add_safe_globals([SessionState, SamplingConfig])
 
 
 class LiveInfer:
@@ -74,6 +75,9 @@ class LiveInfer:
         self.system_prompt = args.system_prompt
         self.inplace_output_ids = torch.zeros(1, 100, dtype=torch.long)  # host buffer: ids are decided on device, read back per token
         self.frame_token_interval_threshold = 0.725
+        # response tokens: None = greedy (the reference's fast_greedy_generate); a SamplingConfig with do_sample draws
+        # them on the device, reproducibly from its seed.  The speak / silent decision is not sampled.
+        self.sampling: Optional[SamplingConfig] = SamplingConfig.from_args(args)
         self.eos_token_id = cfg.eos_token_id
         self.stream_end_id = cfg.stream_end_id
         tok = self.tokenizer
@@ -149,7 +153,7 @@ class LiveInfer:
                 video_time=self.video_time, last_frame_idx=self.last_frame_idx, query_queue=list(self.query_queue),
                 frame_embeds_queue=frames,
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
-                n_calls=self._n_calls, started=self.past_key_values is not None)
+                n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling)
             self.reset()
             return state
 
@@ -175,6 +179,7 @@ class LiveInfer:
                 else:
                     self.drafter.sync(state.kv.n_tokens)
             self._n_calls = state.n_calls
+            self.sampling = state.sampling
             self.past_key_values = self._kv if state.started else None
 
     def load_video(self, video_path_or_tensor, keep_on_host: bool = False):
@@ -256,11 +261,12 @@ class LiveInfer:
         self._n_calls += 1
         return dec
 
-    def _enqueue_step(self, ids: torch.Tensor, frames, n_drafts: int = 0):
+    def _enqueue_step(self, ids: torch.Tensor, frames, n_drafts: int = 0, sample=None):
         """Enqueue one KV-append step over [embed(ids) ; frames[0] ; interval id ; frames[1] ; interval id ; ...].
         With more than one frame every frame is a segment with its own decision (the step is the same arithmetic as
         one step per frame, each fed the interval id of a silent predecessor).  n_drafts (no frames): the last n_drafts
-        ids are one-token segments, each with its own decision.  Returns the segment lengths."""
+        ids are one-token segments, each with its own decision.  sample: Engine.step's, one SampleRow per segment.
+        Returns the segment lengths."""
         eng = self.model.engine
         id_list = [int(x) for x in ids.reshape(-1).tolist()]
         n_ids = len(id_list)
@@ -302,7 +308,7 @@ class LiveInfer:
             pre = torch.cuda.Event()
             pre.record(main)
         eng.step([self._kv.stream_id], [T], packed, row_ids=row_ids,   # token rows gathered on the device
-                 segments=[segs] if len(segs) > 1 else None)
+                 segments=[segs] if len(segs) > 1 else None, sample=sample)
         self.past_key_values = self._kv
         if frames and self.drafter is not None:   # frame rows enter the drafter's history as separators
             hist = list(id_list)
@@ -333,12 +339,14 @@ class LiveInfer:
             self.last_ids = self._added_stream_generation_ids
         ids = [int(x) for x in self.last_ids.reshape(-1).tolist()]
 
-        def step(pending, drafts):
+        def step(pending, drafts, sample=None):
             with self._lock:
-                self._enqueue_step(torch.tensor(pending + drafts, dtype=torch.long), [], n_drafts=len(drafts))
-        # fast_greedy_generate (models/modeling_live.py:173-182), verifying drafts from the session's history
-        out = greedy_generate(self.model.engine, self._kv.stream_id, step, len(ids), self.inplace_output_ids.size(1),
-                              self.eos_token_id, first_ids=ids, drafter=self.drafter, consume=self._consume)
+                self._enqueue_step(torch.tensor(pending + drafts, dtype=torch.long), [], n_drafts=len(drafts),
+                                   sample=sample)
+        # fast_greedy_generate (models/modeling_live.py:173-182), or sampled ids, verifying drafts from the history
+        out = generate_ids(self.model.engine, self._kv.stream_id, step, len(ids), self.inplace_output_ids.size(1),
+                           self.eos_token_id, first_ids=ids, drafter=self.drafter, consume=self._consume,
+                           sampling=self.sampling)
         n = len(out)
         self.inplace_output_ids[0, :n] = torch.tensor(out, dtype=torch.long)
         output_ids = self.inplace_output_ids[:, :n]

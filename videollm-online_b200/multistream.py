@@ -26,8 +26,10 @@ from typing import Callable, Deque, List, Optional, Tuple
 import torch
 
 from ._lib import VloError
-from .engine import KvImage
+from .config import SamplingConfig
+from .engine import KvImage, SampleRow
 from .modeling_live import LiveLlamaForCausalLM
+from .speculative import sample_rows
 
 
 class StreamSession:
@@ -45,6 +47,8 @@ class StreamSession:
             self.stream_id = None
         self.frame_fps = sched.frame_fps
         self.threshold = 0.725
+        # response tokens, as LiveInfer.sampling: None = greedy; each session may have its own config
+        self.sampling: Optional[SamplingConfig] = None
         self.reset()
 
     @property
@@ -127,6 +131,16 @@ class StreamSession:
             ids = list(self.sched.stream_generation_ids)
         self.state, self.resp, self.resp_time, self.resp_query = self.RESPOND, [], video_time, query
         self._next_ids = list(ids)
+        self.resp_prompt = list(ids)   # with the response's ids so far: the repetition penalty's set
+
+    def sample_row(self, n: int) -> Optional[SampleRow]:
+        """The SampleRow of the session's next step of n rows (None: not sampled): a response token, when the session
+        samples.  Position and penalty ids are those LiveInfer gives the same token."""
+        s = self.sampling
+        if self._op is None or self._op[0] != "gen" or s is None or not s.do_sample:
+            return None
+        return sample_rows(s, self.kv_tokens() + n - 1, self.resp_prompt + self.resp, len(self.resp_prompt) +
+                           len(self.resp), 0)[0]
 
     # -- consume the decision of the step this stream took part in
     def advance(self, dec):
@@ -137,7 +151,7 @@ class StreamSession:
         self.started = True
         op, self._op = self._op, None
         if op[0] == "gen":
-            tok = dec.argmax_id
+            tok = dec.argmax_id if dec.sampled_id is None else dec.sampled_id
             self.resp.append(tok)
             if tok == cfg.eos_token_id or len(self.resp) >= self.sched.max_new_tokens:
                 text = self.sched.tokenizer.decode(self.resp, skip_special_tokens=True)
@@ -240,7 +254,9 @@ class StreamScheduler:
         rid = torch.tensor(row_ids, dtype=torch.int64).to(eng.device, non_blocking=True)
         pre = torch.cuda.Event()
         pre.record(main)
-        eng.step([s.stream_id for s, *_ in batch], q_lens, packed, row_ids=rid, want_logits=False)
+        sample = [s.sample_row(n) for s, _, _, n in batch]   # sampling sessions' response rows: one launch for all
+        eng.step([s.stream_id for s, *_ in batch], q_lens, packed, row_ids=rid, want_logits=False,
+                 sample=sample if any(r is not None for r in sample) else None)
         if self.encode_ahead:
             self._launch_encode_ahead(pre)        # enqueued after the step's launches, runs concurrently with it
         decs = eng.read_decisions(len(batch))

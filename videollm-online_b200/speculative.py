@@ -1,4 +1,4 @@
-"""Greedy generation several tokens per decoder step, from n-gram drafts, with the ids of one token per step.
+"""Generation several tokens per decoder step, from n-gram drafts, with the ids of one token per step.
 
 A verify step feeds [pending input | d1 | ... | dk] as k + 1 segments (`Engine.step(..., segments=...)`): every segment
 computes the bits a step of its own computes, so decision j is the one-token loop's decision j as long as d1 .. dj
@@ -7,10 +7,15 @@ cuts the stream back to the inputs that produced them: the ids and the KV cache 
 
 The drafts come from prompt lookup over the session's own token ids (`NgramDrafter`): no second model.  How often they
 are accepted depends on the text; the cost of a rejected draft is the verify step's extra cost over a one-token step.
+
+Sampled responses keep this exactness: the device draws a row's id from its logits, its KV position and the seed only
+(vlo_sample), and segment j of a verify step gets the position and penalty ids the one-token loop has at that token.
 """
 from __future__ import annotations
 
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
+
+from .engine import SampleRow
 
 SEP = -1   # a history entry that is not a token id (a frame row): no n-gram spans it and no draft continues past it
 
@@ -110,17 +115,34 @@ def draft_cap(eng, sid: int, n_prefix: int, remaining: int) -> int:
     return k
 
 
-def greedy_generate(eng, sid: int, step: Callable[[Optional[List[int]], List[int]], None], n_first: int,
-                    max_new: int, eos_token_id: int, *, first_ids: Optional[Sequence[int]] = None, drafter=None,
-                    consume: Optional[Callable] = None, base: int = 0) -> List[int]:
-    """Greedy ids of stream `sid` until EOS or max_new ids, verifying the drafter's proposals on the way.
+def sample_rows(sampling, position0: int, history: List[int], n_history: int, n_drafts: int) -> List[SampleRow]:
+    """The SampleRow of each segment of a step [pending | d1 .. dk] (k = n_drafts): segment j's token sits at KV
+    position position0 + j, and its penalty set is history[:n_history + j] with history = the response's prompt ids,
+    the ids generated so far, then d1 .. dk.  These are the position and the ids the one-token loop has at that token,
+    so segment j draws the id a step of its own would draw."""
+    s = sampling
+    return [SampleRow(s.seed, position0 + j, s.temperature, s.top_k, s.top_p, s.repetition_penalty, history,
+                      n_history + j) for j in range(n_drafts + 1)]
+
+
+def generate_ids(eng, sid: int, step: Callable[..., None], n_first: int, max_new: int, eos_token_id: int, *,
+                 first_ids: Optional[Sequence[int]] = None, drafter=None, consume: Optional[Callable] = None,
+                 base: int = 0, sampling=None) -> List[int]:
+    """Ids of stream `sid` until EOS or max_new ids, verifying the drafter's proposals on the way: the argmax, or with
+    `sampling` (a SamplingConfig with do_sample) the ids the device draws.
 
     step(ids, drafts) enqueues one decoder step of the stream over the pending input ids, then the drafts as one-token
-    segments (segments [[len(ids), 1, ...]]; no drafts: an ordinary step).  The first step's input is n_first rows:
-    ids = first_ids, or None when they are not token ids (the caller feeds its own embeddings).  After it, ids is
-    [previous id].  consume(decision) -> decision sees every decision the one-token loop would act on, in order, and no
-    other.  The drafter's history is the stream's KV from position `base` on (sync / extend / propose)."""
+    segments (segments [[len(ids), 1, ...]]; no drafts: an ordinary step).  When sampling it is called as
+    step(ids, drafts, rows) and passes rows (one SampleRow per segment, `sample_rows`) on as Engine.step(sample=rows).
+    The first step's input is n_first rows: ids = first_ids, or None when they are not token ids (the caller feeds its
+    own embeddings).  After it, ids is [previous id].  consume(decision) -> decision sees every decision the one-token
+    loop would act on, in order, and no other; the loop takes its `sampled_id` when sampling, else its `argmax_id`.
+    The drafter's history is the stream's KV from position `base` on (sync / extend / propose).  The penalty set of a
+    sampled response is first_ids and the ids generated so far."""
+    if sampling is not None and not sampling.do_sample:
+        sampling = None
     out: List[int] = []
+    prompt = list(first_ids) if first_ids is not None else []
     pending: Optional[List[int]] = list(first_ids) if first_ids is not None else None
     n_pending = n_first
     pend_ids = pending if pending is not None else [SEP] * n_first
@@ -134,7 +156,11 @@ def greedy_generate(eng, sid: int, step: Callable[[Optional[List[int]], List[int
             drafts = [int(t) for t in drafter.propose(k)[:k]] if k > 0 else []
             drafter.extend(drafts)
         try:
-            step(pending, drafts)
+            if sampling is None:
+                step(pending, drafts)
+            else:
+                step(pending, drafts, sample_rows(sampling, kv0 + n_pending - 1, prompt + out + drafts,
+                                                  len(prompt) + len(out), len(drafts)))
         except Exception:
             if drafter is not None:
                 drafter.sync(kv0 - base)
@@ -144,7 +170,7 @@ def greedy_generate(eng, sid: int, step: Callable[[Optional[List[int]], List[int
         for j, dec in enumerate(decs):
             if consume is not None:
                 dec = consume(dec)
-            new_id = dec.argmax_id
+            new_id = dec.argmax_id if sampling is None else dec.sampled_id
             out.append(new_id)
             if new_id == eos_token_id or len(out) == max_new or j == len(drafts) or drafts[j] != new_id:
                 break
@@ -157,3 +183,6 @@ def greedy_generate(eng, sid: int, step: Callable[[Optional[List[int]], List[int
         pending = pend_ids = [out[-1]]
         n_pending = 1
     return out
+
+
+greedy_generate = generate_ids   # the loop without `sampling`
