@@ -285,6 +285,15 @@ int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const v
  * current device's SM count. */
 int vlo_op_attn_plan_counts(int n_segs, const int32_t* h_seg_lens, int n_heads, int n_kv_heads, int head_dim, int kv_len,
                             int32_t* h_counts);
+/* The ViT attention kernels of vlo_vit_encode (csrc/vit_kernels.cuh), launched by the same helpers; fp16 tensors,
+ * head_dim 64, hidden = 64 x heads, n_frames frames of n_tok tokens.  Asynchronous.
+ * vit_attn: d_qkv [n_frames * n_tok, 3 * hidden] (q | k | v column blocks, head h at columns 64 h .. of each) ->
+ *   d_out [n_frames * n_tok, hidden] = softmax(q k^T / 8) v over the keys of the query's own frame, per head.
+ * probe_attn (the MAP head): d_kv [n_frames * n_tok, 2 * hidden] (k | v), d_q fp32 [hidden] one query shared by every
+ *   frame -> d_out [n_frames, hidden] = softmax(q k^T / 8) v per head and frame; n_tok <= 12288. */
+int vlo_op_vit_attn(const void* d_qkv, void* d_out, int n_frames, int n_tok, int hidden, void* cuda_stream);
+int vlo_op_probe_attn(const void* d_kv, const float* d_q, void* d_out, int n_frames, int n_tok, int hidden,
+                      void* cuda_stream);
 /* The decoder step's fix-up and decision kernels (csrc/decoder_kernels.cuh), launched by the same helpers as vlo_step
  * (block size, grid, shared memory, PDL).  bf16 tensors unless stated; bf16(.) = round to nearest even.
  * d_part: fp32 stream-K partial planes [plane][T][width] as vlo_op_gemm_ws mode 0 leaves them (plane_stride T * width)

@@ -98,6 +98,8 @@ SIGNATURES = {
     "vlo_op_attn_kvappend_paged": (_I, [_P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P]),
     "vlo_op_attn_kvappend_segments": (_I, [_P, _P, _P, _P, _I, _P, _I, C.POINTER(C.c_int32), _I, _I, _I, _I, _P]),
     "vlo_op_attn_plan_counts": (_I, [_I, C.POINTER(C.c_int32), _I, _I, _I, _I, C.POINTER(C.c_int32)]),
+    "vlo_op_vit_attn": (_I, [_P, _P, _I, _I, _I, _P]),
+    "vlo_op_probe_attn": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "vlo_op_resid_rmsnorm": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
     "vlo_op_qkv_rope_append": (_I, [_P, _I, _I, _P, _P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _I, _P, _P, _P,
                                     _I, _I, _I, _P]),

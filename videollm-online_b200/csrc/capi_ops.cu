@@ -222,6 +222,17 @@ int vlo_op_attn_plan_counts(int n_segs, const int32_t* h_seg_lens, int n_heads, 
   return 0;
 }
 
+int vlo_op_vit_attn(const void* d_qkv, void* d_out, int n_frames, int n_tok, int hidden, void* cuda_stream) {
+  VLO_CHECK(d_qkv != nullptr && d_out != nullptr, "vit_attn: null argument");
+  return vit_attn_launch(d_qkv, d_out, n_frames, n_tok, hidden, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_probe_attn(const void* d_kv, const float* d_q, void* d_out, int n_frames, int n_tok, int hidden,
+                      void* cuda_stream) {
+  VLO_CHECK(d_kv != nullptr && d_q != nullptr && d_out != nullptr, "probe_attn: null argument");
+  return probe_attn_launch(d_kv, d_q, d_out, n_frames, n_tok, hidden, static_cast<cudaStream_t>(cuda_stream));
+}
+
 int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
                          const int32_t* d_last_index, int T, int H, float eps, void* cuda_stream) {
   // the row is staged in shared memory without an opt-in beyond the default 48 KB

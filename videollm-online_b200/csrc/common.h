@@ -170,6 +170,14 @@ int sample_check_rows(const void* h_rows, int n_rows, int n_ids);
 int sample_launch(const void* logits, int n_rows, int vocab, const void* rows, const int* penalty_ids, int* out_ids,
                   void* info, cudaStream_t st);
 
+// ---- ViT attention kernels (vit_kernels.cuh / engine.cu) ------------------------------
+// vit_attn_kernel: non-causal attention of each of B frames of N tokens over its own tokens, head_dim 64, C / 64 heads;
+// qkv fp16 [B * N, 3C] (q | k | v column blocks) -> out fp16 [B * N, C].
+int vit_attn_launch(const void* qkv, void* out, int B, int N, int C, cudaStream_t st);
+// probe_attn_kernel: the MAP head's one fp32 query q [C] over the N tokens of each frame, kv fp16 [B * N, 2C] (k | v)
+// -> out fp16 [B, C].
+int probe_attn_launch(const void* kv, const float* q, void* out, int B, int N, int C, cudaStream_t st);
+
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {
   int q_tok0;          // first packed token of the sequence

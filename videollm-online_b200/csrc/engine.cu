@@ -388,6 +388,35 @@ int decision_launch(const void* logits, int n_rows, int vocab, int interval_id, 
   return 0;
 }
 
+// ------------------------------------------------------------------------------ ViT attention launches
+// vlo_vit_encode and the kernel-level entry points (capi_ops.cu) launch the ViT attention kernels through these only.
+int vit_attn_launch(const void* qkv, void* out, int B, int N, int C, cudaStream_t st) {
+  VLO_CHECK(B > 0 && N > 0 && C > 0 && C % kVitHD == 0, "vit_attn: B, N > 0 and hidden = 64 x heads");
+  VLO_CHECK(static_cast<long long>(B) * N < (1ll << 31), "vit_attn: too many token rows for a TMA map");
+  if (ensure_max_smem(reinterpret_cast<const void*>(vit_attn_kernel), kVitSmemBytes)) return -1;
+  const int rows = B * N;
+  CUtensorMap tm_qkv;
+  if (tmap_2d_sw128(qkv, rows, 3 * C, kVitBlk, FMT_F16, &tm_qkv)) return -1;
+  const float scale_log2 = 1.4426950408889634f / 8.0f;  // head_dim 64
+  prof_begin(PROF_VIT_ATTN, st, 4.0 * rows * C * 2);
+  VLO_CUDA(launch_pdl(vit_attn_kernel, dim3((N + kVitBlk - 1) / kVitBlk, C / kVitHD, B), dim3(kVitThreads), kVitSmemBytes, st,
+                      tm_qkv, static_cast<__half*>(out), N, C, scale_log2));
+  prof_end(st);
+  count_launch();
+  return 0;
+}
+
+int probe_attn_launch(const void* kv, const float* q, void* out, int B, int N, int C, cudaStream_t st) {
+  VLO_CHECK(B > 0 && N > 0 && C > 0 && C % kVitHD == 0, "probe_attn: B, N > 0 and hidden = 64 x heads");
+  // the N scores are staged in shared memory without an opt-in beyond the default 48 KB
+  VLO_CHECK(static_cast<size_t>(N) * sizeof(float) <= 48 * 1024, "probe_attn: N <= 12288 tokens per frame");
+  probe_attn_kernel<<<dim3(C / kVitHD, B), 128, static_cast<size_t>(N) * sizeof(float), st>>>(
+      static_cast<const __half*>(kv), q, static_cast<__half*>(out), N, C, 0.125f);  // head_dim 64
+  VLO_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+
 int sample_check_rows(const void* h_rows, int n_rows, int n_ids) {
   VLO_CHECK(h_rows != nullptr, "sample: null rows");
   const SampleRow* rows = static_cast<const SampleRow*>(h_rows);
@@ -444,7 +473,7 @@ int vlo_engine_create_pooled(const vlo_config* cfg, int64_t kv_pool_tokens, int 
             "max_kv_tokens above " + std::to_string(attn_max_key_blocks() * kKvPageTokens) +
                 " (the attention stages a stream's page table in shared memory)");
   VLO_CHECK(c.max_step_tokens <= 128, "max_step_tokens <= 128 (longer inputs are chunked by the host; chunked == one pass)");
-  VLO_CHECK(c.vit_layers == 0 || (c.vit_hidden % 128 == 0 && c.vit_hidden / c.vit_heads == 64 && c.vit_mlp % 64 == 0),
+  VLO_CHECK(c.vit_layers == 0 || (c.vit_hidden % 128 == 0 && c.vit_hidden == 64 * c.vit_heads && c.vit_mlp % 64 == 0),
             "vision tower: hidden % 64, head_dim == 64");
   VLO_CHECK(c.vit_layers == 0 || (c.image_size % c.patch_size == 0 && (3 * c.patch_size * c.patch_size) % 64 == 0 &&
                                   c.patch_size % 8 == 0),
@@ -902,19 +931,6 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     g.pos_rows = P;
     if (gemm_launch(g, st)) return -1;
   }
-  // ViT attention: mma.sync m16n8k16 over TMA-loaded Q / K / V tiles (vit_kernels.cuh)
-  if (ensure_max_smem(reinterpret_cast<const void*>(vit_attn_kernel), kVitSmemBytes)) return -1;
-  CUtensorMap tm_qkv;
-  if (tmap_2d_sw128(e->v_qkv, rows, 3 * C, kVitBlk, FMT_F16, &tm_qkv)) return -1;
-  const float scale_log2 = 1.4426950408889634f / 8.0f;  // head_dim 64
-  auto launch_vit_attn = [&]() -> int {
-    prof_begin(PROF_VIT_ATTN, st, 4.0 * rows * C * 2);
-    VLO_CUDA(launch_pdl(vit_attn_kernel, dim3((P + kVitBlk - 1) / kVitBlk, c.vit_heads, B), dim3(kVitThreads), kVitSmemBytes, st,
-                        tm_qkv, e->v_attn, P, C, scale_log2));
-    prof_end(st);
-    count_launch();
-    return 0;
-  };
   // Trunk GEMMs: QKV and fc1 run whole tiles with the fused bias / GELU fp16 epilogue; out_proj and fc2 (few
   // output tiles) run stream-K over all SMs on the persistent swap-AB kernel (weights ride MMA-M, the token rows are
   // tiled along MMA-N) and their partial planes are folded into the fp32 residual stream together with the NEXT
@@ -960,7 +976,8 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     const VitLayer& v = e->vit[l];
     GemmWsPlan sk{};
     if (tiles_gemm(e->v_xn, v.qkv_w, 3 * C, C, e->v_qkv, v.qkv_b, ACT_NONE)) return -1;
-    if (launch_vit_attn()) return -1;
+    // ViT attention: mma.sync m16n8k16 over TMA-loaded Q / K / V tiles (vit_kernels.cuh)
+    if (vit_attn_launch(e->v_qkv, e->v_attn, B, P, C, st)) return -1;
     if (partial_gemm(e->v_attn, v.out_w, C, &sk)) return -1;
     if (fix_ln(sk, v.out_b, v.ln2_w, v.ln2_b, nullptr)) return -1;
     if (tiles_gemm(e->v_xn, v.fc1_w, M, C, e->v_mlp, v.fc1_b, ACT_GELU_TANH)) return -1;
@@ -984,8 +1001,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   if (cls) {
     // MAP head: K/V projection of all tokens, 1-query attention, out-proj, LN, MLP, residual
     if (gemm_store16(e->v_xn, rows, e->head_kv_w, 2 * C, C, e->v_qkv, 2 * C, e->head_kv_b, ACT_NONE, st)) return -1;
-    probe_attn_kernel<<<dim3(c.vit_heads, B), 128, static_cast<size_t>(P) * sizeof(float), st>>>(e->v_qkv, e->head_q, e->v_pa, P, C, 0.125f);
-    VLO_LAUNCH_CHECK();
+    if (probe_attn_launch(e->v_qkv, e->head_q, e->v_pa, B, P, C, st)) return -1;
     VLO_CHECK(B <= 128, "MAP head handles <= 128 frames per call");
     if (gemm_ws_store16(FMT_F16, e->head_out_w, C, e->v_pa, B, C, e->v_resid, C, e->head_out_b, ACT_NONE, st)) return -1;
     layernorm_kernel<__half><<<B, 256, ln_smem, st>>>(e->v_resid, e->head_ln_w, e->head_ln_b, e->v_lnh, nullptr, C, c.vit_ln_eps);
@@ -994,7 +1010,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     if (gemm_ws_store16(FMT_F16, e->head_fc2_w, C, e->v_m1, B, M, e->v_m2, C, e->head_fc2_b, ACT_NONE, st)) return -1;
     cls_residual_kernel<<<(B * C + 255) / 256, 256, 0, st>>>(e->v_resid, e->v_m2, e->tokens32, B, C, NT);
     VLO_LAUNCH_CHECK();
-    count_launch(3);
+    count_launch(2);
   }
   const long long ntok_elems = static_cast<long long>(B) * NT * C;
   if (d_vit_tokens)
