@@ -81,9 +81,10 @@ int vlo_engine_create(const vlo_config* cfg, int device, vlo_engine** out);
 /* KV cache = a pool of kv_pool_tokens (rounded up to whole 64-token pages) shared by all streams;
  * max_kv_tokens stays the per-stream cap.  kv_pool_tokens <= 0: max_streams * max_kv_tokens,
  * which is what vlo_engine_create reserves.  A stream holds ceil(kv_len / 64) pages; a step (or
- * vlo_kv_write / vlo_kv_copy_prefix / vlo_kv_fill_synthetic) that needs more pages than are free fails
- * with a "KV page pool exhausted" message and changes no stream.  max_kv_tokens may not exceed 552 896 (the
- * attention stages a split's page table in shared memory). */
+ * vlo_kv_write / vlo_kv_copy_prefix / vlo_kv_fill_synthetic / vlo_kv_swap_in) that needs more pages than are
+ * free fails with a "KV page pool exhausted" message.  Any of these calls that returns non-zero, for this or any
+ * other reason, leaves every stream's kv_len and pages, and the free-page count, as they were before the call.
+ * max_kv_tokens may not exceed 552 896 (the attention stages a split's page table in shared memory). */
 int vlo_engine_create_pooled(const vlo_config* cfg, int64_t kv_pool_tokens, int device, vlo_engine** out);
 int vlo_kv_pool_info(vlo_engine* e, int* page_tokens, int64_t* total_pages, int64_t* free_pages);
 int vlo_engine_destroy(vlo_engine* e);

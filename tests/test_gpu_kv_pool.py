@@ -147,13 +147,19 @@ def test_pool_exhaustion_fails_without_changing_any_stream(tiny):
     assert eng.kv_pool_info()["free_pages"] == 0
     before = {s: (eng.kv_len(s), _kv_all(eng, s)) for s in sids}
     batch, q = [sids[0], sids[4]], [40, 40]   # 600 -> 640 fits its last page, 90 -> 130 needs a third page
-    with pytest.raises(VloError, match="KV page pool exhausted"):
-        eng.step(batch, q, _emb(eng.cfg, sum(q), 7))
-    torch.cuda.synchronize()
-    assert eng.kv_pool_info()["free_pages"] == 0
-    for s in sids:
-        assert eng.kv_len(s) == before[s][0]
-        assert _same_kv(_kv_all(eng, s), before[s][1])
+    rows = torch.ones(eng.cfg.num_key_value_heads, 130, eng.cfg.head_dim, dtype=torch.bfloat16, device="cuda")
+    grows = {"step": lambda: eng.step(batch, q, _emb(eng.cfg, sum(q), 7)),
+             "kv_write": lambda: eng.kv_write(sids[4], 0, False, rows),
+             "kv_fill_synthetic": lambda: eng.kv_fill_synthetic(sids[4], 130, seed=8),
+             "kv_copy_prefix": lambda: eng.kv_copy_prefix(sids[0], sids[4], 200)}
+    for name, grow in grows.items():
+        with pytest.raises(VloError, match="KV page pool exhausted"):
+            grow()
+        torch.cuda.synchronize()
+        assert eng.kv_pool_info()["free_pages"] == 0, name
+        for s in sids:
+            assert eng.kv_len(s) == before[s][0], name
+            assert _same_kv(_kv_all(eng, s), before[s][1]), name
     eng.stream_close(sids[3])
     ref.stream_close(sids[3])
     assert _same_step(_step(eng, batch, q, seed=7), _step(ref, batch, q, seed=7))

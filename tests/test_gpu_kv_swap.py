@@ -110,14 +110,19 @@ def test_round_trip_full_width():
     _round_trip(eng, 1000, seed=7)
 
 
-def test_page_reuse_waits_for_the_swap_out(tiny):
-    """The swap-out runs on a side CUDA stream; right after it, the main stream fills and steps a stream that is handed
-    exactly the released pages (the pool holds nothing else).  The engine makes the main stream wait for the copies, so
-    the image still equals the cache before the swap."""
-    cfg, llm, _ = tiny
-    n = 8000
-    eng = _engine(cfg, llm, 2, 8192, kv_pool_tokens=n)
-    a, b = eng.stream_open(), eng.stream_open()
+def _reuse_after_swap_out(cfg, llm, writer):
+    """a's swap-out runs on a side CUDA stream; right after it, `writer` on the main stream fills stream b, which is
+    handed exactly the released pages (the pool holds nothing else), and b then steps"""
+    n, m = 8000, 7800
+    # kv_copy_prefix needs a source that holds m tokens of its own
+    eng = _engine(cfg, llm, 3, 8192, kv_pool_tokens=n + (m if writer == "kv_copy_prefix" else 0))
+    a, b, src = eng.stream_open(), eng.stream_open(), eng.stream_open()
+    rows = torch.randn(cfg.num_key_value_heads, m, cfg.head_dim, device="cuda").bfloat16()
+    if writer == "kv_copy_prefix":
+        eng.kv_fill_synthetic(src, m, seed=2)
+    if writer == "kv_swap_in":
+        eng.kv_fill_synthetic(b, m, seed=2)
+        img_b = eng.kv_swap_out(b)
     eng.kv_fill_synthetic(a, n, seed=1)
     before = _kv_all(eng, a)
     assert _free(eng) == 0
@@ -126,7 +131,20 @@ def test_page_reuse_waits_for_the_swap_out(tiny):
     with torch.cuda.stream(side):
         img = eng.kv_swap_out(a)
     assert _free(eng) == -(-n // PAGE)        # gated pages count as free
-    eng.kv_fill_synthetic(b, n - 200, seed=2)   # on the main stream, over a's old pages
+    # on the main stream, over a's old pages: b ends up with m tokens
+    if writer == "kv_fill_synthetic":
+        eng.kv_fill_synthetic(b, m, seed=2)
+    elif writer == "kv_write":
+        for layer in range(cfg.num_hidden_layers):
+            for is_v in (False, True):
+                eng.kv_write(b, layer, is_v, rows)
+    elif writer == "kv_copy_prefix":
+        eng.kv_copy_prefix(src, b, m)
+    elif writer == "kv_swap_in":
+        eng.kv_swap_in(b, img_b)
+    else:
+        eng.step([b], [m], _emb(cfg, m, 2))     # split into max_step_tokens pieces, none synchronised
+    assert eng.kv_len(b) == m
     _step(eng, [b], [128], seed=3)
     _step(eng, [b], [72], seed=4)
     assert _free(eng) == 0
@@ -134,6 +152,18 @@ def test_page_reuse_waits_for_the_swap_out(tiny):
     eng.stream_close(b)
     eng.kv_swap_in(a, img)
     assert _same_kv(_kv_all(eng, a), before)
+
+
+def test_page_reuse_waits_for_the_swap_out(tiny):
+    """Whichever call first writes the pages a swap-out released (kv_fill_synthetic, kv_write, kv_copy_prefix,
+    kv_swap_in or a step), the engine makes its CUDA stream wait for the swap-out's copies, so the image still equals
+    the cache before the swap."""
+    cfg, llm, _ = tiny
+    for writer in ("kv_fill_synthetic", "kv_write", "kv_copy_prefix", "kv_swap_in", "step"):
+        try:
+            _reuse_after_swap_out(cfg, llm, writer)
+        except AssertionError as err:
+            raise AssertionError(f"first writer {writer}") from err
 
 
 def test_failed_swap_in_changes_nothing(tiny):

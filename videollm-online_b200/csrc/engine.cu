@@ -63,21 +63,8 @@ struct vlo_engine {
   std::vector<void*> allocs;
   int64_t device_bytes = 0;
   bf16* kv = nullptr;  // [layer][2][page][kv_head][64][128], pages owned through `pool`
-  KvPool pool;
+  KvPool pool;              // every stream slot's cache state
   int* kv_op_pt = nullptr;  // device page tables of the KV copy / fill calls (two streams' worth)
-  std::vector<int> kv_len;
-  std::vector<char> stream_open;
-  // Pages released by vlo_kv_swap_out sit on the free list while the swap-out's device-to-host copies may still read
-  // them: page_gate[p] is the gate (an event recorded after those copies) page p waits for, or -1.  A call that takes a
-  // gated page makes its stream wait on the event; a gate whose event has completed releases its pages for good.
-  struct KvGate {
-    cudaEvent_t ev = nullptr;
-    std::vector<int> pages;
-    bool live = false;
-  };
-  std::vector<KvGate> gates;
-  std::vector<int> page_gate;
-  int live_gates = 0;
   size_t max_pitch = 0;  // cudaDevAttrMaxPitch: the plane stride of a swap's 2D copies must not exceed it
 
   // decoder workspaces
@@ -235,7 +222,7 @@ int stage_page_tables(const vlo_engine* e, uint8_t* hs, int n, const int* sids, 
   int* dst = reinterpret_cast<int*>(hs + e->meta.pt);
   int used = 0;
   for (int i = 0; i < n; ++i) {
-    const std::vector<int>& tab = e->pool.tables[sids[i]];
+    const std::vector<int>& tab = e->pool.table(sids[i]);
     std::memcpy(dst + used, tab.data(), sizeof(int) * tab.size());
     pt0[i] = used;
     used += static_cast<int>(tab.size());
@@ -289,45 +276,9 @@ struct DevGuard {
 
 int check_stream(vlo_engine* e, int sid) {
   if (e == nullptr) return fail("null engine");
-  if (sid < 0 || sid >= e->cfg.max_streams || !e->stream_open[sid]) return fail("invalid stream id " + std::to_string(sid));
+  if (sid < 0 || sid >= e->cfg.max_streams || !e->pool.is_open(sid)) return fail("invalid stream id " + std::to_string(sid));
   return 0;
 }
-
-// Release the gates whose swap-out copies have completed: their pages are ordinary free (or taken) pages again.
-int retire_gates(vlo_engine* e) {
-  for (size_t g = 0; g < e->gates.size() && e->live_gates > 0; ++g) {
-    vlo_engine::KvGate& gate = e->gates[g];
-    if (!gate.live) continue;
-    const cudaError_t q = cudaEventQuery(gate.ev);
-    if (q == cudaErrorNotReady) continue;
-    VLO_CUDA(q);
-    for (int p : gate.pages)
-      if (e->page_gate[p] == static_cast<int>(g)) e->page_gate[p] = -1;
-    gate.pages.clear();
-    gate.live = false;
-    --e->live_gates;
-  }
-  return 0;
-}
-
-// Stream st is about to write the pages stream sid holds from table entry `from` on (just taken from the pool): make
-// it wait for the swap-out copies that may still read any of them.  No gate alive: nothing is enqueued.
-int wait_taken_pages(vlo_engine* e, int sid, size_t from, cudaStream_t st) {
-  if (e->live_gates == 0) return 0;
-  if (retire_gates(e)) return -1;
-  const std::vector<int>& tab = e->pool.tables[sid];
-  std::vector<char> waited(e->gates.size(), 0);
-  for (size_t j = from; j < tab.size(); ++j) {
-    const int g = e->page_gate[tab[j]];
-    if (g < 0 || waited[g]) continue;
-    VLO_CUDA(cudaStreamWaitEvent(st, e->gates[g].ev, 0));
-    waited[g] = 1;
-  }
-  return 0;
-}
-
-// pages stream sid holds: the table entry of the first page a call that grows the stream takes
-inline size_t table_size(const vlo_engine* e, int sid) { return e->pool.tables[sid].size(); }
 
 // bytes of one page in one layer's K or V matrix
 inline size_t kv_page_bytes(const vlo_engine* e) {
@@ -486,8 +437,6 @@ int vlo_engine_create_pooled(const vlo_config* cfg, int64_t kv_pool_tokens, int 
   e->n_patches = e->grid * e->grid;
   e->patch_k = 3 * c.patch_size * c.patch_size;
   e->n_frame_tokens = (c.frame_token_cls ? 1 : 0) + c.pool_h * c.pool_w;
-  e->kv_len.assign(c.max_streams, 0);
-  e->stream_open.assign(c.max_streams, 0);
   const int rc = engine_init(e, kv_pool_tokens);
   if (rc != 0) {   // no half-built engine escapes: free what was allocated, keep the error text
     const std::string msg = last_error();
@@ -511,7 +460,6 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
                                            : static_cast<int64_t>(c.max_streams) * per_stream;
   VLO_CHECK(pages * c.num_kv_heads * kKvPageTokens < (1ll << 31), "KV pool too large for one TMA map per layer");
   e->pool.init(c.max_streams, c.num_kv_heads, static_cast<int>(pages));
-  e->page_gate.assign(static_cast<size_t>(pages), -1);
   int max_pitch = 0;
   VLO_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, e->device));
   e->max_pitch = static_cast<size_t>(max_pitch);
@@ -588,8 +536,6 @@ int vlo_engine_destroy(vlo_engine* e) {
   if (e->stage) cudaFreeHost(e->stage);
   for (int i = 0; i < kStageSlots; ++i)
     if (e->stage_events[i]) cudaEventDestroy(e->stage_events[i]);
-  for (auto& g : e->gates)
-    if (g.ev) cudaEventDestroy(g.ev);
   delete e;
   return 0;
 }
@@ -674,26 +620,16 @@ int vlo_finalize_weights(vlo_engine* e) {
 // ------------------------------------------------------------------------------ streams
 int vlo_stream_open(vlo_engine* e, int* stream_id) {
   VLO_CHECK(e != nullptr && stream_id != nullptr, "null argument");
-  for (int i = 0; i < e->cfg.max_streams; ++i)
-    if (!e->stream_open[i]) {
-      e->stream_open[i] = 1;
-      e->kv_len[i] = 0;
-      *stream_id = i;
-      return 0;
-    }
-  return fail("no free stream slot (max_streams = " + std::to_string(e->cfg.max_streams) + ")");
+  return e->pool.open(stream_id);
 }
 int vlo_stream_reset(vlo_engine* e, int sid) {
   if (check_stream(e, sid)) return -1;
-  e->pool.resize(sid, 0);
-  e->kv_len[sid] = 0;
+  e->pool.commit(sid, 0);
   return 0;
 }
 int vlo_stream_close(vlo_engine* e, int sid) {
   if (check_stream(e, sid)) return -1;
-  e->pool.resize(sid, 0);
-  e->stream_open[sid] = 0;
-  e->kv_len[sid] = 0;
+  e->pool.close(sid);
   return 0;
 }
 int vlo_kv_pool_info(vlo_engine* e, int* page_tokens, int64_t* total_pages, int64_t* free_pages) {
@@ -705,14 +641,13 @@ int vlo_kv_pool_info(vlo_engine* e, int* page_tokens, int64_t* total_pages, int6
 }
 int vlo_kv_len(vlo_engine* e, int sid, int* out_len) {
   if (check_stream(e, sid)) return -1;
-  *out_len = e->kv_len[sid];
+  *out_len = e->pool.len(sid);
   return 0;
 }
 int vlo_kv_truncate(vlo_engine* e, int sid, int new_len) {
   if (check_stream(e, sid)) return -1;
-  VLO_CHECK(new_len >= 0 && new_len <= e->kv_len[sid], "kv_truncate: new_len must be within [0, kv_len]");
-  e->pool.resize(sid, new_len);
-  e->kv_len[sid] = new_len;
+  VLO_CHECK(new_len >= 0 && new_len <= e->pool.len(sid), "kv_truncate: new_len must be within [0, kv_len]");
+  e->pool.commit(sid, new_len);
   return 0;
 }
 int vlo_kv_fill_synthetic(vlo_engine* e, int sid, int n_tokens, uint64_t seed, void* cuda_stream) {
@@ -720,17 +655,17 @@ int vlo_kv_fill_synthetic(vlo_engine* e, int sid, int n_tokens, uint64_t seed, v
   if (check_stream(e, sid)) return -1;
   const vlo_config& c = e->cfg;
   VLO_CHECK(n_tokens >= 0 && n_tokens <= c.max_kv_tokens, "kv_fill: n_tokens out of range");
-  const size_t had = table_size(e, sid);
-  if (e->pool.resize(sid, n_tokens)) return -1;
-  e->kv_len[sid] = n_tokens;
-  if (n_tokens == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  if (wait_taken_pages(e, sid, had, st)) return -1;
-  const int* d_pt;
-  if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
-  kv_fill_kernel<<<dim3(std::min(64, (n_tokens * 128 + 255) / 256), c.num_kv_heads, 2 * c.num_layers), 256, 0, st>>>(
-      kv_paged_side(e, e->kv, d_pt), c.num_kv_heads, n_tokens, sid, c.max_kv_tokens, seed);
-  VLO_LAUNCH_CHECK();
+  KvGrowth growth{e->pool};
+  if (e->pool.grow(1, &sid, &n_tokens, st)) return -1;
+  if (n_tokens > 0) {
+    const int* d_pt;
+    if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
+    kv_fill_kernel<<<dim3(std::min(64, (n_tokens * 128 + 255) / 256), c.num_kv_heads, 2 * c.num_layers), 256, 0, st>>>(
+        kv_paged_side(e, e->kv, d_pt), c.num_kv_heads, n_tokens, sid, c.max_kv_tokens, seed);
+    VLO_LAUNCH_CHECK();
+  }
+  e->pool.commit(sid, n_tokens);
   return 0;
 }
 
@@ -748,7 +683,7 @@ int vlo_kv_read(vlo_engine* e, int sid, int layer, int is_v, void* d_out, void* 
   const vlo_config& c = e->cfg;
   VLO_CHECK(layer >= 0 && layer < c.num_layers, "layer out of range");
   VLO_CHECK((reinterpret_cast<uintptr_t>(d_out) & 15) == 0, "kv_read: d_out must be 16-byte aligned");
-  const int len = e->kv_len[sid];
+  const int len = e->pool.len(sid);
   if (len == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const int* d_pt;
@@ -763,15 +698,16 @@ int vlo_kv_write(vlo_engine* e, int sid, int layer, int is_v, const void* d_in, 
   VLO_CHECK(layer >= 0 && layer < c.num_layers, "layer out of range");
   VLO_CHECK(n_tokens > 0 && n_tokens <= c.max_kv_tokens, "kv_write: n_tokens out of range");
   VLO_CHECK((reinterpret_cast<uintptr_t>(d_in) & 15) == 0, "kv_write: d_in must be 16-byte aligned");
-  const size_t had = table_size(e, sid);
-  if (e->pool.resize(sid, n_tokens)) return -1;
-  e->kv_len[sid] = n_tokens;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  if (wait_taken_pages(e, sid, had, st)) return -1;
+  KvGrowth growth{e->pool};
+  if (e->pool.grow(1, &sid, &n_tokens, st)) return -1;
   const int* d_pt;
   if (upload_op_tables(e, 1, &sid, &d_pt, st)) return -1;
-  return launch_kv_copy(KvSide{static_cast<bf16*>(const_cast<void*>(d_in)), nullptr, 0, n_tokens},
-                        kv_paged_side(e, kv_layer_base(e, layer, is_v), d_pt), c.num_kv_heads, n_tokens, 1, st);
+  if (launch_kv_copy(KvSide{static_cast<bf16*>(const_cast<void*>(d_in)), nullptr, 0, n_tokens},
+                     kv_paged_side(e, kv_layer_base(e, layer, is_v), d_pt), c.num_kv_heads, n_tokens, 1, st))
+    return -1;
+  e->pool.commit(sid, n_tokens);
+  return 0;
 }
 
 int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, void* cuda_stream) {
@@ -779,22 +715,20 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, vo
   if (check_stream(e, src_sid) || check_stream(e, dst_sid)) return -1;
   const vlo_config& c = e->cfg;
   VLO_CHECK(src_sid != dst_sid, "kv_copy_prefix: source and destination streams must differ");
-  VLO_CHECK(n_tokens >= 0 && n_tokens <= e->kv_len[src_sid], "kv_copy_prefix: n_tokens exceeds the source length");
-  // the destination's pages are dropped and fresh ones taken: check first, so a short pool changes nothing
-  const int n_pages = kv_pages_for(n_tokens);
-  const int have = static_cast<int>(e->pool.tables[dst_sid].size());
-  if (n_pages > e->pool.free_pages() + have) return e->pool.resize(dst_sid, n_tokens);  // fails with the pool's message
-  e->pool.resize(dst_sid, 0);
-  e->pool.resize(dst_sid, n_tokens);
-  e->kv_len[dst_sid] = n_tokens;
-  if (n_tokens == 0) return 0;
+  VLO_CHECK(n_tokens >= 0 && n_tokens <= e->pool.len(src_sid), "kv_copy_prefix: n_tokens exceeds the source length");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  if (wait_taken_pages(e, dst_sid, 0, st)) return -1;
-  const int sids[2] = {src_sid, dst_sid};
-  const int* d_pt[2];
-  if (upload_op_tables(e, 2, sids, d_pt, st)) return -1;
-  return launch_kv_copy(kv_paged_side(e, e->kv, d_pt[0]), kv_paged_side(e, e->kv, d_pt[1]), c.num_kv_heads, n_tokens,
-                        2 * c.num_layers, st);
+  KvGrowth growth{e->pool};
+  if (n_tokens > 0) {  // the copy overwrites the destination from position 0: it waits for swap-outs of any of its pages
+    if (e->pool.grow(1, &dst_sid, &n_tokens, st, true)) return -1;
+    const int sids[2] = {src_sid, dst_sid};
+    const int* d_pt[2];
+    if (upload_op_tables(e, 2, sids, d_pt, st)) return -1;
+    if (launch_kv_copy(kv_paged_side(e, e->kv, d_pt[0]), kv_paged_side(e, e->kv, d_pt[1]), c.num_kv_heads, n_tokens,
+                       2 * c.num_layers, st))
+      return -1;
+  }
+  e->pool.commit(dst_sid, n_tokens);
+  return 0;
 }
 
 // ------------------------------------------------------------------------------ host images of a stream's cache
@@ -806,7 +740,7 @@ int swap_copies(vlo_engine* e, int sid, uint8_t* h, bool to_host, cudaStream_t s
   const size_t planes = static_cast<size_t>(2) * e->cfg.num_layers;
   VLO_CHECK(pitch <= e->max_pitch, "kv swap: the pool's plane stride (" + std::to_string(pitch) +
                                        " B) exceeds the device's maximum copy pitch");
-  const std::vector<int>& tab = e->pool.tables[sid];
+  const std::vector<int>& tab = e->pool.table(sid);
   for (size_t j = 0; j < tab.size(); ++j) {
     uint8_t* dev = reinterpret_cast<uint8_t*>(e->kv) + static_cast<size_t>(tab[j]) * pb;
     uint8_t* host = h + j * planes * pb;
@@ -834,47 +768,30 @@ int64_t vlo_kv_image_bytes(vlo_engine* e, int n_tokens) {
 int vlo_kv_swap_out(vlo_engine* e, int sid, void* h_dst, int64_t bytes, void* cuda_stream) {
   DevGuard dev_guard(e);
   if (check_stream(e, sid)) return -1;
-  const int n = e->kv_len[sid];
+  const int n = e->pool.len(sid);
   if (n == 0) return 0;
   VLO_CHECK(h_dst != nullptr && bytes >= vlo_kv_image_bytes(e, n),
             "kv_swap_out: the host image needs " + std::to_string(vlo_kv_image_bytes(e, n)) + " bytes");
   if (check_pinned(h_dst, "kv_swap_out")) return -1;
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   if (swap_copies(e, sid, static_cast<uint8_t*>(h_dst), true, st)) return -1;
-  if (retire_gates(e)) return -1;
-  size_t g = 0;
-  while (g < e->gates.size() && e->gates[g].live) ++g;
-  if (g == e->gates.size()) {
-    e->gates.emplace_back();
-    VLO_CUDA(cudaEventCreateWithFlags(&e->gates[g].ev, cudaEventDisableTiming));
-  }
-  vlo_engine::KvGate& gate = e->gates[g];
-  VLO_CUDA(cudaEventRecord(gate.ev, st));
-  gate.pages = e->pool.tables[sid];
-  gate.live = true;
-  ++e->live_gates;
-  for (int p : gate.pages) e->page_gate[p] = static_cast<int>(g);
-  e->pool.resize(sid, 0);
-  e->kv_len[sid] = 0;
-  return 0;
+  return e->pool.swap_out(sid, st);
 }
 
 int vlo_kv_swap_in(vlo_engine* e, int sid, const void* h_src, int n_tokens, void* cuda_stream) {
   DevGuard dev_guard(e);
   if (check_stream(e, sid)) return -1;
-  VLO_CHECK(e->kv_len[sid] == 0, "kv_swap_in: the stream must be empty (kv_len " + std::to_string(e->kv_len[sid]) + ")");
+  VLO_CHECK(e->pool.len(sid) == 0, "kv_swap_in: the stream must be empty (kv_len " + std::to_string(e->pool.len(sid)) + ")");
   VLO_CHECK(n_tokens >= 0 && n_tokens <= e->cfg.max_kv_tokens, "kv_swap_in: n_tokens out of range");
   if (n_tokens == 0) return 0;
   VLO_CHECK(h_src != nullptr, "kv_swap_in: null host image");
   if (check_pinned(h_src, "kv_swap_in")) return -1;
-  if (e->pool.resize(sid, n_tokens)) return -1;  // fails with the pool's message, nothing taken
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-  if (wait_taken_pages(e, sid, 0, st) ||
-      swap_copies(e, sid, static_cast<uint8_t*>(const_cast<void*>(h_src)), false, st)) {
-    e->pool.resize(sid, 0);
+  KvGrowth growth{e->pool};
+  if (e->pool.grow(1, &sid, &n_tokens, st) ||
+      swap_copies(e, sid, static_cast<uint8_t*>(const_cast<void*>(h_src)), false, st))
     return -1;
-  }
-  e->kv_len[sid] = n_tokens;
+  e->pool.commit(sid, n_tokens);
   return 0;
 }
 
@@ -1051,7 +968,7 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   VLO_CHECK(h_stream_ids != nullptr && h_seg_lens != nullptr, "step: null argument");
   const int H = c.hidden_size;
   int T = 0, n_rows = 0;
-  std::vector<int> q_lens(n_seqs), seg0(n_seqs);  // seg0[i]: index of sequence i's first segment
+  std::vector<int> q_lens(n_seqs), seg0(n_seqs), ends(n_seqs);  // seg0[i]: index of sequence i's first segment
   for (int i = 0; i < n_seqs; ++i) {
     if (check_stream(e, h_stream_ids[i])) return -1;
     for (int j = 0; j < i; ++j) VLO_CHECK(h_stream_ids[j] != h_stream_ids[i], "step: a stream appears twice in one batch");
@@ -1064,41 +981,16 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
       q_lens[i] += q_len;
     }
     n_rows += n_segs;
-    VLO_CHECK(e->kv_len[h_stream_ids[i]] + q_lens[i] <= c.max_kv_tokens,
-              "step: KV cache capacity exceeded for stream " + std::to_string(h_stream_ids[i]));
+    ends[i] = e->pool.len(h_stream_ids[i]) + q_lens[i];
+    VLO_CHECK(ends[i] <= c.max_kv_tokens, "step: KV cache capacity exceeded for stream " + std::to_string(h_stream_ids[i]));
     T += q_lens[i];
   }
   // every segment holds at least one token, so the n_rows <= T decision rows fit the buffers sized in engine_init
   VLO_CHECK(T <= c.max_step_tokens, "step: total new tokens exceed max_step_tokens");
   const int32_t* h_q_lens = q_lens.data();
-  // ---- pages for the new tokens, taken before anything is enqueued; a short pool fails with no stream changed
-  {
-    int need = 0;
-    for (int i = 0; i < n_seqs; ++i) need += e->pool.missing(h_stream_ids[i], e->kv_len[h_stream_ids[i]] + h_q_lens[i]);
-    if (need > e->pool.free_pages())
-      return fail("step: KV page pool exhausted: the step needs " + std::to_string(need) + " more pages of " +
-                  std::to_string(kKvPageTokens) + " tokens, " + std::to_string(e->pool.free_pages()) + " of " +
-                  std::to_string(e->pool.n_pages) + " are free");
-    for (int i = 0; i < n_seqs; ++i) {
-      const size_t had = table_size(e, h_stream_ids[i]);
-      e->pool.resize(h_stream_ids[i], e->kv_len[h_stream_ids[i]] + h_q_lens[i]);
-      if (wait_taken_pages(e, h_stream_ids[i], had, st)) {
-        for (int j = 0; j <= i; ++j) e->pool.resize(h_stream_ids[j], e->kv_len[h_stream_ids[j]]);
-        return -1;
-      }
-    }
-  }
-  // a failure before the lengths are committed gives the pages back: every table stays ceil(kv_len / 64) long
-  struct PageRollback {
-    vlo_engine* e;
-    int n;
-    const int32_t* sids;
-    bool armed = true;
-    ~PageRollback() {
-      if (armed)
-        for (int i = 0; i < n; ++i) e->pool.resize(sids[i], e->kv_len[sids[i]]);
-    }
-  } rollback{e, n_seqs, h_stream_ids};
+  // ---- pages for the new tokens, taken before anything is enqueued
+  KvGrowth growth{e->pool};
+  if (e->pool.grow(n_seqs, h_stream_ids, ends.data(), st)) return -1;
 
   // ---- per-step metadata: built on the host, one pinned slot, uploaded once, reused by all layers
   uint8_t* hs;
@@ -1113,7 +1005,7 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   std::vector<AttnSeq> seqs(n_seqs);
   int t = 0;
   for (int i = 0; i < n_seqs; ++i) {
-    const int sid = h_stream_ids[i], ql = h_q_lens[i], past = e->kv_len[sid];
+    const int sid = h_stream_ids[i], ql = h_q_lens[i], past = e->pool.len(sid);
     const int n_segs = h_seg_counts ? h_seg_counts[i] : 1;
     first_rows[i] = t;
     for (int j = 0; j < ql; ++j) {
@@ -1181,8 +1073,7 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
                       st))
     return -1;
 
-  for (int i = 0; i < n_seqs; ++i) e->kv_len[h_stream_ids[i]] += h_q_lens[i];
-  rollback.armed = false;
+  for (int i = 0; i < n_seqs; ++i) e->pool.commit(h_stream_ids[i], ends[i]);
   e->last_step_tokens = T;
   return 0;
 }
@@ -1248,8 +1139,7 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   for (int i = 0; i < n_seqs; ++i) {
     if (check_stream(e, h_stream_ids[i])) return -1;
-    const int kv_len = e->kv_len[h_stream_ids[i]];
-    VLO_CHECK(kv_len >= n_tok, "bench_attn: need kv_len >= n_tok");
+    VLO_CHECK(e->pool.len(h_stream_ids[i]) >= n_tok, "bench_attn: need kv_len >= n_tok");
   }
   // the streams' page tables go up in the same region and memcpy as a step's
   uint8_t* hs;
@@ -1258,7 +1148,7 @@ int vlo_bench_attn(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, int n
   std::vector<int> pt0(n_seqs);
   const int n_pt = stage_page_tables(e, hs, n_seqs, h_stream_ids, pt0.data());
   std::vector<AttnSeq> seqs(n_seqs);
-  for (int i = 0; i < n_seqs; ++i) seqs[i] = AttnSeq{i * n_tok, n_tok, e->kv_len[h_stream_ids[i]], pt0[i]};
+  for (int i = 0; i < n_seqs; ++i) seqs[i] = AttnSeq{i * n_tok, n_tok, e->pool.len(h_stream_ids[i]), pt0[i]};
   VLO_CUDA(cudaMemcpyAsync(e->meta_dev + e->meta.pt, hs + e->meta.pt, sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
   AttnPlan plan{};
   if (attn_plan(&plan, e->attn_ws, hs + e->meta.bytes, seqs.data(), n_seqs, n_seqs * n_tok, c.num_heads, c.num_kv_heads,
