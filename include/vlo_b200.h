@@ -108,6 +108,21 @@ int vlo_kv_truncate(vlo_engine* e, int stream_id, int new_len);      /* trim_pas
  * The engine-side form of `trim_past_key_values(past_key_values, 0, n)` when the ORIGINAL cache must survive
  * (stream_evaluate's look-ahead, models/modeling_live.py:112-113,170-171). */
 int vlo_kv_copy_prefix(vlo_engine* e, int src_stream_id, int dst_stream_id, int n_tokens, void* cuda_stream);
+/* Sliding window over a stream's cache (StreamingLLM): drop cache positions [first_token, first_token + n_tokens) and
+ * move the later ones down by n_tokens, so positions stay contiguous.  first_token and n_tokens are multiples of the
+ * page size (64), n_tokens > 0, and every dropped page is full: first_token + n_tokens <= 64 * floor(kv_len / 64).
+ * The dropped pages leave the stream's table and go back to the pool; no row moves.  V rows are unchanged; every kept
+ * K row after the dropped range is rotated in place by -n_tokens positions (one kernel over all layers and kv heads):
+ *   k'[d]      = bf16(fl(fl(x1 * cos_d) + fl(x2 * sin_d)))
+ *   k'[d + 64] = bf16(fl(fl(x2 * cos_d) - fl(x1 * sin_d)))        x1 = k[d], x2 = k[d + 64], d < head_dim / 2
+ * with each fl one fp32 round-to-nearest (no FMA), cos_d / sin_d = h_cos[d] / h_sin[d] (host arrays of head_dim / 2
+ * fp32 values: cos / sin of n_tokens * inv_freq[d], weights.rope_rotation).  Rows past kv_len on the last page are
+ * left as they are.  The tables go through the pinned staging ring (no host synchronisation); the kernel is enqueued on
+ * cuda_stream.  Ordering as vlo_kv_truncate: the stream is shorter on return, and the caller orders the call after the
+ * work that wrote the stream and before work that reads it (usual stream / event rules).  A call that fails changes no
+ * stream's length or table and no free-page count. */
+int vlo_kv_evict(vlo_engine* e, int stream_id, int first_token, int n_tokens, const float* h_cos, const float* h_sin,
+                 void* cuda_stream);
 /* test/bench hook: fill a stream's KV cache with deterministic pseudo-random values up to n_tokens
  * (pre-fill for the 12k-context measurements without replaying 1200 frames) */
 int vlo_kv_fill_synthetic(vlo_engine* e, int stream_id, int n_tokens, uint64_t seed, void* cuda_stream);

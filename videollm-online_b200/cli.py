@@ -4,6 +4,8 @@
         [--do_sample --temperature 0.6 --top_p 0.9 --top_k 50 --repetition_penalty 1.1 --sample_seed 0]
 
 Responses are greedy unless --do_sample is given (SamplingConfig; --seed stays the synthetic weights' seed).
+--context_window N keeps the session's cache within N tokens (0: off): the start prompt stays, the oldest pages after it
+are dropped.
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

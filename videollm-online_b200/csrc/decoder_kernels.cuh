@@ -412,4 +412,43 @@ __global__ void __launch_bounds__(256) kv_fill_kernel(const KvSide dst, int n_kv
   }
 }
 
+// KV eviction: rotate the keys of positions [pos0, pos0 + n_tok) of every kv head and layer by -delta in place, so that
+// a key RoPE put at position p sits at p - delta (V has no position in it and is not touched).  With the RoPE pairs
+// (d, d + 64) of qkv_rope_append_kernel and cs = [c_0 .. c_63 | s_0 .. s_63], c_d = cos(delta f_d), s_d = sin(delta f_d):
+//   k'[d]      = bf16(fl(fl(x1 c_d) + fl(x2 s_d)))
+//   k'[d + 64] = bf16(fl(fl(x2 c_d) - fl(x1 s_d)))
+// every fl one fp32 round-to-nearest (no FMA contraction), so an fp32 emulation reproduces it bit for bit.  Each thread
+// rotates eight pairs of one row (two 16-byte loads and stores); no row depends on another.  K of layer l is plane 2 l.
+// grid = (ceil(n_tok * 8 / 256), n_kv_heads, layers), block = 256.
+__global__ void __launch_bounds__(256) kv_rerotate_kernel(const KvSide k, int n_kv, int pos0, int n_tok, const float* cs) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(n_tok) * 8) return;
+  const int pos = pos0 + static_cast<int>(i >> 3), d0 = static_cast<int>(i & 7) * 8, h = blockIdx.y, l = blockIdx.z;
+  __nv_bfloat16* row = k.base + 2ll * l * k.plane_stride + kv_side_row(k, n_kv, h, pos) * 128;
+  uint4* lo = reinterpret_cast<uint4*>(row + d0);
+  uint4* hi = reinterpret_cast<uint4*>(row + 64 + d0);
+  const uint4 a = *lo, b = *hi;
+  float c[8], s[8];
+  *reinterpret_cast<float4*>(c) = *reinterpret_cast<const float4*>(cs + d0);
+  *reinterpret_cast<float4*>(c + 4) = *reinterpret_cast<const float4*>(cs + d0 + 4);
+  *reinterpret_cast<float4*>(s) = *reinterpret_cast<const float4*>(cs + 64 + d0);
+  *reinterpret_cast<float4*>(s + 4) = *reinterpret_cast<const float4*>(cs + 64 + d0 + 4);
+  const uint32_t wa[4] = {a.x, a.y, a.z, a.w}, wb[4] = {b.x, b.y, b.z, b.w};
+  uint32_t oa[4], ob[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 x1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wa[j]));
+    const float2 x2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wb[j]));
+    const float c0 = c[2 * j], c1 = c[2 * j + 1], s0 = s[2 * j], s1 = s[2 * j + 1];
+    const __nv_bfloat162 r1 = __floats2bfloat162_rn(__fadd_rn(__fmul_rn(x1.x, c0), __fmul_rn(x2.x, s0)),
+                                                    __fadd_rn(__fmul_rn(x1.y, c1), __fmul_rn(x2.y, s1)));
+    const __nv_bfloat162 r2 = __floats2bfloat162_rn(__fsub_rn(__fmul_rn(x2.x, c0), __fmul_rn(x1.x, s0)),
+                                                    __fsub_rn(__fmul_rn(x2.y, c1), __fmul_rn(x1.y, s1)));
+    oa[j] = *reinterpret_cast<const uint32_t*>(&r1);
+    ob[j] = *reinterpret_cast<const uint32_t*>(&r2);
+  }
+  *lo = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+  *hi = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+}
+
 }  // namespace vlo

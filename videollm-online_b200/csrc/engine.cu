@@ -24,6 +24,7 @@ namespace {
 constexpr int kStageSlots = 16;
 constexpr int kSamplePenaltyIds = 65536;  // penalty ids one vlo_sample call may pass
 constexpr int kSkFlags = 4096;  // stream-K arrival counters of the fused gate|up GEMM: one per 128-row weight tile
+constexpr int kRotFloats = 128;  // vlo_kv_evict's cos | sin (head_dim / 2 each), staged ahead of the stream's table
 
 using bf16 = __nv_bfloat16;
 
@@ -64,7 +65,8 @@ struct vlo_engine {
   int64_t device_bytes = 0;
   bf16* kv = nullptr;  // [layer][2][page][kv_head][64][128], pages owned through `pool`
   KvPool pool;              // every stream slot's cache state
-  int* kv_op_pt = nullptr;  // device page tables of the KV copy / fill calls (two streams' worth)
+  // device page tables of the KV copy / fill calls (two streams' worth), or an eviction's cos | sin then its table
+  int* kv_op_pt = nullptr;
   size_t max_pitch = 0;  // cudaDevAttrMaxPitch: the plane stride of a swap's 2D copies must not exceed it
 
   // decoder workspaces
@@ -465,7 +467,7 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   e->max_pitch = static_cast<size_t>(max_pitch);
   const size_t kv_elems = static_cast<size_t>(c.num_layers) * 2 * e->pool.rows_per_layer() * c.head_dim;
   if (dev_alloc_t(e, &e->kv, kv_elems, true)) return -1;
-  if (dev_alloc_t(e, &e->kv_op_pt, static_cast<size_t>(2) * per_stream)) return -1;
+  if (dev_alloc_t(e, &e->kv_op_pt, static_cast<size_t>(2) * per_stream + kRotFloats)) return -1;
   if (dev_alloc_t(e, &e->h, static_cast<size_t>(T) * H)) return -1;
   if (dev_alloc_t(e, &e->xn, static_cast<size_t>(T) * H)) return -1;
   // decision rows: one per sequence, or one per segment of a segmented step (each segment holds >= 1 of the T tokens)
@@ -728,6 +730,42 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_sid, int dst_sid, int n_tokens, vo
       return -1;
   }
   e->pool.commit(dst_sid, n_tokens);
+  return 0;
+}
+
+int vlo_kv_evict(vlo_engine* e, int sid, int first_token, int n_tokens, const float* h_cos, const float* h_sin,
+                 void* cuda_stream) {
+  DevGuard dev_guard(e);
+  if (check_stream(e, sid)) return -1;
+  const vlo_config& c = e->cfg;
+  VLO_CHECK(h_cos != nullptr && h_sin != nullptr, "kv_evict: null cos / sin table");
+  VLO_CHECK(n_tokens > 0 && first_token >= 0 && first_token % kKvPageTokens == 0 && n_tokens % kKvPageTokens == 0,
+            "kv_evict: first_token >= 0 and n_tokens > 0 must be multiples of " + std::to_string(kKvPageTokens));
+  const int len = e->pool.len(sid), full = len / kKvPageTokens * kKvPageTokens;
+  VLO_CHECK(static_cast<long long>(first_token) + n_tokens <= full,
+            "kv_evict: every dropped page must be full: first_token + n_tokens <= " + std::to_string(full) + " (kv_len " +
+                std::to_string(len) + ")");
+  const int kept = len - first_token - n_tokens;  // positions after the dropped range: their keys move by -n_tokens
+  if (kept > 0) {
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    // one staging slot, one copy: cos | sin | the stream's current table (the kernel addresses the old positions)
+    uint8_t* hs;
+    int slot;
+    if (stage_acquire(e, &hs, &slot)) return -1;
+    const std::vector<int>& tab = e->pool.table(sid);
+    float* rot = reinterpret_cast<float*>(hs + e->meta.pt);
+    std::memcpy(rot, h_cos, sizeof(float) * c.head_dim / 2);
+    std::memcpy(rot + c.head_dim / 2, h_sin, sizeof(float) * c.head_dim / 2);
+    std::memcpy(rot + kRotFloats, tab.data(), sizeof(int) * tab.size());
+    VLO_CUDA(cudaMemcpyAsync(e->kv_op_pt, rot, sizeof(float) * kRotFloats + sizeof(int) * tab.size(),
+                             cudaMemcpyHostToDevice, st));
+    if (stage_release(e, slot, st)) return -1;
+    kv_rerotate_kernel<<<dim3((kept * 8 + 255) / 256, c.num_kv_heads, c.num_layers), 256, 0, st>>>(
+        kv_paged_side(e, e->kv, e->kv_op_pt + kRotFloats), c.num_kv_heads, first_token + n_tokens, kept,
+        reinterpret_cast<const float*>(e->kv_op_pt));
+    VLO_LAUNCH_CHECK();
+  }
+  e->pool.drop(sid, first_token / kKvPageTokens, n_tokens / kKvPageTokens);
   return 0;
 }
 

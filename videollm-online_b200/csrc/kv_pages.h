@@ -111,6 +111,15 @@ class KvPool {
     grown.clear();
   }
 
+  // Remove pages [first, first + n) from stream sid's table (full pages, the caller checks): they go back to the free
+  // list, first on top; the later pages keep their rows and move n entries down, and the length drops by 64 n.
+  void drop(int sid, int first, int n) {
+    std::vector<int>& t = tables[sid];
+    for (int j = first + n - 1; j >= first; --j) free_list.push_back(t[j]);
+    t.erase(t.begin() + first, t.begin() + first + n);
+    lens[sid] -= n * kKvPageTokens;
+  }
+
   // Empty the non-empty stream sid once its swap-out copies are enqueued on st: its pages go back to the free list,
   // gated by an event recorded on st, and a grow() that takes one of them makes its stream wait on that event.
   int swap_out(int sid, cudaStream_t st) {

@@ -13,6 +13,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 
 from . import _lib
+from . import weights as W
 from ._lib import VloConfig, VloDecision, VloError, VloSampleRow, check
 from .config import LiveConfig
 
@@ -79,6 +80,42 @@ class KvImage:
 
 
 torch.serialization.add_safe_globals([KvImage])
+
+
+def sink_tokens(keep_tokens: int, page: int) -> int:
+    """Cache positions a context window never drops: the first ceil(keep_tokens / page) pages."""
+    return -(-keep_tokens // page) * page
+
+
+def evict_span(kv_len: int, need: int, window: int, keep_tokens: int, page: int) -> tuple[int, int]:
+    """The one eviction policy of a context window: (first, n) = the cache positions to drop before a stream of kv_len
+    positions appends `need` more, n = 0 when kv_len + need <= window.  The sink (`sink_tokens`) stays; after it the
+    fewest whole pages that make kv_len + need <= window go, but at least window / 8 tokens' worth rounded up to pages
+    (as many full pages as there are, if fewer), so the re-rotation of the tail is paid once per window / 8 tokens.
+    Raises VloError when dropping every full page after the sink is not enough."""
+    if kv_len + need <= window:
+        return 0, 0
+    first = sink_tokens(keep_tokens, page)
+    avail = max(0, kv_len // page - first // page)          # full pages after the sink
+    least = -(-(kv_len + need - window) // page)
+    if least > avail:
+        raise VloError(f"context window {window}: {kv_len} cached + {need} new tokens do not fit even after dropping "
+                       f"every full page after the first {first} positions")
+    return first, min(avail, max(least, -(-window // (8 * page)))) * page
+
+
+def check_context_window(window: int, max_kv_tokens: int, keep_tokens: int, largest_need: int, page: int):
+    """Raise ValueError unless a context window of `window` tokens is usable: within max_kv_tokens, and large enough
+    for the sink pages, one eviction chunk (window / 8 in whole pages) and the largest single step or response
+    reserve (`largest_need`)."""
+    if isinstance(window, bool) or not isinstance(window, int) or window <= 0:
+        raise ValueError(f"context_window must be a positive int (tokens), got {window!r}")
+    if window > max_kv_tokens:
+        raise ValueError(f"context_window {window} exceeds the engine's max_kv_tokens ({max_kv_tokens})")
+    least = sink_tokens(keep_tokens, page) + -(-window // (8 * page)) * page + largest_need
+    if window < least:
+        raise ValueError(f"context_window {window} cannot hold the {sink_tokens(keep_tokens, page)}-token sink, one "
+                         f"eviction chunk and a step of {largest_need} tokens: it must be >= {least}")
 
 
 @dataclass
@@ -208,6 +245,23 @@ class Engine:
 
     def kv_copy_prefix(self, src_sid: int, dst_sid: int, n_tokens: int):
         check(self.lib.vlo_kv_copy_prefix(self._h, src_sid, dst_sid, n_tokens, self._stream()), "vlo_kv_copy_prefix")
+
+    def kv_evict(self, sid: int, first: int, n: int):
+        """Drop cache positions [first, first + n) of stream `sid` (whole, full pages) and move the later ones down by
+        n: their keys are re-rotated on the device by -n positions (vlo_kv_evict, current CUDA stream)."""
+        cos, sin = W.rope_rotation(self.cfg, n)
+        fp = C.POINTER(C.c_float)
+        check(self.lib.vlo_kv_evict(self._h, sid, first, n, C.cast(cos.data_ptr(), fp), C.cast(sin.data_ptr(), fp),
+                                    self._stream()), "vlo_kv_evict")
+
+    def kv_make_room(self, sid: int, need: int, window: int, keep_tokens: int) -> int:
+        """Before stream `sid` appends `need` tokens under a context window: evict what `evict_span` says (the sink of
+        keep_tokens positions stays).  Returns the number of positions dropped (0: none); they start at
+        sink_tokens(keep_tokens, page)."""
+        first, n = evict_span(self.kv_len(sid), need, window, keep_tokens, self.kv_pool_info()["page_tokens"])
+        if n:
+            self.kv_evict(sid, first, n)
+        return n
 
     def kv_fill_synthetic(self, sid: int, n_tokens: int, seed: int = 0):
         check(self.lib.vlo_kv_fill_synthetic(self._h, sid, n_tokens, seed, self._stream()), "vlo_kv_fill_synthetic")

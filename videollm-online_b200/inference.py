@@ -24,7 +24,7 @@ from typing import Optional
 import torch
 
 from .config import LiveArguments, SamplingConfig, parse_args
-from .engine import KvImage
+from .engine import KvImage, check_context_window, sink_tokens
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
 from .speculative import SEP, NgramDrafter, generate_ids
 
@@ -46,6 +46,7 @@ class SessionState:
     n_calls: int
     started: bool                # past_key_values was set: a step ran since the last reset
     sampling: Optional[SamplingConfig] = None   # LiveInfer.sampling (None: greedy responses)
+    evicted_tokens: int = 0      # cache positions the session's context window dropped so far
 
 
 torch.serialization.add_safe_globals([SessionState, SamplingConfig])
@@ -93,6 +94,9 @@ class LiveInfer:
         # response ids, the decisions the hook sees and the cache are those of one token per step.
         self.drafter = NgramDrafter()
         self._n_calls = 0
+        # context window (tokens, None: off): the cache keeps the start prompt (the sink) and drops its oldest pages
+        # after it, at fixed points only (before a frame step, before a response), so a session runs in bounded memory
+        self.context_window = args.context_window or None
         # encode-ahead: with a loaded clip the ViT + connector of the NEXT frame run on a side CUDA stream while the
         # decoder works on the current one (same per-frame arithmetic; a live stream delivers the next frame
         # during the current step anyway).  Set prefetch_next = False for strictly sequential behaviour.
@@ -127,6 +131,35 @@ class LiveInfer:
         self._prefetch_event = None
         self._want_prefetch = None
 
+    # ------------------------------------------------------------------ context window
+    @property
+    def context_window(self) -> Optional[int]:
+        return self._context_window
+
+    @context_window.setter
+    def context_window(self, window: Optional[int]):
+        """None: off.  Else it must be <= max_kv_tokens and hold the sink pages, one eviction chunk and the largest
+        frame step or response reserve (ValueError otherwise)."""
+        if window is not None:
+            frame_step = 1 + self._added_stream_prompt_ids.numel() + self.frame_num_tokens
+            reserve = self._added_stream_generation_ids.numel() + self.inplace_output_ids.size(1)
+            eng = self.model.engine
+            check_context_window(window, eng.max_kv_tokens, self._start_ids.numel(), max(frame_step, reserve),
+                                 eng.kv_pool_info()["page_tokens"])
+        self._context_window = window
+
+    def _make_room(self, need: int):
+        """Under a context window: evict before the stream appends `need` tokens (Engine.kv_make_room, the policy
+        StreamScheduler uses as well), and drop the same positions from the drafter's history."""
+        if self._context_window is None:
+            return
+        eng, sid = self._kv.engine, self._kv.stream_id
+        n = eng.kv_make_room(sid, need, self._context_window, self._start_ids.numel())
+        if n:
+            if self.drafter is not None:
+                self.drafter.drop(sink_tokens(self._start_ids.numel(), eng.kv_pool_info()["page_tokens"]), n)
+            self.evicted_tokens += n
+
     # ------------------------------------------------------------------ session control
     def reset(self):
         self.query_queue = collections.deque()
@@ -135,6 +168,7 @@ class LiveInfer:
         self.last_frame_idx = -1
         self.video_tensor = None
         self.last_ids = torch.tensor([[]], dtype=torch.long)
+        self.evicted_tokens = 0
         self._kv.engine.stream_reset(self._kv.stream_id)
         if self.drafter is not None:
             self.drafter.sync(0)
@@ -153,7 +187,8 @@ class LiveInfer:
                 video_time=self.video_time, last_frame_idx=self.last_frame_idx, query_queue=list(self.query_queue),
                 frame_embeds_queue=frames,
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
-                n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling)
+                n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling,
+                evicted_tokens=self.evicted_tokens)
             self.reset()
             return state
 
@@ -180,6 +215,7 @@ class LiveInfer:
                     self.drafter.sync(state.kv.n_tokens)
             self._n_calls = state.n_calls
             self.sampling = state.sampling
+            self.evicted_tokens = state.evicted_tokens
             self.past_key_values = self._kv if state.started else None
 
     def load_video(self, video_path_or_tensor, keep_on_host: bool = False):
@@ -338,6 +374,9 @@ class LiveInfer:
             assert int(self.last_ids) == self.stream_end_id, f'{self.last_ids} != {self.stream_end_id}'  # "]\n" closes the frame list
             self.last_ids = self._added_stream_generation_ids
         ids = [int(x) for x in self.last_ids.reshape(-1).tolist()]
+        # before a response: room for the prompt and every id it may generate.  A verify step's drafts fit in it as
+        # well (draft_cap keeps them within the ids still wanted), so the loop below never evicts.
+        self._make_room(len(ids) + self.inplace_output_ids.size(1))
 
         def step(pending, drafts, sample=None):
             with self._lock:
@@ -346,7 +385,7 @@ class LiveInfer:
         # fast_greedy_generate (models/modeling_live.py:173-182), or sampled ids, verifying drafts from the history
         out = generate_ids(self.model.engine, self._kv.stream_id, step, len(ids), self.inplace_output_ids.size(1),
                            self.eos_token_id, first_ids=ids, drafter=self.drafter, consume=self._consume,
-                           sampling=self.sampling)
+                           sampling=self.sampling, position_base=self.evicted_tokens)
         n = len(out)
         self.inplace_output_ids[0, :n] = torch.tensor(out, dtype=torch.long)
         output_ids = self.inplace_output_ids[:, :n]
@@ -366,6 +405,7 @@ class LiveInfer:
                 self.last_ids = self._start_ids
             elif int(self.last_ids.reshape(-1)[-1]) == self.eos_token_id and self.last_ids.numel() == 1:
                 self.last_ids = torch.cat([self.last_ids.reshape(1, -1), self._added_stream_prompt_ids], dim=1)
+            self._make_room(self.last_ids.numel() + self.frame_embeds_queue[0][1].shape[0])   # before a frame step
             n = self._backlog_run()
             if n > 1:
                 video_time, query, answered = self._stream_backlog(n)
@@ -388,12 +428,17 @@ class LiveInfer:
     def _backlog_run(self) -> int:
         """Queued frames (from the head) that one segmented step can take: the loop above would step them one after
         another, each fed the interval id of a silent predecessor, without a query in between.  So the run stops
-        before a frame that rule 1 would precede, after a frame that rule 2 answers, and at max_step_tokens."""
+        before a frame that rule 1 would precede, after a frame that rule 2 answers, and at max_step_tokens.  Under a
+        context window it also stops before a frame whose own step would evict: no segmented step spans an eviction."""
         iid, q = self.frame_token_interval_id, self.frame_embeds_queue
         if iid is None or len(q) < 2:
             return 1
         due = self.query_queue[0][0] if self.query_queue else None
         room = self.model.engine.max_step_tokens - self.last_ids.numel() - q[0][1].shape[0]
+        win = self._context_window
+        if win is not None:   # window room left after the first frame's step
+            kv = self.model.engine.kv_len(self._kv.stream_id)
+            room = min(room, win - kv - self.last_ids.numel() - q[0][1].shape[0])
         n, prev = 1, q[0][0]
         # input_video_stream appends to the queue from another thread under the same lock: a deque may not change
         # while it is iterated (only this thread pops, so the n frames counted here stay at the head)

@@ -17,6 +17,10 @@ More sessions than the engine holds: a session without work (no pending frame, n
 a pinned host image (`Engine.kv_swap_out`), and then holds neither KV pages nor a stream slot.  Before each tick every
 session with work is made resident again if it fits (`StreamScheduler._make_room`); the policy is fixed and
 deterministic.
+
+Context window: a session with `context_window` set keeps its cache within that many tokens as `LiveInfer` does, with
+the same policy (`engine.evict_span`) at the same points: before a frame step and before a response.  A resident session
+evicts before its pages are counted; a swapped-out one right after its swap-in.
 """
 from __future__ import annotations
 
@@ -27,7 +31,7 @@ import torch
 
 from ._lib import VloError
 from .config import SamplingConfig
-from .engine import KvImage, SampleRow
+from .engine import KvImage, SampleRow, evict_span
 from .modeling_live import LiveLlamaForCausalLM
 from .speculative import sample_rows
 
@@ -49,6 +53,8 @@ class StreamSession:
         self.threshold = 0.725
         # response tokens, as LiveInfer.sampling: None = greedy; each session may have its own config
         self.sampling: Optional[SamplingConfig] = None
+        # as LiveInfer.context_window: None = off; the sink is the scheduler's start_ids
+        self.context_window: Optional[int] = None
         self.reset()
 
     @property
@@ -77,6 +83,7 @@ class StreamSession:
         self.outputs: List[Tuple[float, Optional[str], Optional[str]]] = []   # (time, query, response text)
         self.events: List[tuple] = []
         self.n_calls = 0
+        self.evicted_tokens = 0   # cache positions the context window dropped (sampled positions count them)
         self._op = None
 
     # -- inputs (LiveInfer.load_video / input_video_stream / input_query_stream)
@@ -139,8 +146,21 @@ class StreamSession:
         s = self.sampling
         if self._op is None or self._op[0] != "gen" or s is None or not s.do_sample:
             return None
-        return sample_rows(s, self.kv_tokens() + n - 1, self.resp_prompt + self.resp, len(self.resp_prompt) +
-                           len(self.resp), 0)[0]
+        return sample_rows(s, self.evicted_tokens + self.kv_tokens() + n - 1, self.resp_prompt + self.resp,
+                           len(self.resp_prompt) + len(self.resp), 0)[0]
+
+    def window_need(self, n: int) -> int:
+        """Tokens the context window makes room for before the planned step of n rows: the step itself, or at the start
+        of a response its prompt and every id it may generate (as LiveInfer), so no response step evicts."""
+        if self._op[0] == "gen" and not self.resp:
+            return len(self.resp_prompt) + self.sched.max_new_tokens
+        return n
+
+    def make_room(self, need: int):
+        """Evict (resident session, context window set) before appending `need` tokens."""
+        if self.context_window is not None:
+            self.evicted_tokens += self.sched.model.engine.kv_make_room(self.stream_id, need, self.context_window,
+                                                                        len(self.sched.start_ids))
 
     # -- consume the decision of the step this stream took part in
     def advance(self, dec):
@@ -277,12 +297,17 @@ class StreamScheduler:
         info = eng.kv_pool_info()
         page, total = info["page_tokens"], info["total_pages"]
         pages = lambda t: -(-t // page)
-        kv = s.kv_tokens()
-        if pages(kv + n) > total:
-            raise VloError(f"session {s.index}: {kv + n} tokens need {pages(kv + n)} KV pages, the pool has {total}")
+        w_need = s.window_need(n)
+        if s.resident:
+            s.make_room(w_need)
+        kv = after = s.kv_tokens()
+        if s.context_window is not None and not s.resident:   # it evicts right after its swap-in
+            after -= evict_span(kv, w_need, s.context_window, len(self.start_ids), page)[1]
+        if pages(after + n) > total:
+            raise VloError(f"session {s.index}: {after + n} tokens need {pages(after + n)} KV pages, the pool has {total}")
         # pages the sessions already in the batch take in this step
         reserved = sum(pages(q.kv_tokens() + m) - pages(q.kv_tokens()) for q, _, _, m in batch)
-        need = pages(kv + n) - (pages(kv) if s.resident else 0)
+        need = pages(kv + n) - pages(kv) if s.resident else max(pages(kv), pages(after + n))
         keep = {q.index for q, *_ in batch} | {s.index}
 
         def evict() -> bool:
@@ -311,6 +336,7 @@ class StreamScheduler:
                     raise
             s.stream_id, s.image = sid, None
             self.swaps_in += 1
+            s.make_room(w_need)
         return True
 
     def _swap_out(self, s: StreamSession):

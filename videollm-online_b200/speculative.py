@@ -60,6 +60,13 @@ class NgramDrafter:
                     del ends[key]
             ids_.pop()
 
+    def drop(self, start: int, n: int):
+        """Remove history entries [start, start + n), as a context window drops those cache positions: the index is
+        rebuilt from the kept entries (cheap: frame rows are SEP and index nothing)."""
+        kept = self.ids[:start] + self.ids[start + n:]
+        self.ids, self._ends = [], {}
+        self.extend(kept)
+
     def sync(self, n: int):
         """Make the history n entries long: cut it back, or pad it with SEP for KV rows it never saw (a cache filled
         or copied in from elsewhere)."""
@@ -127,7 +134,7 @@ def sample_rows(sampling, position0: int, history: List[int], n_history: int, n_
 
 def generate_ids(eng, sid: int, step: Callable[..., None], n_first: int, max_new: int, eos_token_id: int, *,
                  first_ids: Optional[Sequence[int]] = None, drafter=None, consume: Optional[Callable] = None,
-                 base: int = 0, sampling=None) -> List[int]:
+                 base: int = 0, sampling=None, position_base: int = 0) -> List[int]:
     """Ids of stream `sid` until EOS or max_new ids, verifying the drafter's proposals on the way: the argmax, or with
     `sampling` (a SamplingConfig with do_sample) the ids the device draws.
 
@@ -138,7 +145,8 @@ def generate_ids(eng, sid: int, step: Callable[..., None], n_first: int, max_new
     own embeddings).  After it, ids is [previous id].  consume(decision) -> decision sees every decision the one-token
     loop would act on, in order, and no other; the loop takes its `sampled_id` when sampling, else its `argmax_id`.
     The drafter's history is the stream's KV from position `base` on (sync / extend / propose).  The penalty set of a
-    sampled response is first_ids and the ids generated so far."""
+    sampled response is first_ids and the ids generated so far.  position_base is added to the KV positions the samples
+    are drawn at: a session under a context window passes the positions it dropped, so no position repeats."""
     if sampling is not None and not sampling.do_sample:
         sampling = None
     out: List[int] = []
@@ -159,7 +167,7 @@ def generate_ids(eng, sid: int, step: Callable[..., None], n_first: int, max_new
             if sampling is None:
                 step(pending, drafts)
             else:
-                step(pending, drafts, sample_rows(sampling, kv0 + n_pending - 1, prompt + out + drafts,
+                step(pending, drafts, sample_rows(sampling, position_base + kv0 + n_pending - 1, prompt + out + drafts,
                                                   len(prompt) + len(out), len(drafts)))
         except Exception:
             if drafter is not None:

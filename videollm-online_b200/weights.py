@@ -141,12 +141,25 @@ def rope_tables(cfg: LiveConfig, n_positions: int, device) -> tuple[torch.Tensor
     position_ids = arange(n) (HF:models/llama/modeling_llama.py:124-135): fp32 outer product,
     fp32 cos/sin, cast to the activation dtype.  Only the first head_dim/2 columns are stored
     (HF concatenates two identical halves)."""
-    d = cfg.head_dim
-    inv_freq = 1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).to(dtype=torch.float) / d))
     pos = torch.arange(n_positions, dtype=torch.float32)
-    freqs = pos[:, None] * inv_freq[None, :]
+    freqs = pos[:, None] * rope_inv_freq(cfg)[None, :]
     return (freqs.cos().to(torch.bfloat16).contiguous().to(device),
             freqs.sin().to(torch.bfloat16).contiguous().to(device))
+
+
+def rope_inv_freq(cfg: LiveConfig) -> torch.Tensor:
+    """fp32 [head_dim / 2]: the RoPE frequencies, as LlamaRotaryEmbedding computes inv_freq (the one definition the
+    tables and the eviction's rotation share)."""
+    d = cfg.head_dim
+    return 1.0 / (cfg.rope_theta ** (torch.arange(0, d, 2, dtype=torch.int64).to(dtype=torch.float) / d))
+
+
+def rope_rotation(cfg: LiveConfig, delta: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """fp32 cos / sin [head_dim / 2] of delta * inv_freq, computed in fp64 from the fp32 inv_freq and rounded once: the
+    rotation vlo_kv_evict applies (by -delta) to the keys it moves delta positions down.  Not the bf16 tables, whose
+    2^-9 relative error would compound over repeated evictions."""
+    ang = rope_inv_freq(cfg).double() * float(delta)
+    return ang.cos().float(), ang.sin().float()
 
 
 def _b32_from16(t: torch.Tensor, dt16) -> torch.Tensor:
