@@ -92,6 +92,10 @@ int vlo_engine_destroy(vlo_engine* e);
  * DESIGN.md "weight layout"; the Python loader does the HF/peft key mapping, LoRA merge and
  * packing at init).  The engine keeps the pointer; the caller keeps the storage alive. */
 int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t n_bytes);
+/* Resolve and size-check the registered tensors.  Each decoder layer matrix L{i}.{qkv,o,gate_up,down} comes in exactly
+ * one form: bf16 `name`, or FP8 weights `name.f8` (e4m3fn bytes [N, K]) + `name.scale` (fp32 [N], one per row).  All
+ * 4 x num_layers matrices must share one form; a mixed set, a missing scale or a wrong size fails with a message that
+ * names the tensor.  The form decides which GEMM kernels the layer loop runs. */
 int vlo_finalize_weights(vlo_engine* e);
 /* bytes of device memory the engine allocated itself (KV + workspaces) */
 int64_t vlo_engine_device_bytes(vlo_engine* e);
@@ -266,6 +270,13 @@ int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, 
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
                    void* cuda_stream);
+/* The same GEMM in mode 0 on e4m3 weights (the decoder's FP8 weight form): d_w8 [rows_w, k] e4m3fn bytes, d_scale fp32
+ * [rows_w] row scales, X bf16 [rows_x, k].  Same token tile and stream-K plan as the bf16 call with these sizes and
+ * n_ctas; each weight k-block is upcast to bf16 exactly and multiplied by the bf16 wgmma chain, so plane p holds
+ * fl(P_p[t][n] * d_scale[n]), P_p being plane p of the bf16 call on the upcast weights.  d_out == NULL only plans
+ * (*h_max_planes).  Asynchronous. */
+int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
+                      long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream);
 /* ViT trunk GEMM (csrc/gemm_vit.cuh), fp16, 128-token x 128-feature tiles:
  * out[t][n] = act(fp16(sum_k X[t,k] W[n,k] + bias[n])), fp16 out[rows_x][ld_out], ld_out even and >= rows_w;
  * n_ctas <= 0: one CTA per SM. */
@@ -340,6 +351,11 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
  * counters, zero before the call and zero again when it has run.  Asynchronous. */
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
                        int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream);
+/* vlo_op_gemm_swiglu on e4m3 weights d_w8 [rows_w, k] with fp32 row scales d_scale [rows_w] (same row order and plan):
+ * g, u = bf16(sum_p fl(P_p * d_scale[n])) summed in plane order, P_p the fp32 partials of the bf16 kernel on the exactly
+ * upcast weights (the finisher's own partial is plane 0).  Asynchronous. */
+int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
+                          float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream);
 /* Speak / silent decision over bf16 logits [n_rows, vocab] (vocab a multiple of 8, rows 16-byte aligned), one
  * vlo_decision per row into d_out (device): first-index argmax, max logit, max - second max (a repeated maximum counts
  * as the second), log-sum-exp, p_interval = bf16(softmax[interval_id]) (0 when interval_id is outside the row), and the

@@ -93,6 +93,7 @@ SIGNATURES = {
     "vlo_bench_gemm": (_I, [_P, _I, _I, C.POINTER(C.c_double), C.POINTER(_I), _P]),
     "vlo_op_gemm": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _P, _P, _I, _I, _P]),
     "vlo_op_gemm_ws": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, C.POINTER(_I), _P]),
+    "vlo_op_gemm_ws_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
     "vlo_op_attn_kvappend": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P]),
@@ -105,6 +106,7 @@ SIGNATURES = {
     "vlo_op_qkv_rope_append": (_I, [_P, _I, _I, _P, _P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _I, _P, _P, _P,
                                     _I, _I, _I, _P]),
     "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
+    "vlo_op_gemm_swiglu_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_op_sample": (_I, [_P, _I, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),

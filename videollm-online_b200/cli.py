@@ -6,6 +6,8 @@
 Responses are greedy unless --do_sample is given (SamplingConfig; --seed stays the synthetic weights' seed).
 --context_window N keeps the session's cache within N tokens (0: off): the start prompt stays, the oldest pages after it
 are dropped.
+--fp8_weights serves the decoder layers from e4m3 weights with per-row scales (half their bytes per step; the model's
+numbers change, so it is off by default).
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

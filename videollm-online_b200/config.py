@@ -155,6 +155,9 @@ class LiveArguments:
     kv_pool_tokens: int = 0  # KV page pool shared by the streams, tokens; 0: max_streams x the per-stream cap
     synthetic_weights: bool = False
     seed: int = 0            # of the synthetic weights
+    # serve the decoder layers' q|k|v, o, gate|up and down matrices from e4m3 codes with one fp32 scale per row (half the
+    # weight bytes per step); changes the model's numbers, so off by default
+    fp8_weights: bool = False
     # LiveInfer.context_window, tokens: keep the start prompt and drop the oldest cache pages after it so the session's
     # cache never exceeds this many tokens; 0: off (the cache grows until max_kv_tokens)
     context_window: int = 0

@@ -137,6 +137,29 @@ int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d
   return rc;
 }
 
+int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
+                      long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
+  VLO_CHECK(d_out == nullptr || d_scale != nullptr, "gemm_ws_f8: null row scales");
+  GemmWsCall c{};
+  c.fmt = FMT_E4M3;
+  c.mode = 0;
+  c.w = d_w8;
+  c.w_scale = d_scale;
+  c.rows_w = rows_w;
+  c.x = d_x;
+  c.rows_x = rows_x;
+  c.k = k;
+  c.out = d_out;
+  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
+  c.ld_out = rows_w;
+  c.plane_stride = plane_stride;
+  c.n_ctas = n_ctas;
+  GemmWsPlan plan{};
+  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
+  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
+  return rc;
+}
+
 int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
                     const float* d_bias, int act, int n_ctas, void* cuda_stream) {
   return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
@@ -272,8 +295,16 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
                        int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu: plane_elems");
-  return gemm_wsf_launch(d_w, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags, n_flags,
-                         static_cast<cudaStream_t>(cuda_stream));
+  return gemm_wsf_launch(d_w, nullptr, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
+                         n_flags, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
+                          float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
+  VLO_CHECK(plane_elems >= 0, "gemm_swiglu_f8: plane_elems");
+  VLO_CHECK(d_scale != nullptr, "gemm_swiglu_f8: null row scales");
+  return gemm_wsf_launch(d_w8, d_scale, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
+                         n_flags, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream) {

@@ -108,7 +108,7 @@ enum WsTiling : int {
                                // shares an SM with a decoder weight-streaming CTA
 };
 struct GemmWsCall {
-  int fmt;            // 0 fp16, 1 bf16
+  int fmt;            // 0 fp16, 1 bf16, 2 e4m3 weights x bf16 activations (mode 0 only)
   int mode;           // 0 stream-K fp32 partial planes, 1 whole tiles + 16-bit epilogue
   const void* w;      // [rows_w, k]
   int rows_w;
@@ -124,6 +124,7 @@ struct GemmWsCall {
   int n_ctas;         // <= 0: one CTA per SM
   int bn;             // token-tile width; 0: chosen by `tiling`
   int tiling;         // WsTiling
+  const float* w_scale;  // fmt 2: [rows_w] fp32 row scales, each partial is multiplied by its row's scale once
 };
 // What a launch decided, for the kernels that fold its partial planes.
 struct GemmWsPlan {
@@ -140,11 +141,12 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan = 
 int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
                     const float* bias, int act, int n_ctas, cudaStream_t stream);
 
-// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), bf16, one CTA per SM:
-// act[rows_x][rows_w / 2] = SwiGLU(x w^T).  planes (plane_elems floats) take the partials of the non-finisher CTAs,
-// flags (n_flags counters, zero between launches) their arrivals.
-int gemm_wsf_launch(const void* w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
-                    size_t plane_elems, int* flags, int n_flags, cudaStream_t stream);
+// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), bf16 x, one CTA per SM:
+// act[rows_x][rows_w / 2] = SwiGLU(x w^T).  w is bf16 (w_scale null) or e4m3 with fp32 row scales w_scale [rows_w].
+// planes (plane_elems floats) take the partials of the non-finisher CTAs, flags (n_flags counters, zero between
+// launches) their arrivals.
+int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
+                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream);
 
 // ---- decoder fix-up and decision kernels (decoder_kernels.cuh / engine.cu) -----------
 // bf16 tensors; `part` holds fp32 stream-K planes [plane][T][width] of the plan `sk`, as gemm_ws_launch mode 0 leaves

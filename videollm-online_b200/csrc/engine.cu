@@ -28,8 +28,14 @@ constexpr int kRotFloats = 128;  // vlo_kv_evict's cos | sin (head_dim / 2 each)
 
 using bf16 = __nv_bfloat16;
 
+// a layer matrix [n, k]: bf16 (scale null) or e4m3 bytes with fp32 row scales [n]
+struct DecW {
+  const void* w;
+  const float* scale;
+};
 struct DecLayer {
-  const bf16 *in_norm, *qkv, *o, *post_norm, *gate_up, *down;
+  const bf16 *in_norm, *post_norm;
+  DecW qkv, o, gate_up, down;
 };
 struct VitLayer {
   const float *ln1_w, *ln1_b, *ln2_w, *ln2_b, *qkv_b, *out_b, *fc1_b, *fc2_b;
@@ -56,6 +62,7 @@ struct vlo_engine {
               *head_fc1_b = nullptr, *head_fc2_b = nullptr, *conn0_b = nullptr, *conn2_b = nullptr;
   const bf16 *conn0_w = nullptr, *conn2_w = nullptr;
   bool has_vit = false, has_connector = false, has_decoder = false;
+  bool fp8_weights = false;  // the layer matrices are e4m3 + row scales (vlo_finalize_weights)
 
   // derived
   int qkv_width = 0, grid = 0, n_patches = 0, n_frame_tokens = 0, patch_k = 0;
@@ -134,9 +141,10 @@ int lookup(vlo_engine* e, const std::string& name, int64_t expect_elems, const T
 // which a fix-up kernel folds.  The fix-up kernels unroll kFixMaxPlanes planes: this is the one check of that limit,
 // made before the fix-up kernel that would read the planes is launched.
 int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int k, float* part, size_t part_elems,
-                 int tiling, GemmWsPlan* plan, cudaStream_t st) {
+                 int tiling, GemmWsPlan* plan, cudaStream_t st, const float* w_scale = nullptr) {
   GemmWsCall c{};
   c.fmt = fmt;
+  c.w_scale = w_scale;
   c.mode = 0;
   c.w = w;
   c.rows_w = n_out;
@@ -153,9 +161,10 @@ int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int
   return 0;
 }
 
-// the decoder's partial GEMMs: bf16, the step's T tokens, planes in e->part
-int dec_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, GemmWsPlan* sk, cudaStream_t st) {
-  return gemm_partial(FMT_BF16, w, n_out, x, T, k, e->part, e->part_elems, WS_TILE_FIT, sk, st);
+// the decoder's partial GEMMs: bf16 or e4m3 weights, the step's T tokens, planes in e->part
+int dec_partial(vlo_engine* e, const DecW& w, int n_out, const bf16* x, int T, int k, GemmWsPlan* sk, cudaStream_t st) {
+  return gemm_partial(w.scale ? FMT_E4M3 : FMT_BF16, w.w, n_out, x, T, k, e->part, e->part_elems, WS_TILE_FIT, sk, st,
+                      w.scale);
 }
 
 // gate|up GEMM + SwiGLU: the stream-K finisher CTAs apply the fix-up themselves (gemm_wsf.cuh).  A finisher's epilogue
@@ -163,8 +172,8 @@ int dec_partial(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, i
 // separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling.  Only the gate|up GEMM has
 // enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB plane round trip of
 // its fix-up; q|k|v, o_proj and down_proj go through gemm_partial and a fix-up kernel (DESIGN.md section 5).
-int gemm_swiglu(vlo_engine* e, const bf16* w, int n_out, const bf16* x, int T, int k, cudaStream_t st) {
-  return gemm_wsf_launch(w, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st);
+int gemm_swiglu(vlo_engine* e, const DecW& w, int n_out, const bf16* x, int T, int k, cudaStream_t st) {
+  return gemm_wsf_launch(w.w, w.scale, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st);
 }
 
 // whole-tile persistent GEMM with the 16-bit epilogue: out[T, n_out] = act(x W^T + bias)
@@ -552,6 +561,34 @@ int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t 
   return 0;
 }
 
+namespace {
+// Layer matrix `name` [n, k] in exactly one form: bf16 `name`, or e4m3 bytes `name.f8` with fp32 row scales `name.scale`.
+// *f8 < 0: the first matrix, which sets the form every later one must share.
+int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* f8, DecW* out) {
+  const bool has16 = e->tensors.count(name) > 0, has8 = e->tensors.count(name + ".f8") > 0,
+             has_s = e->tensors.count(name + ".scale") > 0;
+  if (has16 && (has8 || has_s)) return fail("weight tensor '" + name + "' is loaded both as bf16 and as e4m3");
+  if (!has16 && !has8 && !has_s) return fail("missing weight tensor '" + name + "' (or '" + name + ".f8' + '" + name + ".scale')");
+  if (has8 != has_s) return fail("missing weight tensor '" + name + (has8 ? ".scale'" : ".f8'"));
+  const int form = has8 ? 1 : 0;
+  if (*f8 >= 0 && form != *f8)
+    return fail("weight tensor '" + name + (form ? ".f8' is e4m3" : "' is bf16") +
+                " but an earlier layer matrix is not: all layer matrices must share one form");
+  *f8 = form;
+  out->scale = nullptr;
+  if (!form) {
+    const bf16* w;
+    if (lookup(e, name, n * k, &w)) return -1;
+    out->w = w;
+    return 0;
+  }
+  const uint8_t* w;
+  if (lookup(e, name + ".f8", n * k, &w) || lookup(e, name + ".scale", n, &out->scale)) return -1;
+  out->w = w;
+  return 0;
+}
+}  // namespace
+
 int vlo_finalize_weights(vlo_engine* e) {
   VLO_CHECK(e != nullptr, "null engine");
   const vlo_config& c = e->cfg;
@@ -568,16 +605,18 @@ int vlo_finalize_weights(vlo_engine* e) {
     if (lookup(e, "rope.cos", e->rope_positions * 64, &e->rope_cos)) return -1;
     if (lookup(e, "rope.sin", e->rope_positions * 64, &e->rope_sin)) return -1;
     e->dec.resize(c.num_layers);
+    int f8 = -1;
     for (int l = 0; l < c.num_layers; ++l) {
       const std::string p = "L" + std::to_string(l) + ".";
       DecLayer& d = e->dec[l];
       if (lookup(e, p + "in_norm", H, &d.in_norm)) return -1;
-      if (lookup(e, p + "qkv", static_cast<int64_t>(e->qkv_width) * H, &d.qkv)) return -1;
-      if (lookup(e, p + "o", H * c.num_heads * c.head_dim, &d.o)) return -1;
+      if (lookup_layer_matrix(e, p + "qkv", e->qkv_width, H, &f8, &d.qkv)) return -1;
+      if (lookup_layer_matrix(e, p + "o", H, static_cast<int64_t>(c.num_heads) * c.head_dim, &f8, &d.o)) return -1;
       if (lookup(e, p + "post_norm", H, &d.post_norm)) return -1;
-      if (lookup(e, p + "gate_up", 2 * I * H, &d.gate_up)) return -1;
-      if (lookup(e, p + "down", H * I, &d.down)) return -1;
+      if (lookup_layer_matrix(e, p + "gate_up", 2 * I, H, &f8, &d.gate_up)) return -1;
+      if (lookup_layer_matrix(e, p + "down", H, I, &f8, &d.down)) return -1;
     }
+    e->fp8_weights = f8 == 1;
   }
   e->has_connector = e->tensors.count("conn.0.w") > 0;
   if (e->has_connector) {
@@ -1210,6 +1249,7 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const int H = c.hidden_size, I = c.intermediate_size, A = c.num_heads * c.head_dim;
   double bytes = 0.0;
+  const double w_elem = e->fp8_weights ? 1.0 : 2.0, row_b = e->fp8_weights ? 4.0 : 0.0;   // e4m3: 1 B + a scale per row
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < c.num_layers; ++l) {
       const DecLayer& d = e->dec[l];
@@ -1219,8 +1259,8 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
       if (dec_partial(e, d.gate_up, 2 * I, e->xn, n_tok, H, &sk, st)) return -1;
       if (dec_partial(e, d.down, H, e->act, n_tok, I, &sk, st)) return -1;
       if (it == 0)
-        bytes += 2.0 * (static_cast<double>(e->qkv_width) * H + static_cast<double>(H) * A + 2.0 * I * H + static_cast<double>(H) * I) +
-                 2.0 * n_tok * (2.0 * H + A + I);
+        bytes += w_elem * (static_cast<double>(e->qkv_width) * H + static_cast<double>(H) * A + 2.0 * I * H + static_cast<double>(H) * I) +
+                 row_b * (static_cast<double>(e->qkv_width) + H + 2.0 * I + H) + 2.0 * n_tok * (2.0 * H + A + I);
     }
   if (h_algo_bytes_per_iter) *h_algo_bytes_per_iter = bytes;
   if (h_launches_per_iter) *h_launches_per_iter = 4 * c.num_layers;

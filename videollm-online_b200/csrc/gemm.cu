@@ -9,6 +9,7 @@
 #include <cudaTypedefs.h>
 
 #include <cstdio>
+#include <algorithm>
 #include <cstdlib>
 #include <mutex>
 #include <unordered_map>
@@ -58,7 +59,8 @@ struct TmapHash {
 std::mutex g_tmap_mu;
 std::unordered_map<TmapKey, CUtensorMap, TmapHash> g_tmaps;
 
-// [rows, k] row-major 16-bit matrix, box = 64 (k) x box_rows, 128-byte swizzle.
+// [rows, k] row-major 16-bit matrix, box = 64 (k) x box_rows, 128-byte swizzle; FMT_E4M3: bytes, box = 64 B x box_rows,
+// no swizzle (the consumer reads the stage with plain loads).
 int get_tmap(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out) {
   TmapKey key{ptr, rows, k, box_rows, fmt};
   {
@@ -73,13 +75,17 @@ int get_tmap(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMa
   if (enc == nullptr) return fail("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) return fail("TMA operand not 16-byte aligned");
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(k), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(k) * 2};
+  const bool f8 = fmt == FMT_E4M3;
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(k) * (f8 ? 1 : 2)};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(kGemmBK), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
   CUtensorMap m;
-  CUresult r = enc(&m, fmt == FMT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+  CUresult r = enc(&m,
+                   f8                  ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                   : fmt == FMT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                     : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
                    2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   f8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed, CUresult " + std::to_string(r));
   {
@@ -167,18 +173,29 @@ static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemR
               "decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
 static_assert(GemmWsfCfg<16, wsf_default_stages(16)>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
               "the 8-stage fused decoder GEMM now shares its SM with a ViT trunk GEMM CTA: update the comment above");
+// The e4m3 16-token decoder GEMM keeps that pairing: the deepest ring of 10 KB stages that fits beside the ViT trunk GEMM
+// CTA next to the two converted 16 KB tiles (8 stages, 64 KB of weights in flight; DESIGN.md section 5).
+constexpr int kF8DecoderStages =
+    std::min(16, (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes - GemmWsCfg<16, 0, FMT_E4M3>::kSmemBytes) /
+                     (kF8BytesW + 16 * kGemmBK * 2));
+static_assert(GemmWsCfg<16, kF8DecoderStages, FMT_E4M3>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "e4m3 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
+static_assert(GemmWsCfg<16, kF8DecoderStages, FMT_E4M3>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "e4m3 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
 
 namespace {
-template <int FMT, int BN, int STAGES = ws_default_stages(BN)>
+template <int FMT, int BN, int STAGES = FMT == FMT_E4M3 ? ws_f8_default_stages(BN) : ws_default_stages(BN)>
 int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
   auto kern = gemm_ws_kernel<FMT, BN, STAGES>;
-  if (ensure_max_smem(reinterpret_cast<const void*>(kern), GemmWsCfg<BN, STAGES>::kSmemBytes)) return -1;
+  using Cfg = GemmWsCfg<BN, STAGES, FMT>;
+  if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
   if (prof_on()) {
     const double out_b = a.mode == 0 ? 4.0 * a.rows_x * a.rows_w : 2.0 * a.rows_x * a.rows_w;
-    prof_begin(FMT == FMT_BF16 ? PROF_GEMM_STREAM : PROF_GEMM_VIT, stream,
-               2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x) + out_b);
+    const double in_b = FMT == FMT_E4M3 ? (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x   // 1 B per weight + row scales
+                                        : 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x);
+    prof_begin(FMT == FMT_F16 ? PROF_GEMM_VIT : PROF_GEMM_STREAM, stream, in_b + out_b);
   }
-  VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), GemmWsCfg<BN, STAGES>::kSmemBytes, stream, tw, tx, a));
+  VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a));
   prof_end(stream);
   count_launch();
   return 0;
@@ -186,12 +203,12 @@ int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a,
 
 // Token-tile width for rows_x token rows, of both weight-streaming kernels: the smallest instance covering them (a
 // narrower X tile leaves more of the ring to the weight stream: 88 tokens = 8 streams x 11 take the 96-wide instance).
-// fp16 takes 128 above 64 rows; the fused gate|up GEMM is bf16.  Above 128 rows: 128-wide tiles.
+// fp16 takes 128 above 64 rows; bf16 and e4m3 weights (bf16 activations) take 96.  Above 128 rows: 128-wide tiles.
 int token_tile(int rows_x, int fmt) {
   if (rows_x <= 16) return 16;
   if (rows_x <= 32) return 32;
   if (rows_x <= 64) return 64;
-  return rows_x <= 96 && fmt == FMT_BF16 ? 96 : 128;
+  return rows_x <= 96 && fmt != FMT_F16 ? 96 : 128;
 }
 
 // Token-tile width of the ViT trunk of 3+ frames (many token tiles): the least padding in the last token tile, and in
@@ -239,6 +256,9 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
                  : c.tiling == WS_TILE_TRUNK ? trunk_token_tile(c.rows_x, c.rows_w, c.mode)
                  : token_tile(c.rows_x, c.fmt);
   VLO_CHECK(!beside || (c.fmt == FMT_F16 && bn == 64), "gemm_ws: only the 64-token fp16 instance fits beside a decoder CTA");
+  const bool f8 = c.fmt == FMT_E4M3;
+  VLO_CHECK(!f8 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn)),
+            "gemm_ws: e4m3 weights run stream-K partials (mode 0) on the token tile token_tile() picks");
   const int x_tiles = (c.rows_x + bn - 1) / bn;
   GemmWsArgs a{};
   a.rows_w = c.rows_w;
@@ -258,13 +278,16 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   a.plane_stride = c.plane_stride;
   a.bias = c.bias;
   a.act = c.act;
+  VLO_CHECK(!f8 || c.w_scale != nullptr, "gemm_ws: e4m3 weights need their row scales");
+  a.w_scale = c.w_scale;
   CUtensorMap tw, tx;
   if (get_tmap(c.w, c.rows_w, c.k, kGemmBM, c.fmt, &tw) != 0) return -1;
-  if (get_tmap(c.x, c.rows_x, c.k, bn, c.fmt, &tx) != 0) return -1;
+  if (get_tmap(c.x, c.rows_x, c.k, bn, f8 ? FMT_BF16 : c.fmt, &tx) != 0) return -1;
 #define VLO_WS_CASE(F, N) \
   if (c.fmt == F && bn == N) return launch_ws<F, N>(tw, tx, a, stream);
   // the single-stream decoder GEMM: 6 x 18 KB leaves room on the SM for a co-resident ViT CTA (static_asserts above)
   if (c.fmt == FMT_BF16 && bn == 16) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
+  if (f8 && bn == 16) return launch_ws<FMT_E4M3, 16, kF8DecoderStages>(tw, tx, a, stream);
   if (beside) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
   VLO_WS_CASE(FMT_BF16, 32)
   VLO_WS_CASE(FMT_BF16, 64)
@@ -276,6 +299,10 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   VLO_WS_CASE(FMT_F16, 128)
   VLO_WS_CASE(FMT_F16, 96)
   VLO_WS_CASE(FMT_F16, 192)
+  VLO_WS_CASE(FMT_E4M3, 32)
+  VLO_WS_CASE(FMT_E4M3, 64)
+  VLO_WS_CASE(FMT_E4M3, 96)
+  VLO_WS_CASE(FMT_E4M3, 128)
 #undef VLO_WS_CASE
   return fail("gemm_ws_launch: no kernel instance");
 }
@@ -315,8 +342,22 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 // ------------------------------------------------------------------------------------------------
 // stream-K gate|up GEMM with the SwiGLU finisher epilogue (gemm_wsf.cuh)
 namespace {
+// w_scale null: bf16 weights; else e4m3 weights with these row scales
 template <int BN>
-int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, cudaStream_t stream) {
+int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, const float* w_scale,
+               cudaStream_t stream) {
+  if (w_scale != nullptr) {
+    constexpr int S = wsf_f8_default_stages(BN);
+    auto kern = gemm_wsf_f8_kernel<BN, S>;
+    using Cfg = GemmWsfCfg<BN, S, FMT_E4M3>;
+    if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
+    if (prof_on())   // 1 B per weight + the row scales
+      prof_begin(PROF_GEMM_STREAM, stream, (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x + 2.0 * a.rows_x * a.rows_w);
+    VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a, w_scale));
+    prof_end(stream);
+    count_launch();
+    return 0;
+  }
   constexpr int S = wsf_default_stages(BN);
   auto kern = gemm_wsf_kernel<BN, S>;
   using Cfg = GemmWsfCfg<BN, S>;
@@ -330,8 +371,8 @@ int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& 
 }
 }  // namespace
 
-int gemm_wsf_launch(const void* w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
-                    size_t plane_elems, int* flags, int n_flags, cudaStream_t stream) {
+int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
+                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream) {
   VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(rows_w > 0 && rows_x > 0 && rows_x <= 128, "gemm_wsf: 1..128 token rows");
   VLO_CHECK(rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
@@ -351,13 +392,13 @@ int gemm_wsf_launch(const void* w, int rows_w, const void* x, int rows_x, int k,
   a.act = static_cast<__nv_bfloat16*>(act);
   a.I = rows_w / 2;
   CUtensorMap tw, tx;
-  if (get_tmap(w, rows_w, k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
+  if (get_tmap(w, rows_w, k, kGemmBM, w_scale ? FMT_E4M3 : FMT_BF16, &tw) != 0) return -1;
   if (get_tmap(x, rows_x, k, bn, FMT_BF16, &tx) != 0) return -1;
-  if (bn == 16) return launch_wsf<16>(tw, tx, a, stream);
-  if (bn == 32) return launch_wsf<32>(tw, tx, a, stream);
-  if (bn == 64) return launch_wsf<64>(tw, tx, a, stream);
-  if (bn == 96) return launch_wsf<96>(tw, tx, a, stream);
-  return launch_wsf<128>(tw, tx, a, stream);
+  if (bn == 16) return launch_wsf<16>(tw, tx, a, w_scale, stream);
+  if (bn == 32) return launch_wsf<32>(tw, tx, a, w_scale, stream);
+  if (bn == 64) return launch_wsf<64>(tw, tx, a, w_scale, stream);
+  if (bn == 96) return launch_wsf<96>(tw, tx, a, w_scale, stream);
+  return launch_wsf<128>(tw, tx, a, w_scale, stream);
 }
 
 }  // namespace vlo

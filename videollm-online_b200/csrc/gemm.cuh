@@ -15,6 +15,7 @@
 //   models/live_llama/modeling_live_llama.py:18-22 (connector)
 #pragma once
 #include <cuda.h>
+#include <cuda_fp8.h>
 #include "ptx.cuh"
 #include "wgmma.cuh"
 
@@ -25,7 +26,9 @@ enum GemmEpi : int {
   EPI_PATCH32 = 3,  // out32  = r16(acc + bias) + pos[out_row % pos_rows]     (ViT patch embed)
 };
 enum GemmAct : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF_PY = 2 };
-enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1 };
+// FMT_E4M3: e4m3 weights with one fp32 scale per weight row, bf16 activations; the consumer upcasts each weight k-block
+// to bf16 exactly and runs the bf16 wgmma chain (weight-streaming kernels, stream-K partials only)
+enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2 };
 
 struct GemmArgs {
   int rows_a, rows_b, k;
@@ -88,6 +91,78 @@ __device__ __forceinline__ void wg_mainloop(float (&acc)[2][BN / 2], const uint8
       // +2 per 16 elements (32 B) along K; the second 64-row half of A starts 8 KB (+512) further
       Wgmma<FMT, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
       Wgmma<FMT, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (j > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+    }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  if (nk > 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+  }
+}
+
+// ---- e4m3 weights (FMT_E4M3).  A weight stage is a 128 x 64-byte TMA box without swizzle.  Every finite e4m3 value is
+// a bf16 value, so the upcast is exact; the MMAs then read a bf16 tile laid out as a SWIZZLE_128B TMA box would leave it
+// and issue the same wgmma chain as wg_mainloop<FMT_BF16>, so the fp32 accumulators are those of the bf16 kernel on the
+// upcast weights.
+constexpr int kF8BytesW = kGemmBM * kGemmBK;          // one e4m3 weight stage
+constexpr int kF8BytesCvt = 2 * kGemmBM * kGemmBK * 2;  // two bf16 tiles: k-block j converts while the MMAs of j - 1 run
+
+__device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t two) {
+  const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two & 0xFFFF), __NV_E4M3);
+  const __nv_bfloat162 b = __float22bfloat162_rn(__half22float2(__half2(h)));   // e4m3 -> f16 -> f32 -> bf16: all exact
+  return *reinterpret_cast<const uint32_t*>(&b);
+}
+
+// the warpgroup converts one e4m3 stage src [128][64 B] into the bf16 tile dst [128][128 B], 16-byte chunk c of row r at
+// chunk c ^ (r % 8).  Thread t converts chunks j * 128 + t: a warp reads 256 and writes 512 contiguous bytes per j.
+__device__ __forceinline__ void f8_tile_to_bf16_sw128(const uint8_t* src, uint8_t* dst) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int idx = j * 128 + static_cast<int>(threadIdx.x), r = idx >> 3, c = idx & 7;
+    const uint2 v = *reinterpret_cast<const uint2*>(src + r * 64 + c * 8);
+    const uint4 o = make_uint4(e4m3x2_to_bf16x2(v.x), e4m3x2_to_bf16x2(v.x >> 16), e4m3x2_to_bf16x2(v.y),
+                               e4m3x2_to_bf16x2(v.y >> 16));
+    *reinterpret_cast<uint4*>(dst + r * 128 + ((c ^ (r & 7)) << 4)) = o;
+  }
+}
+
+// wg_mainloop for e4m3 weight stages: k-block j is converted into cvt tile j % 2, then multiplied exactly as the bf16
+// mainloop does.  The barrier before a conversion makes every warp's MMAs of k-block j - 2 (the tile's last readers)
+// retired: each warp has passed wgmma_wait<1> of iteration j - 1 by then.  A stage goes back to the producer when the
+// MMAs of its k-block retire, as in wg_mainloop, since they read its activation tile.
+template <int BN, int S>
+__device__ __forceinline__ void wg_mainloop_f8(float (&acc)[2][BN / 2], uint8_t* smem_cvt, const uint8_t* smem_w8,
+                                               const uint8_t* smem_b, uint64_t* full_bar, uint64_t* empty_bar, int& i,
+                                               int nk) {
+  constexpr int kBytesB = BN * kGemmBK * 2;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+  for (int j = 0; j < nk; ++j, ++i) {
+    const int s = i % S;
+    uint8_t* cvt = smem_cvt + (j & 1) * (kF8BytesCvt / 2);
+    mbar_wait(&full_bar[s], (i / S) & 1);
+    if (j >= 2) wg_sync();
+    f8_tile_to_bf16_sw128(smem_w8 + s * kF8BytesW, cvt);
+    fence_proxy_async();   // the generic-proxy stores become visible to the wgmma operand reads
+    wg_sync();
+    wgmma_fence();
+    const uint64_t da = wgmma_desc_sw128(smem_u32(cvt));
+    const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + s * kBytesB));
+#pragma unroll
+    for (int kk = 0; kk < kGemmBK / 16; ++kk) {
+      Wgmma<FMT_BF16, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
+      Wgmma<FMT_BF16, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
     }
     wgmma_commit();
     wgmma_wait<1>();

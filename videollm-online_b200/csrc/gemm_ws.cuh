@@ -11,7 +11,9 @@
 //     vit_fix_ln) add the planes of each tile in plane order -> deterministic;
 //   * TILES mode (lm_head, connector): whole tiles per CTA, direct 16-bit epilogue, no partials;
 //   * the producer warp keeps the ring full across items, so the weight stream continues while the warpgroup
-//     runs the epilogue of an item.
+//     runs the epilogue of an item;
+//   * FMT_E4M3 (mode 0 only): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop_f8), each partial
+//     multiplied by its row's scale once before it is written.
 #pragma once
 #include <cuda.h>
 #include "gemm.cuh"
@@ -31,32 +33,42 @@ struct GemmWsArgs {
   const float* bias;
   int act;
   unsigned long long hint_w;  // L2 policy for the weight stream (evict-first when read once per launch)
+  const float* w_scale;       // FMT_E4M3: [rows_w] fp32 row scales, applied once to each partial
 };
 
 // deepest ring of at most 8 stages that fits next to the staging tile
 constexpr int ws_default_stages(int bn) { return fit_stages(kGemmBM * kGemmBK * 2 + bn * kGemmBK * 2, kWgStageBytes + 1024 + 256, 8); }
+// e4m3 weights: stages of half the weight bytes, so up to 16 of them (the barrier block holds 16 pairs), next to the
+// staging tile and the two converted bf16 tiles
+constexpr int ws_f8_default_stages(int bn) {
+  return fit_stages(kF8BytesW + bn * kGemmBK * 2, kF8BytesCvt + kWgStageBytes + 1024 + 256, 16);
+}
 
-template <int BN, int STAGES = ws_default_stages(BN)>
+template <int BN, int STAGES = ws_default_stages(BN), int FMT = FMT_BF16>
 struct GemmWsCfg {
   static constexpr int kStages = STAGES;
-  static constexpr int kBytesA = kGemmBM * kGemmBK * 2;
+  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : kGemmBM * kGemmBK * 2;
   static constexpr int kBytesB = BN * kGemmBK * 2;
-  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256 + kWgStageBytes;
+  static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
+  static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kWgStageBytes;
   static_assert(kSmemBytes <= kSmemOptIn, "ring + staging tile exceed the shared memory of one block");
+  static_assert(kStages <= 16, "the barrier block holds 16 full / empty pairs");
 };
 
 template <int FMT, int BN, int STAGES = ws_default_stages(BN)>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
                const GemmWsArgs p) {
-  using Cfg = GemmWsCfg<BN, STAGES>;
+  using Cfg = GemmWsCfg<BN, STAGES, FMT>;
+  constexpr bool kF8 = FMT == FMT_E4M3;
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + S * Cfg::kBytesA;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * (Cfg::kBytesA + Cfg::kBytesB));
+  uint8_t* smem_cvt = smem;               // kF8: the converted bf16 weight tiles
+  uint8_t* smem_a = smem + Cfg::kBytesCvt;
+  uint8_t* smem_b = smem + Cfg::kBytesCvt + S * Cfg::kBytesA;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBytesCvt + S * (Cfg::kBytesA + Cfg::kBytesB));
   uint64_t* empty_bar = full_bar + S;
   float* stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
 
@@ -128,13 +140,20 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
       u += nk;
       float acc[2][BN / 2];
-      wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      if constexpr (kF8)
+        wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      else
+        wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int wt = tile / p.x_tiles, xt = tile - wt * p.x_tiles;
       const int n = wt * kGemmBM + row;  // output feature (row of W)
       const int t0 = xt * BN;            // first token row of this tile
       const bool n_ok = n < p.rows_w;
       float* plane = nullptr;
       float bias_n = 0.f;
+      float scale_n = 0.f;
+      if constexpr (kF8) {
+        if (n_ok) scale_n = __ldg(p.w_scale + n);
+      }
       if (p.mode == 0) {
         const int pl = c - sk_first_cta(tile, p.sk);
         plane = reinterpret_cast<float*>(p.out) + static_cast<size_t>(pl) * p.plane_stride;
@@ -154,7 +173,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           const int t = t0 + c0 + j;
           if (t >= p.rows_x) break;
           const float acc = v[j];
-          if (p.mode == 0) {
+          if constexpr (kF8) {
+            plane[static_cast<size_t>(t) * p.rows_w + n] = __fmul_rn(acc, scale_n);   // the one rounding of the scale
+          } else if (p.mode == 0) {
             plane[static_cast<size_t>(t) * p.rows_w + n] = acc;
           } else {
             float x = r16<FMT>(acc + bias_n);

@@ -13,6 +13,8 @@
 //     gate and up are finished by different threads: they are exchanged through a small shared-memory tile.
 // Only gate|up has enough tiles to amortise the finisher tail; q|k|v, o_proj and down_proj leave fp32 planes to the
 // fix-up kernels of decoder_kernels.cuh, whose rounding points this epilogue shares.
+// gemm_wsf_f8_kernel runs the same schedule on e4m3 weights (FMT_E4M3, gemm.cuh): every contributor, the finisher's own
+// accumulator included, multiplies its fp32 partial of feature n by the row scale w_scale[n] once before the plane sum.
 // All CTAs of the grid are co-resident or become so without depending on a waiting CTA (grid <= #SMs, the PDL successor
 // cannot start before every CTA of this grid has started), so the finisher's wait cannot dead-lock; it is bounded anyway.
 #pragma once
@@ -35,18 +37,24 @@ struct GemmWsfArgs {
 
 constexpr int kWsfXchStride = 17;   // floats per feature row of the exchange tile (16 tokens + 1: conflict-free)
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, int FMT = FMT_BF16>
 struct GemmWsfCfg {
   static constexpr int kStages = STAGES;
-  static constexpr int kBytesA = kGemmBM * kGemmBK * 2;
+  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : kGemmBM * kGemmBK * 2;
   static constexpr int kBytesB = BN * kGemmBK * 2;
+  static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
   static constexpr int kXchBytes = kGemmBM * kWsfXchStride * 4;
-  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + 1024 + 256 + kXchBytes + kWgStageBytes;
+  static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kXchBytes + kWgStageBytes;
   static_assert(kSmemBytes <= kSmemOptIn, "ring + exchange + staging tiles exceed the shared memory of one block");
+  static_assert(kStages <= 16, "the barrier block holds 16 full / empty pairs");
 };
 // deepest ring of at most 8 stages that fits next to the exchange and staging tiles
 constexpr int wsf_default_stages(int bn) {
   return fit_stages(kGemmBM * kGemmBK * 2 + bn * kGemmBK * 2, 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 8);
+}
+// e4m3 weights: up to 16 half-size stages next to the converted bf16 tiles, the exchange and the staging tile
+constexpr int wsf_f8_default_stages(int bn) {
+  return fit_stages(kF8BytesW + bn * kGemmBK * 2, kF8BytesCvt + 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 16);
 }
 
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
@@ -55,19 +63,20 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-// p is __grid_constant__ so that its fields are read from parameter space where used: ptxas otherwise copies a struct
-// this small up front, which costs the 64- and 128-token instances registers.
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
-                const __grid_constant__ GemmWsfArgs p) {
-  using Cfg = GemmWsfCfg<BN, STAGES>;
+// The body of both kernels below; FMT is FMT_BF16 or FMT_E4M3 (the weight format).  p by value: ptxas then still reads
+// the fields from parameter space where used (the bf16 kernels compile to the same code as with the body inline).
+template <int FMT, int BN, int STAGES>
+__device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUtensorMap& tm_x, const GemmWsfArgs p,
+                                              const float* w_scale) {
+  using Cfg = GemmWsfCfg<BN, STAGES, FMT>;
+  constexpr bool kF8 = FMT == FMT_E4M3;
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + S * Cfg::kBytesA;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * (Cfg::kBytesA + Cfg::kBytesB));
+  uint8_t* smem_cvt = smem;               // kF8: the converted bf16 weight tiles
+  uint8_t* smem_a = smem + Cfg::kBytesCvt;
+  uint8_t* smem_b = smem + Cfg::kBytesCvt + S * Cfg::kBytesA;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBytesCvt + S * (Cfg::kBytesA + Cfg::kBytesB));
   uint64_t* empty_bar = full_bar + S;
   float* xch = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);   // [128][17] exchange tile
   float* stage = xch + kGemmBM * kWsfXchStride;
@@ -128,11 +137,18 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
       const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
       u += nk;
       float acc[2][BN / 2];
-      wg_mainloop<FMT_BF16, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      if constexpr (kF8)
+        wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      else
+        wg_mainloop<FMT_BF16, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int pl = c - sk_first_cta(tile, p.sk);
       const int n_planes = sk_planes(tile, p.sk);
       const int n = tile * kGemmBM + d;
       const bool n_ok = n < p.rows_w;
+      float scale_n = 0.f;
+      if constexpr (kF8) {
+        if (n_ok) scale_n = __ldg(w_scale + n);
+      }
       if (pl > 0) {
         // ---- contributor: publish the partial plane, then bump the tile's arrival counter
         float* plane = p.planes + static_cast<size_t>(pl - 1) * p.plane_stride;
@@ -148,7 +164,10 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
           for (int j = 0; j < 16; ++j) {
             const int t = c0 + j;
             if (t >= p.rows_x) break;
-            __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, v[j]);
+            if constexpr (kF8)
+              __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, __fmul_rn(v[j], scale_n));
+            else
+              __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, v[j]);
           }
         }
         __threadfence();
@@ -182,6 +201,10 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
         wg_sync();
         float x[16];
         wg_load16(stage, d, x);
+        if constexpr (kF8) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) x[j] = __fmul_rn(x[j], scale_n);   // the finisher's own partial, before the sum
+        }
         for (int s2 = 1; s2 < n_planes; ++s2) {   // plane order: deterministic
           const float* plane = p.planes + static_cast<size_t>(s2 - 1) * p.plane_stride + n;
           float a[16];
@@ -213,6 +236,22 @@ gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant_
       }
     }
   }
+}
+
+// p is __grid_constant__ so that its fields are read from parameter space where used: ptxas otherwise copies a struct
+// this small up front, which costs the 64- and 128-token instances registers.
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_wsf_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
+                const __grid_constant__ GemmWsfArgs p) {
+  gemm_wsf_body<FMT_BF16, BN, STAGES>(tm_w, tm_x, p, nullptr);
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_wsf_f8_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
+                   const __grid_constant__ GemmWsfArgs p, const float* __restrict__ w_scale) {
+  gemm_wsf_body<FMT_E4M3, BN, STAGES>(tm_w, tm_x, p, w_scale);
 }
 
 }  // namespace vlo

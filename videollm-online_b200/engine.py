@@ -214,6 +214,11 @@ class Engine:
     def weights(self) -> Dict[str, torch.Tensor]:
         return self._weights
 
+    @property
+    def fp8_weights(self) -> bool:
+        """True when the decoder layer matrices were loaded as e4m3 codes + row scales (weights.quantize_fp8_rows)."""
+        return "L0.qkv.f8" in self._weights
+
     def device_bytes(self) -> int:
         return int(self.lib.vlo_engine_device_bytes(self._h))
 

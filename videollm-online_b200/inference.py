@@ -23,6 +23,7 @@ from typing import Optional
 
 import torch
 
+from ._lib import VloError
 from .config import LiveArguments, SamplingConfig, parse_args
 from .engine import KvImage, check_context_window, sink_tokens
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
@@ -47,6 +48,7 @@ class SessionState:
     started: bool                # past_key_values was set: a step ran since the last reset
     sampling: Optional[SamplingConfig] = None   # LiveInfer.sampling (None: greedy responses)
     evicted_tokens: int = 0      # cache positions the session's context window dropped so far
+    fp8_weights: bool = False    # the cache was written by a model with FP8 layer weights (Engine.fp8_weights)
 
 
 torch.serialization.add_safe_globals([SessionState, SamplingConfig])
@@ -188,7 +190,7 @@ class LiveInfer:
                 frame_embeds_queue=frames,
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
                 n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling,
-                evicted_tokens=self.evicted_tokens)
+                evicted_tokens=self.evicted_tokens, fp8_weights=self._kv.engine.fp8_weights)
             self.reset()
             return state
 
@@ -196,10 +198,15 @@ class LiveInfer:
         """Continue a session `suspend()` returned: the cache is copied back into this session's (emptied) stream and
         every queue and counter `__call__` reads is restored.  The video is not part of the state: load it again
         (before or after resuming).  Raises VloError if the pool is short or the image belongs to another config; the
-        session's stream is then empty and the rest of the session unchanged."""
+        session's stream is then empty and the rest of the session unchanged.  A state whose cache was written with the
+        other weight form (FP8 or bf16 layer weights: a different model) is refused before anything changes."""
         with self._lock:
-            self._drop_prefetch()
             eng = self._kv.engine
+            if state.fp8_weights != eng.fp8_weights:
+                form = {True: "FP8", False: "bf16"}
+                raise VloError(f"resume: the state's cache was written with {form[state.fp8_weights]} layer weights, "
+                               f"this model has {form[eng.fp8_weights]} ones")
+            self._drop_prefetch()
             eng.stream_reset(self._kv.stream_id)
             eng.kv_swap_in(self._kv.stream_id, state.kv)
             dev = self.device

@@ -17,6 +17,9 @@ Engine layout (name -> tensor), all contiguous on the engine's device:
   vit.L{i}.{ln1,ln2}.{w,b} f32, vit.L{i}.qkv.w [3C,C] f16 (+ .b f32), out.w [C,C], fc1.w [M,C], fc2.w [C,M]
   vit.head.q [C] f32 (= in_proj_q(probe), fp16-rounded), vit.head.kv.{w,b}, out.{w,b}, ln.{w,b}, fc1, fc2
 16-bit biases are stored as fp32 copies of their 16-bit values (the GEMM epilogue adds them in fp32).
+FP8 weights (fp8_weights=True): each layer matrix L{i}.{qkv,o,gate_up,down} [N, K] is replaced by L{i}.{m}.f8 (e4m3fn
+bytes [N, K], uint8) and L{i}.{m}.scale (fp32 [N], one scale per output row), quantized by quantize_fp8_rows from the
+bf16 matrix above (after the LoRA merge and the gate|up interleave).  Everything else stays 16-bit.
 """
 from __future__ import annotations
 
@@ -174,7 +177,46 @@ def interleave_gate_up(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
     return torch.stack([gate.view(I // 64, 64, H), up.view(I // 64, 64, H)], 1).reshape(2 * I, H).contiguous()
 
 
-def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: int) -> StateDict:
+FP8_MAX = 448.0   # largest finite e4m3fn value
+LAYER_MATRICES = ("qkv", "o", "gate_up", "down")   # the decoder layer matrices fp8_weights quantizes
+
+
+def quantize_fp8_rows(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """[N, K] weight -> (e4m3fn codes as uint8 [N, K], fp32 scales [N]) on w's device:
+    s[n] = fp32(max_k |W[n, k]|) / 448 (1 for an all-zero row), q[n, k] = e4m3fn(clamp(fp32(W[n, k]) / s[n], -448, 448))
+    rounded to nearest even, so W[n, k] ~ fp32(q[n, k]) * s[n] and no code is NaN."""
+    if w.dim() != 2:
+        raise ValueError(f"quantize_fp8_rows: a 2-D weight, got shape {tuple(w.shape)}")
+    w32 = w.float()
+    if not bool(torch.isfinite(w32).all()):
+        raise ValueError("quantize_fp8_rows: the weight holds a non-finite value")
+    amax = w32.abs().amax(dim=1)
+    scale = torch.where(amax > 0, amax / FP8_MAX, torch.ones_like(amax))
+    q = (w32 / scale[:, None]).clamp_(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn)
+    return q.view(torch.uint8), scale.contiguous()
+
+
+def dequantize_fp8_rows(codes: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
+    """fp32 [N, K] = fp32(q) * s: the weight the FP8 kernels multiply by (up to where the scale is applied)."""
+    return codes.view(torch.float8_e4m3fn).float() * scale[:, None]
+
+
+def layer_matrix_spec(name: str, shape: tuple, fp8_weights: bool) -> Dict[str, tuple]:
+    """Engine tensor name -> (shape, dtype) of one layer matrix [N, K] in the chosen form."""
+    if not fp8_weights:
+        return {name: (shape, torch.bfloat16)}
+    return {name + ".f8": (shape, torch.uint8), name + ".scale": ((shape[0],), torch.float32)}
+
+
+def _put_layer_matrix(out: StateDict, name: str, w: torch.Tensor, fp8_weights: bool) -> None:
+    # quantized on w's device, one matrix at a time: the bf16 matrix is dropped as soon as its codes exist
+    if fp8_weights:
+        out[name + ".f8"], out[name + ".scale"] = quantize_fp8_rows(w)
+    else:
+        out[name] = w
+
+
+def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: int, fp8_weights: bool = False) -> StateDict:
     bf = torch.bfloat16
     out: StateDict = {}
 
@@ -190,11 +232,13 @@ def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: i
         p = f"model.layers.{i}."
         out[f"L{i}.in_norm"] = take(p + "input_layernorm.weight")
         out[f"L{i}.post_norm"] = take(p + "post_attention_layernorm.weight")
-        out[f"L{i}.qkv"] = torch.cat([take(p + "self_attn.q_proj.weight"), take(p + "self_attn.k_proj.weight"),
-                                      take(p + "self_attn.v_proj.weight")], 0).contiguous()
-        out[f"L{i}.o"] = take(p + "self_attn.o_proj.weight")
-        out[f"L{i}.gate_up"] = interleave_gate_up(take(p + "mlp.gate_proj.weight"), take(p + "mlp.up_proj.weight"))
-        out[f"L{i}.down"] = take(p + "mlp.down_proj.weight")
+        _put_layer_matrix(out, f"L{i}.qkv", torch.cat([take(p + "self_attn.q_proj.weight"),
+                                                       take(p + "self_attn.k_proj.weight"),
+                                                       take(p + "self_attn.v_proj.weight")], 0).contiguous(), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.o", take(p + "self_attn.o_proj.weight"), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.gate_up", interleave_gate_up(take(p + "mlp.gate_proj.weight"),
+                                                                   take(p + "mlp.up_proj.weight")), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.down", take(p + "mlp.down_proj.weight"), fp8_weights)
     if "connector.0.weight" in sd:
         out["conn.0.w"] = take("connector.0.weight")
         out["conn.0.b"] = _b32_from16(sd["connector.0.bias"].to(device), bf)
@@ -245,9 +289,11 @@ def pack_vision_for_engine(cfg: LiveConfig, sd: StateDict, device) -> StateDict:
     return out
 
 
-def synthetic_engine_weights(cfg: LiveConfig, device, max_positions: int, seed: int = 0, std: float = 0.02) -> StateDict:
+def synthetic_engine_weights(cfg: LiveConfig, device, max_positions: int, seed: int = 0, std: float = 0.02,
+                             fp8_weights: bool = False) -> StateDict:
     """Full-size synthetic weights generated directly in the engine layout on `device` (bench path: no
-    16 GB host round trip).  Same distributions as synthetic_*_state, different random stream."""
+    16 GB host round trip).  Same distributions as synthetic_*_state, different random stream.  fp8_weights: the layer
+    matrices of the same seed, quantized."""
     g = torch.Generator(device=device).manual_seed(seed)
     bf, f16, f32 = torch.bfloat16, torch.float16, torch.float32
     H, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
@@ -261,10 +307,10 @@ def synthetic_engine_weights(cfg: LiveConfig, device, max_positions: int, seed: 
     for i in range(cfg.num_hidden_layers):
         out[f"L{i}.in_norm"] = _gen((H,), 0.1, g, device, bf, 1.0)
         out[f"L{i}.post_norm"] = _gen((H,), 0.1, g, device, bf, 1.0)
-        out[f"L{i}.qkv"] = _gen(((nh + 2 * nkv) * hd, H), std, g, device, bf)
-        out[f"L{i}.o"] = _gen((H, nh * hd), std, g, device, bf)
-        out[f"L{i}.gate_up"] = _gen((2 * I, H), std, g, device, bf)
-        out[f"L{i}.down"] = _gen((H, I), std, g, device, bf)
+        _put_layer_matrix(out, f"L{i}.qkv", _gen(((nh + 2 * nkv) * hd, H), std, g, device, bf), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.o", _gen((H, nh * hd), std, g, device, bf), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.gate_up", _gen((2 * I, H), std, g, device, bf), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.down", _gen((H, I), std, g, device, bf), fp8_weights)
     out["conn.0.w"] = _gen((H, C), std, g, device, bf)
     out["conn.0.b"] = _gen((H,), std, g, device, bf).float()
     out["conn.2.w"] = _gen((H, H), std, g, device, bf)
