@@ -127,6 +127,20 @@ int vlo_kv_copy_prefix(vlo_engine* e, int src_stream_id, int dst_stream_id, int 
  * stream's length or table and no free-page count. */
 int vlo_kv_evict(vlo_engine* e, int stream_id, int first_token, int n_tokens, const float* h_cos, const float* h_sin,
                  void* cuda_stream);
+/* Token-granular window over a stream's cache: keep only the cache positions in n_spans spans
+ * [keep_first[i], keep_first[i] + keep_len[i]) of stream_id (sorted, non-overlapping, each len > 0, inside [0, kv_len),
+ * at least one position dropped).  Span i moves down to new_first[i] = sum_{j<i} keep_len[j]; its shift is
+ * d_i = keep_first[i] - new_first[i].  V rows move unchanged.  K rows move and are rotated by -d_i with the exact formula
+ * of vlo_kv_evict, using h_rot[i] = cos[head_dim/2] | sin[head_dim/2] of d_i (weights.rope_rotation), so h_rot holds
+ * n_spans * head_dim fp32 values.  Rows with d_i = 0 are not touched.  The new kv_len is sum(keep_len).  Pages past
+ * ceil(new_len / 64) go back to the pool; the rows past the new kv_len on the last page keep old, finite values.
+ * The rows move in place, page by page in increasing order, through the decoder step's partial-sum workspace: the call
+ * takes no free page and no device memory, and works on a full pool.  Because it uses that workspace it is ordered
+ * like a step: enqueue it on the CUDA stream the engine's steps run on.  The tables go through one slot of the pinned
+ * staging ring, which caps n_spans (hundreds at least; the error message of a larger call names the cap).  A call
+ * that fails changes no stream's length, table or row and no free-page count. */
+int vlo_kv_compact(vlo_engine* e, int stream_id, int n_spans, const int32_t* h_keep_first, const int32_t* h_keep_len,
+                   const float* h_rot, void* cuda_stream);
 /* test/bench hook: fill a stream's KV cache with deterministic pseudo-random values up to n_tokens
  * (pre-fill for the 12k-context measurements without replaying 1200 frames) */
 int vlo_kv_fill_synthetic(vlo_engine* e, int stream_id, int n_tokens, uint64_t seed, void* cuda_stream);

@@ -73,6 +73,7 @@ SIGNATURES = {
     "vlo_kv_truncate": (_I, [_P, _I, _I]),
     "vlo_kv_copy_prefix": (_I, [_P, _I, _I, _I, _P]),
     "vlo_kv_evict": (_I, [_P, _I, _I, _I, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
+    "vlo_kv_compact": (_I, [_P, _I, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_float), _P]),
     "vlo_kv_fill_synthetic": (_I, [_P, _I, _I, C.c_uint64, _P]),
     "vlo_kv_read": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_kv_write": (_I, [_P, _I, _I, _I, _P, _I, _P]),

@@ -6,6 +6,8 @@
 Responses are greedy unless --do_sample is given (SamplingConfig; --seed stays the synthetic weights' seed).
 --context_window N keeps the session's cache within N tokens (0: off): the start prompt stays, the oldest pages after it
 are dropped.
+--context_keep_turns (with --context_window) drops the oldest frames token by token instead, and keeps the questions and
+answers.
 --fp8_weights serves the decoder layers from e4m3 weights with per-row scales (half their bytes per step; the model's
 numbers change, so it is off by default).
 

@@ -161,6 +161,9 @@ class LiveArguments:
     # LiveInfer.context_window, tokens: keep the start prompt and drop the oldest cache pages after it so the session's
     # cache never exceeds this many tokens; 0: off (the cache grows until max_kv_tokens)
     context_window: int = 0
+    # LiveInfer.context_keep_turns: with a context window, drop old frames token by token and keep the questions and
+    # answers (engine.retain_spans) instead of dropping whole pages; no effect without a window
+    context_keep_turns: bool = False
     # response sampling (SamplingConfig; HF GenerationConfig names, sample_seed = its seed); greedy without --do_sample
     do_sample: bool = False
     temperature: float = 1.0

@@ -412,22 +412,12 @@ __global__ void __launch_bounds__(256) kv_fill_kernel(const KvSide dst, int n_kv
   }
 }
 
-// KV eviction: rotate the keys of positions [pos0, pos0 + n_tok) of every kv head and layer by -delta in place, so that
-// a key RoPE put at position p sits at p - delta (V has no position in it and is not touched).  With the RoPE pairs
-// (d, d + 64) of qkv_rope_append_kernel and cs = [c_0 .. c_63 | s_0 .. s_63], c_d = cos(delta f_d), s_d = sin(delta f_d):
-//   k'[d]      = bf16(fl(fl(x1 c_d) + fl(x2 s_d)))
-//   k'[d + 64] = bf16(fl(fl(x2 c_d) - fl(x1 s_d)))
-// every fl one fp32 round-to-nearest (no FMA contraction), so an fp32 emulation reproduces it bit for bit.  Each thread
-// rotates eight pairs of one row (two 16-byte loads and stores); no row depends on another.  K of layer l is plane 2 l.
-// grid = (ceil(n_tok * 8 / 256), n_kv_heads, layers), block = 256.
-__global__ void __launch_bounds__(256) kv_rerotate_kernel(const KvSide k, int n_kv, int pos0, int n_tok, const float* cs) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long long>(n_tok) * 8) return;
-  const int pos = pos0 + static_cast<int>(i >> 3), d0 = static_cast<int>(i & 7) * 8, h = blockIdx.y, l = blockIdx.z;
-  __nv_bfloat16* row = k.base + 2ll * l * k.plane_stride + kv_side_row(k, n_kv, h, pos) * 128;
-  uint4* lo = reinterpret_cast<uint4*>(row + d0);
-  uint4* hi = reinterpret_cast<uint4*>(row + 64 + d0);
-  const uint4 a = *lo, b = *hi;
+// The re-rotation of eight RoPE pairs (d, d + 64), d = d0 .. d0 + 7, of one key row: a holds x1 = k[d0 .. d0 + 8),
+// b holds x2 = k[64 + d0 .. 64 + d0 + 8), cs = [c_0 .. c_63 | s_0 .. s_63].  On return
+//   a[d] = bf16(fl(fl(x1 c_d) + fl(x2 s_d)))      b[d] = bf16(fl(fl(x2 c_d) - fl(x1 s_d)))
+// every fl one fp32 round-to-nearest (no FMA contraction), so an fp32 emulation reproduces it bit for bit.  The one
+// definition of the arithmetic kv_rerotate_kernel and kv_compact_kernel share.
+__device__ __forceinline__ void rope_rerotate8(uint4& a, uint4& b, const float* cs, int d0) {
   float c[8], s[8];
   *reinterpret_cast<float4*>(c) = *reinterpret_cast<const float4*>(cs + d0);
   *reinterpret_cast<float4*>(c + 4) = *reinterpret_cast<const float4*>(cs + d0 + 4);
@@ -447,8 +437,76 @@ __global__ void __launch_bounds__(256) kv_rerotate_kernel(const KvSide k, int n_
     oa[j] = *reinterpret_cast<const uint32_t*>(&r1);
     ob[j] = *reinterpret_cast<const uint32_t*>(&r2);
   }
-  *lo = make_uint4(oa[0], oa[1], oa[2], oa[3]);
-  *hi = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+  a = make_uint4(oa[0], oa[1], oa[2], oa[3]);
+  b = make_uint4(ob[0], ob[1], ob[2], ob[3]);
+}
+
+// KV eviction: rotate the keys of positions [pos0, pos0 + n_tok) of every kv head and layer by -delta in place, so that
+// a key RoPE put at position p sits at p - delta (V has no position in it and is not touched).  With the RoPE pairs
+// (d, d + 64) of qkv_rope_append_kernel and cs = [c_0 .. c_63 | s_0 .. s_63], c_d = cos(delta f_d), s_d = sin(delta f_d),
+// each key is rotated by rope_rerotate8.  Each thread rotates eight pairs of one row (two 16-byte loads and stores); no
+// row depends on another.  K of layer l is plane 2 l.
+// grid = (ceil(n_tok * 8 / 256), n_kv_heads, layers), block = 256.
+__global__ void __launch_bounds__(256) kv_rerotate_kernel(const KvSide k, int n_kv, int pos0, int n_tok, const float* cs) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= static_cast<long long>(n_tok) * 8) return;
+  const int pos = pos0 + static_cast<int>(i >> 3), d0 = static_cast<int>(i & 7) * 8, h = blockIdx.y, l = blockIdx.z;
+  __nv_bfloat16* row = k.base + 2ll * l * k.plane_stride + kv_side_row(k, n_kv, h, pos) * 128;
+  uint4* lo = reinterpret_cast<uint4*>(row + d0);
+  uint4* hi = reinterpret_cast<uint4*>(row + 64 + d0);
+  uint4 a = *lo, b = *hi;
+  rope_rerotate8(a, b, cs, d0);
+  *lo = a;
+  *hi = b;
+}
+
+// Token-granular KV compaction (vlo_kv_compact), one batch of (destination page, plane) units.  Kept span i moves from
+// cache positions [src[i], src[i] + len) to [dst[i], dst[i] + len), dst[i] <= src[i]; its keys are rotated by
+// rope_rerotate8 with cs + 128 i (cos | sin of d_i = src[i] - dst[i]), its values are copied.  Unit u of the batch is
+// destination page j = j0 + (u0 + u) / planes of plane (u0 + u) % planes (K of layer l is plane 2 l, V plane 2 l + 1).
+//   gather (to_stage): read the sources of the unit's positions q in [q_lo, new_len) through the stream's table, rotate
+//     the K rows, write them to stage[u][kv head][q % 64][128];
+//   scatter: copy those stage rows to the unit's own positions, through the same table.
+// A destination page j only reads source positions >= 64 j (every d_i >= 0), so the batches, run in increasing unit
+// order with a batch's scatter after its gather, never overwrite a row a later batch still reads: the compaction runs in
+// place, and its bits do not depend on the batching.  Positions below q_lo (spans with d_i = 0) and past new_len are not
+// written.  Each thread moves eight RoPE pairs (or 16 V elements) of one row.
+// grid = (ceil(n_units * n_kv * 64 * 8 / 256)), block = 256.
+struct CompactSpans {
+  const float* cs;   // [n][128]: cos | sin of each span's shift
+  const int* src;    // [n] first source position of each span
+  const int* dst;    // [n] first destination position, ascending, dst[0] = 0
+  int n;
+};
+__global__ void __launch_bounds__(256) kv_compact_kernel(const KvSide kv, int n_kv, int planes, int j0, int u0, int n_units,
+                                                         int q_lo, int new_len, const CompactSpans sp,
+                                                         __nv_bfloat16* stage, int to_stage) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int per_unit = n_kv * 64 * 8;
+  if (i >= static_cast<long long>(n_units) * per_unit) return;
+  const int u = static_cast<int>(i / per_unit), t = static_cast<int>(i % per_unit);
+  const int h = t >> 9, r = (t >> 3) & 63, d0 = (t & 7) * 8;
+  const int unit = u0 + u, pl = unit % planes, q = (j0 + unit / planes) * 64 + r;
+  if (q < q_lo || q >= new_len) return;
+  __nv_bfloat16* st = stage + ((static_cast<long long>(u) * n_kv + h) * 64 + r) * 128;
+  __nv_bfloat16* plane = kv.base + pl * kv.plane_stride;
+  if (!to_stage) {
+    __nv_bfloat16* row = plane + kv_side_row(kv, n_kv, h, q) * 128;
+    *reinterpret_cast<uint4*>(row + d0) = *reinterpret_cast<const uint4*>(st + d0);
+    *reinterpret_cast<uint4*>(row + 64 + d0) = *reinterpret_cast<const uint4*>(st + 64 + d0);
+    return;
+  }
+  int lo = 0, hi = sp.n - 1;   // the span holding q: the last one with dst <= q
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (sp.dst[mid] <= q) lo = mid;
+    else hi = mid - 1;
+  }
+  const __nv_bfloat16* row = plane + kv_side_row(kv, n_kv, h, sp.src[lo] + q - sp.dst[lo]) * 128;
+  uint4 a = *reinterpret_cast<const uint4*>(row + d0), b = *reinterpret_cast<const uint4*>(row + 64 + d0);
+  if ((pl & 1) == 0) rope_rerotate8(a, b, sp.cs + 128ll * lo, d0);
+  *reinterpret_cast<uint4*>(st + d0) = a;
+  *reinterpret_cast<uint4*>(st + 64 + d0) = b;
 }
 
 }  // namespace vlo

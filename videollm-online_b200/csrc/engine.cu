@@ -808,6 +808,87 @@ int vlo_kv_evict(vlo_engine* e, int sid, int first_token, int n_tokens, const fl
   return 0;
 }
 
+namespace {
+// vlo_kv_compact's tables, laid out the same way in a staging slot and at the start of e->part:
+// cos | sin [n][head_dim] fp32, then src [n], dst [n] and the stream's page table, int32
+size_t compact_table_bytes(const vlo_engine* e, int n_spans) {
+  return sizeof(float) * n_spans * e->cfg.head_dim + sizeof(int) * (2 * static_cast<size_t>(n_spans) +
+                                                                     kv_pages_for(e->cfg.max_kv_tokens));
+}
+// most spans one call may pass: its tables fill at most one staging slot
+int compact_max_spans(const vlo_engine* e) {
+  const size_t per_span = sizeof(float) * e->cfg.head_dim + 2 * sizeof(int);
+  return static_cast<int>((e->stage_slot_bytes - compact_table_bytes(e, 0)) / per_span);
+}
+}  // namespace
+
+int vlo_kv_compact(vlo_engine* e, int sid, int n_spans, const int32_t* h_keep_first, const int32_t* h_keep_len,
+                   const float* h_rot, void* cuda_stream) {
+  DevGuard dev_guard(e);
+  if (check_stream(e, sid)) return -1;
+  const vlo_config& c = e->cfg;
+  const int cap = compact_max_spans(e);
+  VLO_CHECK(n_spans > 0 && n_spans <= cap, "kv_compact: n_spans must be within [1, " + std::to_string(cap) + "], got " +
+                                               std::to_string(n_spans));
+  VLO_CHECK(h_keep_first != nullptr && h_keep_len != nullptr && h_rot != nullptr, "kv_compact: null span table");
+  const int len = e->pool.len(sid);
+  long long kept = 0, end = 0;  // end: first position after the previous span
+  int first_moved = -1;         // first span with a shift > 0: every later one has one as well
+  for (int i = 0; i < n_spans; ++i) {
+    const long long f = h_keep_first[i], n = h_keep_len[i];
+    VLO_CHECK(n > 0, "kv_compact: span " + std::to_string(i) + " is empty");
+    VLO_CHECK(f >= end, "kv_compact: spans must be sorted and non-overlapping (span " + std::to_string(i) + ")");
+    VLO_CHECK(f + n <= len, "kv_compact: span " + std::to_string(i) + " ends past kv_len " + std::to_string(len));
+    if (first_moved < 0 && f > kept) first_moved = i;
+    kept += n;
+    end = f + n;
+  }
+  VLO_CHECK(kept < len, "kv_compact: the spans keep every position: nothing is dropped");
+  const int new_len = static_cast<int>(kept);
+  const size_t unit_bytes = kv_page_bytes(e), head = align256(compact_table_bytes(e, n_spans));
+  const size_t part_bytes = e->part_elems * sizeof(float);
+  const long long batch_units = part_bytes > head ? static_cast<long long>((part_bytes - head) / unit_bytes) : 0;
+  VLO_CHECK(batch_units > 0, "kv_compact: the step workspace cannot stage one KV page");
+  if (first_moved >= 0) {
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    uint8_t* hs;
+    int slot;
+    if (stage_acquire(e, &hs, &slot)) return -1;
+    const std::vector<int>& tab = e->pool.table(sid);
+    float* cs = reinterpret_cast<float*>(hs);
+    int* src = reinterpret_cast<int*>(cs + static_cast<size_t>(n_spans) * c.head_dim);
+    int* dst = src + n_spans;
+    std::memcpy(cs, h_rot, sizeof(float) * n_spans * c.head_dim);
+    std::memcpy(src, h_keep_first, sizeof(int) * n_spans);
+    for (int i = 0, q = 0; i < n_spans; q += h_keep_len[i++]) dst[i] = q;
+    const int q_lo = dst[first_moved];
+    std::memcpy(dst + n_spans, tab.data(), sizeof(int) * tab.size());
+    uint8_t* d_tab = reinterpret_cast<uint8_t*>(e->part);
+    VLO_CUDA(cudaMemcpyAsync(d_tab, hs, compact_table_bytes(e, n_spans), cudaMemcpyHostToDevice, st));
+    if (stage_release(e, slot, st)) return -1;
+    const float* d_cs = reinterpret_cast<const float*>(d_tab);
+    const int* d_src = reinterpret_cast<const int*>(d_cs + static_cast<size_t>(n_spans) * c.head_dim);
+    const CompactSpans sp{d_cs, d_src, d_src + n_spans, n_spans};
+    const KvSide kv = kv_paged_side(e, e->kv, d_src + 2 * n_spans);
+    bf16* stage = reinterpret_cast<bf16*>(d_tab + head);
+    // (destination page, plane) units from the page of q_lo on, page-major: page j's units run before page j + 1's
+    const int planes = 2 * c.num_layers, j0 = q_lo / kKvPageTokens;
+    const long long units = static_cast<long long>(kv_pages_for(new_len) - j0) * planes;
+    const long long per_unit = static_cast<long long>(c.num_kv_heads) * kKvPageTokens * 8;
+    for (long long u0 = 0; u0 < units; u0 += batch_units) {
+      const int n = static_cast<int>(std::min(batch_units, units - u0));
+      const dim3 grid(static_cast<unsigned>((n * per_unit + 255) / 256));
+      for (int to_stage = 1; to_stage >= 0; --to_stage) {
+        kv_compact_kernel<<<grid, 256, 0, st>>>(kv, c.num_kv_heads, planes, j0, static_cast<int>(u0), n, q_lo, new_len,
+                                                sp, stage, to_stage);
+        VLO_LAUNCH_CHECK();
+      }
+    }
+  }
+  e->pool.commit(sid, new_len);
+  return 0;
+}
+
 // ------------------------------------------------------------------------------ host images of a stream's cache
 // One cudaMemcpy2DAsync per page moves the page's 2L planes (K and V of every layer, each at the plane stride of the
 // pool) to or from `kv_page_bytes x 2L` contiguous host bytes: copy engines only, no SM is taken from other streams.

@@ -104,14 +104,110 @@ def evict_span(kv_len: int, need: int, window: int, keep_tokens: int, page: int)
     return first, min(avail, max(least, -(-window // (8 * page)))) * page
 
 
-def check_context_window(window: int, max_kv_tokens: int, keep_tokens: int, largest_need: int, page: int):
-    """Raise ValueError unless a context window of `window` tokens is usable: within max_kv_tokens, and large enough
-    for the sink pages, one eviction chunk (window / 8 in whole pages) and the largest single step or response
-    reserve (`largest_need`)."""
+def retain_spans(row_ids: Sequence[int], need: int, window: int, keep_tokens: int, interval_id: Optional[int],
+                 frame_num_tokens: int) -> List[tuple[int, int]]:
+    """The policy of a context window that keeps the conversation (`context_keep_turns`): the spans [(first, n), ...] of
+    cache positions to keep before a stream appends `need` more, [] when len(row_ids) + need <= window.
+
+    row_ids holds the id fed at every cache position, -1 for a frame row.  After the start prompt [0, keep_tokens),
+    which stays exactly, the history is read as stream messages (frames of frame_num_tokens rows, one interval_id row
+    between two frames of a message; none when interval_id is None) and the text between them: a turn is the text from
+    the "]" that closes a message to the "\\n[" that reopens one.  What goes, in whole units:
+      1. while the turn rows kept after the prompt exceed window / 2: the oldest whole turn, together with the last
+         frame of the message before it, so the two messages merge as "... F , G ...";
+      2. the oldest frames, each with the interval row after it; the last frame of a message never goes alone;
+      3. older turns as in 1, if the frames were not enough.
+    It stops once at least max(len(row_ids) + need - window, window / 8) positions go (window / 8 at least, so the
+    compaction is paid once per window / 8 tokens), and raises VloError when dropping every unit is not enough.  The
+    kept ids are then what the chat template renders for the same conversation with those frames and turns deleted,
+    and every message that stays keeps at least one frame.  Text before the first or after the last frame stays."""
+    kv_len = len(row_ids)
+    excess = kv_len + need - window
+    if excess <= 0:
+        return []
+    fnt, sep = frame_num_tokens, (0 if interval_id is None else 1)
+    frames, texts = [], []           # frame starts; text runs (start, end) after the prompt, in order
+    i = keep_tokens
+    while i < kv_len:
+        j = i
+        if row_ids[i] < 0:
+            while j < kv_len and row_ids[j] < 0:
+                j += 1
+            if (j - i) % fnt:
+                raise VloError(f"context window: {j - i} frame rows at position {i} are not whole frames of {fnt}")
+            frames.extend(range(i, j, fnt))
+        else:
+            while j < kv_len and row_ids[j] >= 0:
+                j += 1
+            texts.append((i, j))
+        i = j
+    is_frame = set(frames)
+    # a frame continues its message when the next frame follows it after `sep` interval rows
+    next_frame = lambda f: f + fnt + sep in is_frame and (not sep or row_ids[f + fnt] == interval_id)
+    frame_units = [(f, f + fnt + sep) for f in frames if next_frame(f)]
+    seps = {f + fnt for f in frames if sep and next_frame(f)}
+    turns = [(s, e) for s, e in texts if s not in seps]          # the text rows the turn budget counts
+    # a droppable turn lies between two messages: from the last frame before it to the first frame after it
+    turn_units = [(s - fnt, e, e - s) for s, e in turns if s - fnt in is_frame and e in is_frame]
+    text_rows = sum(e - s for s, e in turns)
+    target = max(excess, -(-window // 8))
+    dropped, n_drop, t = [], 0, 0
+    while t < len(turn_units) and text_rows > window // 2:      # 1. the turn budget
+        dropped.append(turn_units[t][:2])
+        n_drop += turn_units[t][1] - turn_units[t][0]
+        text_rows -= turn_units[t][2]
+        t += 1
+    for u in frame_units:                                        # 2. the oldest frames
+        if n_drop >= target:
+            break
+        dropped.append(u)
+        n_drop += u[1] - u[0]
+    for u in turn_units[t:]:                                     # 3. older turns
+        if n_drop >= target:
+            break
+        dropped.append(u[:2])
+        n_drop += u[1] - u[0]
+    if n_drop < excess:
+        raise VloError(f"context window {window}: {kv_len} cached + {need} new tokens do not fit even after dropping "
+                       f"every frame and turn that may go")
+    spans, pos = [], 0
+    for s, e in sorted(dropped):
+        if s > pos:
+            spans.append((pos, s - pos))
+        pos = e
+    if pos < kv_len:
+        spans.append((pos, kv_len - pos))
+    return spans
+
+
+def kept_rows(seq: Sequence, spans: Sequence[tuple[int, int]]) -> list:
+    """The entries of seq (one per cache position) that `spans` keep, in order."""
+    return [x for f, n in spans for x in seq[f:f + n]]
+
+
+def _check_window_arg(window, max_kv_tokens: int):
     if isinstance(window, bool) or not isinstance(window, int) or window <= 0:
         raise ValueError(f"context_window must be a positive int (tokens), got {window!r}")
     if window > max_kv_tokens:
         raise ValueError(f"context_window {window} exceeds the engine's max_kv_tokens ({max_kv_tokens})")
+
+
+def check_context_window_turns(window: int, max_kv_tokens: int, keep_tokens: int, largest_need: int):
+    """check_context_window for a window that keeps the conversation (`retain_spans`): within max_kv_tokens, and large
+    enough for the start prompt, the turn budget (window / 2), one eviction chunk (window / 8) and the largest single
+    step or response reserve (`largest_need`)."""
+    _check_window_arg(window, max_kv_tokens)
+    least = keep_tokens + window // 2 + -(-window // 8) + largest_need
+    if window < least:
+        raise ValueError(f"context_window {window} cannot hold the {keep_tokens}-token prompt, the turn budget "
+                         f"({window // 2}), one eviction chunk and a step of {largest_need} tokens")
+
+
+def check_context_window(window: int, max_kv_tokens: int, keep_tokens: int, largest_need: int, page: int):
+    """Raise ValueError unless a context window of `window` tokens is usable: within max_kv_tokens, and large enough
+    for the sink pages, one eviction chunk (window / 8 in whole pages) and the largest single step or response
+    reserve (`largest_need`)."""
+    _check_window_arg(window, max_kv_tokens)
     least = sink_tokens(keep_tokens, page) + -(-window // (8 * page)) * page + largest_need
     if window < least:
         raise ValueError(f"context_window {window} cannot hold the {sink_tokens(keep_tokens, page)}-token sink, one "
@@ -267,6 +363,31 @@ class Engine:
         if n:
             self.kv_evict(sid, first, n)
         return n
+
+    def kv_compact(self, sid: int, spans: Sequence[tuple[int, int]]):
+        """Keep only the cache positions of stream `sid` in `spans` [(first, n), ...] (sorted, non-overlapping): span i
+        moves down to the sum of the earlier spans' lengths and its keys are re-rotated on the device by that shift
+        (vlo_kv_compact, current CUDA stream: the one the steps run on)."""
+        first = torch.tensor([f for f, _ in spans], dtype=torch.int32)
+        lens = torch.tensor([n for _, n in spans], dtype=torch.int32)
+        rot, q = [], 0
+        for f, n in spans:
+            rot.extend(W.rope_rotation(self.cfg, f - q))
+            q += n
+        rot = torch.cat(rot) if rot else torch.zeros(1)
+        i32, fp = C.POINTER(C.c_int32), C.POINTER(C.c_float)
+        check(self.lib.vlo_kv_compact(self._h, sid, len(spans), C.cast(first.data_ptr(), i32),
+                                      C.cast(lens.data_ptr(), i32), C.cast(rot.data_ptr(), fp), self._stream()),
+              "vlo_kv_compact")
+
+    def kv_retain(self, sid: int, row_ids: Sequence[int], need: int, window: int, keep_tokens: int,
+                  interval_id: Optional[int], frame_num_tokens: int) -> List[tuple[int, int]]:
+        """Before stream `sid` appends `need` tokens under a context window that keeps the conversation: compact the
+        cache to what `retain_spans` keeps of its history row_ids.  Returns the spans kept ([]: nothing dropped)."""
+        spans = retain_spans(row_ids, need, window, keep_tokens, interval_id, frame_num_tokens)
+        if spans:
+            self.kv_compact(sid, spans)
+        return spans
 
     def kv_fill_synthetic(self, sid: int, n_tokens: int, seed: int = 0):
         check(self.lib.vlo_kv_fill_synthetic(self._h, sid, n_tokens, seed, self._stream()), "vlo_kv_fill_synthetic")

@@ -25,7 +25,7 @@ import torch
 
 from ._lib import VloError
 from .config import LiveArguments, SamplingConfig, parse_args
-from .engine import KvImage, check_context_window, sink_tokens
+from .engine import KvImage, check_context_window, check_context_window_turns, kept_rows, sink_tokens
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
 from .speculative import SEP, NgramDrafter, generate_ids
 
@@ -48,6 +48,7 @@ class SessionState:
     started: bool                # past_key_values was set: a step ran since the last reset
     sampling: Optional[SamplingConfig] = None   # LiveInfer.sampling (None: greedy responses)
     evicted_tokens: int = 0      # cache positions the session's context window dropped so far
+    fed_ids: Optional[list] = None   # the id fed at every cache position (-1: frame row) when no NgramDrafter holds them
     fp8_weights: bool = False    # the cache was written by a model with FP8 layer weights (Engine.fp8_weights)
 
 
@@ -98,6 +99,7 @@ class LiveInfer:
         self._n_calls = 0
         # context window (tokens, None: off): the cache keeps the start prompt (the sink) and drops its oldest pages
         # after it, at fixed points only (before a frame step, before a response), so a session runs in bounded memory
+        self._context_keep_turns = args.context_keep_turns
         self.context_window = args.context_window or None
         # encode-ahead: with a loaded clip the ViT + connector of the NEXT frame run on a side CUDA stream while the
         # decoder works on the current one (same per-frame arithmetic; a live stream delivers the next frame
@@ -141,14 +143,43 @@ class LiveInfer:
     @context_window.setter
     def context_window(self, window: Optional[int]):
         """None: off.  Else it must be <= max_kv_tokens and hold the sink pages, one eviction chunk and the largest
-        frame step or response reserve (ValueError otherwise)."""
+        frame step or response reserve; with context_keep_turns the prompt, the turn budget (window / 2), one eviction
+        chunk and that reserve (ValueError otherwise)."""
         if window is not None:
             frame_step = 1 + self._added_stream_prompt_ids.numel() + self.frame_num_tokens
             reserve = self._added_stream_generation_ids.numel() + self.inplace_output_ids.size(1)
             eng = self.model.engine
-            check_context_window(window, eng.max_kv_tokens, self._start_ids.numel(), max(frame_step, reserve),
-                                 eng.kv_pool_info()["page_tokens"])
+            if self._context_keep_turns:
+                check_context_window_turns(window, eng.max_kv_tokens, self._start_ids.numel(), max(frame_step, reserve))
+            else:
+                check_context_window(window, eng.max_kv_tokens, self._start_ids.numel(), max(frame_step, reserve),
+                                     eng.kv_pool_info()["page_tokens"])
         self._context_window = window
+
+    @property
+    def context_keep_turns(self) -> bool:
+        return self._context_keep_turns
+
+    @context_keep_turns.setter
+    def context_keep_turns(self, keep: bool):
+        """With a context window: False (default) drops whole pages after the start prompt (engine.evict_span); True
+        drops the oldest frames token by token and keeps the questions and answers (engine.retain_spans)."""
+        old, self._context_keep_turns = self._context_keep_turns, bool(keep)
+        try:
+            self.context_window = self._context_window   # validated for the new mode
+        except ValueError:
+            self._context_keep_turns = old
+            raise
+
+    def _fed_ids(self) -> list:
+        """The id fed at every cache position (-1: a frame row): the NgramDrafter's history when the session has one,
+        else its own list; both are cut back here to the cache, which a take-back or a rejected draft may have cut."""
+        n = self._kv.engine.kv_len(self._kv.stream_id)
+        if isinstance(self.drafter, NgramDrafter):
+            self.drafter.sync(n)
+            return self.drafter.ids
+        del self._fed[n:]
+        return self._fed
 
     def _make_room(self, need: int):
         """Under a context window: evict before the stream appends `need` tokens (Engine.kv_make_room, the policy
@@ -156,6 +187,17 @@ class LiveInfer:
         if self._context_window is None:
             return
         eng, sid = self._kv.engine, self._kv.stream_id
+        if self._context_keep_turns:
+            fed = self._fed_ids()
+            spans = eng.kv_retain(sid, fed, need, self._context_window, self._start_ids.numel(),
+                                  self.frame_token_interval_id, self.frame_num_tokens)
+            if spans:
+                self.evicted_tokens += len(fed) - sum(n for _, n in spans)
+                if self.drafter is not None:
+                    self.drafter.keep(spans)
+                if not isinstance(self.drafter, NgramDrafter):
+                    self._fed = kept_rows(fed, spans)
+            return
         n = eng.kv_make_room(sid, need, self._context_window, self._start_ids.numel())
         if n:
             if self.drafter is not None:
@@ -171,6 +213,7 @@ class LiveInfer:
         self.video_tensor = None
         self.last_ids = torch.tensor([[]], dtype=torch.long)
         self.evicted_tokens = 0
+        self._fed = []   # _fed_ids without an NgramDrafter
         self._kv.engine.stream_reset(self._kv.stream_id)
         if self.drafter is not None:
             self.drafter.sync(0)
@@ -184,13 +227,15 @@ class LiveInfer:
         with self._lock:
             self._drop_prefetch()   # encoded-ahead frames are dropped as reset() drops them
             frames = [(t, f.to("cpu")) for t, f in self.frame_embeds_queue]   # before the cache copy: this one syncs
+            fed = None if isinstance(self.drafter, NgramDrafter) else list(self._fed_ids())   # before the swap-out too
             state = SessionState(
                 kv=self._kv.engine.kv_swap_out(self._kv.stream_id), last_ids=self.last_ids.clone(),
                 video_time=self.video_time, last_frame_idx=self.last_frame_idx, query_queue=list(self.query_queue),
                 frame_embeds_queue=frames,
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
                 n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling,
-                evicted_tokens=self.evicted_tokens, fp8_weights=self._kv.engine.fp8_weights)
+                evicted_tokens=self.evicted_tokens, fp8_weights=self._kv.engine.fp8_weights,
+                fed_ids=fed)
             self.reset()
             return state
 
@@ -214,12 +259,15 @@ class LiveInfer:
             self.video_time, self.last_frame_idx = state.video_time, state.last_frame_idx
             self.query_queue = collections.deque(state.query_queue)
             self.frame_embeds_queue = collections.deque((t, f.to(dev, torch.bfloat16)) for t, f in state.frame_embeds_queue)
+            fed = state.drafter_ids if state.drafter_ids is not None else state.fed_ids
             if self.drafter is not None:
                 self.drafter.sync(0)
-                if state.drafter_ids is not None and isinstance(self.drafter, NgramDrafter):
-                    self.drafter.extend(state.drafter_ids)
+                if fed is not None and isinstance(self.drafter, NgramDrafter):
+                    self.drafter.extend(fed)
                 else:
                     self.drafter.sync(state.kv.n_tokens)
+            if not isinstance(self.drafter, NgramDrafter):
+                self._fed = list(fed) if fed is not None else [SEP] * state.kv.n_tokens
             self._n_calls = state.n_calls
             self.sampling = state.sampling
             self.evicted_tokens = state.evicted_tokens
@@ -353,12 +401,15 @@ class LiveInfer:
         eng.step([self._kv.stream_id], [T], packed, row_ids=row_ids,   # token rows gathered on the device
                  segments=[segs] if len(segs) > 1 else None, sample=sample)
         self.past_key_values = self._kv
+        hist = list(id_list)
+        for j, n in enumerate(n_frs):
+            hist += ([self.frame_token_interval_id] if j else []) + [SEP] * n
         if frames and self.drafter is not None:   # frame rows enter the drafter's history as separators
-            hist = list(id_list)
-            for j, n in enumerate(n_frs):
-                hist += ([self.frame_token_interval_id] if j else []) + [SEP] * n
             self.drafter.sync(eng.kv_len(self._kv.stream_id) - T)
             self.drafter.extend(hist)
+        if not isinstance(self.drafter, NgramDrafter):   # the session's own history (_fed_ids)
+            del self._fed[eng.kv_len(self._kv.stream_id) - T:]
+            self._fed.extend(hist)
         if pre is not None:
             # encode-ahead of the next frame, enqueued AFTER the step's launches (the host is the critical path right
             # after a decision read-back) but ordered only behind what preceded the step: it runs concurrently with it

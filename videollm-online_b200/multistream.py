@@ -19,8 +19,9 @@ session with work is made resident again if it fits (`StreamScheduler._make_room
 deterministic.
 
 Context window: a session with `context_window` set keeps its cache within that many tokens as `LiveInfer` does, with
-the same policy (`engine.evict_span`) at the same points: before a frame step and before a response.  A resident session
-evicts before its pages are counted; a swapped-out one right after its swap-in.
+the same policy (`engine.evict_span`, or `engine.retain_spans` with `context_keep_turns`) at the same points: before a
+frame step and before a response.  A resident session evicts before its pages are counted; a swapped-out one right after
+its swap-in.
 """
 from __future__ import annotations
 
@@ -31,7 +32,7 @@ import torch
 
 from ._lib import VloError
 from .config import SamplingConfig
-from .engine import KvImage, SampleRow, evict_span
+from .engine import KvImage, SampleRow, evict_span, kept_rows, retain_spans
 from .modeling_live import LiveLlamaForCausalLM
 from .speculative import sample_rows
 
@@ -55,6 +56,8 @@ class StreamSession:
         self.sampling: Optional[SamplingConfig] = None
         # as LiveInfer.context_window: None = off; the sink is the scheduler's start_ids
         self.context_window: Optional[int] = None
+        # as LiveInfer.context_keep_turns: with a window, keep the questions and answers and drop old frames token by token
+        self.context_keep_turns = False
         self.reset()
 
     @property
@@ -84,6 +87,7 @@ class StreamSession:
         self.events: List[tuple] = []
         self.n_calls = 0
         self.evicted_tokens = 0   # cache positions the context window dropped (sampled positions count them)
+        self.fed_ids: List[int] = []   # the id fed at every cache position, -1 for a frame row (retain_spans reads it)
         self._op = None
 
     # -- inputs (LiveInfer.load_video / input_video_stream / input_query_stream)
@@ -156,11 +160,34 @@ class StreamSession:
             return len(self.resp_prompt) + self.sched.max_new_tokens
         return n
 
+    def _retain(self, need: int):
+        cfg = self.sched.model.config
+        return retain_spans(self.fed_ids, need, self.context_window, len(self.sched.start_ids),
+                            cfg.frame_token_interval_id, cfg.frame_num_tokens)
+
+    def window_drop(self, need: int) -> int:
+        """Cache positions the context window would drop before appending `need` tokens (0: none or no window)."""
+        if self.context_window is None:
+            return 0
+        if self.context_keep_turns:
+            spans = self._retain(need)
+            return len(self.fed_ids) - sum(n for _, n in spans) if spans else 0
+        page = self.sched.model.engine.kv_pool_info()["page_tokens"]
+        return evict_span(self.kv_tokens(), need, self.context_window, len(self.sched.start_ids), page)[1]
+
     def make_room(self, need: int):
         """Evict (resident session, context window set) before appending `need` tokens."""
-        if self.context_window is not None:
-            self.evicted_tokens += self.sched.model.engine.kv_make_room(self.stream_id, need, self.context_window,
-                                                                        len(self.sched.start_ids))
+        if self.context_window is None:
+            return
+        eng = self.sched.model.engine
+        if self.context_keep_turns:
+            spans = self._retain(need)
+            if spans:
+                eng.kv_compact(self.stream_id, spans)
+                self.evicted_tokens += len(self.fed_ids) - sum(n for _, n in spans)
+                self.fed_ids = kept_rows(self.fed_ids, spans)
+            return
+        self.evicted_tokens += eng.kv_make_room(self.stream_id, need, self.context_window, len(self.sched.start_ids))
 
     # -- consume the decision of the step this stream took part in
     def advance(self, dec):
@@ -279,6 +306,8 @@ class StreamScheduler:
                  sample=sample if any(r is not None for r in sample) else None)
         if self.encode_ahead:
             self._launch_encode_ahead(pre)        # enqueued after the step's launches, runs concurrently with it
+        for s, ids, fidx, _ in batch:
+            s.fed_ids.extend(ids + ([-1] * cfg.frame_num_tokens if fidx is not None else []))
         decs = eng.read_decisions(len(batch))
         for (s, *_), d in zip(batch, decs):
             s.last_step = self.ticks
@@ -301,8 +330,8 @@ class StreamScheduler:
         if s.resident:
             s.make_room(w_need)
         kv = after = s.kv_tokens()
-        if s.context_window is not None and not s.resident:   # it evicts right after its swap-in
-            after -= evict_span(kv, w_need, s.context_window, len(self.start_ids), page)[1]
+        if not s.resident:   # it evicts right after its swap-in
+            after -= s.window_drop(w_need)
         if pages(after + n) > total:
             raise VloError(f"session {s.index}: {after + n} tokens need {pages(after + n)} KV pages, the pool has {total}")
         # pages the sessions already in the batch take in this step

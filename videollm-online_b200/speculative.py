@@ -67,6 +67,13 @@ class NgramDrafter:
         self.ids, self._ends = [], {}
         self.extend(kept)
 
+    def keep(self, spans: Sequence[Tuple[int, int]]):
+        """Keep only history entries [first, first + n) of every (first, n) in spans (sorted), as a context window that
+        keeps the conversation compacts the cache to them: the index is rebuilt from the kept entries."""
+        kept = [t for f, n in spans for t in self.ids[f:f + n]]
+        self.ids, self._ends = [], {}
+        self.extend(kept)
+
     def sync(self, n: int):
         """Make the history n entries long: cut it back, or pad it with SEP for KV rows it never saw (a cache filled
         or copied in from elsewhere)."""
