@@ -99,6 +99,22 @@ int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t 
 int vlo_finalize_weights(vlo_engine* e);
 /* bytes of device memory the engine allocated itself (KV + workspaces) */
 int64_t vlo_engine_device_bytes(vlo_engine* e);
+/* FP8 activations (W8A8), on top of FP8 layer weights.  Valid before vlo_finalize_weights (fails after it); finalize then
+ * fails with a message if the mode is on and the layer matrices are bf16.  on != 0 allocates the e4m3 activation copies
+ * (max_step_tokens x (hidden + heads x head_dim + intermediate) bytes plus three fp32 scales per token); a default
+ * engine never holds them.  Numerics of the mode, for each of the four layer GEMMs:
+ *   - the activation operand is the bf16 tensor the FP8-weight path multiplies: xn after the input RMSNorm (q|k|v), the
+ *     attention output (o_proj), xn after the post-attention RMSNorm (gate|up), the SwiGLU output act (down_proj);
+ *   - per token row t it is quantized as weights.quantize_fp8_rows quantizes a weight row:
+ *       a_s[t] = fp32(max_k |X[t,k]|) / 448 (1 for an all-zero row),
+ *       q[t,k] = e4m3fn(clamp(fp32(X[t,k]) / a_s[t], +-448)), IEEE fp32 division, rounded to nearest even;
+ *   - contributor p of a tile writes fl(fl(P_p[t][n] * w_s[n]) * a_s[t]) into its plane, P_p the e4m3 x e4m3 products
+ *     summed over that CTA's k-blocks by the FP8 wgmma chain, whose accumulation is not full IEEE fp32 (exact only while
+ *     the partial sums are small integers); the fix-up kernels and the gate|up finisher add the planes as before.
+ * The lm_head, embedding, norms, residual stream, RoPE, KV cache, connector and ViT keep their formats; xn (hence
+ * xn_last and vlo_last_step_hidden) is still written in bf16.  Two more launches per layer: the quantizers of the
+ * attention output and of act (the norms write the e4m3 xn themselves). */
+int vlo_set_fp8_activations(vlo_engine* e, int on);
 
 /* ------------------------------------------------------------------ streams (KV ownership)
  * replaces: the DynamicCache handed around as past_key_values (HF:cache_utils.py:88-121;
@@ -291,6 +307,12 @@ int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d
  * (*h_max_planes).  Asynchronous. */
 int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
                       long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream);
+/* The same GEMM in mode 0 on e4m3 weights AND e4m3 activations (the fp8_activations form): d_w8 / d_scale as above, d_x8
+ * [rows_x, k] e4m3fn bytes with fp32 token scales d_xscale [rows_x].  Same token tile and stream-K plan as the bf16
+ * call; plane p holds fl(fl(P_p[t][n] * d_scale[n]) * d_xscale[t]), P_p the FP8 wgmma sum of the codes over plane p's
+ * k-blocks.  d_out == NULL only plans (*h_max_planes).  Asynchronous. */
+int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale, int rows_x,
+                      int k, float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream);
 /* ViT trunk GEMM (csrc/gemm_vit.cuh), fp16, 128-token x 128-feature tiles:
  * out[t][n] = act(fp16(sum_k X[t,k] W[n,k] + bias[n])), fp16 out[rows_x][ld_out], ld_out even and >= rows_w;
  * n_ctas <= 0: one CTA per SM. */
@@ -349,6 +371,14 @@ int vlo_op_probe_attn(const void* d_kv, const float* d_q, void* d_out, int n_fra
  * Asynchronous. */
 int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
                          const int32_t* d_last_index, int T, int H, float eps, void* cuda_stream);
+/* vlo_op_resid_rmsnorm that also writes the e4m3 row d_xq [T, H] of each bf16 xn row and its fp32 scale d_xs [T], by
+ * the rule of vlo_set_fp8_activations; d_xn (not NULL here) gets the same bits as from vlo_op_resid_rmsnorm.
+ * Asynchronous. */
+int vlo_op_resid_rmsnorm_q8(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
+                            const int32_t* d_last_index, void* d_xq, float* d_xs, int T, int H, float eps, void* cuda_stream);
+/* The per-token e4m3 quantizer of the attention output and of act: bf16 d_x [T, K] (K a multiple of 8) -> e4m3fn
+ * d_q [T, K] and fp32 d_s [T], by the rule of vlo_set_fp8_activations.  Asynchronous. */
+int vlo_op_quant_rows_e4m3(const void* d_x, int T, int K, void* d_q, float* d_s, void* cuda_stream);
 /* q|k|v fix-up + RoPE + KV append, width = (n_heads + 2 n_kv_heads) * 128, head hh = features [128 hh, 128 hh + 128):
  * heads < n_heads are q, then n_kv_heads k heads, then n_kv_heads v heads.  For d < 64, x1 = y[d], x2 = y[d + 64]:
  *   q and k: out[d] = bf16(bf16(x1 c) + bf16(-x2 s)), out[d + 64] = bf16(bf16(x2 c) + bf16(x1 s)),
@@ -370,6 +400,12 @@ int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x,
  * upcast weights (the finisher's own partial is plane 0).  Asynchronous. */
 int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
                           float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream);
+/* vlo_op_gemm_swiglu on e4m3 weights (d_w8, d_scale) and e4m3 activations d_x8 [rows_x, k] with fp32 token scales
+ * d_xscale: g, u = bf16(sum_p fl(fl(P_p * d_scale[n]) * d_xscale[t])) in plane order, P_p the FP8 wgmma partials (the
+ * finisher's own partial is plane 0).  Asynchronous. */
+int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale,
+                          int rows_x, int k, void* d_act, float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags,
+                          void* cuda_stream);
 /* Speak / silent decision over bf16 logits [n_rows, vocab] (vocab a multiple of 8, rows 16-byte aligned), one
  * vlo_decision per row into d_out (device): first-index argmax, max logit, max - second max (a repeated maximum counts
  * as the second), log-sum-exp, p_interval = bf16(softmax[interval_id]) (0 when interval_id is outside the row), and the

@@ -66,6 +66,7 @@ SIGNATURES = {
     "vlo_load_tensor": (_I, [_P, C.c_char_p, _P, C.c_int64]),
     "vlo_finalize_weights": (_I, [_P]),
     "vlo_engine_device_bytes": (C.c_int64, [_P]),
+    "vlo_set_fp8_activations": (_I, [_P, _I]),
     "vlo_stream_open": (_I, [_P, C.POINTER(_I)]),
     "vlo_stream_reset": (_I, [_P, _I]),
     "vlo_stream_close": (_I, [_P, _I]),
@@ -95,6 +96,7 @@ SIGNATURES = {
     "vlo_op_gemm": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _P, _P, _I, _I, _P]),
     "vlo_op_gemm_ws": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_ws_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
+    "vlo_op_gemm_ws_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
     "vlo_op_attn_kvappend": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _P]),
@@ -104,10 +106,13 @@ SIGNATURES = {
     "vlo_op_vit_attn": (_I, [_P, _P, _I, _I, _I, _P]),
     "vlo_op_probe_attn": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "vlo_op_resid_rmsnorm": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
+    "vlo_op_resid_rmsnorm_q8": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
+    "vlo_op_quant_rows_e4m3": (_I, [_P, _I, _I, _P, _P, _P]),
     "vlo_op_qkv_rope_append": (_I, [_P, _I, _I, _P, _P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _I, _P, _P, _P,
                                     _I, _I, _I, _P]),
     "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_swiglu_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
+    "vlo_op_gemm_swiglu_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_op_sample": (_I, [_P, _I, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),

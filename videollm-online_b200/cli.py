@@ -10,6 +10,8 @@ are dropped.
 answers.
 --fp8_weights serves the decoder layers from e4m3 weights with per-row scales (half their bytes per step; the model's
 numbers change, so it is off by default).
+--fp8_activations (with --fp8_weights) also quantizes the layer GEMMs' activations to e4m3 per token and multiplies them on
+the FP8 tensor cores (W8A8); off by default for the same reason.
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

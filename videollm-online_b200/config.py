@@ -158,6 +158,9 @@ class LiveArguments:
     # serve the decoder layers' q|k|v, o, gate|up and down matrices from e4m3 codes with one fp32 scale per row (half the
     # weight bytes per step); changes the model's numbers, so off by default
     fp8_weights: bool = False
+    # with fp8_weights: quantize each layer GEMM's activations to e4m3 per token and multiply on the FP8 tensor cores
+    # (W8A8); changes the model's numbers again, so off by default
+    fp8_activations: bool = False
     # LiveInfer.context_window, tokens: keep the start prompt and drop the oldest cache pages after it so the session's
     # cache never exceeds this many tokens; 0: off (the cache grows until max_kv_tokens)
     context_window: int = 0

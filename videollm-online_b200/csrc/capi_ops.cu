@@ -160,6 +160,30 @@ int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const 
   return rc;
 }
 
+int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale, int rows_x,
+                      int k, float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
+  VLO_CHECK(d_out == nullptr || (d_scale != nullptr && d_xscale != nullptr), "gemm_ws_a8: null row or token scales");
+  GemmWsCall c{};
+  c.fmt = FMT_E4M3_A8;
+  c.mode = 0;
+  c.w = d_w8;
+  c.w_scale = d_scale;
+  c.rows_w = rows_w;
+  c.x = d_x8;
+  c.a_scale = d_xscale;
+  c.rows_x = rows_x;
+  c.k = k;
+  c.out = d_out;
+  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
+  c.ld_out = rows_w;
+  c.plane_stride = plane_stride;
+  c.n_ctas = n_ctas;
+  GemmWsPlan plan{};
+  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
+  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
+  return rc;
+}
+
 int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
                     const float* d_bias, int act, int n_ctas, void* cuda_stream) {
   return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
@@ -267,6 +291,22 @@ int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, cons
                               static_cast<cudaStream_t>(cuda_stream));
 }
 
+int vlo_op_resid_rmsnorm_q8(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,
+                            const int32_t* d_last_index, void* d_xq, float* d_xs, int T, int H, float eps, void* cuda_stream) {
+  VLO_CHECK(T > 0 && H > 0 && H % 4 == 0 && H * sizeof(float) <= 48 * 1024, "resid_rmsnorm_q8: H a multiple of 4, <= 12288");
+  VLO_CHECK(d_last_index == nullptr || d_xn_last != nullptr, "resid_rmsnorm_q8: last_index without xn_last");
+  VLO_CHECK(d_xn != nullptr && d_xq != nullptr && d_xs != nullptr, "resid_rmsnorm_q8: null xn, xq or xs");
+  SkInfo sk{};
+  if (d_part != nullptr && op_fix_plan(H, T, k, n_ctas, &sk)) return -1;
+  return resid_rmsnorm_q8_launch(d_part, &sk, d_h, d_w, d_xn, d_xn_last, d_last_index, static_cast<uint8_t*>(d_xq), d_xs, T,
+                                 H, eps, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_quant_rows_e4m3(const void* d_x, int T, int K, void* d_q, float* d_s, void* cuda_stream) {
+  VLO_CHECK(d_x != nullptr && d_q != nullptr && d_s != nullptr, "quant_rows_e4m3: null argument");
+  return quant_rows_launch(d_x, T, K, static_cast<uint8_t*>(d_q), d_s, static_cast<cudaStream_t>(cuda_stream));
+}
+
 int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d_cos, const void* d_sin, int n_rope_pos,
                            const int32_t* h_tok_pos, const int64_t* h_tok_kvrow, int kv_head_stride, void* d_q, void* d_k,
                            void* d_v, int T, int n_heads, int n_kv_heads, void* cuda_stream) {
@@ -305,6 +345,15 @@ int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, co
   VLO_CHECK(d_scale != nullptr, "gemm_swiglu_f8: null row scales");
   return gemm_wsf_launch(d_w8, d_scale, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
                          n_flags, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale,
+                          int rows_x, int k, void* d_act, float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags,
+                          void* cuda_stream) {
+  VLO_CHECK(plane_elems >= 0, "gemm_swiglu_a8: plane_elems");
+  VLO_CHECK(d_scale != nullptr && d_xscale != nullptr, "gemm_swiglu_a8: null row or token scales");
+  return gemm_wsf_launch(d_w8, d_scale, rows_w, d_x8, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
+                         n_flags, static_cast<cudaStream_t>(cuda_stream), d_xscale);
 }
 
 int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream) {

@@ -108,7 +108,7 @@ enum WsTiling : int {
                                // shares an SM with a decoder weight-streaming CTA
 };
 struct GemmWsCall {
-  int fmt;            // 0 fp16, 1 bf16, 2 e4m3 weights x bf16 activations (mode 0 only)
+  int fmt;            // 0 fp16, 1 bf16, 2 e4m3 weights x bf16 activations, 3 e4m3 weights x e4m3 activations (2, 3: mode 0)
   int mode;           // 0 stream-K fp32 partial planes, 1 whole tiles + 16-bit epilogue
   const void* w;      // [rows_w, k]
   int rows_w;
@@ -124,7 +124,8 @@ struct GemmWsCall {
   int n_ctas;         // <= 0: one CTA per SM
   int bn;             // token-tile width; 0: chosen by `tiling`
   int tiling;         // WsTiling
-  const float* w_scale;  // fmt 2: [rows_w] fp32 row scales, each partial is multiplied by its row's scale once
+  const float* w_scale;  // fmt 2, 3: [rows_w] fp32 row scales, each partial is multiplied by its row's scale once
+  const float* a_scale;  // fmt 3: [rows_x] fp32 token scales, each partial is then multiplied by its token's scale once
 };
 // What a launch decided, for the kernels that fold its partial planes.
 struct GemmWsPlan {
@@ -142,11 +143,13 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
                     const float* bias, int act, int n_ctas, cudaStream_t stream);
 
 // ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), bf16 x, one CTA per SM:
-// act[rows_x][rows_w / 2] = SwiGLU(x w^T).  w is bf16 (w_scale null) or e4m3 with fp32 row scales w_scale [rows_w].
+// act[rows_x][rows_w / 2] = SwiGLU(x w^T).  w is bf16 (w_scale null) or e4m3 with fp32 row scales w_scale [rows_w];
+// a_scale non-null: x is e4m3 with fp32 token scales a_scale [rows_x] (e4m3 weights only).
 // planes (plane_elems floats) take the partials of the non-finisher CTAs, flags (n_flags counters, zero between
 // launches) their arrivals.
 int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
-                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream);
+                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream,
+                    const float* a_scale = nullptr);
 
 // ---- decoder fix-up and decision kernels (decoder_kernels.cuh / engine.cu) -----------
 // bf16 tensors; `part` holds fp32 stream-K planes [plane][T][width] of the plan `sk`, as gemm_ws_launch mode 0 leaves
@@ -155,6 +158,12 @@ int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void*
 // last_index[t] >= 0 (both may be null); one CTA per row of min(1024, max(32, H / 4)) threads.
 int resid_rmsnorm_launch(const float* part, const SkInfo* sk, void* h, const void* w, void* xn, void* xn_last,
                          const int* last_index, int T, int H, float eps, cudaStream_t st);
+// resid_rmsnorm_q8_kernel: resid_rmsnorm_kernel that also writes the e4m3 row xq[t] of xn[t] and its fp32 scale xs[t]
+// (the per-token rule of quant_rows_e4m3_kernel); xn is the same as without.
+int resid_rmsnorm_q8_launch(const float* part, const SkInfo* sk, void* h, const void* w, void* xn, void* xn_last,
+                            const int* last_index, uint8_t* xq, float* xs, int T, int H, float eps, cudaStream_t st);
+// quant_rows_e4m3_kernel: bf16 x[T, K] (K % 8 == 0) -> e4m3 q[T, K] and fp32 token scales s[T], one CTA per row.
+int quant_rows_launch(const void* x, int T, int K, uint8_t* q, float* s, cudaStream_t st);
 // qkv_rope_append_kernel: q[T, n_heads, 128] and K / V rows of the token's position (device tables tok_pos / tok_kvrow)
 // from the fix-up of the q|k|v planes, RoPE from the bf16 [pos][64] cos / sin tables.
 int qkv_rope_launch(const float* part, const SkInfo& sk, const void* cos_tab, const void* sin_tab, const int* tok_pos,

@@ -2,6 +2,7 @@
 // path (HF:models/llama/modeling_llama.py) so that the only numeric difference left against the
 // reference forward is the accumulation order inside the GEMMs and the attention.
 #pragma once
+#include <cuda_fp8.h>
 #include "ptx.cuh"
 #include "streamk.h"
 
@@ -25,6 +26,33 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   return red[0];
 }
 
+// block-wide max for <= 1024 threads
+__device__ __forceinline__ float block_max(float v, float* red) {
+  v = warp_max(v);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = (blockDim.x + 31) >> 5;
+  __syncthreads();
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  float t = (threadIdx.x < nw) ? red[threadIdx.x] : 0.f;
+  if (warp == 0) {
+    t = warp_max(t);
+    if (lane == 0) red[0] = t;
+  }
+  __syncthreads();
+  return red[0];
+}
+
+// ---------------------------------------------------------------------------------------------
+// Per-token e4m3 quantization of a bf16 row X[t, :] (weights.quantize_fp8_rows applied to activation rows):
+//   s[t] = fp32(max_k |X[t, k]|) / 448   (1 for an all-zero row)
+//   q[t, k] = e4m3fn(clamp(fp32(X[t, k]) / s[t], +-448))   IEEE division, round to nearest even
+// The saturating conversion is the clamp: a quotient past 448 can only be the rounding of amax / s.
+constexpr float kE4m3Max = 448.f;
+__device__ __forceinline__ float e4m3_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, kE4m3Max) : 1.f; }
+__device__ __forceinline__ uint16_t e4m3x2(float a, float b, float s) {
+  return __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(a, s), __fdiv_rn(b, s)), __NV_SATFINITE, __NV_E4M3);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Stream-K fix-up + residual add + RMSNorm in one pass over a token row:
 //   y      = bf16(sum_s part[s][t][:])                (the Linear output, o_proj / down_proj)
@@ -46,7 +74,10 @@ struct ResidNormParams {
   float eps;
 };
 
-__global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormParams p) {
+// kQ8 (resid_rmsnorm_q8_kernel): also the e4m3 row xq[t] and its scale xs[t] of the bf16 xn row, quantized as above;
+// xn itself is the same as without.
+template <bool kQ8>
+__device__ __forceinline__ void resid_rmsnorm_body(const ResidNormParams p, uint8_t* xq, float* xs) {
   // one CTA per token row, 4 contiguous elements per thread per sweep; the plane loads of a sweep are
   // independent (predicated, fully unrolled) so they are all in flight together.
   extern __shared__ float row[];  // H floats
@@ -94,6 +125,7 @@ __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormPara
   }
   const float tot = block_sum(ss, red);
   const float rstd = rsqrtf(tot / static_cast<float>(p.H) + p.eps);
+  float amax = 0.f;
   for (int i = threadIdx.x * 4; i < p.H; i += blockDim.x * 4) {
     const uint2 wraw = (i == i0) ? w_pre : *reinterpret_cast<const uint2*>(p.w + i);
     const float2 w01 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wraw.x));
@@ -105,7 +137,61 @@ __global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormPara
                                                                      bf16_round(w23.y * bf16_round(row[i + 3] * rstd)));
     if (p.xn) *reinterpret_cast<uint2*>(p.xn + static_cast<size_t>(t) * p.H + i) = o;
     if (li >= 0) *reinterpret_cast<uint2*>(p.xn_last + static_cast<size_t>(li) * p.H + i) = o;
+    if constexpr (kQ8) {   // this thread's own row[] entries now hold the bf16 xn values
+      const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&o.x));
+      const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&o.y));
+      row[i] = a.x; row[i + 1] = a.y; row[i + 2] = b.x; row[i + 3] = b.y;
+      amax = fmaxf(fmaxf(amax, fmaxf(fabsf(a.x), fabsf(a.y))), fmaxf(fabsf(b.x), fabsf(b.y)));
+    }
   }
+  if constexpr (kQ8) {
+    const float sc = e4m3_row_scale(block_max(amax, red));
+    for (int i = threadIdx.x * 4; i < p.H; i += blockDim.x * 4)
+      *reinterpret_cast<uint32_t*>(xq + static_cast<size_t>(t) * p.H + i) =
+          e4m3x2(row[i], row[i + 1], sc) | (static_cast<uint32_t>(e4m3x2(row[i + 2], row[i + 3], sc)) << 16);
+    if (threadIdx.x == 0) xs[t] = sc;
+  }
+}
+
+__global__ void __launch_bounds__(1024) resid_rmsnorm_kernel(const ResidNormParams p) {
+  resid_rmsnorm_body<false>(p, nullptr, nullptr);
+}
+__global__ void __launch_bounds__(1024) resid_rmsnorm_q8_kernel(const ResidNormParams p, uint8_t* xq, float* xs) {
+  resid_rmsnorm_body<true>(p, xq, xs);
+}
+
+// One CTA per row of a bf16 [T, K] tensor (K % 8 == 0): e4m3 q[T, K] and fp32 s[T] by the rule above.  The row is read
+// twice (amax, then the codes); the second read hits L1 / L2.
+__global__ void __launch_bounds__(256) quant_rows_e4m3_kernel(const __nv_bfloat16* x, int K, uint8_t* q, float* s) {
+  __shared__ float red[32];
+  const int t = blockIdx.x;
+  const __nv_bfloat16* xr = x + static_cast<size_t>(t) * K;
+  pdl_trigger();
+  pdl_wait();
+  float amax = 0.f;
+  for (int i = threadIdx.x * 8; i < K; i += blockDim.x * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(xr + i);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[j]));
+      amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+    }
+  }
+  const float sc = e4m3_row_scale(block_max(amax, red));
+  for (int i = threadIdx.x * 8; i < K; i += blockDim.x * 8) {
+    const uint4 v = *reinterpret_cast<const uint4*>(xr + i);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t c[2];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const float2 f0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[2 * j]));
+      const float2 f1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[2 * j + 1]));
+      c[j] = e4m3x2(f0.x, f0.y, sc) | (static_cast<uint32_t>(e4m3x2(f1.x, f1.y, sc)) << 16);
+    }
+    *reinterpret_cast<uint2*>(q + static_cast<size_t>(t) * K + i) = make_uint2(c[0], c[1]);
+  }
+  if (threadIdx.x == 0) s[t] = sc;
 }
 
 // ---------------------------------------------------------------------------------------------

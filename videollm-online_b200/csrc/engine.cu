@@ -63,6 +63,7 @@ struct vlo_engine {
   const bf16 *conn0_w = nullptr, *conn2_w = nullptr;
   bool has_vit = false, has_connector = false, has_decoder = false;
   bool fp8_weights = false;  // the layer matrices are e4m3 + row scales (vlo_finalize_weights)
+  bool fp8_act = false;      // vlo_set_fp8_activations: the layer GEMMs take e4m3 activations with token scales
 
   // derived
   int qkv_width = 0, grid = 0, n_patches = 0, n_frame_tokens = 0, patch_k = 0;
@@ -81,6 +82,9 @@ struct vlo_engine {
        *logits = nullptr;
   float* part = nullptr;
   size_t part_elems = 0;
+  // fp8_act only: e4m3 copies of xn, attn_out and act with their fp32 token scales
+  uint8_t *xq = nullptr, *aq = nullptr, *actq = nullptr;
+  float *xs = nullptr, *as = nullptr, *acts = nullptr;
   int* sk_flags = nullptr;          // kSkFlags counters, zero between launches
   uint8_t* attn_ws = nullptr;
   uint8_t* meta_dev = nullptr;  // the step's tables, laid out as `meta` says
@@ -141,10 +145,12 @@ int lookup(vlo_engine* e, const std::string& name, int64_t expect_elems, const T
 // which a fix-up kernel folds.  The fix-up kernels unroll kFixMaxPlanes planes: this is the one check of that limit,
 // made before the fix-up kernel that would read the planes is launched.
 int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int k, float* part, size_t part_elems,
-                 int tiling, GemmWsPlan* plan, cudaStream_t st, const float* w_scale = nullptr) {
+                 int tiling, GemmWsPlan* plan, cudaStream_t st, const float* w_scale = nullptr,
+                 const float* a_scale = nullptr) {
   GemmWsCall c{};
   c.fmt = fmt;
   c.w_scale = w_scale;
+  c.a_scale = a_scale;
   c.mode = 0;
   c.w = w;
   c.rows_w = n_out;
@@ -161,10 +167,12 @@ int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int
   return 0;
 }
 
-// the decoder's partial GEMMs: bf16 or e4m3 weights, the step's T tokens, planes in e->part
-int dec_partial(vlo_engine* e, const DecW& w, int n_out, const bf16* x, int T, int k, GemmWsPlan* sk, cudaStream_t st) {
-  return gemm_partial(w.scale ? FMT_E4M3 : FMT_BF16, w.w, n_out, x, T, k, e->part, e->part_elems, WS_TILE_FIT, sk, st,
-                      w.scale);
+// the decoder's partial GEMMs: bf16 or e4m3 weights, the step's T tokens, planes in e->part.  x_scale non-null: x is the
+// e4m3 copy of the activations with these token scales (fp8_act).
+int dec_partial(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, int k, GemmWsPlan* sk, cudaStream_t st,
+                const float* x_scale = nullptr) {
+  return gemm_partial(x_scale ? FMT_E4M3_A8 : w.scale ? FMT_E4M3 : FMT_BF16, w.w, n_out, x, T, k, e->part, e->part_elems,
+                      WS_TILE_FIT, sk, st, w.scale, x_scale);
 }
 
 // gate|up GEMM + SwiGLU: the stream-K finisher CTAs apply the fix-up themselves (gemm_wsf.cuh).  A finisher's epilogue
@@ -172,8 +180,9 @@ int dec_partial(vlo_engine* e, const DecW& w, int n_out, const bf16* x, int T, i
 // separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling.  Only the gate|up GEMM has
 // enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB plane round trip of
 // its fix-up; q|k|v, o_proj and down_proj go through gemm_partial and a fix-up kernel (DESIGN.md section 5).
-int gemm_swiglu(vlo_engine* e, const DecW& w, int n_out, const bf16* x, int T, int k, cudaStream_t st) {
-  return gemm_wsf_launch(w.w, w.scale, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st);
+int gemm_swiglu(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, int k, cudaStream_t st,
+                const float* x_scale = nullptr) {
+  return gemm_wsf_launch(w.w, w.scale, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st, x_scale);
 }
 
 // whole-tile persistent GEMM with the 16-bit epilogue: out[T, n_out] = act(x W^T + bias)
@@ -317,6 +326,36 @@ int resid_rmsnorm_launch(const float* part, const SkInfo* sk, void* h, const voi
   p.eps = eps;
   VLO_CUDA(launch_pdl(resid_rmsnorm_kernel, dim3(T), dim3(std::min(1024, std::max(32, H / 4))),
                       static_cast<size_t>(H) * sizeof(float), st, p));
+  count_launch();
+  return 0;
+}
+
+int resid_rmsnorm_q8_launch(const float* part, const SkInfo* sk, void* h, const void* w, void* xn, void* xn_last,
+                            const int* last_index, uint8_t* xq, float* xs, int T, int H, float eps, cudaStream_t st) {
+  ResidNormParams p{};
+  p.part = part;
+  if (part) p.sk = *sk;
+  p.split_stride = static_cast<long long>(T) * H;
+  p.h = static_cast<bf16*>(h);
+  p.w = static_cast<const bf16*>(w);
+  p.xn = static_cast<bf16*>(xn);
+  p.xn_last = static_cast<bf16*>(xn_last);
+  p.last_index = last_index;
+  p.H = H;
+  p.eps = eps;
+  prof_begin(PROF_OTHER, st, 2.0 * T * H * (part ? 3.0 : 2.0) + 1.0 * T * H);
+  VLO_CUDA(launch_pdl(resid_rmsnorm_q8_kernel, dim3(T), dim3(std::min(1024, std::max(32, H / 4))),
+                      static_cast<size_t>(H) * sizeof(float), st, p, xq, xs));
+  prof_end(st);
+  count_launch();
+  return 0;
+}
+
+int quant_rows_launch(const void* x, int T, int K, uint8_t* q, float* s, cudaStream_t st) {
+  VLO_CHECK(T > 0 && K > 0 && K % 8 == 0, "quant_rows: T > 0 and K a positive multiple of 8");
+  prof_begin(PROF_OTHER, st, 3.0 * T * K + 4.0 * T);
+  VLO_CUDA(launch_pdl(quant_rows_e4m3_kernel, dim3(T), dim3(256), 0, st, static_cast<const bf16*>(x), K, q, s));
+  prof_end(st);
   count_launch();
   return 0;
 }
@@ -553,6 +592,22 @@ int vlo_engine_destroy(vlo_engine* e) {
 
 int64_t vlo_engine_device_bytes(vlo_engine* e) { return e ? e->device_bytes : 0; }
 
+int vlo_set_fp8_activations(vlo_engine* e, int on) {
+  DevGuard dev_guard(e);
+  VLO_CHECK(e != nullptr, "null engine");
+  VLO_CHECK(!e->finalized, "set_fp8_activations: the mode is chosen before vlo_finalize_weights");
+  e->fp8_act = on != 0;
+  if (e->fp8_act && e->xq == nullptr) {   // the e4m3 activation copies exist only in this mode (zeroed: vlo_bench_gemm)
+    const vlo_config& c = e->cfg;
+    const size_t T = c.max_step_tokens;
+    if (dev_alloc_t(e, &e->xq, T * c.hidden_size, true)) return -1;
+    if (dev_alloc_t(e, &e->aq, T * c.num_heads * c.head_dim, true)) return -1;
+    if (dev_alloc_t(e, &e->actq, T * c.intermediate_size, true)) return -1;
+    if (dev_alloc_t(e, &e->xs, T, true) || dev_alloc_t(e, &e->as, T, true) || dev_alloc_t(e, &e->acts, T, true)) return -1;
+  }
+  return 0;
+}
+
 int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t n_bytes) {
   VLO_CHECK(e != nullptr && name != nullptr && d_ptr != nullptr && n_bytes > 0, "bad argument");
   VLO_CHECK((reinterpret_cast<uintptr_t>(d_ptr) & 15) == 0, std::string("tensor '") + name + "' is not 16-byte aligned");
@@ -617,6 +672,9 @@ int vlo_finalize_weights(vlo_engine* e) {
       if (lookup_layer_matrix(e, p + "down", H, I, &f8, &d.down)) return -1;
     }
     e->fp8_weights = f8 == 1;
+    VLO_CHECK(!e->fp8_act || e->fp8_weights,
+              "fp8_activations needs FP8 (e4m3) layer weights, but the layer matrices are bf16: the FP8 tensor cores "
+              "take both operands in e4m3");
   }
   e->has_connector = e->tensors.count("conn.0.w") > 0;
   if (e->has_connector) {
@@ -1196,11 +1254,19 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
     count_launch();
   }
 
-  // sk == null: no partials (the first layer's input norm)
+  // sk == null: no partials (the first layer's input norm).  With fp8_act every norm but the final one also writes the
+  // e4m3 copy of xn that the next GEMM reads.
+  const bool a8 = e->fp8_act;
   auto resid_norm = [&](const GemmWsPlan* sk, const bf16* w, bool last) -> int {
+    if (a8 && !last)
+      return resid_rmsnorm_q8_launch(sk ? e->part : nullptr, sk ? &sk->sk : nullptr, e->h, w, e->xn, nullptr, nullptr,
+                                     e->xq, e->xs, T, H, c.rms_norm_eps, st);
     return resid_rmsnorm_launch(sk ? e->part : nullptr, sk ? &sk->sk : nullptr, e->h, w, e->xn, last ? e->xn_last : nullptr,
                                 last ? d_last_index : nullptr, T, H, c.rms_norm_eps, st);
   };
+  const void* xn_in = a8 ? static_cast<const void*>(e->xq) : e->xn;
+  const void* attn_in = a8 ? static_cast<const void*>(e->aq) : e->attn_out;
+  const void* act_in = a8 ? static_cast<const void*>(e->actq) : e->act;
 
   if (resid_norm(nullptr, e->dec[0].in_norm, false)) return -1;
   const int attn_width = c.num_heads * c.head_dim;
@@ -1209,18 +1275,20 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
     GemmWsPlan sk{};
     const bool is_last = (l == c.num_layers - 1);
     // ---- q|k|v projection, then RoPE + in-place KV append
-    if (dec_partial(e, d.qkv, e->qkv_width, e->xn, T, H, &sk, st)) return -1;
+    if (dec_partial(e, d.qkv, e->qkv_width, xn_in, T, H, &sk, st, a8 ? e->xs : nullptr)) return -1;
     if (qkv_rope_launch(e->part, sk.sk, e->rope_cos, e->rope_sin, d_tok_pos, d_tok_kvrow, KvPool::head_stride_rows(), e->q,
                         kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), T, c.num_heads, c.num_kv_heads, st))
       return -1;
     if (attn_layer(e, plan, l, st)) return -1;
     // ---- o_proj + residual, then post-attention RMSNorm
-    if (dec_partial(e, d.o, H, e->attn_out, T, attn_width, &sk, st)) return -1;
+    if (a8 && quant_rows_launch(e->attn_out, T, attn_width, e->aq, e->as, st)) return -1;
+    if (dec_partial(e, d.o, H, attn_in, T, attn_width, &sk, st, a8 ? e->as : nullptr)) return -1;
     if (resid_norm(&sk, d.post_norm, false)) return -1;
     // ---- gate|up + SwiGLU
-    if (gemm_swiglu(e, d.gate_up, 2 * c.intermediate_size, e->xn, T, H, st)) return -1;
+    if (gemm_swiglu(e, d.gate_up, 2 * c.intermediate_size, xn_in, T, H, st, a8 ? e->xs : nullptr)) return -1;
     // ---- down_proj + residual, then the next RMSNorm (next layer's input norm, or the final norm + last-row compaction)
-    if (dec_partial(e, d.down, H, e->act, T, c.intermediate_size, &sk, st)) return -1;
+    if (a8 && quant_rows_launch(e->act, T, c.intermediate_size, e->actq, e->acts, st)) return -1;
+    if (dec_partial(e, d.down, H, act_in, T, c.intermediate_size, &sk, st, a8 ? e->acts : nullptr)) return -1;
     if (resid_norm(&sk, is_last ? e->final_norm : e->dec[l + 1].in_norm, is_last)) return -1;
   }
   // ---- last-position lm_head + on-device decision (one row per segment)
@@ -1331,17 +1399,28 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
   const int H = c.hidden_size, I = c.intermediate_size, A = c.num_heads * c.head_dim;
   double bytes = 0.0;
   const double w_elem = e->fp8_weights ? 1.0 : 2.0, row_b = e->fp8_weights ? 4.0 : 0.0;   // e4m3: 1 B + a scale per row
+  // fp8_act: the W8A8 GEMMs on the e4m3 activation copies, 1 B per activation + a scale per token
+  const bool a8 = e->fp8_act;
+  const double x_elem = a8 ? 1.0 : 2.0, tok_b = a8 ? 4.0 : 0.0;
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < c.num_layers; ++l) {
       const DecLayer& d = e->dec[l];
       GemmWsPlan sk{};
-      if (dec_partial(e, d.qkv, e->qkv_width, e->xn, n_tok, H, &sk, st)) return -1;
-      if (dec_partial(e, d.o, H, e->attn_out, n_tok, A, &sk, st)) return -1;
-      if (dec_partial(e, d.gate_up, 2 * I, e->xn, n_tok, H, &sk, st)) return -1;
-      if (dec_partial(e, d.down, H, e->act, n_tok, I, &sk, st)) return -1;
+      if (a8) {
+        if (dec_partial(e, d.qkv, e->qkv_width, e->xq, n_tok, H, &sk, st, e->xs)) return -1;
+        if (dec_partial(e, d.o, H, e->aq, n_tok, A, &sk, st, e->as)) return -1;
+        if (dec_partial(e, d.gate_up, 2 * I, e->xq, n_tok, H, &sk, st, e->xs)) return -1;
+        if (dec_partial(e, d.down, H, e->actq, n_tok, I, &sk, st, e->acts)) return -1;
+      } else {
+        if (dec_partial(e, d.qkv, e->qkv_width, e->xn, n_tok, H, &sk, st)) return -1;
+        if (dec_partial(e, d.o, H, e->attn_out, n_tok, A, &sk, st)) return -1;
+        if (dec_partial(e, d.gate_up, 2 * I, e->xn, n_tok, H, &sk, st)) return -1;
+        if (dec_partial(e, d.down, H, e->act, n_tok, I, &sk, st)) return -1;
+      }
       if (it == 0)
         bytes += w_elem * (static_cast<double>(e->qkv_width) * H + static_cast<double>(H) * A + 2.0 * I * H + static_cast<double>(H) * I) +
-                 row_b * (static_cast<double>(e->qkv_width) + H + 2.0 * I + H) + 2.0 * n_tok * (2.0 * H + A + I);
+                 row_b * (static_cast<double>(e->qkv_width) + H + 2.0 * I + H) + x_elem * n_tok * (2.0 * H + A + I) +
+                 tok_b * 4.0 * n_tok;
     }
   if (h_algo_bytes_per_iter) *h_algo_bytes_per_iter = bytes;
   if (h_launches_per_iter) *h_launches_per_iter = 4 * c.num_layers;

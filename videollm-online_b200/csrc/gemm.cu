@@ -60,7 +60,8 @@ std::mutex g_tmap_mu;
 std::unordered_map<TmapKey, CUtensorMap, TmapHash> g_tmaps;
 
 // [rows, k] row-major 16-bit matrix, box = 64 (k) x box_rows, 128-byte swizzle; FMT_E4M3: bytes, box = 64 B x box_rows,
-// no swizzle (the consumer reads the stage with plain loads).
+// no swizzle (the consumer reads the stage with plain loads); FMT_E4M3_A8: bytes, box = 64 B x box_rows, 64-byte swizzle
+// (the FP8 wgmma reads the stage).
 int get_tmap(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out) {
   TmapKey key{ptr, rows, k, box_rows, fmt};
   {
@@ -75,7 +76,8 @@ int get_tmap(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMa
   if (enc == nullptr) return fail("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
   if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0) return fail("TMA operand not 16-byte aligned");
   cuuint64_t dims[2] = {static_cast<cuuint64_t>(k), static_cast<cuuint64_t>(rows)};
-  const bool f8 = fmt == FMT_E4M3;
+  const bool a8 = fmt == FMT_E4M3_A8;
+  const bool f8 = fmt == FMT_E4M3 || a8;
   cuuint64_t strides[1] = {static_cast<cuuint64_t>(k) * (f8 ? 1 : 2)};
   cuuint32_t box[2] = {static_cast<cuuint32_t>(kGemmBK), static_cast<cuuint32_t>(box_rows)};
   cuuint32_t estr[2] = {1, 1};
@@ -85,7 +87,7 @@ int get_tmap(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMa
                    : fmt == FMT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
                                      : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
                    2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   f8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   a8 ? CU_TENSOR_MAP_SWIZZLE_64B : f8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed, CUresult " + std::to_string(r));
   {
@@ -182,17 +184,28 @@ static_assert(GemmWsCfg<16, kF8DecoderStages, FMT_E4M3>::kSmemBytes + GemmVitCfg
               "e4m3 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
 static_assert(GemmWsCfg<16, kF8DecoderStages, FMT_E4M3>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
               "e4m3 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
+// The W8A8 16-token decoder GEMM keeps the pairing too.  Without conversion tiles its 9 KB stages (8 KB of weights, 1 KB
+// of activations) go as deep as the ViT trunk GEMM CTA leaves room for, up to the 16 barrier pairs.
+constexpr int kA8DecoderStages =
+    std::min(16, (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes - GemmWsCfg<16, 0, FMT_E4M3_A8>::kSmemBytes) /
+                     (kA8BytesW + 16 * kGemmBK));
+static_assert(GemmWsCfg<16, kA8DecoderStages, FMT_E4M3_A8>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "W8A8 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
+static_assert(GemmWsCfg<16, kA8DecoderStages, FMT_E4M3_A8>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "W8A8 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
 
 namespace {
-template <int FMT, int BN, int STAGES = FMT == FMT_E4M3 ? ws_f8_default_stages(BN) : ws_default_stages(BN)>
+template <int FMT, int BN,
+          int STAGES = FMT == FMT_E4M3 ? ws_f8_default_stages(BN) : FMT == FMT_E4M3_A8 ? ws_a8_default_stages(BN) : ws_default_stages(BN)>
 int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
   auto kern = gemm_ws_kernel<FMT, BN, STAGES>;
   using Cfg = GemmWsCfg<BN, STAGES, FMT>;
   if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
   if (prof_on()) {
     const double out_b = a.mode == 0 ? 4.0 * a.rows_x * a.rows_w : 2.0 * a.rows_x * a.rows_w;
-    const double in_b = FMT == FMT_E4M3 ? (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x   // 1 B per weight + row scales
-                                        : 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x);
+    const double in_b = FMT == FMT_E4M3      ? (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x   // 1 B per weight + row scales
+                        : FMT == FMT_E4M3_A8 ? (a.k + 4.0) * (static_cast<double>(a.rows_w) + a.rows_x)   // + token scales
+                                             : 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x);
     prof_begin(FMT == FMT_F16 ? PROF_GEMM_VIT : PROF_GEMM_STREAM, stream, in_b + out_b);
   }
   VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a));
@@ -256,7 +269,8 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
                  : c.tiling == WS_TILE_TRUNK ? trunk_token_tile(c.rows_x, c.rows_w, c.mode)
                  : token_tile(c.rows_x, c.fmt);
   VLO_CHECK(!beside || (c.fmt == FMT_F16 && bn == 64), "gemm_ws: only the 64-token fp16 instance fits beside a decoder CTA");
-  const bool f8 = c.fmt == FMT_E4M3;
+  const bool a8 = c.fmt == FMT_E4M3_A8;
+  const bool f8 = c.fmt == FMT_E4M3 || a8;
   VLO_CHECK(!f8 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn)),
             "gemm_ws: e4m3 weights run stream-K partials (mode 0) on the token tile token_tile() picks");
   const int x_tiles = (c.rows_x + bn - 1) / bn;
@@ -280,13 +294,16 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   a.act = c.act;
   VLO_CHECK(!f8 || c.w_scale != nullptr, "gemm_ws: e4m3 weights need their row scales");
   a.w_scale = c.w_scale;
+  VLO_CHECK(!a8 || c.a_scale != nullptr, "gemm_ws: e4m3 activations need their token scales");
+  a.a_scale = c.a_scale;
   CUtensorMap tw, tx;
   if (get_tmap(c.w, c.rows_w, c.k, kGemmBM, c.fmt, &tw) != 0) return -1;
-  if (get_tmap(c.x, c.rows_x, c.k, bn, f8 ? FMT_BF16 : c.fmt, &tx) != 0) return -1;
+  if (get_tmap(c.x, c.rows_x, c.k, bn, a8 ? FMT_E4M3_A8 : f8 ? FMT_BF16 : c.fmt, &tx) != 0) return -1;
 #define VLO_WS_CASE(F, N) \
   if (c.fmt == F && bn == N) return launch_ws<F, N>(tw, tx, a, stream);
   // the single-stream decoder GEMM: 6 x 18 KB leaves room on the SM for a co-resident ViT CTA (static_asserts above)
   if (c.fmt == FMT_BF16 && bn == 16) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
+  if (a8 && bn == 16) return launch_ws<FMT_E4M3_A8, 16, kA8DecoderStages>(tw, tx, a, stream);
   if (f8 && bn == 16) return launch_ws<FMT_E4M3, 16, kF8DecoderStages>(tw, tx, a, stream);
   if (beside) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
   VLO_WS_CASE(FMT_BF16, 32)
@@ -303,6 +320,10 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   VLO_WS_CASE(FMT_E4M3, 64)
   VLO_WS_CASE(FMT_E4M3, 96)
   VLO_WS_CASE(FMT_E4M3, 128)
+  VLO_WS_CASE(FMT_E4M3_A8, 32)
+  VLO_WS_CASE(FMT_E4M3_A8, 64)
+  VLO_WS_CASE(FMT_E4M3_A8, 96)
+  VLO_WS_CASE(FMT_E4M3_A8, 128)
 #undef VLO_WS_CASE
   return fail("gemm_ws_launch: no kernel instance");
 }
@@ -342,10 +363,22 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 // ------------------------------------------------------------------------------------------------
 // stream-K gate|up GEMM with the SwiGLU finisher epilogue (gemm_wsf.cuh)
 namespace {
-// w_scale null: bf16 weights; else e4m3 weights with these row scales
+// w_scale null: bf16 weights; else e4m3 weights with these row scales, and with a_scale also e4m3 activations
 template <int BN>
 int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, const float* w_scale,
-               cudaStream_t stream) {
+               const float* a_scale, cudaStream_t stream) {
+  if (a_scale != nullptr) {
+    constexpr int S = wsf_a8_default_stages(BN);
+    auto kern = gemm_wsf_a8_kernel<BN, S>;
+    using Cfg = GemmWsfCfg<BN, S, FMT_E4M3_A8>;
+    if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
+    if (prof_on())   // 1 B per weight and activation + their scales
+      prof_begin(PROF_GEMM_STREAM, stream, (a.k + 4.0) * (static_cast<double>(a.rows_w) + a.rows_x) + 2.0 * a.rows_x * a.rows_w);
+    VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a, w_scale, a_scale));
+    prof_end(stream);
+    count_launch();
+    return 0;
+  }
   if (w_scale != nullptr) {
     constexpr int S = wsf_f8_default_stages(BN);
     auto kern = gemm_wsf_f8_kernel<BN, S>;
@@ -372,7 +405,7 @@ int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& 
 }  // namespace
 
 int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
-                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream) {
+                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream, const float* a_scale) {
   VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(rows_w > 0 && rows_x > 0 && rows_x <= 128, "gemm_wsf: 1..128 token rows");
   VLO_CHECK(rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
@@ -391,14 +424,16 @@ int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void*
   a.hint_w = kEvictFirst;
   a.act = static_cast<__nv_bfloat16*>(act);
   a.I = rows_w / 2;
+  VLO_CHECK(a_scale == nullptr || w_scale != nullptr, "gemm_wsf: e4m3 activations need e4m3 weights");
+  const int fw = a_scale ? FMT_E4M3_A8 : w_scale ? FMT_E4M3 : FMT_BF16;
   CUtensorMap tw, tx;
-  if (get_tmap(w, rows_w, k, kGemmBM, w_scale ? FMT_E4M3 : FMT_BF16, &tw) != 0) return -1;
-  if (get_tmap(x, rows_x, k, bn, FMT_BF16, &tx) != 0) return -1;
-  if (bn == 16) return launch_wsf<16>(tw, tx, a, w_scale, stream);
-  if (bn == 32) return launch_wsf<32>(tw, tx, a, w_scale, stream);
-  if (bn == 64) return launch_wsf<64>(tw, tx, a, w_scale, stream);
-  if (bn == 96) return launch_wsf<96>(tw, tx, a, w_scale, stream);
-  return launch_wsf<128>(tw, tx, a, w_scale, stream);
+  if (get_tmap(w, rows_w, k, kGemmBM, fw, &tw) != 0) return -1;
+  if (get_tmap(x, rows_x, k, bn, a_scale ? FMT_E4M3_A8 : FMT_BF16, &tx) != 0) return -1;
+  if (bn == 16) return launch_wsf<16>(tw, tx, a, w_scale, a_scale, stream);
+  if (bn == 32) return launch_wsf<32>(tw, tx, a, w_scale, a_scale, stream);
+  if (bn == 64) return launch_wsf<64>(tw, tx, a, w_scale, a_scale, stream);
+  if (bn == 96) return launch_wsf<96>(tw, tx, a, w_scale, a_scale, stream);
+  return launch_wsf<128>(tw, tx, a, w_scale, a_scale, stream);
 }
 
 }  // namespace vlo

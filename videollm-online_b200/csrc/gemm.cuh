@@ -28,7 +28,9 @@ enum GemmEpi : int {
 enum GemmAct : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF_PY = 2 };
 // FMT_E4M3: e4m3 weights with one fp32 scale per weight row, bf16 activations; the consumer upcasts each weight k-block
 // to bf16 exactly and runs the bf16 wgmma chain (weight-streaming kernels, stream-K partials only)
-enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2 };
+// FMT_E4M3_A8: e4m3 weights (row scales) x e4m3 activations (token scales), multiplied by the FP8 wgmma (QGMMA) on
+// SWIZZLE_64B stages; each partial is scaled once in the epilogue (weight-streaming kernels, stream-K partials only)
+enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2, FMT_E4M3_A8 = 3 };
 
 struct GemmArgs {
   int rows_a, rows_b, k;
@@ -163,6 +165,48 @@ __device__ __forceinline__ void wg_mainloop_f8(float (&acc)[2][BN / 2], uint8_t*
     for (int kk = 0; kk < kGemmBK / 16; ++kk) {
       Wgmma<FMT_BF16, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
       Wgmma<FMT_BF16, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (j > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+    }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  if (nk > 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+  }
+}
+
+// ---- e4m3 weights x e4m3 activations (FMT_E4M3_A8).  A weight stage is a 128 x 64-byte TMA box and an activation stage
+// a BN x 64-byte box, both with the 64-byte swizzle the FP8 wgmma descriptor reads directly: no conversion, no
+// generic-proxy stores, no warpgroup barrier.  Two k32 MMAs per 64-wide k-block on each 64-row half, in k order.
+constexpr int kA8BytesW = kGemmBM * kGemmBK;   // one e4m3 weight stage (8 KB)
+
+template <int BN, int S>
+__device__ __forceinline__ void wg_mainloop_a8(float (&acc)[2][BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
+                                               uint64_t* full_bar, uint64_t* empty_bar, int& i, int nk) {
+  constexpr int kBytesB = BN * kGemmBK;
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+  for (int j = 0; j < nk; ++j, ++i) {
+    const int s = i % S;
+    mbar_wait(&full_bar[s], (i / S) & 1);
+    wgmma_fence();
+    const uint64_t da = wgmma_desc_sw64(smem_u32(smem_a + s * kA8BytesW));
+    const uint64_t db = wgmma_desc_sw64(smem_u32(smem_b + s * kBytesB));
+#pragma unroll
+    for (int kk = 0; kk < kGemmBK / 32; ++kk) {
+      // +2 per 32 elements (32 B) along K; the second 64-row half of A starts 4 KB (+256) further
+      WgmmaE4M3<BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
+      WgmmaE4M3<BN>::mma(acc[1], da + 256 + 2 * kk, db + 2 * kk);
     }
     wgmma_commit();
     wgmma_wait<1>();

@@ -13,7 +13,9 @@
 //   * the producer warp keeps the ring full across items, so the weight stream continues while the warpgroup
 //     runs the epilogue of an item;
 //   * FMT_E4M3 (mode 0 only): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop_f8), each partial
-//     multiplied by its row's scale once before it is written.
+//     multiplied by its row's scale once before it is written;
+//   * FMT_E4M3_A8 (mode 0 only): e4m3 weight and e4m3 activation stages straight into the FP8 wgmma (wg_mainloop_a8);
+//     each partial is multiplied by its row's weight scale, then by its token's activation scale, before it is written.
 #pragma once
 #include <cuda.h>
 #include "gemm.cuh"
@@ -33,7 +35,8 @@ struct GemmWsArgs {
   const float* bias;
   int act;
   unsigned long long hint_w;  // L2 policy for the weight stream (evict-first when read once per launch)
-  const float* w_scale;       // FMT_E4M3: [rows_w] fp32 row scales, applied once to each partial
+  const float* w_scale;       // FMT_E4M3 / FMT_E4M3_A8: [rows_w] fp32 row scales, applied once to each partial
+  const float* a_scale;       // FMT_E4M3_A8: [rows_x] fp32 token scales, applied after the row scale
 };
 
 // deepest ring of at most 8 stages that fits next to the staging tile
@@ -44,11 +47,14 @@ constexpr int ws_f8_default_stages(int bn) {
   return fit_stages(kF8BytesW + bn * kGemmBK * 2, kF8BytesCvt + kWgStageBytes + 1024 + 256, 16);
 }
 
+// e4m3 weights and activations: up to 16 stages of 8 KB + BN x 64 B next to the staging tile (no conversion tiles)
+constexpr int ws_a8_default_stages(int bn) { return fit_stages(kA8BytesW + bn * kGemmBK, kWgStageBytes + 1024 + 256, 16); }
+
 template <int BN, int STAGES = ws_default_stages(BN), int FMT = FMT_BF16>
 struct GemmWsCfg {
   static constexpr int kStages = STAGES;
-  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : kGemmBM * kGemmBK * 2;
-  static constexpr int kBytesB = BN * kGemmBK * 2;
+  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW : kGemmBM * kGemmBK * 2;
+  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2);
   static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
   static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kWgStageBytes;
   static_assert(kSmemBytes <= kSmemOptIn, "ring + staging tile exceed the shared memory of one block");
@@ -61,6 +67,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
                const GemmWsArgs p) {
   using Cfg = GemmWsCfg<BN, STAGES, FMT>;
   constexpr bool kF8 = FMT == FMT_E4M3;
+  constexpr bool kA8 = FMT == FMT_E4M3_A8;
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -142,6 +149,8 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       float acc[2][BN / 2];
       if constexpr (kF8)
         wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      else if constexpr (kA8)
+        wg_mainloop_a8<BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       else
         wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int wt = tile / p.x_tiles, xt = tile - wt * p.x_tiles;
@@ -151,7 +160,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       float* plane = nullptr;
       float bias_n = 0.f;
       float scale_n = 0.f;
-      if constexpr (kF8) {
+      if constexpr (kF8 || kA8) {
         if (n_ok) scale_n = __ldg(p.w_scale + n);
       }
       if (p.mode == 0) {
@@ -175,6 +184,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
           const float acc = v[j];
           if constexpr (kF8) {
             plane[static_cast<size_t>(t) * p.rows_w + n] = __fmul_rn(acc, scale_n);   // the one rounding of the scale
+          } else if constexpr (kA8) {
+            // a_scale is the quantizer's output: a plain load, after pdl_wait
+            plane[static_cast<size_t>(t) * p.rows_w + n] = __fmul_rn(__fmul_rn(acc, scale_n), p.a_scale[t]);
           } else if (p.mode == 0) {
             plane[static_cast<size_t>(t) * p.rows_w + n] = acc;
           } else {

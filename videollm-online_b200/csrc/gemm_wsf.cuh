@@ -15,6 +15,8 @@
 // fix-up kernels of decoder_kernels.cuh, whose rounding points this epilogue shares.
 // gemm_wsf_f8_kernel runs the same schedule on e4m3 weights (FMT_E4M3, gemm.cuh): every contributor, the finisher's own
 // accumulator included, multiplies its fp32 partial of feature n by the row scale w_scale[n] once before the plane sum.
+// gemm_wsf_a8_kernel runs it on e4m3 weights and e4m3 activations (FMT_E4M3_A8): every partial of feature n, token t is
+// fl(fl(P * w_scale[n]) * a_scale[t]) before the plane sum.
 // All CTAs of the grid are co-resident or become so without depending on a waiting CTA (grid <= #SMs, the PDL successor
 // cannot start before every CTA of this grid has started), so the finisher's wait cannot dead-lock; it is bounded anyway.
 #pragma once
@@ -40,8 +42,8 @@ constexpr int kWsfXchStride = 17;   // floats per feature row of the exchange ti
 template <int BN, int STAGES, int FMT = FMT_BF16>
 struct GemmWsfCfg {
   static constexpr int kStages = STAGES;
-  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : kGemmBM * kGemmBK * 2;
-  static constexpr int kBytesB = BN * kGemmBK * 2;
+  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW : kGemmBM * kGemmBK * 2;
+  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2);
   static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
   static constexpr int kXchBytes = kGemmBM * kWsfXchStride * 4;
   static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kXchBytes + kWgStageBytes;
@@ -56,6 +58,10 @@ constexpr int wsf_default_stages(int bn) {
 constexpr int wsf_f8_default_stages(int bn) {
   return fit_stages(kF8BytesW + bn * kGemmBK * 2, kF8BytesCvt + 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 16);
 }
+// e4m3 weights and activations: up to 16 stages next to the exchange and the staging tile
+constexpr int wsf_a8_default_stages(int bn) {
+  return fit_stages(kA8BytesW + bn * kGemmBK, 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 16);
+}
 
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
@@ -63,13 +69,14 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-// The body of both kernels below; FMT is FMT_BF16 or FMT_E4M3 (the weight format).  p by value: ptxas then still reads
+// The body of the kernels below; FMT is FMT_BF16, FMT_E4M3 or FMT_E4M3_A8.  p by value: ptxas then still reads
 // the fields from parameter space where used (the bf16 kernels compile to the same code as with the body inline).
 template <int FMT, int BN, int STAGES>
 __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUtensorMap& tm_x, const GemmWsfArgs p,
-                                              const float* w_scale) {
+                                              const float* w_scale, const float* a_scale = nullptr) {
   using Cfg = GemmWsfCfg<BN, STAGES, FMT>;
   constexpr bool kF8 = FMT == FMT_E4M3;
+  constexpr bool kA8 = FMT == FMT_E4M3_A8;
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -139,6 +146,8 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
       float acc[2][BN / 2];
       if constexpr (kF8)
         wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      else if constexpr (kA8)
+        wg_mainloop_a8<BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       else
         wg_mainloop<FMT_BF16, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int pl = c - sk_first_cta(tile, p.sk);
@@ -146,7 +155,7 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
       const int n = tile * kGemmBM + d;
       const bool n_ok = n < p.rows_w;
       float scale_n = 0.f;
-      if constexpr (kF8) {
+      if constexpr (kF8 || kA8) {
         if (n_ok) scale_n = __ldg(w_scale + n);
       }
       if (pl > 0) {
@@ -166,6 +175,8 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
             if (t >= p.rows_x) break;
             if constexpr (kF8)
               __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, __fmul_rn(v[j], scale_n));
+            else if constexpr (kA8)
+              __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, __fmul_rn(__fmul_rn(v[j], scale_n), a_scale[t]));
             else
               __stcg(plane + static_cast<size_t>(t) * p.rows_w + n, v[j]);
           }
@@ -204,6 +215,10 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
         if constexpr (kF8) {
 #pragma unroll
           for (int j = 0; j < 16; ++j) x[j] = __fmul_rn(x[j], scale_n);   // the finisher's own partial, before the sum
+        }
+        if constexpr (kA8) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) x[j] = c0 + j < p.rows_x ? __fmul_rn(__fmul_rn(x[j], scale_n), a_scale[c0 + j]) : 0.f;
         }
         for (int s2 = 1; s2 < n_planes; ++s2) {   // plane order: deterministic
           const float* plane = p.planes + static_cast<size_t>(s2 - 1) * p.plane_stride + n;
@@ -252,6 +267,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wsf_f8_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
                    const __grid_constant__ GemmWsfArgs p, const float* __restrict__ w_scale) {
   gemm_wsf_body<FMT_E4M3, BN, STAGES>(tm_w, tm_x, p, w_scale);
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_wsf_a8_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
+                   const __grid_constant__ GemmWsfArgs p, const float* __restrict__ w_scale, const float* a_scale) {
+  gemm_wsf_body<FMT_E4M3_A8, BN, STAGES>(tm_w, tm_x, p, w_scale, a_scale);
 }
 
 }  // namespace vlo

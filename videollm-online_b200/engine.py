@@ -234,10 +234,12 @@ class SampleRow:
 class Engine:
     def __init__(self, cfg: LiveConfig, device: str | torch.device = "cuda:0", *, max_streams: int = 1,
                  max_kv_tokens: int = 16384, max_step_tokens: int = 128, max_vit_batch: int = 8,
-                 kv_pool_tokens: Optional[int] = None):
+                 kv_pool_tokens: Optional[int] = None, fp8_activations: bool = False):
         """kv_pool_tokens: size of the KV page pool all streams share (rounded up to 64-token pages); None reserves
         max_streams * max_kv_tokens, so every stream can reach max_kv_tokens at once.  A smaller pool over-subscribes:
-        a step that needs more pages than are free raises VloError and leaves every stream as it was."""
+        a step that needs more pages than are free raises VloError and leaves every stream as it was.
+        fp8_activations: the layer GEMMs quantize their activations to e4m3 per token and multiply on the FP8 tensor
+        cores (W8A8, vlo_set_fp8_activations); load_weights then needs FP8 layer weights."""
         self.lib = _lib.load()
         self.cfg = cfg
         self.device = torch.device(device)
@@ -266,6 +268,9 @@ class Engine:
         with torch.cuda.device(self.index):
             check(self.lib.vlo_engine_create_pooled(C.byref(c), int(kv_pool_tokens or 0), self.index, C.byref(self._h)),
                   "vlo_engine_create_pooled")
+            self._fp8_act = bool(fp8_activations)
+            if self._fp8_act:
+                check(self.lib.vlo_set_fp8_activations(self._h, 1), "vlo_set_fp8_activations")
         # device scratch for results (decisions, last logits): one row per sequence, or per segment of a segmented step
         # and the sampled ids right behind the decisions, so that one copy brings both back
         rows = max(max_streams, max_step_tokens)
@@ -314,6 +319,11 @@ class Engine:
     def fp8_weights(self) -> bool:
         """True when the decoder layer matrices were loaded as e4m3 codes + row scales (weights.quantize_fp8_rows)."""
         return "L0.qkv.f8" in self._weights
+
+    @property
+    def fp8_activations(self) -> bool:
+        """True when the layer GEMMs take e4m3 activations with per-token scales (W8A8; Engine(fp8_activations=True))."""
+        return self._fp8_act
 
     def device_bytes(self) -> int:
         return int(self.lib.vlo_engine_device_bytes(self._h))

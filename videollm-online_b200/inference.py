@@ -50,6 +50,7 @@ class SessionState:
     evicted_tokens: int = 0      # cache positions the session's context window dropped so far
     fed_ids: Optional[list] = None   # the id fed at every cache position (-1: frame row) when no NgramDrafter holds them
     fp8_weights: bool = False    # the cache was written by a model with FP8 layer weights (Engine.fp8_weights)
+    fp8_activations: bool = False   # ... and with FP8 activations (Engine.fp8_activations)
 
 
 torch.serialization.add_safe_globals([SessionState, SamplingConfig])
@@ -235,7 +236,7 @@ class LiveInfer:
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
                 n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling,
                 evicted_tokens=self.evicted_tokens, fp8_weights=self._kv.engine.fp8_weights,
-                fed_ids=fed)
+                fp8_activations=self._kv.engine.fp8_activations, fed_ids=fed)
             self.reset()
             return state
 
@@ -244,13 +245,18 @@ class LiveInfer:
         every queue and counter `__call__` reads is restored.  The video is not part of the state: load it again
         (before or after resuming).  Raises VloError if the pool is short or the image belongs to another config; the
         session's stream is then empty and the rest of the session unchanged.  A state whose cache was written with the
-        other weight form (FP8 or bf16 layer weights: a different model) is refused before anything changes."""
+        other weight form (FP8 or bf16 layer weights: a different model), or with the other activation form (W8A8 or not),
+        is refused before anything changes."""
         with self._lock:
             eng = self._kv.engine
             if state.fp8_weights != eng.fp8_weights:
                 form = {True: "FP8", False: "bf16"}
                 raise VloError(f"resume: the state's cache was written with {form[state.fp8_weights]} layer weights, "
                                f"this model has {form[eng.fp8_weights]} ones")
+            if state.fp8_activations != eng.fp8_activations:
+                form = {True: "FP8", False: "bf16"}
+                raise VloError(f"resume: the state's cache was written with {form[state.fp8_activations]} layer "
+                               f"activations, this model has {form[eng.fp8_activations]} ones")
             self._drop_prefetch()
             eng.stream_reset(self._kv.stream_id)
             eng.kv_swap_in(self._kv.stream_id, state.kv)

@@ -296,13 +296,17 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
                synthetic_weights: bool = False, seed: int = 0, max_streams: int = 1, max_kv_tokens: int = 16384,
                max_step_tokens: int = 128, max_vit_batch: int = 8, llm_state=None, vision_state=None,
                lora_r: int = 128, lora_alpha: int = 256, kv_pool_tokens: Optional[int] = None, fp8_weights: bool = False,
-               **kwargs):
+               fp8_activations: bool = False, **kwargs):
     """models/modeling_live.py:184-222 for inference: build config + tokenizer, load (or synthesise)
     weights, merge LoRA, hand everything to the engine.  kv_pool_tokens: size of the KV page pool the streams
     share (None or <= 0: max_streams * max_kv_tokens).  fp8_weights: quantize the decoder layer matrices to e4m3 with
-    per-row scales after the LoRA merge (weights.quantize_fp8_rows); the engine then runs its FP8-weight GEMMs."""
+    per-row scales after the LoRA merge (weights.quantize_fp8_rows); the engine then runs its FP8-weight GEMMs.
+    fp8_activations (needs fp8_weights): the layer GEMMs also quantize their activations to e4m3 per token and run on
+    the FP8 tensor cores (W8A8)."""
     if is_training:
         raise NotImplementedError("the vlo_b200 engine covers the streaming-inference path only")
+    if fp8_activations and not fp8_weights:
+        raise ValueError("fp8_activations needs fp8_weights: the FP8 tensor cores take both operands in e4m3")
     cfg = config or llama3_8b_siglip_l()
     for k in ("frame_resolution", "frame_token_cls", "frame_token_pooled", "frame_num_tokens", "frame_token_interval",
               "vision_pretrained"):
@@ -310,7 +314,8 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
             setattr(cfg, k, kwargs[k])
     tokenizer = build_live_tokenizer_and_update_config(llm_pretrained or "", cfg)
     engine = Engine(cfg, device, max_streams=max_streams, max_kv_tokens=max_kv_tokens,
-                    max_step_tokens=max_step_tokens, max_vit_batch=max_vit_batch, kv_pool_tokens=kv_pool_tokens)
+                    max_step_tokens=max_step_tokens, max_vit_batch=max_vit_batch, kv_pool_tokens=kv_pool_tokens,
+                    fp8_activations=fp8_activations)
     if llm_state is not None:
         packed = W.pack_llm_for_engine(cfg, llm_state, engine.device, max_kv_tokens, fp8_weights=fp8_weights)
         if set_vision_inside:
