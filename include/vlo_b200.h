@@ -300,6 +300,13 @@ int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, 
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
                    void* cuda_stream);
+/* vlo_op_gemm_ws with the token tile chosen by `tiling` when bn <= 0 (0: the smallest covering instance, as
+ * vlo_op_gemm_ws; 1: the ViT trunk tiling of 3+ frames; 2: the 64-token fp16 instance that runs beside a decoder step,
+ * which is the one vlo_vit_encode uses for 1-2 frames).  h_plan (may be NULL) receives {bn, token tiles, most planes of
+ * one tile}.  Asynchronous. */
+int vlo_op_gemm_ws_tiled(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
+                         int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int tiling,
+                         int32_t* h_plan, void* cuda_stream);
 /* The same GEMM in mode 0 on e4m3 weights (the decoder's FP8 weight form): d_w8 [rows_w, k] e4m3fn bytes, d_scale fp32
  * [rows_w] row scales, X bf16 [rows_x, k].  Same token tile and stream-K plan as the bf16 call with these sizes and
  * n_ctas; each weight k-block is upcast to bf16 exactly and multiplied by the bf16 wgmma chain, so plane p holds
@@ -357,6 +364,39 @@ int vlo_op_attn_plan_counts(int n_segs, const int32_t* h_seg_lens, int n_heads, 
 int vlo_op_vit_attn(const void* d_qkv, void* d_out, int n_frames, int n_tok, int hidden, void* cuda_stream);
 int vlo_op_probe_attn(const void* d_kv, const float* d_q, void* d_out, int n_frames, int n_tok, int hidden,
                       void* cuda_stream);
+/* The GEMM configuration vlo_vit_encode runs for n_frames frames of n_patches tokens (rows = n_frames * n_patches),
+ * without launching anything: h_out[0..11) =
+ *   [0] QKV / fc1 kernel: 0 = vlo_op_gemm_vit, else the vlo_op_gemm_ws_tiled tiling of its mode-1 call
+ *   [1] QKV and [2] fc1 token tile;  [3] the vlo_op_gemm_ws_tiled tiling of the out_proj / fc2 mode-0 calls
+ *   [4] out_proj token tile and [5] its most planes of one tile;  [6] fc2 token tile and [7] its most planes
+ *   [8] the patch-embed and [9] the MAP-head K/V bn of vlo_op_gemm;  [10] the MAP head's token tile (n_frames rows). */
+int vlo_op_vit_tiling(int n_frames, int n_patches, int hidden, int mlp, int32_t* h_out);
+/* The other kernels of vlo_vit_encode (csrc/vit_kernels.cuh), launched by the same helpers.  Asynchronous.
+ * patchify: u8 d_frames [n_frames, 3, S, S] -> fp16 d_out [n_frames * g * g, 3 ps ps] (g = S / ps, ps a multiple of 8),
+ *   row b g^2 + py g + px, column (c ps + iy) ps + ix = fp16((x / 255 - 0.5) / 0.5) of pixel (c, py ps + iy, px ps + ix).
+ * vit_layernorm: d_in [rows, C] (fp16 if in_is_f16, else fp32) -> LayerNorm with fp32 statistics, affine d_w / d_b, to
+ *   d_out16 fp16 and / or d_out32 fp32 (either may be NULL); C <= 12288.
+ * vit_fix_ln: d_part fp32 stream-K planes [plane][rows][C] of the fp16 vlo_op_gemm_ws mode-0 call with rows_w = C, this
+ *   k, bn and n_ctas (plane_stride rows * C), of which only the planes of each (128-feature, bn-token) tile are read:
+ *     h[t][n] = h[t][n] + fp16(sum_s part[s][t][n] + bias[n])   (fp32 residual d_h, summed in plane order)
+ *     then LayerNorm(h[t]) -> d_out16 / d_out32 as vit_layernorm.  C a multiple of 4, <= 12288, at most 8 planes;
+ *     the fp32 arrays 16-byte and d_out16 8-byte aligned.
+ * vit_pool: adaptive average pool of each frame's grid x grid tokens d_in fp32 [n_frames, grid^2, C] to ph x pw cells,
+ *   cell i pw + j of frame b -> d_tokens[b n_tok + tok_off + i pw + j] (window rows [i g / ph, ceil((i + 1) g / ph)), cols
+ *   alike; summed row by row in fp32, divided once).
+ * cls_residual: d_tokens[b n_tok][c] = fp16(d_resid16[b][c] + d_mlp16[b][c]) for the n_frames x C fp16 inputs. */
+/* tanh.approx.f32 (the MUFU.TANH the GELU-tanh epilogue evaluates) of n fp32 values: d_y[i] = tanh_approx(d_x[i]).
+ * Asynchronous. */
+int vlo_op_tanh_approx(const float* d_x, float* d_y, long long n, void* cuda_stream);
+int vlo_op_patchify(const uint8_t* d_frames, int n_frames, int image_size, int patch_size, void* d_out, void* cuda_stream);
+int vlo_op_vit_layernorm(const void* d_in, int in_is_f16, int rows, int C, const float* d_w, const float* d_b, void* d_out16,
+                         float* d_out32, float eps, void* cuda_stream);
+int vlo_op_vit_fix_ln(const float* d_part, int rows, int C, int k, int bn, int n_ctas, const float* d_bias, float* d_h,
+                      const float* d_ln_w, const float* d_ln_b, void* d_out16, float* d_out32, float eps, void* cuda_stream);
+int vlo_op_vit_pool(const float* d_in, int n_frames, int grid, int C, int ph, int pw, int n_tok, int tok_off, float* d_tokens,
+                    void* cuda_stream);
+int vlo_op_cls_residual(const void* d_resid16, const void* d_mlp16, float* d_tokens, int n_frames, int C, int n_tok,
+                        void* cuda_stream);
 /* The decoder step's fix-up and decision kernels (csrc/decoder_kernels.cuh), launched by the same helpers as vlo_step
  * (block size, grid, shared memory, PDL).  bf16 tensors unless stated; bf16(.) = round to nearest even.
  * d_part: fp32 stream-K partial planes [plane][T][width] as vlo_op_gemm_ws mode 0 leaves them (plane_stride T * width)

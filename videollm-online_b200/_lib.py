@@ -95,6 +95,7 @@ SIGNATURES = {
     "vlo_bench_gemm": (_I, [_P, _I, _I, C.POINTER(C.c_double), C.POINTER(_I), _P]),
     "vlo_op_gemm": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _P, _P, _I, _I, _P]),
     "vlo_op_gemm_ws": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, C.POINTER(_I), _P]),
+    "vlo_op_gemm_ws_tiled": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, _I, C.POINTER(C.c_int32), _P]),
     "vlo_op_gemm_ws_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_ws_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
@@ -105,6 +106,13 @@ SIGNATURES = {
     "vlo_op_attn_plan_counts": (_I, [_I, C.POINTER(C.c_int32), _I, _I, _I, _I, C.POINTER(C.c_int32)]),
     "vlo_op_vit_attn": (_I, [_P, _P, _I, _I, _I, _P]),
     "vlo_op_probe_attn": (_I, [_P, _P, _P, _I, _I, _I, _P]),
+    "vlo_op_vit_tiling": (_I, [_I, _I, _I, _I, C.POINTER(C.c_int32)]),
+    "vlo_op_tanh_approx": (_I, [_P, _P, _LL, _P]),
+    "vlo_op_patchify": (_I, [_P, _I, _I, _I, _P, _P]),
+    "vlo_op_vit_layernorm": (_I, [_P, _I, _I, _I, _P, _P, _P, _P, C.c_float, _P]),
+    "vlo_op_vit_fix_ln": (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, C.c_float, _P]),
+    "vlo_op_vit_pool": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "vlo_op_cls_residual": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "vlo_op_resid_rmsnorm": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
     "vlo_op_resid_rmsnorm_q8": (_I, [_P, _I, _I, _P, _P, _P, _P, _P, _P, _P, _I, _I, C.c_float, _P]),
     "vlo_op_quant_rows_e4m3": (_I, [_P, _I, _I, _P, _P, _P]),

@@ -1,6 +1,7 @@
 // C-ABI: library-level and kernel-level entry points (see include/vlo_b200.h).
 #include "vlo_b200.h"
 
+#include <algorithm>
 #include <vector>
 
 #include "common.h"
@@ -60,6 +61,12 @@ int op_fix_plan(int width, int T, int k, int n_ctas, SkInfo* sk) {
   return 0;
 }
 
+__global__ void tanh_approx_kernel(const float* x, float* y, long long n) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    y[i] = tanh_approx(x[i]);
+}
+
 // Device scratch of a synchronous kernel-level entry point, freed on every return path.
 struct OpScratch {
   void* p = nullptr;
@@ -115,6 +122,17 @@ int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, 
 int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
                    int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int* h_max_planes,
                    void* cuda_stream) {
+  int32_t plan[3] = {0, 0, 0};
+  const int rc = vlo_op_gemm_ws_tiled(fmt, mode, d_w, rows_w, d_x, rows_x, k, d_out, ld_out, plane_stride, d_bias, act,
+                                      n_ctas, bn, WS_TILE_FIT, plan, cuda_stream);
+  if (rc == 0 && h_max_planes) *h_max_planes = plan[2];
+  return rc;
+}
+
+int vlo_op_gemm_ws_tiled(int fmt, int mode, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out,
+                         int ld_out, long long plane_stride, const float* d_bias, int act, int n_ctas, int bn, int tiling,
+                         int32_t* h_plan, void* cuda_stream) {
+  VLO_CHECK(tiling == WS_TILE_FIT || tiling == WS_TILE_TRUNK || tiling == WS_TILE_BESIDE_DECODER, "gemm_ws: unknown tiling");
   GemmWsCall c{};
   c.fmt = fmt;
   c.mode = mode;
@@ -131,9 +149,14 @@ int vlo_op_gemm_ws(int fmt, int mode, const void* d_w, int rows_w, const void* d
   c.act = act;
   c.n_ctas = n_ctas;
   c.bn = bn;
+  c.tiling = tiling;
   GemmWsPlan plan{};
   const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
-  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
+  if (rc == 0 && h_plan) {
+    h_plan[0] = plan.bn;
+    h_plan[1] = plan.x_tiles;
+    h_plan[2] = plan.planes;
+  }
   return rc;
 }
 
@@ -278,6 +301,112 @@ int vlo_op_probe_attn(const void* d_kv, const float* d_q, void* d_out, int n_fra
                       void* cuda_stream) {
   VLO_CHECK(d_kv != nullptr && d_q != nullptr && d_out != nullptr, "probe_attn: null argument");
   return probe_attn_launch(d_kv, d_q, d_out, n_frames, n_tok, hidden, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_vit_tiling(int n_frames, int n_patches, int hidden, int mlp, int32_t* h_out) {
+  VLO_CHECK(n_frames > 0 && n_patches > 0 && hidden > 0 && mlp > 0 && h_out != nullptr, "vit_tiling: sizes");
+  const int rows = n_frames * n_patches;
+  const bool beside = vit_beside_decoder(n_frames);
+  // the planning query of each gemm_ws_launch vlo_vit_encode makes (mode, output features, k, tiling)
+  auto query = [&](int mode, int n_out, int k, int tiling, int tok_rows, GemmWsPlan* plan) -> int {
+    GemmWsCall c{};
+    c.fmt = FMT_F16;
+    c.mode = mode;
+    c.rows_w = n_out;
+    c.rows_x = tok_rows;
+    c.k = k;
+    c.tiling = tiling;
+    return gemm_ws_launch(c, nullptr, plan);
+  };
+  GemmWsPlan qkv{}, fc1{}, out{}, fc2{}, head{};
+  const int part_tiling = beside ? WS_TILE_BESIDE_DECODER : WS_TILE_TRUNK;
+  if (!beside && (query(1, 3 * hidden, hidden, WS_TILE_TRUNK, rows, &qkv) || query(1, mlp, hidden, WS_TILE_TRUNK, rows, &fc1)))
+    return -1;
+  if (query(0, hidden, hidden, part_tiling, rows, &out) || query(0, hidden, mlp, part_tiling, rows, &fc2) ||
+      query(1, hidden, hidden, WS_TILE_FIT, n_frames, &head))
+    return -1;
+  h_out[0] = beside ? 0 : WS_TILE_TRUNK;
+  h_out[1] = beside ? kGemmBM : qkv.bn;
+  h_out[2] = beside ? kGemmBM : fc1.bn;
+  h_out[3] = part_tiling;
+  h_out[4] = out.bn;
+  h_out[5] = out.planes;
+  h_out[6] = fc2.bn;
+  h_out[7] = fc2.planes;
+  h_out[8] = vit_bn(rows, hidden);
+  h_out[9] = vit_bn(rows, 2 * hidden);
+  h_out[10] = head.bn;
+  return 0;
+}
+
+int vlo_op_tanh_approx(const float* d_x, float* d_y, long long n, void* cuda_stream) {
+  VLO_CHECK(d_x != nullptr && d_y != nullptr && n > 0, "tanh_approx: null argument or n <= 0");
+  tanh_approx_kernel<<<static_cast<unsigned>(std::min<long long>((n + 255) / 256, 4096)), 256, 0,
+                       static_cast<cudaStream_t>(cuda_stream)>>>(d_x, d_y, n);
+  VLO_LAUNCH_CHECK();
+  return 0;
+}
+
+int vlo_op_patchify(const uint8_t* d_frames, int n_frames, int image_size, int patch_size, void* d_out, void* cuda_stream) {
+  VLO_CHECK(d_frames != nullptr && d_out != nullptr, "patchify: null argument");
+  VLO_CHECK(n_frames > 0 && patch_size > 0 && patch_size % 8 == 0 && image_size >= patch_size && image_size % patch_size == 0,
+            "patchify: n_frames > 0, patch_size a multiple of 8 dividing image_size");
+  VLO_CHECK((reinterpret_cast<uintptr_t>(d_frames) & 7) == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0,
+            "patchify: frames 8-byte and patches 16-byte aligned");
+  return patchify_launch(d_frames, d_out, n_frames, image_size, patch_size, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_vit_layernorm(const void* d_in, int in_is_f16, int rows, int C, const float* d_w, const float* d_b, void* d_out16,
+                         float* d_out32, float eps, void* cuda_stream) {
+  VLO_CHECK(d_in != nullptr && d_w != nullptr && d_b != nullptr && (d_out16 != nullptr || d_out32 != nullptr),
+            "vit_layernorm: null argument");
+  // the row is staged in shared memory without an opt-in beyond the default 48 KB
+  VLO_CHECK(rows > 0 && C > 0 && C * sizeof(float) <= 48 * 1024, "vit_layernorm: rows > 0, 0 < C <= 12288");
+  return vit_layernorm_launch(d_in, in_is_f16 != 0, rows, C, d_w, d_b, d_out16, d_out32, eps,
+                              static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_vit_fix_ln(const float* d_part, int rows, int C, int k, int bn, int n_ctas, const float* d_bias, float* d_h,
+                      const float* d_ln_w, const float* d_ln_b, void* d_out16, float* d_out32, float eps, void* cuda_stream) {
+  VLO_CHECK(d_part != nullptr && d_bias != nullptr && d_h != nullptr && d_ln_w != nullptr && d_ln_b != nullptr,
+            "vit_fix_ln: null argument");
+  VLO_CHECK(rows > 0 && C > 0 && C % 4 == 0 && C * sizeof(float) <= 48 * 1024, "vit_fix_ln: rows > 0, C a multiple of 4, <= 12288");
+  VLO_CHECK(bn > 0, "vit_fix_ln: the producer's token tile bn must be given");
+  auto aligned = [](const void* q, uintptr_t a) { return (reinterpret_cast<uintptr_t>(q) & (a - 1)) == 0; };
+  // the kernel moves 4 channels per access: float4 for the fp32 rows and vectors, uint2 for out16
+  VLO_CHECK(aligned(d_part, 16) && aligned(d_h, 16) && aligned(d_bias, 16) && aligned(d_ln_w, 16) && aligned(d_ln_b, 16) &&
+                aligned(d_out32, 16) && aligned(d_out16, 8),
+            "vit_fix_ln: fp32 arrays 16-byte and out16 8-byte aligned");
+  GemmWsCall c{};
+  c.fmt = FMT_F16;
+  c.mode = 0;
+  c.rows_w = C;
+  c.rows_x = rows;
+  c.k = k;
+  c.n_ctas = n_ctas;
+  c.bn = bn;
+  GemmWsPlan plan{};
+  if (gemm_ws_launch(c, nullptr, &plan)) return -1;
+  VLO_CHECK(plan.planes <= kFixMaxPlanes, "the plan needs " + std::to_string(plan.planes) +
+                                              " partial planes, more than the fix-up kernels unroll");
+  return vit_fix_ln_launch(d_part, plan, rows, C, d_bias, d_h, d_ln_w, d_ln_b, d_out16, d_out32, eps,
+                           static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_vit_pool(const float* d_in, int n_frames, int grid, int C, int ph, int pw, int n_tok, int tok_off, float* d_tokens,
+                    void* cuda_stream) {
+  VLO_CHECK(d_in != nullptr && d_tokens != nullptr, "vit_pool: null argument");
+  VLO_CHECK(n_frames > 0 && grid > 0 && C > 0 && ph > 0 && ph <= grid && pw > 0 && pw <= grid,
+            "vit_pool: sizes (1 <= ph, pw <= grid)");
+  VLO_CHECK(tok_off >= 0 && tok_off + ph * pw <= n_tok, "vit_pool: the pooled cells must fit in n_tok token slots");
+  return pool_launch(d_in, d_tokens, n_frames, grid, C, ph, pw, n_tok, tok_off, static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_cls_residual(const void* d_resid16, const void* d_mlp16, float* d_tokens, int n_frames, int C, int n_tok,
+                        void* cuda_stream) {
+  VLO_CHECK(d_resid16 != nullptr && d_mlp16 != nullptr && d_tokens != nullptr, "cls_residual: null argument");
+  VLO_CHECK(n_frames > 0 && C > 0 && n_tok > 0, "cls_residual: sizes");
+  return cls_residual_launch(d_resid16, d_mlp16, d_tokens, n_frames, C, n_tok, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, const void* d_w, void* d_xn, void* d_xn_last,

@@ -98,6 +98,8 @@ struct GemmCall {
   int bn;    // 64 or 128 (0: one wave of CTAs if possible, else the less wasted last wave; gemm.cu)
 };
 int gemm_launch(const GemmCall& c, cudaStream_t stream);
+// the bn gemm_launch picks when GemmCall::bn is 0
+int vit_bn(int rows, int n_out);
 
 // ---- persistent weight-streaming GEMM (gemm_ws.cuh / gemm.cu)
 // How gemm_ws_launch picks the token-tile width when GemmWsCall::bn is 0 (the rules sit next to the instances in gemm.cu)
@@ -188,6 +190,28 @@ int vit_attn_launch(const void* qkv, void* out, int B, int N, int C, cudaStream_
 // probe_attn_kernel: the MAP head's one fp32 query q [C] over the N tokens of each frame, kv fp16 [B * N, 2C] (k | v)
 // -> out fp16 [B, C].
 int probe_attn_launch(const void* kv, const float* q, void* out, int B, int N, int C, cudaStream_t st);
+
+// ---- the other ViT kernels (vit_kernels.cuh / engine.cu), fp16 / fp32 as vlo_vit_encode holds them -------------
+// B frames run their trunk GEMMs beside a decoder step (gemm_vit_kernel, WS_TILE_BESIDE_DECODER) rather than on the
+// WS_TILE_TRUNK tiling
+bool vit_beside_decoder(int B);
+// patchify_kernel: u8 frames [B, 3, S, S] -> fp16 patches [B * (S / ps)^2, 3 ps ps]; ps % 8 == 0
+int patchify_launch(const uint8_t* frames, void* out, int B, int S, int ps, cudaStream_t st);
+// layernorm_kernel: in [rows, C] (fp16 if in_f16, else fp32) -> out16 fp16 and / or out32 fp32 (either may be null)
+int vit_layernorm_launch(const void* in, bool in_f16, int rows, int C, const float* w, const float* b, void* out16,
+                         float* out32, float eps, cudaStream_t st);
+// vit_fix_ln_kernel: the stream-K planes `part` [plane][rows][C] of the fp16 GEMM that made `plan` folded with bias into
+// the fp32 residual h [rows, C], then LayerNorm(h) -> out16 (and out32 if not null); C % 4 == 0
+int vit_fix_ln_launch(const float* part, const GemmWsPlan& plan, int rows, int C, const float* bias, float* h,
+                      const float* ln_w, const float* ln_b, void* out16, float* out32, float eps, cudaStream_t st);
+// pool_kernel: adaptive average pool of each frame's g x g grid of in [B, g * g, C] to ph x pw cells, cell j of frame b
+// -> tokens[b * n_tok + tok_off + j]
+int pool_launch(const float* in, float* tokens, int B, int g, int C, int ph, int pw, int n_tok, int tok_off,
+                cudaStream_t st);
+// cls_residual_kernel: tokens[b * n_tok] = fp16(resid[b] + mlp[b]), fp16 [B, C] inputs
+int cls_residual_launch(const void* resid, const void* mlp, float* tokens, int B, int C, int n_tok, cudaStream_t st);
+// f32_to_bf16_kernel: out[i] = bf16(in[i]), i < n
+int f32_to_bf16_launch(const float* in, void* out, long long n, cudaStream_t st);
 
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {

@@ -418,6 +418,80 @@ int probe_attn_launch(const void* kv, const float* q, void* out, int B, int N, i
   return 0;
 }
 
+// ------------------------------------------------------------------------------ ViT element-wise launches
+// vlo_vit_encode and the kernel-level entry points (capi_ops.cu) launch the other ViT kernels through these only.
+bool vit_beside_decoder(int B) { return B <= 2; }
+
+int patchify_launch(const uint8_t* frames, void* out, int B, int S, int ps, cudaStream_t st) {
+  const int g = S / ps;
+  const long long total = static_cast<long long>(B) * g * g * 3 * ps * ps / 8;
+  VLO_CUDA(launch_pdl(patchify_kernel, dim3(static_cast<unsigned>(std::min<long long>((total + 255) / 256, 4096))), dim3(256), 0, st,
+                      frames, static_cast<__half*>(out), B, S, ps));
+  count_launch();
+  return 0;
+}
+
+int vit_layernorm_launch(const void* in, bool in_f16, int rows, int C, const float* w, const float* b, void* out16,
+                         float* out32, float eps, cudaStream_t st) {
+  const size_t smem = static_cast<size_t>(C) * sizeof(float);
+  if (in_f16) {
+    layernorm_kernel<__half><<<rows, 256, smem, st>>>(static_cast<const __half*>(in), w, b, static_cast<__half*>(out16),
+                                                      out32, C, eps);
+    VLO_LAUNCH_CHECK();
+  } else {
+    VLO_CUDA(launch_pdl(layernorm_kernel<float>, dim3(rows), dim3(256), smem, st, static_cast<const float*>(in), w, b,
+                        static_cast<__half*>(out16), out32, C, eps));
+  }
+  count_launch();
+  return 0;
+}
+
+int vit_fix_ln_launch(const float* part, const GemmWsPlan& plan, int rows, int C, const float* bias, float* h,
+                      const float* ln_w, const float* ln_b, void* out16, float* out32, float eps, cudaStream_t st) {
+  VitFixLnParams p{};
+  p.part = part;
+  p.sk = plan.sk;
+  p.sk_bn = plan.bn;
+  p.sk_xtiles = plan.x_tiles;
+  p.split_stride = static_cast<long long>(rows) * C;
+  p.bias = bias;
+  p.h = h;
+  p.ln_w = ln_w;
+  p.ln_b = ln_b;
+  p.out16 = static_cast<__half*>(out16);
+  p.out32 = out32;
+  p.C = C;
+  p.eps = eps;
+  VLO_CUDA(launch_pdl(vit_fix_ln_kernel, dim3(rows), dim3(256), static_cast<size_t>(C) * sizeof(float), st, p));
+  count_launch();
+  return 0;
+}
+
+int pool_launch(const float* in, float* tokens, int B, int g, int C, int ph, int pw, int n_tok, int tok_off,
+                cudaStream_t st) {
+  const long long total = static_cast<long long>(B) * ph * pw * C;
+  pool_kernel<<<static_cast<int>(std::min<long long>((total + 255) / 256, 2048)), 256, 0, st>>>(in, tokens, B, g, C, ph, pw,
+                                                                                                 n_tok, tok_off);
+  VLO_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+
+int cls_residual_launch(const void* resid, const void* mlp, float* tokens, int B, int C, int n_tok, cudaStream_t st) {
+  cls_residual_kernel<<<(B * C + 255) / 256, 256, 0, st>>>(static_cast<const __half*>(resid), static_cast<const __half*>(mlp),
+                                                           tokens, B, C, n_tok);
+  VLO_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+
+int f32_to_bf16_launch(const float* in, void* out, long long n, cudaStream_t st) {
+  f32_to_bf16_kernel<<<static_cast<int>(std::min<long long>((n + 255) / 256, 2048)), 256, 0, st>>>(in, static_cast<bf16*>(out), n);
+  VLO_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+
 int sample_check_rows(const void* h_rows, int n_rows, int n_ids) {
   VLO_CHECK(h_rows != nullptr, "sample: null rows");
   const SampleRow* rows = static_cast<const SampleRow*>(h_rows);
@@ -1042,14 +1116,10 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   VLO_CHECK(e->n_frame_tokens > 0, "no frame tokens configured");
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const int C = c.vit_hidden, M = c.vit_mlp, P = e->n_patches, rows = B * P;
-  const size_t ln_smem = static_cast<size_t>(C) * sizeof(float);
 
   // K1/K2: normalise + patchify, then patch-embed GEMM with bias + position embedding epilogue
   {
-    const long long total = static_cast<long long>(rows) * e->patch_k / 8;
-    VLO_CUDA(launch_pdl(patchify_kernel, dim3(static_cast<unsigned>(std::min<long long>((total + 255) / 256, 4096))), dim3(256), 0, st,
-                        d_frames, e->patches, B, c.image_size, c.patch_size));
-    count_launch();
+    if (patchify_launch(d_frames, e->patches, B, c.image_size, c.patch_size, st)) return -1;
     GemmCall g{};
     g.epi = EPI_PATCH32;
     g.a = e->patches;
@@ -1074,7 +1144,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   // 97 KB), out_proj and fc2 with 64-token tiles and a 3-stage ring (83 KB).  gemm_vit_kernel gives QKV / fc1 the
   // same bits as 64-token swap-AB tiles would; the stream-K planes keep the 64-token decomposition, whose summation
   // order the frame embeddings depend on.
-  const bool small = B <= 2;
+  const bool small = vit_beside_decoder(B);
   auto tiles_gemm = [&](const __half* x, const __half* w, int n_out, int k, __half* out, const float* bias, int act) -> int {
     if (small) return gemm_vit_launch(x, rows, w, n_out, k, out, n_out, bias, act, 0, st);
     return gemm_ws_store16(FMT_F16, w, n_out, x, rows, k, out, n_out, bias, act, st, WS_TILE_TRUNK);
@@ -1084,27 +1154,10 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
                         small ? WS_TILE_BESIDE_DECODER : WS_TILE_TRUNK, plan, st);
   };
   auto fix_ln = [&](const GemmWsPlan& plan, const float* bias, const float* lw, const float* lb, float* out32) -> int {
-    VitFixLnParams p{};
-    p.part = e->v_part;
-    p.sk = plan.sk;
-    p.sk_bn = plan.bn;
-    p.sk_xtiles = plan.x_tiles;
-    p.split_stride = static_cast<long long>(rows) * C;
-    p.bias = bias;
-    p.h = e->v_h;
-    p.ln_w = lw;
-    p.ln_b = lb;
-    p.out16 = e->v_xn;
-    p.out32 = out32;
-    p.C = C;
-    p.eps = c.vit_ln_eps;
-    VLO_CUDA(launch_pdl(vit_fix_ln_kernel, dim3(rows), dim3(256), ln_smem, st, p));
-    count_launch();
-    return 0;
+    return vit_fix_ln_launch(e->v_part, plan, rows, C, bias, e->v_h, lw, lb, e->v_xn, out32, c.vit_ln_eps, st);
   };
-  VLO_CUDA(launch_pdl(layernorm_kernel<float>, dim3(rows), dim3(256), ln_smem, st, static_cast<const float*>(e->v_h),
-                      e->vit[0].ln1_w, e->vit[0].ln1_b, e->v_xn, static_cast<float*>(nullptr), C, c.vit_ln_eps));
-  count_launch();
+  if (vit_layernorm_launch(e->v_h, false, rows, C, e->vit[0].ln1_w, e->vit[0].ln1_b, e->v_xn, nullptr, c.vit_ln_eps, st))
+    return -1;
   for (int l = 0; l < c.vit_layers; ++l) {
     const VitLayer& v = e->vit[l];
     GemmWsPlan sk{};
@@ -1124,34 +1177,25 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   }
   const int NT = e->n_frame_tokens;
   const int cls = c.frame_token_cls ? 1 : 0;
-  if (c.pool_h * c.pool_w > 0) {
-    const long long total = static_cast<long long>(B) * c.pool_h * c.pool_w * C;
-    pool_kernel<<<static_cast<int>(std::min<long long>((total + 255) / 256, 2048)), 256, 0, st>>>(
-        e->v_ln32, e->tokens32, B, e->grid, C, c.pool_h, c.pool_w, NT, cls);
-    VLO_LAUNCH_CHECK();
-    count_launch();
-  }
+  if (c.pool_h * c.pool_w > 0 && pool_launch(e->v_ln32, e->tokens32, B, e->grid, C, c.pool_h, c.pool_w, NT, cls, st))
+    return -1;
   if (cls) {
     // MAP head: K/V projection of all tokens, 1-query attention, out-proj, LN, MLP, residual
     if (gemm_store16(e->v_xn, rows, e->head_kv_w, 2 * C, C, e->v_qkv, 2 * C, e->head_kv_b, ACT_NONE, st)) return -1;
     if (probe_attn_launch(e->v_qkv, e->head_q, e->v_pa, B, P, C, st)) return -1;
     VLO_CHECK(B <= 128, "MAP head handles <= 128 frames per call");
     if (gemm_ws_store16(FMT_F16, e->head_out_w, C, e->v_pa, B, C, e->v_resid, C, e->head_out_b, ACT_NONE, st)) return -1;
-    layernorm_kernel<__half><<<B, 256, ln_smem, st>>>(e->v_resid, e->head_ln_w, e->head_ln_b, e->v_lnh, nullptr, C, c.vit_ln_eps);
-    VLO_LAUNCH_CHECK();
+    if (vit_layernorm_launch(e->v_resid, true, B, C, e->head_ln_w, e->head_ln_b, e->v_lnh, nullptr, c.vit_ln_eps, st))
+      return -1;
     if (gemm_ws_store16(FMT_F16, e->head_fc1_w, M, e->v_lnh, B, C, e->v_m1, M, e->head_fc1_b, ACT_GELU_TANH, st)) return -1;
     if (gemm_ws_store16(FMT_F16, e->head_fc2_w, C, e->v_m1, B, M, e->v_m2, C, e->head_fc2_b, ACT_NONE, st)) return -1;
-    cls_residual_kernel<<<(B * C + 255) / 256, 256, 0, st>>>(e->v_resid, e->v_m2, e->tokens32, B, C, NT);
-    VLO_LAUNCH_CHECK();
-    count_launch(2);
+    if (cls_residual_launch(e->v_resid, e->v_m2, e->tokens32, B, C, NT, st)) return -1;
   }
   const long long ntok_elems = static_cast<long long>(B) * NT * C;
   if (d_vit_tokens)
     VLO_CUDA(cudaMemcpyAsync(d_vit_tokens, e->tokens32, ntok_elems * sizeof(float), cudaMemcpyDeviceToDevice, st));
   if (d_out) {
-    f32_to_bf16_kernel<<<static_cast<int>(std::min<long long>((ntok_elems + 255) / 256, 2048)), 256, 0, st>>>(e->tokens32, e->tokens16, ntok_elems);
-    VLO_LAUNCH_CHECK();
-    count_launch();
+    if (f32_to_bf16_launch(e->tokens32, e->tokens16, ntok_elems, st)) return -1;
     return vlo_connector(e, e->tokens16, B * NT, d_out, cuda_stream);
   }
   return 0;

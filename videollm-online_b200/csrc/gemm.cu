@@ -115,6 +115,8 @@ int launch_one(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& arg
   return 0;
 }
 
+}  // namespace
+
 // N-tile width of the ViT's one-tile GEMMs: prefer a single wave of CTAs (one CTA per SM); two waves cost 2x.
 int vit_bn(int rows, int n_out) {
   const int mt = (rows + 127) / 128;
@@ -126,8 +128,6 @@ int vit_bn(int rows, int n_out) {
   const double e128 = static_cast<double>(t128) / (((t128 + num_sms() - 1) / num_sms()) * num_sms());
   return e64 > e128 + 0.15 ? 64 : 128;
 }
-
-}  // namespace
 
 int tmap_2d_sw128(const void* ptr, int rows, int k, int box_rows, int fmt, CUtensorMap* out) {
   return get_tmap(ptr, rows, k, box_rows, fmt, out);

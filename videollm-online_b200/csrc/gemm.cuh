@@ -264,6 +264,13 @@ __device__ __forceinline__ uint16_t to16(float x) {
   return __half_as_ushort(__float2half_rn(x));
 }
 
+// MUFU.TANH (PTX ISA: maximum relative error 2^-10.987 over the entire range); vlo_op_tanh_approx exposes it to tests
+__device__ __forceinline__ float tanh_approx(float x) {
+  float y;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
 // Activations evaluated the way the reference evaluates them on 16-bit tensors.
 template <int FMT>
 __device__ __forceinline__ float apply_act(float v, int act) {
@@ -272,8 +279,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     // the 16-bit input, one rounding at the end.
     const float k0 = 0.7978845608028654f, k1 = 0.044715f;
     const float inner = k0 * (v + k1 * v * v * v);
-    float th;
-    asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(inner));  // MUFU.TANH: |err| ~ 2^-11, below fp16 output resolution
+    const float th = tanh_approx(inner);  // |err| ~ 2^-11, below fp16 output resolution
     return r16<FMT>(0.5f * v * (1.0f + th));
   }
   if (act == ACT_GELU_ERF_PY) {

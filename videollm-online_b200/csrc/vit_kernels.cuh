@@ -387,7 +387,7 @@ __global__ void __launch_bounds__(256) pool_kernel(const float* in, float* token
 // ---------------------------------------------------------------------------------------------
 // K7 (part): MAP-head attention of the single learned probe over the N tokens
 // (SiglipMultiheadAttentionPoolingHead, HF:...siglip.py:628-651 -> nn.MultiheadAttention).
-// kv: fp16 [B*N, 2C] (k | v), q: fp32 [C] (= in_proj_q(probe), rounded to fp16 at load).
+// kv: fp16 [B*N, 2C] (k | v), q: fp32 [C] (= in_proj_q(probe), rounded to fp16 on the host by pack_vision_for_engine).
 // grid = (heads, B), block = 128; dynamic smem = N floats.
 __global__ void __launch_bounds__(128) probe_attn_kernel(const __half* kv, const float* q, __half* out, int N, int C,
                                                          float scale) {
