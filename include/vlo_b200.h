@@ -149,7 +149,7 @@ int vlo_kv_evict(vlo_engine* e, int stream_id, int first_token, int n_tokens, co
  * d_i = keep_first[i] - new_first[i].  V rows move unchanged.  K rows move and are rotated by -d_i with the exact formula
  * of vlo_kv_evict, using h_rot[i] = cos[head_dim/2] | sin[head_dim/2] of d_i (weights.rope_rotation), so h_rot holds
  * n_spans * head_dim fp32 values.  Rows with d_i = 0 are not touched.  The new kv_len is sum(keep_len).  Pages past
- * ceil(new_len / 64) go back to the pool; the rows past the new kv_len on the last page keep old, finite values.
+ * ceil(new_len / 64) go back to the pool; the rows past the new kv_len on the last page keep their old values.
  * The rows move in place, page by page in increasing order, through the decoder step's partial-sum workspace: the call
  * takes no free page and no device memory, and works on a full pool.  Because it uses that workspace it is ordered
  * like a step: enqueue it on the CUDA stream the engine's steps run on.  The tables go through one slot of the pinned
@@ -167,8 +167,8 @@ int vlo_kv_write(vlo_engine* e, int stream_id, int layer, int is_v, const void* 
 /* Host images of a stream's cache, so an idle session can give its pages (and stream slot) back and resume later.
  * Image layout: [page j][layer][K|V][kv_head][64][128] bf16, pages in page-table order; page_bytes = n_kv_heads * 64 *
  * 128 * 2 (131 072 B for Llama-3-8B).  vlo_kv_image_bytes = ceil(n_tokens / 64) * 2 * num_layers * page_bytes.
- * The last page of an image also carries that page's rows past n_tokens: stale but finite pool rows, so the pool's
- * finiteness invariant (csrc/kv_pages.h) survives a round trip.
+ * The last page of an image also carries that page's rows past n_tokens: stale pool rows.  They are masked rows of the
+ * attention and may hold anything, non-finite values included.
  * vlo_kv_swap_out: enqueues on cuda_stream one cudaMemcpy2DAsync per page (2 * num_layers rows of page_bytes at the
  * pool's plane stride; copy engines only, no kernel) into h_dst (pinned host memory of >= vlo_kv_image_bytes(kv_len)
  * bytes), then empties the stream: kv_len 0, pages released, slot still open.  The caller orders the copies after the
@@ -329,13 +329,16 @@ int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, in
  *   d_q bf16 [n_tok, n_heads, head_dim] (RoPE applied); d_k/d_v bf16 [n_kv_heads, kv_stride, head_dim];
  *   keys 0..kv_len-1 valid, the n_tok query tokens sit at positions kv_len-n_tok .. kv_len-1 (causal with
  *   offset, HF:masking_utils.py:263-272); d_out bf16 [n_tok, n_heads*head_dim]; d_ws fp32 scratch of
- *   vlo_op_attn_ws_bytes(). Replaces HF:models/llama/modeling_llama.py:272-285 (SDPA / flash-attn 2). */
+ *   vlo_op_attn_ws_bytes(). Replaces HF:models/llama/modeling_llama.py:272-285 (SDPA / flash-attn 2).
+ *   Rows kv_len .. kv_stride - 1 are masked and may hold anything, NaN and Inf included.  The n_tok new rows must be
+ *   finite: a row multiplies the V rows of the later new tokens of its work item by P = 0 (DESIGN §3). */
 int64_t vlo_op_attn_ws_bytes(int n_tok, int n_heads, int head_dim, int kv_len);
 int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void* d_out, float* d_ws, int n_tok,
                          int n_heads, int n_kv_heads, int head_dim, int kv_len, long long kv_stride, void* cuda_stream);
 /* kernel-level: the decoder attention over a paged pool [n_pages, n_kv_heads, 64, 128] (tests).  d_page_table: device
  * int32 [ceil(kv_len / 64)], the page of each 64-key block; other arguments as vlo_op_attn_kvappend.  Rows of the last
- * page past kv_len must be finite. */
+ * page past kv_len are masked: they may hold anything, NaN and Inf included.  The new rows must be finite, as for
+ * vlo_op_attn_kvappend. */
 int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
                                int n_pages, void* d_out, float* d_ws, int n_tok, int n_heads, int n_kv_heads,
                                int head_dim, int kv_len, void* cuda_stream);
@@ -344,7 +347,8 @@ int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void
  * kv_len - 1 of d_q [n_tok, n_heads, head_dim]; row r attends causally to keys 0..(its position).  Segment j (rows
  * o_j .. o_j + len_j - 1, ending at key e_j = kv_len - n_tok + o_j + len_j) gets in d_out exactly the bits
  * vlo_op_attn_kvappend_paged gives its rows alone with kv_len = e_j on the same pool.  n_segs = 1 is that call.
- * Keys past a row's position are masked: they may hold any finite values.  Scratch is allocated internally;
+ * Keys past a row's position are masked.  Rows past kv_len may hold anything, NaN and Inf included; the new rows must
+ * be finite, since a row multiplies the V rows of the later tokens of its work item or packed run by P = 0 (DESIGN §3).  Scratch is allocated internally;
  * synchronous. */
 int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const void* d_v_pool, const int32_t* d_page_table,
                                   int n_pages, void* d_out, int n_segs, const int32_t* h_seg_lens, int n_heads,

@@ -322,16 +322,14 @@ def engines():
 
 class _Kv:
     """one layer's K or V cache of the replayed sequence: contiguous [n_kv][cap][128] (vlo_op_attn_kvappend's layout) or
-    64-token pages [cap / 64][n_kv][64][128] under an identity page table (vlo_op_attn_kvappend_segments').
-
-    Rows past the cached ones start at zero, not at a NaN sentinel: the attention loads whole 64-key blocks and
-    multiplies the V rows past kv_len by probabilities of exactly 0, so their values drop out only while they are
-    finite.  A row the replayed append fails to write still differs from the engine's."""
+    64-token pages [cap / 64][n_kv][64][128] under an identity page table (vlo_op_attn_kvappend_segments').  Rows past
+    the cached ones start at a NaN sentinel: the attention must not see the rows past kv_len it loads, and a row the
+    replayed append fails to write stays NaN."""
 
     def __init__(self, rows, cap, paged):
         nkv, n, hd = rows.shape
         self.nkv, self.cap, self.paged = nkv, cap, paged
-        c = torch.zeros(nkv, cap, hd, dtype=torch.bfloat16, device="cuda")
+        c = torch.full((nkv, cap, hd), float("nan"), dtype=torch.bfloat16, device="cuda")
         c[:, :n] = rows
         self.buf = c.view(nkv, cap // 64, 64, hd).permute(1, 0, 2, 3).contiguous() if paged else c
 

@@ -31,8 +31,8 @@ def _st():
 @pytest.mark.parametrize("kv_len,n_tok,G", [(kv, n, g) for kv in (1, 63, 64, 65, 12011, 66011) for n in (1, 11, 40)
                                              for g in (2, 4) if n <= kv] + [(66011, 272, 4)])
 def test_paged_attention_op_matches_contiguous(lib, kv_len, n_tok, G):
-    """scattered pages in an oversized pool whose unused pages hold NaN and whose last page has finite garbage past
-    kv_len: bit-identical to the contiguous op on the same logical K / V.  272 queries at G = 4 are 17 work items: with
+    """scattered pages in an oversized pool whose unused pages hold NaN and whose last page has garbage past kv_len
+    (+-Inf, NaN and values ~100): bit-identical to the contiguous op on the same logical K / V.  272 queries at G = 4 are 17 work items: with
     8 kv heads the plan gets one split per item, so one CTA walks all 1032 key blocks."""
     from videollm_online_b200._lib import check
     torch.manual_seed(kv_len * 7 + n_tok * 3 + G)
@@ -50,9 +50,11 @@ def test_paged_attention_op_matches_contiguous(lib, kv_len, n_tok, G):
     kp[perm] = k.view(Hk, nblk, PAGE, D).transpose(0, 1)
     vp[perm] = v.view(Hk, nblk, PAGE, D).transpose(0, 1)
     tail = kv_len - (nblk - 1) * PAGE
-    if tail < PAGE:   # rows past kv_len in the last page: finite, but not what the contiguous cache holds
-        kp[perm[-1], :, tail:] = (torch.randn(Hk, PAGE - tail, D, device="cuda") * 100).bfloat16()
-        vp[perm[-1], :, tail:] = (torch.randn(Hk, PAGE - tail, D, device="cuda") * 100).bfloat16()
+    if tail < PAGE:   # rows past kv_len in the last page: not what the contiguous cache holds, some not finite
+        for pool in (kp, vp):
+            junk = torch.randn(Hk, PAGE - tail, D, device="cuda") * 100
+            junk[:, 0::4, 0::3], junk[:, 1::4, 1::3], junk[:, 2::4] = float("inf"), float("-inf"), float("nan")
+            pool[perm[-1], :, tail:] = junk.bfloat16()
     pt = perm.to(torch.int32).contiguous()
     ws = torch.empty(lib.vlo_op_attn_ws_bytes(n_tok, H, D, kv_len), device="cuda", dtype=torch.uint8)
     out_c = torch.empty(n_tok, H * D, device="cuda", dtype=torch.bfloat16)

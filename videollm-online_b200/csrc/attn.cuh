@@ -268,6 +268,23 @@ __device__ __forceinline__ void attn_kvappend_cta(const CUtensorMap& tm_k, const
         o_acc[nd][2] *= al1;
         o_acc[nd][3] *= al1;
       }
+      // The block that holds kv_end loads rows past it: stale rows of a reused page or this stream's rows left past a
+      // truncate, evict or compact.  Their P is exactly 0, but 0 * Inf and 0 * NaN are NaN, so the group's warps zero
+      // those V rows in the stage before the P V product reads it.  A finite row's 0 * v adds nothing, so the bits stay
+      // those of the unmasked product; every other block skips this branch (the test is block-uniform).
+      if (key0 + kAttnBlk > kv_end) {
+        uint8_t* vst = smem + (grp * kAttnStages + s) * kAttnStageBytes + 2 * kAttnSubTile;
+        const int first = kv_end - key0;  // rows first .. 63 of both 64-dim halves: 16 chunks of 16 B per row
+        for (int c = mt * 32 + lane; c < (kAttnBlk - first) * 16; c += mt_active * 32) {
+          const int row = first + (c >> 4), ch = c & 15;
+          *reinterpret_cast<uint4*>(vst + (ch >> 3) * kAttnSubTile + row * 128 + (ch & 7) * 16) = make_uint4(0, 0, 0, 0);
+        }
+        fence_proxy_async();                       // the stage's next TMA fill is ordered after these stores
+        if (grp == 0)                              // every warp of the group sees the whole cleared tail
+          named_bar_sync<1>(mt_active * 32);
+        else
+          named_bar_sync<2>(mt_active * 32);
+      }
       // O += P V   (16 x 128), V tile rows = keys, transposed ldmatrix
       const uint32_t sv = st + 2 * kAttnSubTile;
 #pragma unroll

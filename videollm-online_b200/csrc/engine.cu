@@ -577,8 +577,8 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   const vlo_config& c = e->cfg;
   const int T = c.max_step_tokens;
   const int H = c.hidden_size;
-  // KV cache: a pool of 64-token pages shared by all streams, zero-initialised once.  Attention reads (masked) rows
-  // past kv_len inside a stream's last page; they must be finite.
+  // KV cache: a pool of 64-token pages shared by all streams, zero-initialised once.  Attention loads (masked) rows
+  // past kv_len inside a stream's last page; they may hold anything.
   const int per_stream = kv_pages_for(c.max_kv_tokens);
   const int64_t pages = kv_pool_tokens > 0 ? (kv_pool_tokens + kKvPageTokens - 1) / kKvPageTokens
                                            : static_cast<int64_t>(c.max_streams) * per_stream;

@@ -8,10 +8,11 @@
 // Between calls a stream holds exactly ceil(len / 64) pages.  A call that adds rows takes the pages (grow), enqueues
 // the work that writes them, then sets the length (commit); a call that fails first gives the pages back (rollback).
 //
-// A page handed out may hold stale rows from an earlier owner; they are finite (the pool is zero-filled once, and only
-// finite K / V rows are ever written), which is what a masked key of the attention needs (it contributes 0 x V).  A
-// host image of a stream (vlo_kv_swap_out / vlo_kv_swap_in) moves whole pages, so a swapped-in last page carries the
-// rows past kv_len that it had in the pool: finite as well.
+// A page handed out may hold stale rows from an earlier owner, and a stream's last page keeps whatever its rows past
+// kv_len held before a truncate, evict or compact.  Masked rows may hold anything, NaN and Inf included: the attention
+// masks their scores and zeroes their V rows in the shared-memory stage (csrc/attn.cuh).  A host image of a stream
+// (vlo_kv_swap_out / vlo_kv_swap_in) moves whole pages, so a swapped-in last page carries the rows past kv_len that it
+// had in the pool, or whatever the image holds there.
 #pragma once
 #include <algorithm>
 #include <string>

@@ -31,6 +31,11 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
 }
+// bar.sync on named barrier kId (1 .. 15; 0 is __syncthreads) for `n` threads (a multiple of 32)
+template <int kId>
+__device__ __forceinline__ void named_bar_sync(int n) {
+  asm volatile("bar.sync %0, %1;\n" ::"n"(kId), "r"(n) : "memory");
+}
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }

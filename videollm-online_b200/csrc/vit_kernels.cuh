@@ -328,6 +328,17 @@ vit_attn_kernel(const __grid_constant__ CUtensorMap tm_qkv, __half* out, int N, 
       o_acc[nd][2] *= al1;
       o_acc[nd][3] *= al1;
     }
+    // keys >= N of the last block are the next frame's first rows (or the TMA zero fill past the last frame): P is 0
+    // there, but 0 * Inf and 0 * NaN are NaN, so the 4 MMA warps zero those V rows in the stage before the P V product
+    // reads it.  A finite row's 0 * v adds nothing, so the bits stay those of the unmasked product.
+    if (key0 + kVitBlk > N) {
+      uint8_t* vst = kv_tiles + s * 2 * kVitTile + kVitTile;
+      const int first = N - key0;  // rows first .. 63: 8 chunks of 16 B per row
+      for (int c = mt * 32 + lane; c < (kVitBlk - first) * 8; c += 4 * 32)
+        *reinterpret_cast<uint4*>(vst + (first + (c >> 3)) * 128 + (c & 7) * 16) = make_uint4(0, 0, 0, 0);
+      fence_proxy_async();    // the stage's next TMA fill is ordered after these stores
+      named_bar_sync<1>(4 * 32);  // the 4 MMA warps
+    }
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       const int vrow = kk * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
