@@ -42,8 +42,11 @@ def lib():
 @pytest.fixture(scope="module", autouse=True)
 def _scrub_poisoned_memory():
     """the caching allocator would hand the memory these tests filled with NaN and Inf to later tests: give it back to
-    the driver zeroed.  test_gpu_vit_kernels.py::test_tower_replay_bit_exact[11] chains the tower from torch.empty
-    buffers, and once lost its run-to-run repeatability after this module; which kernel reads there is not known."""
+    the driver zeroed, so that a later test's torch.empty buffers start clean.  Once, after this module,
+    test_gpu_vit_kernels.py::test_tower_replay_bit_exact[11] did not repeat its bits; the record does not say whether
+    vit_encode or the replay changed.  The replay's own stages read only what they wrote:
+    test_gpu_ordering.py::test_tower_replay_reads_only_what_it_wrote runs it over NaN- and pattern-filled buffers with
+    poisoned tails at every frame batch.  The engine's ViT workspaces inside vit_encode are not covered by that test."""
     yield
     torch.cuda.synchronize()
     free = torch.cuda.memory_reserved() - torch.cuda.memory_allocated()
