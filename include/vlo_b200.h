@@ -193,6 +193,30 @@ int vlo_kv_swap_in(vlo_engine* e, int stream_id, const void* h_src, int n_tokens
  * pre-connector tokens (what build_live_vision's encode_fn returns). */
 int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int n_frames, void* d_out, float* d_vit_tokens,
                    void* cuda_stream);
+/* vlo_letterbox replaces the host preprocessing of a clip: ffmpeg_once's `scale` + `pad` to image x image (data/utils.py:51-66,
+ * called from demo/cli.py:15-20), which video_ingest.read_video_resampled applies with OpenCV's INTER_CUBIC.  It turns
+ * n_frames native frames, each of its own size, into the canvases vlo_vit_encode reads: d_out uint8
+ * [n_frames, 3, image, image], RGB.  One descriptor per frame (host array, passed to the kernel by value):
+ *   d_pixels   uint8 [height][width][3], packed, RGB or BGR (bgr != 0);
+ *   1 <= width, height <= 8192;
+ *   d_taps     int32 tap tables (16-byte aligned): the horizontal table starts at row x_taps, the vertical one at row
+ *              y_taps; a row is {i0, i1, i2, i3, w0, w1, w2, w3}, one per output column (sw rows) / line (sh rows).
+ * Geometry: (sw, sh, x0, y0) = video_ingest.letterbox_geometry(width, height, image); every byte outside the scaled image
+ * is 0 and every byte of the canvas is written.  The scaled pixel (dx, dy), channel c, is
+ *   h_k = sum_j src[iy_k][ix_j][c] * wx_j   (int32; i = the row's indices clamped to the image, w = its weights)
+ *   v   = sum_k h_k * wy_k                  (int32)
+ *   out = clamp((v + 2^21) >> 22, 0, 255)
+ * which is OpenCV's fixed-point INTER_CUBIC when the tables are video_ingest.cubic_taps (11-bit weights of A = -0.75).
+ * Checks null pointers, sizes, n_frames <= max_vit_batch, the table alignment and that bgr is 0 or 1; one launch per 64
+ * frames, asynchronous, ordered behind the previous work on cuda_stream (the canvas may still be read by it). */
+typedef struct vlo_letterbox_frame {
+  const uint8_t* d_pixels;
+  const int32_t* d_taps;
+  int32_t width, height, bgr;
+  int32_t x_taps, y_taps;
+  int32_t reserved;
+} vlo_letterbox_frame;
+int vlo_letterbox(vlo_engine* e, const vlo_letterbox_frame* h_frames, int n_frames, uint8_t* d_out, void* cuda_stream);
 /* connector only: visual_embed without a vision tower (models/modeling_live.py:22-27 with
  * pre-extracted features). d_tokens: bf16 [n_rows, vit_hidden] */
 int vlo_connector(vlo_engine* e, const void* d_tokens, int n_rows, void* d_out, void* cuda_stream);

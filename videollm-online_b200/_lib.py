@@ -48,6 +48,13 @@ class VloSampleRow(C.Structure):
     ]
 
 
+class VloLetterboxFrame(C.Structure):
+    _fields_ = [
+        ("d_pixels", C.c_void_p), ("d_taps", C.c_void_p), ("width", C.c_int32), ("height", C.c_int32),
+        ("bgr", C.c_int32), ("x_taps", C.c_int32), ("y_taps", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _LL = C.c_longlong
@@ -82,6 +89,7 @@ SIGNATURES = {
     "vlo_kv_swap_out": (_I, [_P, _I, _P, C.c_int64, _P]),
     "vlo_kv_swap_in": (_I, [_P, _I, _P, _I, _P]),
     "vlo_vit_encode": (_I, [_P, _P, _I, _P, _P, _P]),
+    "vlo_letterbox": (_I, [_P, C.POINTER(VloLetterboxFrame), _I, _P, _P]),
     "vlo_connector": (_I, [_P, _P, _I, _P, _P]),
     "vlo_embed_tokens": (_I, [_P, _P, _I, _P, _P]),
     "vlo_step": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _I, _P]),

@@ -1,13 +1,16 @@
 """Headless driver + FPS measurement: the engine-backed counterpart of demo/cli.py:12-50.
 
     python -m videollm_online_b200.cli --synthetic_weights true [--frames 100] [--video clip.mp4] [--whole_video]
-        [--do_sample --temperature 0.6 --top_p 0.9 --top_k 50 --repetition_penalty 1.1 --sample_seed 0]
+        [--live] [--do_sample --temperature 0.6 --top_p 0.9 --top_k 50 --repetition_penalty 1.1 --sample_seed 0]
 
 Responses are greedy unless --do_sample is given (SamplingConfig; --seed stays the synthetic weights' seed).
 --context_window N keeps the session's cache within N tokens (0: off): the start prompt stays, the oldest pages after it
 are dropped.
 --context_keep_turns (with --context_window) drops the oldest frames token by token instead, and keeps the questions and
 answers.
+--live (with --video) feeds the clip as a camera would: decoded at its native size without a resize, one frame per
+1 / frame_fps of video time pushed through LiveInfer.push_frames (BGR, letterboxed on the device), each one frame ahead
+of the frame being processed.
 --fp8_weights serves the decoder layers from e4m3 weights with per-row scales (half their bytes per step; the model's
 numbers change, so it is off by default).
 --fp8_activations (with --fp8_weights) also quantizes the layer GEMMs' activations to e4m3 per token and multiplies them on
@@ -35,17 +38,34 @@ def synthetic_clip(n_frames: int, resolution: int, seed: int = 0) -> torch.Tenso
 
 
 def main(liveinfer: LiveInfer, video=None, n_iters: int = 100, save_history_path: str = None, quiet: bool = False,
-         whole_video: bool = False):
-    if video is None:
-        video = synthetic_clip(n_iters, liveinfer.frame_resolution)
-    liveinfer.load_video(video)
+         whole_video: bool = False, live: bool = False):
+    camera = None
+    if live:
+        if not isinstance(video, str) or whole_video:
+            raise ValueError("--live takes a clip on disk (--video) and does not combine with --whole_video")
+        from .video_ingest import iter_video_frames
+        camera = iter_video_frames(video, fps=liveinfer.frame_fps)
+    else:
+        if video is None:
+            video = synthetic_clip(n_iters, liveinfer.frame_resolution)
+        liveinfer.load_video(video)
     liveinfer.input_query_stream('Please narrate the video in real time.', video_time=0.0)
     timecosts, history = [], {'frame_fps': liveinfer.frame_fps, 'conversation': []}
     fps = 0.0
     if whole_video:
         return _drain_whole_video(liveinfer, min(n_iters, liveinfer.num_video_frames), history, save_history_path, quiet)
-    for i in range(min(n_iters, liveinfer.num_video_frames)):
+    frame = next(camera, None) if live else None   # the camera frame of video time i / frame_fps
+    for i in range(n_iters if live else min(n_iters, liveinfer.num_video_frames)):
+        if live and frame is None:
+            break
         start = time.time()
+        if live:
+            # frame i + 1 is delivered while frame i is processed, so encode-ahead takes it as it takes a loaded clip's
+            if i == 0:
+                liveinfer.push_frames([torch.from_numpy(frame)], bgr=True)
+            frame = next(camera, None)
+            if frame is not None and i + 1 < n_iters:
+                liveinfer.push_frames([torch.from_numpy(frame)], bgr=True)
         liveinfer.input_video_stream(i / liveinfer.frame_fps)
         query, response = liveinfer()
         timecosts.append(time.time() - start)
@@ -98,4 +118,5 @@ if __name__ == '__main__':
     if '--video' in sys.argv:   # a clip on disk: resampled to frame_fps and letterboxed to frame_resolution on load
         video = sys.argv[sys.argv.index('--video') + 1]
     # --whole_video: queue the whole clip at t = 0 and drain it (narrate a recorded file as fast as possible)
-    main(LiveInfer(parse_args()), video=video, n_iters=n, whole_video='--whole_video' in sys.argv)
+    # --live: push the clip's frames at their native size, one per frame interval (a camera feed)
+    main(LiveInfer(parse_args()), video=video, n_iters=n, whole_video='--whole_video' in sys.argv, live='--live' in sys.argv)

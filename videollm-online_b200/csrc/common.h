@@ -7,6 +7,8 @@
 
 #include "streamk.h"
 
+struct vlo_letterbox_frame;  // include/vlo_b200.h
+
 namespace vlo {
 
 // ---- error plumbing: every C-ABI entry returns 0 / negative and leaves a message here.
@@ -212,6 +214,12 @@ int pool_launch(const float* in, float* tokens, int B, int g, int C, int ph, int
 int cls_residual_launch(const void* resid, const void* mlp, float* tokens, int B, int C, int n_tok, cudaStream_t st);
 // f32_to_bf16_kernel: out[i] = bf16(in[i]), i < n
 int f32_to_bf16_launch(const float* in, void* out, long long n, cudaStream_t st);
+
+// ---- letterbox (letterbox.cu) ---------------------------------------------------------
+// letterbox_kernel: the frames of vlo_letterbox (include/vlo_b200.h) -> uint8 out [n, 3, R, R]; checks each descriptor,
+// then one launch per kLetterboxMaxFrames frames (their descriptors travel as kernel parameters)
+constexpr int kLetterboxMaxFrames = 64;
+int letterbox_launch(const vlo_letterbox_frame* frames, int n, int R, uint8_t* out, cudaStream_t st);
 
 // ---- attention (attn.cu) ------------------------------------------------------------
 struct AttnSeq {

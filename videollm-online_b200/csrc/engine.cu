@@ -1201,6 +1201,13 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
   return 0;
 }
 
+int vlo_letterbox(vlo_engine* e, const vlo_letterbox_frame* h_frames, int n_frames, uint8_t* d_out, void* cuda_stream) {
+  DevGuard dev_guard(e);
+  VLO_CHECK(e != nullptr, "null engine");
+  VLO_CHECK(n_frames > 0 && n_frames <= e->cfg.max_vit_batch, "letterbox: n_frames must lie in [1, max_vit_batch]");
+  return letterbox_launch(h_frames, n_frames, e->cfg.image_size, d_out, static_cast<cudaStream_t>(cuda_stream));
+}
+
 // ------------------------------------------------------------------------------ decoder
 int vlo_embed_tokens(vlo_engine* e, const int64_t* d_ids, int n, void* d_out, void* cuda_stream) {
   DevGuard dev_guard(e);

@@ -284,6 +284,8 @@ class Engine:
         # pinned image buffers a swap copy may still write or read: kept alive until their event has completed, so the
         # caching host allocator cannot hand them to someone else under a copy
         self._swap_inflight: List[tuple] = []
+        self._taps: Dict[tuple, tuple] = {}             # (W, H) -> letterbox tap tables on the device (letterbox)
+        self._frame_staging: List[tuple] = []          # (pinned buffer, event after the copy out of it) (letterbox)
 
     # ------------------------------------------------------------------ life cycle
     def close(self):
@@ -492,6 +494,78 @@ class Engine:
         if return_vit_tokens:
             return out, torch.cat(toks, 0)
         return out
+
+    def letterbox(self, frames: Sequence[torch.Tensor], bgr: bool = False) -> torch.Tensor:
+        """Native frames -> uint8 [B, 3, R, R] RGB canvases (R = frame_resolution), what vit_encode takes: each frame is
+        scaled into the square with the integer INTER_CUBIC of video_ingest.cubic_taps and centred on black bars
+        (video_ingest.letterbox_geometry), on the device (vlo_letterbox, current CUDA stream).  frames: HWC uint8 tensors
+        with 3 channels (RGB, or BGR with bgr=True), each of its own size up to 8192 x 8192, on the CPU or this device.
+        CPU frames are staged through pinned buffers and copied asynchronously; a buffer is reused only once the copy
+        out of it has completed.  Raises VloError on a frame of another dtype, shape, device or size."""
+        from .video_ingest import MAX_FRAME_SIDE
+        frames = list(frames)
+        if not frames:
+            raise VloError("letterbox: no frames")
+        R = self.cfg.frame_resolution
+        out = torch.empty(len(frames), 3, R, R, dtype=torch.uint8, device=self.device)
+        descs = (_lib.VloLetterboxFrame * len(frames))()
+        held = []   # device frames and tap tables: alive until every launch is enqueued (stream-ordered reuse after it)
+        for d, f in zip(descs, frames):
+            if not isinstance(f, torch.Tensor) or f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+                raise VloError(f"letterbox: frames must be uint8 HWC tensors with 3 channels, got "
+                               f"{getattr(f, 'dtype', type(f))} {tuple(getattr(f, 'shape', ()))}")
+            H, W = int(f.shape[0]), int(f.shape[1])
+            if not (1 <= W <= MAX_FRAME_SIDE and 1 <= H <= MAX_FRAME_SIDE):
+                raise VloError(f"letterbox: a {W} x {H} frame; both sides must lie in [1, {MAX_FRAME_SIDE}]")
+            taps, sw = self._letterbox_taps(W, H)
+            dev = self._frame_on_device(f)
+            held += [dev, taps]
+            d.d_pixels, d.d_taps, d.width, d.height = dev.data_ptr(), taps.data_ptr(), W, H
+            d.bgr, d.x_taps, d.y_taps = int(bool(bgr)), 0, sw
+        size = C.sizeof(_lib.VloLetterboxFrame)
+        for b0 in range(0, len(frames), self.max_vit_batch):
+            n = min(self.max_vit_batch, len(frames) - b0)
+            check(self.lib.vlo_letterbox(self._h, C.cast(C.addressof(descs) + b0 * size, C.POINTER(_lib.VloLetterboxFrame)),
+                                         n, _ptr(out[b0:]), self._stream()), "vlo_letterbox")
+        return out
+
+    def _letterbox_taps(self, W: int, H: int):
+        """(device int32 tap tables of a W x H frame, rows of the horizontal table), built once per size"""
+        hit = self._taps.get((W, H))
+        if hit is None:
+            from .video_ingest import letterbox_geometry, letterbox_taps
+            sw = letterbox_geometry(W, H, self.cfg.frame_resolution)[0]
+            taps = torch.from_numpy(letterbox_taps(W, H, self.cfg.frame_resolution)).to(self.device)
+            # once per frame size: the upload has landed before any stream reads the table; tables are never freed, so no
+            # stream can read one after its memory is reused (a table is at most 768 rows of 32 bytes)
+            torch.cuda.current_stream(self.device).synchronize()
+            hit = self._taps[(W, H)] = (taps, sw)
+        return hit
+
+    def _frame_on_device(self, f: torch.Tensor) -> torch.Tensor:
+        if f.device.type == "cuda":
+            if f.device != self.device:
+                raise VloError(f"letterbox: a frame on {f.device}, the engine runs on {self.device}")
+            return f.contiguous()
+        n = f.numel()
+        pool = self._frame_staging
+        # Idle buffers (their copy has completed) more than 4x this frame go, and so do the largest idle ones beyond
+        # max_vit_batch: after a burst of large frames the pool shrinks to the frames now pushed.  Buffers under a copy
+        # stay until their event has completed.
+        idle = [i for i, (b, ev) in enumerate(pool) if ev.query()]
+        drop = {i for i in idle if pool[i][0].numel() > 4 * n}
+        keep = sorted((i for i in idle if i not in drop), key=lambda i: pool[i][0].numel())
+        drop |= set(keep[self.max_vit_batch:])
+        fit = next((i for i in keep[:self.max_vit_batch] if pool[i][0].numel() >= n), None)   # the smallest that fits
+        buf = pool[fit][0] if fit is not None else torch.empty(n, dtype=torch.uint8, pin_memory=True)
+        self._frame_staging = pool = [e for i, e in enumerate(pool) if i not in drop and i != fit]
+        buf[:n].copy_(f.reshape(-1))
+        dev = torch.empty(n, dtype=torch.uint8, device=self.device)
+        dev.copy_(buf[:n], non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.device))
+        pool.append((buf, ev))
+        return dev.view(f.shape)
 
     def connector(self, tokens: torch.Tensor) -> torch.Tensor:
         tokens = tokens.to(device=self.device, dtype=torch.bfloat16).contiguous().view(-1, self.cfg.vision_hidden_size)

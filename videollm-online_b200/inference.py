@@ -28,6 +28,7 @@ from .config import LiveArguments, SamplingConfig, parse_args
 from .engine import KvImage, check_context_window, check_context_window_turns, kept_rows, sink_tokens
 from .modeling_live import LiveLlamaForCausalLM, StreamKV, build_model_and_tokenizer, fast_greedy_generate
 from .speculative import SEP, NgramDrafter, generate_ids
+from .video_ingest import FrameRing
 
 logger = logging.getLogger("liveinfer")
 
@@ -300,6 +301,23 @@ class LiveInfer:
         logger.warning(f'{"tensor" if isinstance(video_path_or_tensor, torch.Tensor) else video_path_or_tensor} -> '
                        f'{tuple(self.video_tensor.shape)}, {self.frame_fps} FPS')
 
+    def push_frames(self, frames, bgr: bool = False):
+        """Append live frames to the session's video at frame_fps: frame i of the session is the i-th frame pushed since
+        the last reset (counted on from the last frame input_video_stream reached, after a resume), so a camera feeds
+        input_video_stream(t) as a loaded clip does.  frames: HWC uint8 tensors at their native sizes (RGB, or BGR with
+        bgr=True; CPU or CUDA); they are copied and letterboxed to frame_resolution on the encode-ahead stream
+        (Engine.letterbox) and held until encoded (video_ingest.FrameRing).  A session plays one source at a time: after
+        load_video, reset() before pushing frames (ValueError otherwise); reset and load_video drop the pushed frames."""
+        with self._lock:
+            ring = self.video_tensor
+            if ring is None:
+                ring = self.video_tensor = FrameRing(self.model.engine, self._side, first=self.last_frame_idx + 1)
+            elif not isinstance(ring, FrameRing):
+                raise ValueError("push_frames: the session plays a loaded clip; reset() it before pushing frames")
+            ring.push(frames, bgr=bgr)
+            self.num_video_frames = ring.size(0)
+            self.video_duration = ring.size(0) / self.frame_fps
+
     def input_query_stream(self, query, history=None, video_time=None):
         self.query_queue.append((self.video_time if video_time is None else video_time, query))
         if not self.past_key_values:
@@ -312,6 +330,8 @@ class LiveInfer:
 
     def _input_video_stream(self, video_time):
         frame_idx = int(video_time * self.frame_fps)
+        if frame_idx > self.last_frame_idx and isinstance(self.video_tensor, FrameRing):
+            self.video_tensor.check_pushed(frame_idx)   # a camera frame not delivered yet: nothing changes, retry later
         if frame_idx > self.last_frame_idx:
             ranger = range(self.last_frame_idx + 1, frame_idx + 1)
             main = torch.cuda.current_stream(self.device)

@@ -35,6 +35,7 @@ from .config import SamplingConfig
 from .engine import KvImage, SampleRow, evict_span, kept_rows, retain_spans
 from .modeling_live import LiveLlamaForCausalLM
 from .speculative import sample_rows
+from .video_ingest import FrameRing
 
 
 class StreamSession:
@@ -95,8 +96,19 @@ class StreamSession:
         self.video = video_u8.to(self.sched.model.device)
         getattr(self.sched, "_ahead", {}).pop(self.index, None)
 
+    def push_frames(self, frames, bgr: bool = False):
+        """As LiveInfer.push_frames: append live frames at their native sizes to the session's video, letterboxed on the
+        scheduler's encode-ahead stream.  After load_video, reset() before pushing frames (ValueError otherwise)."""
+        if self.video is None:
+            self.video = FrameRing(self.sched.model.engine, self.sched._side, first=self.last_frame_idx + 1)
+        elif not isinstance(self.video, FrameRing):
+            raise ValueError("push_frames: the session plays a loaded clip; reset() it before pushing frames")
+        self.video.push(frames, bgr=bgr)
+
     def input_video_stream(self, video_time: float):
         idx = int(video_time * self.frame_fps)
+        if idx > self.last_frame_idx and isinstance(self.video, FrameRing):
+            self.video.check_pushed(idx)   # before a frame that is not there becomes pending: nothing changes
         if idx > self.last_frame_idx:
             for r in range(self.last_frame_idx + 1, idx + 1):
                 self.pending_frames.append((r / self.frame_fps, r))

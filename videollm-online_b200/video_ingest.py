@@ -13,13 +13,23 @@ same geometry and sampling rule are applied here in one pass with OpenCV:
     square ((ow-iw)/2, (oh-ih)/2 rounded down).
 
 Not bit-identical to libswscale's bicubic taps (documented; the frames then go through the same uint8 -> ViT path).
-Host-side only: returns a uint8 [T, 3, R, R] CPU tensor in RGB that `LiveInfer.load_video` moves to the GPU.
+`read_video_resampled` runs on the host: it returns a uint8 [T, 3, R, R] CPU tensor in RGB that `LiveInfer.load_video`
+moves to the GPU.
+
+Live frames (`push_frames`) are letterboxed on the device instead (`Engine.letterbox`, vlo_letterbox): `cubic_taps` builds
+the integer INTER_CUBIC tap tables the kernel reads, and `FrameRing` holds a session's pushed frames until they are
+encoded.
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+import collections
+from typing import Iterator, Optional, Tuple
 
+import numpy as np
 import torch
+
+MAX_FRAME_SIDE = 8192   # widest / tallest native frame vlo_letterbox takes
+TAP_BITS = 11           # integer tap weights are round(w * 2^11), OpenCV's INTER_RESIZE_COEF_BITS
 
 
 def letterbox_geometry(width: int, height: int, resolution: int) -> Tuple[int, int, int, int]:
@@ -34,6 +44,135 @@ def letterbox_geometry(width: int, height: int, resolution: int) -> Tuple[int, i
     return sw, sh, (resolution - sw) // 2, (resolution - sh) // 2
 
 
+def cubic_taps(n_in: int, n_out: int) -> np.ndarray:
+    """int32 [n_out, 8] tap table of one axis for vlo_letterbox: per output coordinate d the source indices
+    clamp(s - 1 + k, 0, n_in - 1) then the weights round_half_even(w_k * 2048), k = 0..3, with
+      f = fp32((d + 0.5) * (n_in / n_out) - 0.5)   (in fp64, rounded once),  s = floor(f),  t = f - s   (fp32)
+    and OpenCV's cubic weights of A = -0.75, every operation rounded in fp32:
+      w0 = ((A(t+1) - 5A)(t+1) + 8A)(t+1) - 4A,  w1 = ((A+2)t - (A+3))t t + 1,  w2 = w1 at 1 - t,  w3 = 1 - w0 - w1 - w2.
+    Raises ValueError unless 1 <= n_in <= MAX_FRAME_SIDE and n_out >= 1."""
+    if not (1 <= n_in <= MAX_FRAME_SIDE) or n_out < 1:
+        raise ValueError(f"cubic_taps: a side of {n_in} pixels is outside [1, {MAX_FRAME_SIDE}] (or {n_out} outputs)")
+    f32 = np.float32
+    d = np.arange(n_out, dtype=np.float64)
+    f = ((d + 0.5) * (n_in / n_out) - 0.5).astype(f32)
+    s = np.floor(f)
+    t = f - s
+    A, one = f32(-0.75), f32(1)
+    x = t + one
+    w0 = ((A * x - f32(5) * A) * x + f32(8) * A) * x - f32(4) * A
+    w1 = ((A + f32(2)) * t - (A + f32(3))) * t * t + one
+    u = one - t
+    w2 = ((A + f32(2)) * u - (A + f32(3))) * u * u + one
+    w3 = one - w0 - w1 - w2
+    w = np.stack([w0, w1, w2, w3], 1)
+    assert w.dtype == np.float32
+    iw = np.rint(w * f32(1 << TAP_BITS)).astype(np.int32)
+    idx = np.clip(s.astype(np.int64)[:, None] - 1 + np.arange(4)[None, :], 0, n_in - 1).astype(np.int32)
+    return np.ascontiguousarray(np.concatenate([idx, iw], 1))
+
+
+def letterbox_taps(width: int, height: int, resolution: int) -> np.ndarray:
+    """The tap tables of a width x height frame letterboxed to resolution^2, as one int32 array: the horizontal table
+    (sw rows of 8) then the vertical one (sh rows), (sw, sh) from letterbox_geometry.  Raises ValueError unless both
+    sides lie in [1, MAX_FRAME_SIDE]."""
+    for side in (width, height):
+        if not (isinstance(side, int) and 1 <= side <= MAX_FRAME_SIDE):
+            raise ValueError(f"letterbox: a frame side of {side!r} pixels is outside [1, {MAX_FRAME_SIDE}]")
+    sw, sh, _, _ = letterbox_geometry(width, height, resolution)
+    return np.concatenate([cubic_taps(width, sw), cubic_taps(height, sh)], 0)
+
+
+class FrameRing:
+    """The frames pushed into a session, indexed as the session indexes a loaded clip (`video[r:r2]`, `video[i]`,
+    `video.size(0)`): frame `first + j` is the j-th frame pushed.  Each push letterboxes its native frames on `stream`
+    (Engine.letterbox, the session's encode-ahead stream) and records one event; reading frames makes the reading stream
+    wait on the events of their pushes, so they may be encoded on any stream, and the reading stream never waits for a
+    native-frame copy otherwise.  A frame is released when it is read (the session encodes each frame once): the
+    canvases of a push are dropped once all of them have been read, after which their memory is reused only behind the
+    work already enqueued on the streams that read them.  So the ring holds the frames pushed and not yet encoded."""
+
+    def __init__(self, engine, stream: torch.cuda.Stream, first: int = 0):
+        self.engine, self.stream = engine, stream
+        self.first = self.end = int(first)
+        self._pushes = collections.deque()   # [first index, canvases [n, 3, R, R], event, unread indices]
+
+    def push(self, frames, bgr: bool = False):
+        """Letterbox `frames` (HWC uint8 tensors, CPU or CUDA, any sizes) into the ring, as the next frames.  CUDA frames
+        may still be being written on the caller's current stream: `stream` reads them only after the work enqueued there
+        so far, and their memory is not reused before that read, even if the caller drops them at once."""
+        frames = list(frames)
+        if not frames:
+            return
+        on_device = [f for f in frames if isinstance(f, torch.Tensor) and f.device == self.engine.device]
+        if on_device:
+            ready = torch.cuda.Event()
+            ready.record(torch.cuda.current_stream(self.engine.device))
+            self.stream.wait_event(ready)
+            for f in on_device:
+                f.record_stream(self.stream)
+        with torch.cuda.stream(self.stream):
+            canvases = self.engine.letterbox(frames, bgr=bgr)
+            ev = torch.cuda.Event()
+            ev.record(self.stream)
+        self._pushes.append([self.end, canvases, ev, set(range(self.end, self.end + len(frames)))])
+        self.end += len(frames)
+
+    def size(self, dim: int = 0) -> int:
+        if dim != 0:
+            raise IndexError("FrameRing.size: only dim 0 (frames pushed, counted from frame 0)")
+        return self.end
+
+    def __len__(self) -> int:
+        return self.end
+
+    def __getitem__(self, key):
+        if isinstance(key, slice):
+            start, stop, step = key.indices(self.end)
+            if step != 1:
+                raise IndexError("FrameRing: only contiguous slices")
+            if key.stop is not None and key.stop > self.end:   # never fewer frames than asked for
+                raise IndexError(f"FrameRing: frames up to {key.stop - 1} asked for, {self.end} pushed")
+            idx = range(start, max(start, stop))
+        else:
+            i = int(key)
+            idx = range(i, i + 1)
+        owners = []
+        for i in idx:
+            p = next((p for p in self._pushes if i in p[3]), None)
+            if p is None:
+                what = "not pushed yet" if i >= self.end else "already encoded and released" if i >= self.first else \
+                    "before the first frame pushed into this session"
+                raise IndexError(f"FrameRing: frame {i} is {what}")
+            owners.append(p)
+        cur = torch.cuda.current_stream(self.engine.device)
+        parts = []   # [push, first, end): runs of consecutive frames of one push
+        for i, p in zip(idx, owners):
+            if not any(q[0] is p for q in parts):
+                cur.wait_event(p[2])
+                p[1].record_stream(cur)
+            j = i - p[0]
+            if parts and parts[-1][0] is p and parts[-1][2] == j:
+                parts[-1][2] = j + 1
+            else:
+                parts.append([p, j, j + 1])
+            p[3].discard(i)   # released: a push whose frames have all been read is dropped below
+        self._pushes = collections.deque(p for p in self._pushes if p[3])
+        out = [p[1][a:b] for p, a, b in parts]
+        out = out[0] if len(out) == 1 else torch.cat(out) if out else self._empty()
+        return out if isinstance(key, slice) else out[0]
+
+    def check_pushed(self, frame_idx: int):
+        """Raise IndexError unless frame `frame_idx` has been pushed: a session checks before it changes any state."""
+        if frame_idx >= self.end:
+            raise IndexError(f"frame {frame_idx} is not pushed yet ({self.end} frames pushed): push_frames before "
+                             f"input_video_stream reaches it")
+
+    def _empty(self):
+        R = self.engine.cfg.frame_resolution
+        return torch.empty(0, 3, R, R, dtype=torch.uint8, device=self.engine.device)
+
+
 def resample_indices(n_src: int, src_fps: float, fps: float) -> list:
     """Source frame index shown by every output frame of a constant-frame-rate conversion to `fps`."""
     if n_src <= 0 or src_fps <= 0 or fps <= 0:
@@ -42,11 +181,10 @@ def resample_indices(n_src: int, src_fps: float, fps: float) -> list:
     return [min(n_src - 1, int(round(k / fps * src_fps))) for k in range(n_out)]
 
 
-def read_video_resampled(path: str, fps: Optional[float] = None, resolution: Optional[int] = None) -> torch.Tensor:
-    """Decode `path`; optionally convert to `fps` frames/s and letterbox to `resolution`.  uint8 [T,3,H,W], RGB.
-    Streaming: only the frames the output keeps are converted and held (a 107 s 1440x1080 clip is 3204 source frames =
-    15 GB decoded, but 214 frames of 384x384 at 2 FPS)."""
-    import numpy as np
+def iter_video_frames(path: str, fps: Optional[float] = None) -> Iterator[np.ndarray]:
+    """Decode `path` with OpenCV and yield its frames at their native size (uint8 HWC, BGR), converted to `fps` frames/s
+    by `resample_indices` (a source frame shown by several output frames is yielded once per output frame, as the same
+    array).  Streaming: only the frames the output keeps are decoded to pixels."""
     try:
         import cv2
     except Exception as e:  # pragma: no cover
@@ -72,7 +210,37 @@ def read_video_resampled(path: str, fps: Optional[float] = None, resolution: Opt
         raise RuntimeError(f"could not decode any frame from {path}")
     wanted = resample_indices(n_src, src_fps, float(fps)) if (fps is not None and src_fps > 0) else list(range(n_src))
 
+    k, i, last = 0, 0, None
+    try:
+        while k < len(wanted):
+            if wanted[k] > i:                # skip without decoding to pixels
+                if not cap.grab():
+                    break
+                i += 1
+                continue
+            ok, fr = cap.read()              # source frame i is wanted (possibly several times: fps above the source rate)
+            if not ok:
+                break
+            last = fr
+            while k < len(wanted) and wanted[k] == i:
+                yield fr
+                k += 1
+            i += 1
+    finally:
+        cap.release()
+    if last is None:
+        raise RuntimeError(f"could not decode any frame from {path}")
+    while k < len(wanted):               # the container over-reported its length: hold the last frame (ffmpeg -r pads the same way)
+        yield last
+        k += 1
+
+
+def read_video_resampled(path: str, fps: Optional[float] = None, resolution: Optional[int] = None) -> torch.Tensor:
+    """Decode `path`; optionally convert to `fps` frames/s and letterbox to `resolution`.  uint8 [T,3,H,W], RGB.
+    Streaming: only the frames the output keeps are converted and held (a 107 s 1440x1080 clip is 3204 source frames =
+    15 GB decoded, but 214 frames of 384x384 at 2 FPS)."""
     def convert(fr):
+        import cv2
         h, w = fr.shape[:2]
         if resolution is not None and (h != resolution or w != resolution):
             sw, sh, x0, y0 = letterbox_geometry(w, h, resolution)
@@ -82,25 +250,9 @@ def read_video_resampled(path: str, fps: Optional[float] = None, resolution: Opt
             fr = canvas
         return torch.from_numpy(cv2.cvtColor(fr, cv2.COLOR_BGR2RGB)).permute(2, 0, 1).contiguous()
 
-    out, k, i, last = [], 0, 0, None
-    while k < len(wanted):
-        if wanted[k] > i:                # skip without decoding to pixels
-            if not cap.grab():
-                break
-            i += 1
-            continue
-        ok, fr = cap.read()              # source frame i is wanted (possibly several times: fps above the source rate)
-        if not ok:
-            break
-        last = convert(fr)
-        while k < len(wanted) and wanted[k] == i:
-            out.append(last)
-            k += 1
-        i += 1
-    cap.release()
-    if last is None:
-        raise RuntimeError(f"could not decode any frame from {path}")
-    while k < len(wanted):               # the container over-reported its length: hold the last frame (ffmpeg -r pads the same way)
+    out, src, last = [], None, None
+    for fr in iter_video_frames(path, fps):
+        if fr is not src:                # a repeated source frame is converted once
+            src, last = fr, convert(fr)
         out.append(last)
-        k += 1
     return torch.stack(out).contiguous()
