@@ -207,7 +207,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int n_frames, void* d
  *   v   = sum_k h_k * wy_k                  (int32)
  *   out = clamp((v + 2^21) >> 22, 0, 255)
  * which is OpenCV's fixed-point INTER_CUBIC when the tables are video_ingest.cubic_taps (11-bit weights of A = -0.75).
- * Checks null pointers, sizes, n_frames <= max_vit_batch, the table alignment and that bgr is 0 or 1; one launch per 64
+ * Checks null pointers, sizes, n_frames <= max_vit_batch, the table alignment and that bgr is 0 or 1; one launch per 48
  * frames, asynchronous, ordered behind the previous work on cuda_stream (the canvas may still be read by it). */
 typedef struct vlo_letterbox_frame {
   const uint8_t* d_pixels;
@@ -217,6 +217,36 @@ typedef struct vlo_letterbox_frame {
   int32_t reserved;
 } vlo_letterbox_frame;
 int vlo_letterbox(vlo_engine* e, const vlo_letterbox_frame* h_frames, int n_frames, uint8_t* d_out, void* cuda_stream);
+/* vlo_letterbox_planes is vlo_letterbox for frames given as planes, as camera and decoder pipelines deliver them: the
+ * same geometry, tap tables, integer INTER_CUBIC and canvases, with each source pixel converted to RGB where the cubic
+ * sums read it.  One descriptor per frame; a launch may mix formats and sizes.  format (plane p at d_planes[p], row r of
+ * it at d_planes[p] + r * pitch[p], pitch[p] >= the plane's row bytes; padding past the row bytes is never read):
+ *   VLO_PIX_RGB24 / VLO_PIX_BGR24  1 plane  uint8 [height][width][3] packed           (1 <= width, height <= 8192)
+ *   VLO_PIX_NV12                   2 planes Y [height][width], UV [height/2][width/2][2] interleaved
+ *   VLO_PIX_I420                   3 planes Y [height][width], U [height/2][width/2], V [height/2][width/2]
+ *   VLO_PIX_YUYV                   1 plane  [height][width/2] pairs {Y0, U, Y1, V}     (ffmpeg's yuyv422)
+ * The YUV formats take 2 <= width, height <= 8192, width even, height even for NV12 and I420.  Pixel (x, y) has luma
+ * Y = its Y sample and chroma U, V = the sample of (x/2, y/2) (NV12, I420) or of pair x/2 (YUYV), taken nearest; it
+ * enters the cubic sums as OpenCV's fixed-point BT.601 limited-range cvtColor(COLOR_YUV2RGB_NV12 / _I420 / _YUYV):
+ *   y = max(Y - 16, 0) * 1220542,  u = U - 128,  v = V - 128
+ *   R = clamp((y + 2^19 + 1673527 v) >> 20, 0, 255)
+ *   G = clamp((y + 2^19 - 852492 v - 409993 u) >> 20, 0, 255)
+ *   B = clamp((y + 2^19 + 2116026 u) >> 20, 0, 255)
+ * (int32, arithmetic shift).  The clamp precedes the cubic sums, so the canvas is exactly vlo_letterbox's canvas of
+ * cvtColor's RGB frame.  Checks, before any launch, and leaves d_out untouched on failure: null planes, tables or output,
+ * an unknown format, sides outside the limits above, odd sides, a pitch below the row bytes, the table alignment,
+ * negative table offsets and n_frames in [1, max_vit_batch].  The descriptors travel as kernel parameters within the
+ * 4 KB parameter space: one launch per 48 frames, asynchronous, ordered as vlo_letterbox. */
+enum { VLO_PIX_RGB24 = 0, VLO_PIX_BGR24 = 1, VLO_PIX_NV12 = 2, VLO_PIX_I420 = 3, VLO_PIX_YUYV = 4 };
+typedef struct vlo_frame_planes {
+  const uint8_t* d_planes[3];   /* unused planes may be NULL */
+  const int32_t* d_taps;        /* as vlo_letterbox_frame, tables of the luma width x height */
+  int32_t pitch[3];             /* bytes from one row of a plane to the next */
+  int32_t format, width, height;
+  int32_t x_taps, y_taps;
+} vlo_frame_planes;
+int vlo_letterbox_planes(vlo_engine* e, const vlo_frame_planes* h_frames, int n_frames, uint8_t* d_out,
+                         void* cuda_stream);
 /* connector only: visual_embed without a vision tower (models/modeling_live.py:22-27 with
  * pre-extracted features). d_tokens: bf16 [n_rows, vit_hidden] */
 int vlo_connector(vlo_engine* e, const void* d_tokens, int n_rows, void* d_out, void* cuda_stream);

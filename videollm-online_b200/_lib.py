@@ -55,6 +55,17 @@ class VloLetterboxFrame(C.Structure):
     ]
 
 
+class VloFramePlanes(C.Structure):
+    _fields_ = [
+        ("d_planes", C.c_void_p * 3), ("d_taps", C.c_void_p), ("pitch", C.c_int32 * 3), ("format", C.c_int32),
+        ("width", C.c_int32), ("height", C.c_int32), ("x_taps", C.c_int32), ("y_taps", C.c_int32),
+    ]
+
+
+# vlo_frame_planes.format (include/vlo_b200.h)
+PIX_RGB24, PIX_BGR24, PIX_NV12, PIX_I420, PIX_YUYV = range(5)
+
+
 _P = C.c_void_p
 _I = C.c_int
 _LL = C.c_longlong
@@ -90,6 +101,7 @@ SIGNATURES = {
     "vlo_kv_swap_in": (_I, [_P, _I, _P, _I, _P]),
     "vlo_vit_encode": (_I, [_P, _P, _I, _P, _P, _P]),
     "vlo_letterbox": (_I, [_P, C.POINTER(VloLetterboxFrame), _I, _P, _P]),
+    "vlo_letterbox_planes": (_I, [_P, C.POINTER(VloFramePlanes), _I, _P, _P]),
     "vlo_connector": (_I, [_P, _P, _I, _P, _P]),
     "vlo_embed_tokens": (_I, [_P, _P, _I, _P, _P]),
     "vlo_step": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _I, _P]),

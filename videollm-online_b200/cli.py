@@ -1,7 +1,7 @@
 """Headless driver + FPS measurement: the engine-backed counterpart of demo/cli.py:12-50.
 
     python -m videollm_online_b200.cli --synthetic_weights true [--frames 100] [--video clip.mp4] [--whole_video]
-        [--live] [--do_sample --temperature 0.6 --top_p 0.9 --top_k 50 --repetition_penalty 1.1 --sample_seed 0]
+        [--live | --live_raw WxH:FORMAT] [--do_sample --temperature 0.6 --top_p 0.9 --top_k 50 --repetition_penalty 1.1 --sample_seed 0]
 
 Responses are greedy unless --do_sample is given (SamplingConfig; --seed stays the synthetic weights' seed).
 --context_window N keeps the session's cache within N tokens (0: off): the start prompt stays, the oldest pages after it
@@ -11,6 +11,10 @@ answers.
 --live (with --video) feeds the clip as a camera would: decoded at its native size without a resize, one frame per
 1 / frame_fps of video time pushed through LiveInfer.push_frames (BGR, letterboxed on the device), each one frame ahead
 of the frame being processed.
+--live_raw WxH:FORMAT (with --video PATH, or --video - for stdin) does the same with raw frames, one per frame interval,
+in ffmpeg's rawvideo layout: FORMAT is nv12, yuv420p or yuyv422 (ffmpeg's -pix_fmt names), converted to RGB on the
+device.  A stream that ends inside a frame drops it with a warning.  A camera at 2 frames/s:
+    ffmpeg -i <camera> -r 2 -f rawvideo -pix_fmt nv12 - | python -m videollm_online_b200.cli --live_raw 1920x1080:nv12 --video -
 --fp8_weights serves the decoder layers from e4m3 weights with per-row scales (half their bytes per step; the model's
 numbers change, so it is off by default).
 --fp8_activations (with --fp8_weights) also quantizes the layer GEMMs' activations to e4m3 per token and multiplies them on
@@ -38,13 +42,21 @@ def synthetic_clip(n_frames: int, resolution: int, seed: int = 0) -> torch.Tenso
 
 
 def main(liveinfer: LiveInfer, video=None, n_iters: int = 100, save_history_path: str = None, quiet: bool = False,
-         whole_video: bool = False, live: bool = False):
-    camera = None
-    if live:
+         whole_video: bool = False, live: bool = False, live_raw: str = None):
+    camera, fmt = None, dict(bgr=True)
+    if live and live_raw:
+        raise ValueError("--live and --live_raw do not combine")
+    if live or live_raw:
         if not isinstance(video, str) or whole_video:
-            raise ValueError("--live takes a clip on disk (--video) and does not combine with --whole_video")
-        from .video_ingest import iter_video_frames
-        camera = iter_video_frames(video, fps=liveinfer.frame_fps)
+            raise ValueError("--live and --live_raw take a clip (--video) and do not combine with --whole_video")
+        from .video_ingest import iter_raw_frames, iter_video_frames, parse_raw_spec
+        if live_raw:
+            W, H, pixel_format = parse_raw_spec(live_raw)
+            camera = iter_raw_frames(sys.stdin.buffer if video == '-' else open(video, 'rb'), W, H, pixel_format)
+            fmt = dict(pixel_format=pixel_format)
+        else:
+            camera = iter_video_frames(video, fps=liveinfer.frame_fps)
+        live = True
     else:
         if video is None:
             video = synthetic_clip(n_iters, liveinfer.frame_resolution)
@@ -62,10 +74,10 @@ def main(liveinfer: LiveInfer, video=None, n_iters: int = 100, save_history_path
         if live:
             # frame i + 1 is delivered while frame i is processed, so encode-ahead takes it as it takes a loaded clip's
             if i == 0:
-                liveinfer.push_frames([torch.from_numpy(frame)], bgr=True)
+                liveinfer.push_frames([torch.from_numpy(frame)], **fmt)
             frame = next(camera, None)
             if frame is not None and i + 1 < n_iters:
-                liveinfer.push_frames([torch.from_numpy(frame)], bgr=True)
+                liveinfer.push_frames([torch.from_numpy(frame)], **fmt)
         liveinfer.input_video_stream(i / liveinfer.frame_fps)
         query, response = liveinfer()
         timecosts.append(time.time() - start)
@@ -119,4 +131,7 @@ if __name__ == '__main__':
         video = sys.argv[sys.argv.index('--video') + 1]
     # --whole_video: queue the whole clip at t = 0 and drain it (narrate a recorded file as fast as possible)
     # --live: push the clip's frames at their native size, one per frame interval (a camera feed)
-    main(LiveInfer(parse_args()), video=video, n_iters=n, whole_video='--whole_video' in sys.argv, live='--live' in sys.argv)
+    # --live_raw WxH:FORMAT: the same from raw YUV frames (--video PATH, or - for stdin)
+    live_raw = sys.argv[sys.argv.index('--live_raw') + 1] if '--live_raw' in sys.argv else None
+    main(LiveInfer(parse_args()), video=video, n_iters=n, whole_video='--whole_video' in sys.argv, live='--live' in sys.argv,
+         live_raw=live_raw)

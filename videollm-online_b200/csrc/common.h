@@ -8,6 +8,7 @@
 #include "streamk.h"
 
 struct vlo_letterbox_frame;  // include/vlo_b200.h
+struct vlo_frame_planes;     // include/vlo_b200.h
 
 namespace vlo {
 
@@ -216,9 +217,11 @@ int cls_residual_launch(const void* resid, const void* mlp, float* tokens, int B
 int f32_to_bf16_launch(const float* in, void* out, long long n, cudaStream_t st);
 
 // ---- letterbox (letterbox.cu) ---------------------------------------------------------
-// letterbox_kernel: the frames of vlo_letterbox (include/vlo_b200.h) -> uint8 out [n, 3, R, R]; checks each descriptor,
-// then one launch per kLetterboxMaxFrames frames (their descriptors travel as kernel parameters)
-constexpr int kLetterboxMaxFrames = 64;
+// letterbox_kernel: the frames of vlo_letterbox_planes (include/vlo_b200.h) -> uint8 out [n, 3, R, R]; checks each
+// descriptor, then one launch per kLetterboxMaxFrames frames (their descriptors travel as kernel parameters, 4 KB)
+constexpr int kLetterboxMaxFrames = 48;
+int letterbox_planes_launch(const vlo_frame_planes* frames, int n, int R, uint8_t* out, cudaStream_t st);
+// vlo_letterbox's packed frames: checks bgr, then letterbox_planes_launch of RGB24 / BGR24 descriptors
 int letterbox_launch(const vlo_letterbox_frame* frames, int n, int R, uint8_t* out, cudaStream_t st);
 
 // ---- attention (attn.cu) ------------------------------------------------------------

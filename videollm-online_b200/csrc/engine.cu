@@ -1208,6 +1208,13 @@ int vlo_letterbox(vlo_engine* e, const vlo_letterbox_frame* h_frames, int n_fram
   return letterbox_launch(h_frames, n_frames, e->cfg.image_size, d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
+int vlo_letterbox_planes(vlo_engine* e, const vlo_frame_planes* h_frames, int n_frames, uint8_t* d_out, void* cuda_stream) {
+  DevGuard dev_guard(e);
+  VLO_CHECK(e != nullptr, "null engine");
+  VLO_CHECK(n_frames > 0 && n_frames <= e->cfg.max_vit_batch, "letterbox: n_frames must lie in [1, max_vit_batch]");
+  return letterbox_planes_launch(h_frames, n_frames, e->cfg.image_size, d_out, static_cast<cudaStream_t>(cuda_stream));
+}
+
 // ------------------------------------------------------------------------------ decoder
 int vlo_embed_tokens(vlo_engine* e, const int64_t* d_ids, int n, void* d_out, void* cuda_stream) {
   DevGuard dev_guard(e);

@@ -495,38 +495,46 @@ class Engine:
             return out, torch.cat(toks, 0)
         return out
 
-    def letterbox(self, frames: Sequence[torch.Tensor], bgr: bool = False) -> torch.Tensor:
+    def letterbox(self, frames: Sequence, bgr: bool = False, pixel_format: Optional[str] = None) -> torch.Tensor:
         """Native frames -> uint8 [B, 3, R, R] RGB canvases (R = frame_resolution), what vit_encode takes: each frame is
         scaled into the square with the integer INTER_CUBIC of video_ingest.cubic_taps and centred on black bars
-        (video_ingest.letterbox_geometry), on the device (vlo_letterbox, current CUDA stream).  frames: HWC uint8 tensors
-        with 3 channels (RGB, or BGR with bgr=True), each of its own size up to 8192 x 8192, on the CPU or this device.
+        (video_ingest.letterbox_geometry), on the device (vlo_letterbox_planes, current CUDA stream).  frames: HWC uint8
+        tensors with 3 channels (RGB, or BGR with bgr=True), each of its own size up to 8192 x 8192, on the CPU or this
+        device; or, with pixel_format "nv12", "yuv420p" or "yuyv422" (ffmpeg's names), YUV frames as
+        video_ingest.frame_layout describes them, converted to RGB per source pixel with OpenCV's BT.601 integer
+        arithmetic, so the canvas is exactly that of cv2.cvtColor's RGB frame.  Device planes are read in place.
         CPU frames are staged through pinned buffers and copied asynchronously; a buffer is reused only once the copy
-        out of it has completed.  Raises VloError on a frame of another dtype, shape, device or size."""
-        from .video_ingest import MAX_FRAME_SIDE
+        out of it has completed.  Every frame is checked before any device work: VloError on a frame of another dtype,
+        shape, device, size or format."""
+        from .video_ingest import frame_layout
         frames = list(frames)
         if not frames:
             raise VloError("letterbox: no frames")
+        try:
+            layouts = [frame_layout(f, pixel_format, bgr) for f in frames]
+        except ValueError as e:
+            raise VloError(f"letterbox: {e}") from None
+        for _, _, _, parts, _ in layouts:
+            for t in parts:
+                if t.device.type == "cuda" and t.device != self.device:
+                    raise VloError(f"letterbox: a frame on {t.device}, the engine runs on {self.device}")
         R = self.cfg.frame_resolution
         out = torch.empty(len(frames), 3, R, R, dtype=torch.uint8, device=self.device)
-        descs = (_lib.VloLetterboxFrame * len(frames))()
+        descs = (_lib.VloFramePlanes * len(frames))()
         held = []   # device frames and tap tables: alive until every launch is enqueued (stream-ordered reuse after it)
-        for d, f in zip(descs, frames):
-            if not isinstance(f, torch.Tensor) or f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-                raise VloError(f"letterbox: frames must be uint8 HWC tensors with 3 channels, got "
-                               f"{getattr(f, 'dtype', type(f))} {tuple(getattr(f, 'shape', ()))}")
-            H, W = int(f.shape[0]), int(f.shape[1])
-            if not (1 <= W <= MAX_FRAME_SIDE and 1 <= H <= MAX_FRAME_SIDE):
-                raise VloError(f"letterbox: a {W} x {H} frame; both sides must lie in [1, {MAX_FRAME_SIDE}]")
+        for d, (W, H, fmt, parts, planes) in zip(descs, layouts):
             taps, sw = self._letterbox_taps(W, H)
-            dev = self._frame_on_device(f)
-            held += [dev, taps]
-            d.d_pixels, d.d_taps, d.width, d.height = dev.data_ptr(), taps.data_ptr(), W, H
-            d.bgr, d.x_taps, d.y_taps = int(bool(bgr)), 0, sw
-        size = C.sizeof(_lib.VloLetterboxFrame)
+            # one tensor: its contiguous device copy; planes: read in place (device only, frame_layout)
+            parts = [self._frame_on_device(parts[0])] if len(parts) == 1 else parts
+            held += [*parts, taps]
+            for q, (k, offset, pitch) in enumerate(planes):
+                d.d_planes[q], d.pitch[q] = parts[k].data_ptr() + offset, pitch
+            d.d_taps, d.format, d.width, d.height, d.x_taps, d.y_taps = taps.data_ptr(), fmt, W, H, 0, sw
+        size = C.sizeof(_lib.VloFramePlanes)
         for b0 in range(0, len(frames), self.max_vit_batch):
             n = min(self.max_vit_batch, len(frames) - b0)
-            check(self.lib.vlo_letterbox(self._h, C.cast(C.addressof(descs) + b0 * size, C.POINTER(_lib.VloLetterboxFrame)),
-                                         n, _ptr(out[b0:]), self._stream()), "vlo_letterbox")
+            check(self.lib.vlo_letterbox_planes(self._h, C.cast(C.addressof(descs) + b0 * size, C.POINTER(_lib.VloFramePlanes)),
+                                                n, _ptr(out[b0:]), self._stream()), "vlo_letterbox_planes")
         return out
 
     def _letterbox_taps(self, W: int, H: int):
@@ -544,8 +552,6 @@ class Engine:
 
     def _frame_on_device(self, f: torch.Tensor) -> torch.Tensor:
         if f.device.type == "cuda":
-            if f.device != self.device:
-                raise VloError(f"letterbox: a frame on {f.device}, the engine runs on {self.device}")
             return f.contiguous()
         n = f.numel()
         pool = self._frame_staging

@@ -301,20 +301,22 @@ class LiveInfer:
         logger.warning(f'{"tensor" if isinstance(video_path_or_tensor, torch.Tensor) else video_path_or_tensor} -> '
                        f'{tuple(self.video_tensor.shape)}, {self.frame_fps} FPS')
 
-    def push_frames(self, frames, bgr: bool = False):
+    def push_frames(self, frames, bgr: bool = False, pixel_format: Optional[str] = None):
         """Append live frames to the session's video at frame_fps: frame i of the session is the i-th frame pushed since
         the last reset (counted on from the last frame input_video_stream reached, after a resume), so a camera feeds
         input_video_stream(t) as a loaded clip does.  frames: HWC uint8 tensors at their native sizes (RGB, or BGR with
-        bgr=True; CPU or CUDA); they are copied and letterboxed to frame_resolution on the encode-ahead stream
-        (Engine.letterbox) and held until encoded (video_ingest.FrameRing).  A session plays one source at a time: after
-        load_video, reset() before pushing frames (ValueError otherwise); reset and load_video drop the pushed frames."""
+        bgr=True; CPU or CUDA), or with pixel_format "nv12", "yuv420p" or "yuyv422" the YUV frames of
+        video_ingest.frame_layout (a decoder's device planes among them); they are copied, converted and letterboxed to
+        frame_resolution on the encode-ahead stream (Engine.letterbox) and held until encoded (video_ingest.FrameRing).
+        Bad frames raise VloError before anything is enqueued.  A session plays one source at a time: after load_video,
+        reset() before pushing frames (ValueError otherwise); reset and load_video drop the pushed frames."""
         with self._lock:
             ring = self.video_tensor
             if ring is None:
                 ring = self.video_tensor = FrameRing(self.model.engine, self._side, first=self.last_frame_idx + 1)
             elif not isinstance(ring, FrameRing):
                 raise ValueError("push_frames: the session plays a loaded clip; reset() it before pushing frames")
-            ring.push(frames, bgr=bgr)
+            ring.push(frames, bgr=bgr, pixel_format=pixel_format)
             self.num_video_frames = ring.size(0)
             self.video_duration = ring.size(0) / self.frame_fps
 

@@ -96,14 +96,15 @@ class StreamSession:
         self.video = video_u8.to(self.sched.model.device)
         getattr(self.sched, "_ahead", {}).pop(self.index, None)
 
-    def push_frames(self, frames, bgr: bool = False):
-        """As LiveInfer.push_frames: append live frames at their native sizes to the session's video, letterboxed on the
-        scheduler's encode-ahead stream.  After load_video, reset() before pushing frames (ValueError otherwise)."""
+    def push_frames(self, frames, bgr: bool = False, pixel_format: Optional[str] = None):
+        """As LiveInfer.push_frames: append live frames at their native sizes (packed RGB / BGR, or YUV in pixel_format) to
+        the session's video, letterboxed on the scheduler's encode-ahead stream.  After load_video, reset() before pushing
+        frames (ValueError otherwise)."""
         if self.video is None:
             self.video = FrameRing(self.sched.model.engine, self.sched._side, first=self.last_frame_idx + 1)
         elif not isinstance(self.video, FrameRing):
             raise ValueError("push_frames: the session plays a loaded clip; reset() it before pushing frames")
-        self.video.push(frames, bgr=bgr)
+        self.video.push(frames, bgr=bgr, pixel_format=pixel_format)
 
     def input_video_stream(self, video_time: float):
         idx = int(video_time * self.frame_fps)

@@ -18,18 +18,25 @@ moves to the GPU.
 
 Live frames (`push_frames`) are letterboxed on the device instead (`Engine.letterbox`, vlo_letterbox): `cubic_taps` builds
 the integer INTER_CUBIC tap tables the kernel reads, and `FrameRing` holds a session's pushed frames until they are
-encoded.
+encoded.  Frames may come as packed RGB / BGR or, named by ffmpeg's `-pix_fmt`, as NV12, I420 (`yuv420p`) or YUYV
+(`yuyv422`), converted to RGB on the device (vlo_letterbox_planes); `frame_layout` checks them on the host, and
+`iter_raw_frames` splits a raw byte stream of them (ffmpeg `-f rawvideo`) into frames.
 """
 from __future__ import annotations
 
 import collections
-from typing import Iterator, Optional, Tuple
+import warnings
+from typing import BinaryIO, Iterator, Optional, Tuple
 
 import numpy as np
 import torch
 
+from ._lib import VloError
+
 MAX_FRAME_SIDE = 8192   # widest / tallest native frame vlo_letterbox takes
 TAP_BITS = 11           # integer tap weights are round(w * 2^11), OpenCV's INTER_RESIZE_COEF_BITS
+# pixel_format (ffmpeg's -pix_fmt names) -> vlo_frame_planes.format; None is packed RGB (0) or BGR (1), chosen by bgr
+PIXEL_FORMATS = {"nv12": 2, "yuv420p": 3, "yuyv422": 4}
 
 
 def letterbox_geometry(width: int, height: int, resolution: int) -> Tuple[int, int, int, int]:
@@ -83,6 +90,125 @@ def letterbox_taps(width: int, height: int, resolution: int) -> np.ndarray:
     return np.concatenate([cubic_taps(width, sw), cubic_taps(height, sh)], 0)
 
 
+def raw_frame_shape(width: int, height: int, pixel_format: str) -> Tuple[int, ...]:
+    """The uint8 shape of one width x height frame in pixel_format as one tensor (the layout of ffmpeg's rawvideo and of
+    cv2): [H * 3 / 2, W] for the 4:2:0 formats (the Y plane, then the chroma planes packed), [H, W, 2] for YUYV."""
+    if pixel_format not in PIXEL_FORMATS:
+        raise ValueError(f"unknown pixel format {pixel_format!r}; one of {sorted(PIXEL_FORMATS)} (or None: RGB / BGR)")
+    return (height, width, 2) if pixel_format == "yuyv422" else (height * 3 // 2, width)
+
+
+def _check_sides(width: int, height: int, pixel_format: Optional[str]):
+    lo = 1 if pixel_format is None else 2
+    if not (lo <= width <= MAX_FRAME_SIDE and lo <= height <= MAX_FRAME_SIDE):
+        raise ValueError(f"a {width} x {height} frame; both sides must lie in [{lo}, {MAX_FRAME_SIDE}]")
+    if pixel_format is not None and width % 2:
+        raise ValueError(f"a {pixel_format} frame {width} pixels wide; the width must be even")
+    if pixel_format in ("nv12", "yuv420p") and height % 2:
+        raise ValueError(f"a {pixel_format} frame {height} lines high; the height must be even")
+
+
+def frame_layout(frame, pixel_format: Optional[str] = None, bgr: bool = False):
+    """Check one frame of `push_frames` / `Engine.letterbox` on the host, before any device work, and return
+    (width, height, vlo_frame_planes.format, parts, planes): the frame's tensors and, per plane, (index into parts, byte
+    offset, pitch).  Raises ValueError on anything vlo_letterbox_planes would refuse.  A frame is
+      pixel_format None               uint8 [H, W, 3] packed RGB (BGR with bgr=True), 1 <= W, H <= 8192, CPU or device;
+      "nv12", "yuv420p" (I420)        uint8 [H * 3 / 2, W], the planes one after the other (raw_frame_shape), CPU or
+                                      device; or, on the device only, a tuple of 2-D uint8 planes (Y [H, W] and UV
+                                      [H / 2, W] for NV12; Y, U [H / 2, W / 2] and V for I420) whose rows may be padded
+                                      (stride(1) == 1, stride(0) >= the row bytes): a decoder's surface, read in place;
+      "yuyv422"                       uint8 [H, W, 2] (pairs Y0 U Y1 V), CPU or device.
+    The YUV formats take 2 <= W, H <= 8192 with W even, and H even for the 4:2:0 formats.  The offsets and pitches of a
+    single tensor are those of its contiguous copy, which is what Engine.letterbox reads."""
+    if pixel_format is not None and pixel_format not in PIXEL_FORMATS:
+        raise ValueError(f"unknown pixel format {pixel_format!r}; one of {sorted(PIXEL_FORMATS)} (or None: RGB / BGR)")
+    if pixel_format is not None and bgr:
+        raise ValueError(f"bgr=True names a packed RGB order; it does not combine with pixel_format={pixel_format!r}")
+    if isinstance(frame, (tuple, list)):
+        if pixel_format not in ("nv12", "yuv420p"):
+            raise ValueError(f"frames as separate planes are NV12 or yuv420p; got a tuple with pixel_format={pixel_format!r}")
+        n = 2 if pixel_format == "nv12" else 3
+        if len(frame) != n or not all(isinstance(p, torch.Tensor) for p in frame):
+            raise ValueError(f"a {pixel_format} frame as planes is a tuple of {n} tensors")
+        for p in frame:
+            if p.dtype != torch.uint8 or p.dim() != 2 or p.device.type != "cuda":
+                raise ValueError(f"{pixel_format} planes must be 2-D uint8 device tensors, got {p.dtype} "
+                                 f"{tuple(p.shape)} on {p.device}")
+        H, W = int(frame[0].shape[0]), int(frame[0].shape[1])
+        _check_sides(W, H, pixel_format)
+        want = [(H, W), (H // 2, W)] if n == 2 else [(H, W), (H // 2, W // 2), (H // 2, W // 2)]
+        planes = []
+        for k, (p, shape) in enumerate(zip(frame, want)):
+            if tuple(p.shape) != shape:
+                raise ValueError(f"{pixel_format} plane {k} of a {W} x {H} frame must be {list(shape)}, got {list(p.shape)}")
+            pitch = p.stride(0)
+            if p.stride(1) != 1 or pitch < shape[1] or pitch >= 2 ** 31:
+                raise ValueError(f"{pixel_format} plane {k}: rows must be unit-stride with a pitch in [{shape[1]}, 2^31), "
+                                 f"got strides {p.stride()}")
+            planes.append((k, 0, pitch))
+        return W, H, PIXEL_FORMATS[pixel_format], tuple(frame), planes
+    if not isinstance(frame, torch.Tensor) or frame.dtype != torch.uint8:
+        raise ValueError(f"frames must be uint8 tensors, got {getattr(frame, 'dtype', type(frame))}")
+    shape = tuple(frame.shape)
+    if pixel_format is None:
+        if len(shape) != 3 or shape[2] != 3:
+            raise ValueError(f"packed RGB / BGR frames are uint8 HWC tensors with 3 channels, got {list(shape)}")
+        H, W = shape[:2]
+        _check_sides(W, H, None)
+        return W, H, int(bool(bgr)), (frame,), [(0, 0, 3 * W)]
+    if pixel_format == "yuyv422":
+        if len(shape) != 3 or shape[2] != 2:
+            raise ValueError(f"yuyv422 frames are uint8 [H, W, 2] tensors, got {list(shape)}")
+        H, W = shape[:2]
+        _check_sides(W, H, pixel_format)
+        return W, H, PIXEL_FORMATS[pixel_format], (frame,), [(0, 0, 2 * W)]
+    if len(shape) != 2 or shape[0] % 3:
+        raise ValueError(f"{pixel_format} frames are uint8 [H * 3 / 2, W] tensors (or a tuple of device planes), "
+                         f"got {list(shape)}")
+    H, W = shape[0] // 3 * 2, shape[1]
+    _check_sides(W, H, pixel_format)
+    if pixel_format == "nv12":
+        planes = [(0, 0, W), (0, W * H, W)]
+    else:
+        planes = [(0, 0, W), (0, W * H, W // 2), (0, W * H + (W // 2) * (H // 2), W // 2)]
+    return W, H, PIXEL_FORMATS[pixel_format], (frame,), planes
+
+
+def parse_raw_spec(spec: str) -> Tuple[int, int, str]:
+    """`WxH:FORMAT` (cli --live_raw, e.g. 1920x1080:nv12) -> (width, height, pixel_format); ValueError if malformed or
+    outside frame_layout's limits."""
+    try:
+        size, pixel_format = spec.split(":")
+        width, height = (int(v) for v in size.lower().split("x"))
+    except ValueError:
+        raise ValueError(f"a raw video spec is WxH:FORMAT, e.g. 1920x1080:nv12; got {spec!r}") from None
+    raw_frame_shape(width, height, pixel_format)
+    _check_sides(width, height, pixel_format)
+    return width, height, pixel_format
+
+
+def iter_raw_frames(stream: BinaryIO, width: int, height: int, pixel_format: str) -> Iterator[np.ndarray]:
+    """Split a raw video byte stream (ffmpeg `-f rawvideo -pix_fmt <pixel_format>`, a pipe or a file) into frames of
+    raw_frame_shape, yielded as uint8 arrays as they arrive.  A stream that ends inside a frame drops that frame with a
+    warning."""
+    shape = raw_frame_shape(width, height, pixel_format)
+    _check_sides(width, height, pixel_format)
+    n = int(np.prod(shape))
+    while True:
+        buf = bytearray(n)
+        view, got = memoryview(buf), 0
+        while got < n:   # a pipe returns what it has: read until the frame is whole or the stream ends
+            k = stream.readinto(view[got:])
+            if not k:
+                break
+            got += k
+        if got < n:
+            if got:
+                warnings.warn(f"raw video ended {got} bytes into a {n}-byte {pixel_format} frame; that frame is dropped")
+            return
+        yield np.frombuffer(buf, dtype=np.uint8).reshape(shape)
+
+
 class FrameRing:
     """The frames pushed into a session, indexed as the session indexes a loaded clip (`video[r:r2]`, `video[i]`,
     `video.size(0)`): frame `first + j` is the j-th frame pushed.  Each push letterboxes its native frames on `stream`
@@ -97,14 +223,19 @@ class FrameRing:
         self.first = self.end = int(first)
         self._pushes = collections.deque()   # [first index, canvases [n, 3, R, R], event, unread indices]
 
-    def push(self, frames, bgr: bool = False):
-        """Letterbox `frames` (HWC uint8 tensors, CPU or CUDA, any sizes) into the ring, as the next frames.  CUDA frames
-        may still be being written on the caller's current stream: `stream` reads them only after the work enqueued there
-        so far, and their memory is not reused before that read, even if the caller drops them at once."""
+    def push(self, frames, bgr: bool = False, pixel_format: Optional[str] = None):
+        """Letterbox `frames` (as frame_layout takes them: HWC uint8 tensors or, in pixel_format, YUV frames or device
+        planes; CPU or CUDA, any sizes) into the ring, as the next frames.  Every frame is checked before any device work.
+        CUDA frames may still be being written on the caller's current stream: `stream` reads them only after the work
+        enqueued there so far, and their memory is not reused before that read, even if the caller drops them at once."""
         frames = list(frames)
         if not frames:
             return
-        on_device = [f for f in frames if isinstance(f, torch.Tensor) and f.device == self.engine.device]
+        try:
+            parts = [frame_layout(f, pixel_format, bgr)[3] for f in frames]
+        except ValueError as e:
+            raise VloError(f"push_frames: {e}") from None
+        on_device = [t for ts in parts for t in ts if t.device == self.engine.device]
         if on_device:
             ready = torch.cuda.Event()
             ready.record(torch.cuda.current_stream(self.engine.device))
@@ -112,7 +243,7 @@ class FrameRing:
             for f in on_device:
                 f.record_stream(self.stream)
         with torch.cuda.stream(self.stream):
-            canvases = self.engine.letterbox(frames, bgr=bgr)
+            canvases = self.engine.letterbox(frames, bgr=bgr, pixel_format=pixel_format)
             ev = torch.cuda.Event()
             ev.record(self.stream)
         self._pushes.append([self.end, canvases, ev, set(range(self.end, self.end + len(frames)))])
