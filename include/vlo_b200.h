@@ -319,6 +319,22 @@ typedef struct vlo_sample_row {
 int vlo_sample(vlo_engine* e, const void* d_logits, int n_rows, const vlo_sample_row* h_rows, const int32_t* h_penalty_ids,
                int n_penalty_ids, int32_t* d_out_ids, void* cuda_stream);
 
+/* Prefill: one stream's n_tokens rows (1 <= n_tokens <= vlo_max_prefill_tokens(e)) through all
+ * layers in one pass, with the bits of the same rows fed as vlo_step calls of max_step_tokens (the chunked path).  The
+ * layer GEMMs run on gemm_prefill_kernel (tokens on wgmma M, the chunked path's stream-K k-ranges summed in its plane
+ * order, csrc/gemm_prefill.cuh); the KV append, fix-up, RMSNorm, lm_head and decision kernels are the step's; each layer's
+ * attention is one vlo_step_segments-style launch whose segments are the max_step_tokens pieces, each planned as its own
+ * step.  d_row_ids (device int64 [n_tokens] or NULL) as in vlo_step_ids; d_last_logits: bf16 [1, vocab] or NULL;
+ * d_decision: one vlo_decision or NULL, at the last row.  vlo_last_step_logits / vlo_last_step_hidden then cover all
+ * n_tokens rows.  The stream's pages are taken all or none; on any error the stream is unchanged.  bf16 layer weights
+ * only: an engine with e4m3 weights (or W8A8) returns an error. */
+int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row_ids, const void* d_embeds,
+                void* d_last_logits, vlo_decision* d_decision, int interval_id, void* cuda_stream);
+/* 8 x max_step_tokens once vlo_finalize_weights has loaded bf16 layer weights on an engine without fp8 activations: it
+ * then grows the token-row workspaces (h, xn, q, attn_out, act, attention workspace, step tables) to that many rows.
+ * 0 before, and on engines with e4m3 layer weights or activations, which keep them at max_step_tokens rows. */
+int vlo_max_prefill_tokens(vlo_engine* e);
+
 /* all-position logits for the last vlo_step's tokens (the reference's logits_to_keep=0 behaviour,
  * HF:models/llama/modeling_llama.py:485-487); d_logits bf16 [sum(q_lens), vocab]. Test/compat path. */
 int vlo_last_step_logits(vlo_engine* e, void* d_logits, void* cuda_stream);
@@ -493,6 +509,13 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
  * counters, zero before the call and zero again when it has run.  Asynchronous. */
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
                        int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream);
+/* Prefill GEMM (csrc/gemm_prefill.cuh), bf16 W [rows_w, k], X [rows_x, k] (any rows_x): for each output the k-ranges of
+ * the stream-K plan vlo_op_gemm_ws (mode 0, one token tile) makes over n_ctas CTAs (0: all SMs), each an in-order chain
+ * from zero, summed in plane order.  epi 0: d_out fp32 [rows_x, rows_w] = 0 + P0 + P1 + ..., what the fix-up kernels sum
+ * from the chunked path's planes; epi 1: d_out bf16 [rows_x, rows_w / 2], the SwiGLU of vlo_op_gemm_swiglu's tile layout
+ * (rows_w % 128 == 0, all SMs' plan) on g, u = P0 + P1 + ....  Rows past rows_x are not written.  Asynchronous. */
+int vlo_op_gemm_prefill(int epi, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, int n_ctas, void* d_out,
+                        void* cuda_stream);
 /* vlo_op_gemm_swiglu on e4m3 weights d_w8 [rows_w, k] with fp32 row scales d_scale [rows_w] (same row order and plan):
  * g, u = bf16(sum_p fl(P_p * d_scale[n])) summed in plane order, P_p the fp32 partials of the bf16 kernel on the exactly
  * upcast weights (the finisher's own partial is plane 0).  Asynchronous. */

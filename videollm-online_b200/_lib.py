@@ -109,6 +109,8 @@ SIGNATURES = {
     "vlo_step_segments": (_I, [_P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _P, _P, _P, _P,
                                _I, _P]),
     "vlo_sample": (_I, [_P, _P, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P]),
+    "vlo_prefill": (_I, [_P, _I, _I, _P, _P, _P, _P, _I, _P]),
+    "vlo_max_prefill_tokens": (_I, [_P]),
     "vlo_last_step_logits": (_I, [_P, _P, _P]),
     "vlo_last_step_hidden": (_I, [_P, _P, _P]),
     "vlo_bench_attn": (_I, [_P, _I, C.POINTER(C.c_int32), _I, _I, _I, C.POINTER(C.c_double), _P]),
@@ -139,6 +141,7 @@ SIGNATURES = {
     "vlo_op_qkv_rope_append": (_I, [_P, _I, _I, _P, _P, _I, C.POINTER(C.c_int32), C.POINTER(C.c_int64), _I, _P, _P, _P,
                                     _I, _I, _I, _P]),
     "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
+    "vlo_op_gemm_prefill": (_I, [_I, _P, _I, _P, _I, _I, _I, _P, _P]),
     "vlo_op_gemm_swiglu_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_swiglu_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),

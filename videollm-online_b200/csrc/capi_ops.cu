@@ -461,6 +461,12 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
   return 0;
 }
 
+int vlo_op_gemm_prefill(int epi, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, int n_ctas, void* d_out,
+                        void* cuda_stream) {
+  VLO_CHECK(n_ctas >= 0, "gemm_prefill: n_ctas");
+  return gemm_prefill_launch(epi, d_w, rows_w, d_x, rows_x, k, n_ctas, d_out, static_cast<cudaStream_t>(cuda_stream));
+}
+
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
                        int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu: plane_elems");

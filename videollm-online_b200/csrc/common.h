@@ -152,6 +152,13 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 // a_scale non-null: x is e4m3 with fp32 token scales a_scale [rows_x] (e4m3 weights only).
 // planes (plane_elems floats) take the partials of the non-finisher CTAs, flags (n_flags counters, zero between
 // launches) their arrivals.
+// ---- prefill GEMM, tokens on wgmma M (gemm_prefill.cuh / gemm.cu): bf16 x [rows_x, k], w [rows_w, k], any rows_x; the
+// k-ranges and plane order of the chunked path's stream-K plan over n_ctas CTAs (<= 0: one per SM).  epi 0: one fp32
+// plane out[rows_x][rows_w] (fill *sk with the one-plane SkInfo its fix-up kernel reads); epi 1: gate|up + SwiGLU into
+// bf16 out[rows_x][rows_w / 2] (rows_w % 128 == 0)
+int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
+                        cudaStream_t stream, SkInfo* sk = nullptr);
+
 int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
                     float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream,
                     const float* a_scale = nullptr);

@@ -106,6 +106,10 @@ struct vlo_engine {
   bool stage_used[kStageSlots]{};
   int stage_next = 0;
   int last_step_tokens = 0;
+  int token_rows = 0;    // rows the token-row workspaces hold (size_token_rows)
+  // rows of one vlo_prefill: kFixMaxPlanes x max_step_tokens (one fp32 plane fits `part`) once vlo_finalize_weights has
+  // grown the token-row workspaces of a bf16 engine; 0 before, and on engines with e4m3 layer weights or activations
+  int max_prefill = 0;
 
   // ViT workspaces
   __half *patches = nullptr, *v_xn = nullptr, *v_qkv = nullptr, *v_attn = nullptr, *v_mlp = nullptr, *v_pa = nullptr,
@@ -128,6 +132,65 @@ int dev_alloc(vlo_engine* e, void** p, size_t bytes, bool zero) {
 template <typename T>
 int dev_alloc_t(vlo_engine* e, T** p, size_t n, bool zero = false) {
   return dev_alloc(e, reinterpret_cast<void**>(p), n * sizeof(T), zero);
+}
+// gives back an allocation of dev_alloc (bytes as passed to it)
+template <typename T>
+void dev_free(vlo_engine* e, T** p, size_t bytes) {
+  if (*p == nullptr) return;
+  for (size_t i = 0; i < e->allocs.size(); ++i)
+    if (e->allocs[i] == *p) {
+      e->allocs.erase(e->allocs.begin() + static_cast<long>(i));
+      cudaFree(*p);
+      e->device_bytes -= static_cast<int64_t>(align256(bytes ? bytes : 256));
+      break;
+    }
+  *p = nullptr;
+}
+
+// The workspaces whose size follows the rows of one pass: h, xn, q, attn_out, act, the attention workspace, the step
+// tables (and with them the layout of every pinned staging slot).  `rows` = max_step_tokens at creation; a bf16 engine
+// grows them to max_prefill rows in vlo_finalize_weights.  Growing frees the old buffers: no work may be in flight.
+int size_token_rows(vlo_engine* e, int rows) {
+  const vlo_config& c = e->cfg;
+  const size_t H = c.hidden_size, A = static_cast<size_t>(c.num_heads) * c.head_dim, I = c.intermediate_size;
+  const int per_stream = kv_pages_for(c.max_kv_tokens);
+  const size_t per_token = align256(sizeof(int) * rows);
+  const size_t meta_bytes = 3 * per_token + align256(sizeof(long long) * rows) +
+                            align256(sizeof(int) * std::max(2, c.max_streams) * per_stream);
+  const size_t sample_bytes = e->sample_ids + sizeof(int) * kSamplePenaltyIds;
+  if (e->h != nullptr) {
+    const size_t old = e->token_rows;
+    dev_free(e, &e->h, old * H * sizeof(bf16));
+    dev_free(e, &e->xn, old * H * sizeof(bf16));
+    dev_free(e, &e->q, old * A * sizeof(bf16));
+    dev_free(e, &e->attn_out, old * A * sizeof(bf16));
+    dev_free(e, &e->act, old * I * sizeof(bf16));
+    dev_free(e, &e->attn_ws, attn_ws_bytes(e->token_rows, c.max_streams, c.num_heads, c.num_kv_heads));
+    dev_free(e, &e->meta_dev, e->meta.bytes);
+    VLO_CUDA(cudaFreeHost(e->stage));
+    e->stage = nullptr;
+    for (int i = 0; i < kStageSlots; ++i) e->stage_used[i] = false;
+  }
+  e->token_rows = rows;
+  if (dev_alloc_t(e, &e->h, rows * H)) return -1;
+  if (dev_alloc_t(e, &e->xn, rows * H)) return -1;
+  if (dev_alloc_t(e, &e->q, rows * A)) return -1;
+  if (dev_alloc_t(e, &e->attn_out, rows * A)) return -1;
+  if (dev_alloc_t(e, &e->act, rows * I)) return -1;
+  const size_t aws = attn_ws_bytes(rows, c.max_streams, c.num_heads, c.num_kv_heads);
+  if (dev_alloc(e, reinterpret_cast<void**>(&e->attn_ws), aws, false)) return -1;
+  // the table region also stages the two streams' tables of a KV copy (upload_op_tables)
+  e->meta.pos = 0;
+  e->meta.last = per_token;
+  e->meta.first = 2 * per_token;
+  e->meta.kvrow = 3 * per_token;
+  e->meta.pt = e->meta.kvrow + align256(sizeof(long long) * rows);
+  e->meta.bytes = meta_bytes;
+  if (dev_alloc(e, reinterpret_cast<void**>(&e->meta_dev), e->meta.bytes, false)) return -1;
+  e->sample_stage = align256(e->meta.bytes + attn_stage_bytes(rows, c.max_streams, c.num_heads, c.num_kv_heads));
+  e->stage_slot_bytes = align256(e->sample_stage + sample_bytes);
+  VLO_CUDA(cudaMallocHost(reinterpret_cast<void**>(&e->stage), e->stage_slot_bytes * kStageSlots));
+  return 0;
 }
 
 template <typename T>
@@ -547,7 +610,7 @@ int vlo_engine_create_pooled(const vlo_config* cfg, int64_t kv_pool_tokens, int 
   VLO_CHECK(kv_pages_for(c.max_kv_tokens) <= attn_max_key_blocks(),
             "max_kv_tokens above " + std::to_string(attn_max_key_blocks() * kKvPageTokens) +
                 " (the attention stages a stream's page table in shared memory)");
-  VLO_CHECK(c.max_step_tokens <= 128, "max_step_tokens <= 128 (longer inputs are chunked by the host; chunked == one pass)");
+  VLO_CHECK(c.max_step_tokens <= 128, "max_step_tokens <= 128 (longer inputs run as prefills or are chunked by the host; chunked == one pass)");
   VLO_CHECK(c.vit_layers == 0 || (c.vit_hidden % 128 == 0 && c.vit_hidden == 64 * c.vit_heads && c.vit_mlp % 64 == 0),
             "vision tower: hidden % 64, head_dim == 64");
   VLO_CHECK(c.vit_layers == 0 || (c.image_size % c.patch_size == 0 && (3 * c.patch_size * c.patch_size) % 64 == 0 &&
@@ -590,38 +653,21 @@ static int engine_init(vlo_engine* e, int64_t kv_pool_tokens) {
   const size_t kv_elems = static_cast<size_t>(c.num_layers) * 2 * e->pool.rows_per_layer() * c.head_dim;
   if (dev_alloc_t(e, &e->kv, kv_elems, true)) return -1;
   if (dev_alloc_t(e, &e->kv_op_pt, static_cast<size_t>(2) * per_stream + kRotFloats)) return -1;
-  if (dev_alloc_t(e, &e->h, static_cast<size_t>(T) * H)) return -1;
-  if (dev_alloc_t(e, &e->xn, static_cast<size_t>(T) * H)) return -1;
   // decision rows: one per sequence, or one per segment of a segmented step (each segment holds >= 1 of the T tokens)
   const int rows = std::max(c.max_streams, T);
   if (dev_alloc_t(e, &e->xn_last, static_cast<size_t>(rows) * H)) return -1;
-  if (dev_alloc_t(e, &e->q, static_cast<size_t>(T) * c.num_heads * c.head_dim)) return -1;
-  if (dev_alloc_t(e, &e->attn_out, static_cast<size_t>(T) * c.num_heads * c.head_dim)) return -1;
-  if (dev_alloc_t(e, &e->act, static_cast<size_t>(T) * c.intermediate_size)) return -1;
   if (dev_alloc_t(e, &e->logits, static_cast<size_t>(rows) * c.vocab_size)) return -1;
   if (dev_alloc_t(e, &e->decisions, static_cast<size_t>(rows))) return -1;
   const int widest = std::max(std::max(e->qkv_width, 2 * c.intermediate_size), H);
-  e->part_elems = static_cast<size_t>(8) * T * widest;  // stream-K needs <= kb/floor(U/G) + 2 planes (<= 4 in practice)
+  // stream-K needs <= kb/floor(U/G) + 2 planes (<= 4 in practice); a prefill's one plane of max_prefill rows fills it
+  e->part_elems = static_cast<size_t>(kFixMaxPlanes) * T * widest;
   if (dev_alloc_t(e, &e->part, e->part_elems)) return -1;
   if (dev_alloc_t(e, &e->sk_flags, kSkFlags, true)) return -1;
-  const size_t aws = attn_ws_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads);
-  if (dev_alloc(e, reinterpret_cast<void**>(&e->attn_ws), aws, false)) return -1;
-  // the table region also stages the two streams' tables of a KV copy (upload_op_tables)
-  const size_t per_token = align256(sizeof(int) * T);
-  e->meta.pos = 0;
-  e->meta.last = per_token;
-  e->meta.first = 2 * per_token;
-  e->meta.kvrow = 3 * per_token;
-  e->meta.pt = e->meta.kvrow + align256(sizeof(long long) * T);
-  e->meta.bytes = e->meta.pt + align256(sizeof(int) * std::max(2, c.max_streams) * per_stream);
-  if (dev_alloc(e, reinterpret_cast<void**>(&e->meta_dev), e->meta.bytes, false)) return -1;
   e->sample_rows = rows;
   e->sample_ids = align256(sizeof(SampleRow) * rows);
   const size_t sample_bytes = e->sample_ids + sizeof(int) * kSamplePenaltyIds;
   if (dev_alloc(e, reinterpret_cast<void**>(&e->sample_dev), sample_bytes, false)) return -1;
-  e->sample_stage = align256(e->meta.bytes + attn_stage_bytes(T, c.max_streams, c.num_heads, c.num_kv_heads));
-  e->stage_slot_bytes = align256(e->sample_stage + sample_bytes);
-  VLO_CUDA(cudaMallocHost(reinterpret_cast<void**>(&e->stage), e->stage_slot_bytes * kStageSlots));
+  if (size_token_rows(e, T)) return -1;
   for (int i = 0; i < kStageSlots; ++i) VLO_CUDA(cudaEventCreateWithFlags(&e->stage_events[i], cudaEventDisableTiming));
 
   if (c.vit_layers > 0) {
@@ -719,6 +765,7 @@ int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64
 }  // namespace
 
 int vlo_finalize_weights(vlo_engine* e) {
+  DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr, "null engine");
   const vlo_config& c = e->cfg;
   const int64_t H = c.hidden_size, I = c.intermediate_size, V = c.vocab_size;
@@ -785,6 +832,13 @@ int vlo_finalize_weights(vlo_engine* e) {
       if (lookup(e, "vit.head.fc1.w", M * C, &e->head_fc1_w) || lookup(e, "vit.head.fc1.b", M, &e->head_fc1_b)) return -1;
       if (lookup(e, "vit.head.fc2.w", C * M, &e->head_fc2_w) || lookup(e, "vit.head.fc2.b", C, &e->head_fc2_b)) return -1;
     }
+  }
+  // A bf16 engine prefills (vlo_prefill): its token-row workspaces grow once to max_prefill rows.  Engines with e4m3 layer
+  // weights or activations chunk long inputs into steps and keep them at max_step_tokens.
+  if (e->has_decoder && !e->fp8_weights && !e->fp8_act && e->max_prefill == 0) {
+    VLO_CUDA(cudaDeviceSynchronize());   // no step, copy or staging slot of this engine may be in flight
+    if (size_token_rows(e, kFixMaxPlanes * c.max_step_tokens)) return -1;
+    e->max_prefill = kFixMaxPlanes * c.max_step_tokens;
   }
   e->finalized = true;
   return 0;
@@ -1232,9 +1286,12 @@ namespace {
 
 // The decoder step.  Sequence i carries h_seg_counts[i] consecutive segments (h_seg_counts == NULL: one each) whose
 // lengths follow one another in h_seg_lens; one lm_head row and one decision per segment, read at its last row.
+// prefill (vlo_prefill): one sequence of one segment, up to max_prefill rows, whose layer GEMMs run on
+// gemm_prefill_kernel and whose attention plans each max_step_tokens piece as a step of its own: the bits of the same
+// rows fed as max_step_tokens steps.
 int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_seg_counts,
                   const int32_t* h_seg_lens, const int64_t* d_row_ids, const void* d_embeds, void* d_last_logits,
-                  vlo_decision* d_decisions, int interval_id, cudaStream_t st) {
+                  vlo_decision* d_decisions, int interval_id, cudaStream_t st, bool prefill = false) {
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
   const vlo_config& c = e->cfg;
@@ -1260,7 +1317,11 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
     T += q_lens[i];
   }
   // every segment holds at least one token, so the n_rows <= T decision rows fit the buffers sized in engine_init
-  VLO_CHECK(T <= c.max_step_tokens, "step: total new tokens exceed max_step_tokens");
+  if (prefill)
+    VLO_CHECK(n_seqs == 1 && n_rows == 1 && T <= e->max_prefill,
+              "prefill: one stream of 1.." + std::to_string(e->max_prefill) + " tokens (max_prefill_tokens)");
+  else
+    VLO_CHECK(T <= c.max_step_tokens, "step: total new tokens exceed max_step_tokens");
   const int32_t* h_q_lens = q_lens.data();
   // ---- pages for the new tokens, taken before anything is enqueued
   KvGrowth growth{e->pool};
@@ -1277,6 +1338,8 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   std::vector<int> pt0(n_seqs);
   const int n_pt = stage_page_tables(e, hs, n_seqs, h_stream_ids, pt0.data());
   std::vector<AttnSeq> seqs(n_seqs);
+  std::vector<int> pieces;   // prefill: the max_step_tokens pieces of the chunked path, each attended as its own step
+  for (int o = 0; prefill && o < T; o += c.max_step_tokens) pieces.push_back(std::min(c.max_step_tokens, T - o));
   int t = 0;
   for (int i = 0; i < n_seqs; ++i) {
     const int sid = h_stream_ids[i], ql = h_q_lens[i], past = e->pool.len(sid);
@@ -1291,7 +1354,8 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
       end += h_seg_lens[seg0[i] + s];
       last_index[t + end - 1] = seg0[i] + s;
     }
-    seqs[i] = AttnSeq{t, ql, past + ql, pt0[i], n_segs, h_seg_lens + seg0[i]};
+    seqs[i] = prefill ? AttnSeq{t, ql, past + ql, pt0[i], static_cast<int>(pieces.size()), pieces.data()}
+                      : AttnSeq{t, ql, past + ql, pt0[i], n_segs, h_seg_lens + seg0[i]};
     t += ql;
   }
   VLO_CUDA(cudaMemcpyAsync(e->meta_dev, hs, e->meta.pt + sizeof(int) * n_pt, cudaMemcpyHostToDevice, st));
@@ -1325,6 +1389,16 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   const void* xn_in = a8 ? static_cast<const void*>(e->xq) : e->xn;
   const void* attn_in = a8 ? static_cast<const void*>(e->aq) : e->attn_out;
   const void* act_in = a8 ? static_cast<const void*>(e->actq) : e->act;
+  // the layer GEMMs: stream-K partial planes of the step's plan, or the prefill GEMM's one plane (fix-up plan: G = 1)
+  auto partial = [&](const DecW& w, int n_out, const void* x, int k, GemmWsPlan* sk, const float* x_scale) -> int {
+    if (!prefill) return dec_partial(e, w, n_out, x, T, k, sk, st, x_scale);
+    VLO_CHECK(static_cast<size_t>(T) * n_out <= e->part_elems, "prefill: the plane exceeds the partial workspace");
+    return gemm_prefill_launch(PREFILL_PLANE, w.w, n_out, x, T, k, 0, e->part, st, &sk->sk);
+  };
+  auto swiglu = [&](const DecW& w) -> int {
+    if (!prefill) return gemm_swiglu(e, w, 2 * c.intermediate_size, xn_in, T, H, st, a8 ? e->xs : nullptr);
+    return gemm_prefill_launch(PREFILL_SWIGLU, w.w, 2 * c.intermediate_size, e->xn, T, H, 0, e->act, st);
+  };
 
   if (resid_norm(nullptr, e->dec[0].in_norm, false)) return -1;
   const int attn_width = c.num_heads * c.head_dim;
@@ -1333,20 +1407,20 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
     GemmWsPlan sk{};
     const bool is_last = (l == c.num_layers - 1);
     // ---- q|k|v projection, then RoPE + in-place KV append
-    if (dec_partial(e, d.qkv, e->qkv_width, xn_in, T, H, &sk, st, a8 ? e->xs : nullptr)) return -1;
+    if (partial(d.qkv, e->qkv_width, xn_in, H, &sk, a8 ? e->xs : nullptr)) return -1;
     if (qkv_rope_launch(e->part, sk.sk, e->rope_cos, e->rope_sin, d_tok_pos, d_tok_kvrow, KvPool::head_stride_rows(), e->q,
                         kv_layer_base(e, l, 0), kv_layer_base(e, l, 1), T, c.num_heads, c.num_kv_heads, st))
       return -1;
     if (attn_layer(e, plan, l, st)) return -1;
     // ---- o_proj + residual, then post-attention RMSNorm
     if (a8 && quant_rows_launch(e->attn_out, T, attn_width, e->aq, e->as, st)) return -1;
-    if (dec_partial(e, d.o, H, attn_in, T, attn_width, &sk, st, a8 ? e->as : nullptr)) return -1;
+    if (partial(d.o, H, attn_in, attn_width, &sk, a8 ? e->as : nullptr)) return -1;
     if (resid_norm(&sk, d.post_norm, false)) return -1;
     // ---- gate|up + SwiGLU
-    if (gemm_swiglu(e, d.gate_up, 2 * c.intermediate_size, xn_in, T, H, st, a8 ? e->xs : nullptr)) return -1;
+    if (swiglu(d.gate_up)) return -1;
     // ---- down_proj + residual, then the next RMSNorm (next layer's input norm, or the final norm + last-row compaction)
     if (a8 && quant_rows_launch(e->act, T, c.intermediate_size, e->actq, e->acts, st)) return -1;
-    if (dec_partial(e, d.down, H, act_in, T, c.intermediate_size, &sk, st, a8 ? e->acts : nullptr)) return -1;
+    if (partial(d.down, H, act_in, c.intermediate_size, &sk, a8 ? e->acts : nullptr)) return -1;
     if (resid_norm(&sk, is_last ? e->final_norm : e->dec[l + 1].in_norm, is_last)) return -1;
   }
   // ---- last-position lm_head + on-device decision (one row per segment)
@@ -1378,6 +1452,20 @@ int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, co
   return step_segments(e, n_seqs, h_stream_ids, h_seg_counts, h_seg_lens, d_row_ids, d_embeds, d_seg_logits, d_decisions,
                        interval_id, static_cast<cudaStream_t>(cuda_stream));
 }
+
+int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row_ids, const void* d_embeds,
+                void* d_last_logits, vlo_decision* d_decision, int interval_id, void* cuda_stream) {
+  VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
+  VLO_CHECK(!e->fp8_weights && !e->fp8_act && e->max_prefill > 0,
+            "prefill: bf16 layer weights and activations only (e4m3 engines chunk long inputs into steps)");
+  VLO_CHECK(n_tokens > 0 && n_tokens <= e->max_prefill,
+            "prefill: n_tokens must lie in [1, max_prefill_tokens] = [1, " + std::to_string(e->max_prefill) + "]");
+  VLO_CHECK(d_embeds != nullptr, "prefill: null embeddings");
+  return step_segments(e, 1, &stream_id, nullptr, &n_tokens, d_row_ids, d_embeds, d_last_logits, d_decision, interval_id,
+                       static_cast<cudaStream_t>(cuda_stream), true);
+}
+
+int vlo_max_prefill_tokens(vlo_engine* e) { return e ? e->max_prefill : 0; }
 
 int vlo_step(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_q_lens, const void* d_embeds,
              void* d_last_logits, vlo_decision* d_decisions, int interval_id, void* cuda_stream) {

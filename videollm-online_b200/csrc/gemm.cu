@@ -2,6 +2,7 @@
 // resolved at run time, so the library loads on a box without libcuda), tile-shape
 // selection, stream-K planning and kernel dispatch.
 #include "gemm.cuh"
+#include "gemm_prefill.cuh"
 #include "gemm_vit.cuh"
 #include "gemm_ws.cuh"
 #include "gemm_wsf.cuh"
@@ -355,6 +356,45 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
   if (prof_on())
     prof_begin(PROF_GEMM_VIT, stream, 2.0 * k * (static_cast<double>(rows_w) + rows_x) + 2.0 * rows_x * rows_w);
   VLO_CUDA(launch_pdl(kern, dim3(G), dim3(kVitGemmThreads), GemmVitCfg::kSmemBytes, stream, tx, tw, a));
+  prof_end(stream);
+  count_launch();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// prefill GEMM, tokens on wgmma M, with the chunked path's stream-K k-ranges (gemm_prefill.cuh)
+
+int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
+                        cudaStream_t stream, SkInfo* sk) {
+  VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
+  VLO_CHECK(rows_w > 0 && rows_x > 0, "empty GEMM operand");
+  VLO_CHECK(epi == PREFILL_PLANE || epi == PREFILL_SWIGLU, "gemm_prefill: unknown epilogue");
+  VLO_CHECK(epi != PREFILL_SWIGLU || rows_w % kGemmBM == 0, "gemm_prefill: the SwiGLU epilogue needs whole 128-row tiles");
+  VLO_CHECK(out != nullptr, "gemm_prefill: null output");
+  GemmPrefillArgs a{};
+  a.rows_x = rows_x;
+  a.rows_w = rows_w;
+  a.k = k;
+  a.m_tiles = (rows_x + kGemmBM - 1) / kGemmBM;
+  const int w_tiles = (rows_w + kGemmBM - 1) / kGemmBM;
+  a.tiles = a.m_tiles * w_tiles;
+  gemm_ws_plan(w_tiles, k, 0, n_ctas, &a.sk);   // the plan of one chunk: one token tile
+  if (epi == PREFILL_PLANE)
+    a.plane = static_cast<float*>(out);
+  else
+    a.act = static_cast<__nv_bfloat16*>(out);
+  if (sk) *sk = SkInfo{a.sk.U, a.sk.kb, 1};      // G = 1: every tile has one plane
+  const int G = std::min(num_sms(), a.tiles);
+  CUtensorMap tx, tw;
+  if (get_tmap(x, rows_x, k, kGemmBM, FMT_BF16, &tx) != 0) return -1;
+  if (get_tmap(w, rows_w, k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
+  auto kern = epi == PREFILL_PLANE ? gemm_prefill_kernel<PREFILL_PLANE> : gemm_prefill_kernel<PREFILL_SWIGLU>;
+  if (ensure_max_smem(reinterpret_cast<const void*>(kern), GemmPrefillCfg::kSmemBytes)) return -1;
+  if (prof_on()) {
+    const double out_b = epi == PREFILL_PLANE ? 4.0 * rows_x * rows_w : 1.0 * rows_x * rows_w;
+    prof_begin(PROF_GEMM_STREAM, stream, 2.0 * k * (static_cast<double>(rows_w) + rows_x) + out_b);
+  }
+  VLO_CUDA(launch_pdl(kern, dim3(G), dim3(kPrefillThreads), GemmPrefillCfg::kSmemBytes, stream, tx, tw, a));
   prof_end(stream);
   count_launch();
   return 0;

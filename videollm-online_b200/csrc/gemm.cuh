@@ -31,6 +31,8 @@ enum GemmAct : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF_PY = 2 };
 // FMT_E4M3_A8: e4m3 weights (row scales) x e4m3 activations (token scales), multiplied by the FP8 wgmma (QGMMA) on
 // SWIZZLE_64B stages; each partial is scaled once in the epilogue (weight-streaming kernels, stream-K partials only)
 enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2, FMT_E4M3_A8 = 3 };
+// epilogues of the prefill GEMM (gemm_prefill.cuh): one fp32 plane for the fix-up kernels, or gate|up + SwiGLU
+enum PrefillEpi : int { PREFILL_PLANE = 0, PREFILL_SWIGLU = 1 };
 
 struct GemmArgs {
   int rows_a, rows_b, k;
@@ -263,6 +265,10 @@ __device__ __forceinline__ uint16_t to16(float x) {
   if (FMT == FMT_BF16) return __bfloat16_as_ushort(__float2bfloat16_rn(x));
   return __half_as_ushort(__float2half_rn(x));
 }
+
+// LlamaMLP's act_fn(gate) * up on bf16 values g, u (HF:...llama.py:182-184): bf16(silu(g)) * u in fp32, which the caller
+// rounds to bf16 once.  The gate|up finisher (gemm_wsf.cuh) and the prefill GEMM (gemm_prefill.cuh) share it.
+__device__ __forceinline__ float swiglu_bf16(float g, float u) { return bf16_round(g / (1.0f + expf(-g))) * u; }
 
 // MUFU.TANH (PTX ISA: maximum relative error 2^-10.987 over the entire range); vlo_op_tanh_approx exposes it to tests
 __device__ __forceinline__ float tanh_approx(float x) {

@@ -242,9 +242,7 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
           for (int j = 0; j < 16; ++j) {
             const int t = c0 + j;
             if (t >= p.rows_x) break;
-            const float g = x[j], up = xch[d * kWsfXchStride + j];
-            const float a = bf16_round(g / (1.0f + expf(-g)));
-            p.act[static_cast<size_t>(t) * p.I + f] = __float2bfloat16_rn(a * up);
+            p.act[static_cast<size_t>(t) * p.I + f] = __float2bfloat16_rn(swiglu_bf16(x[j], xch[d * kWsfXchStride + j]));
           }
         }
         wg_sync();

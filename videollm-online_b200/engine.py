@@ -323,6 +323,25 @@ class Engine:
         return "L0.qkv.f8" in self._weights
 
     @property
+    def max_prefill_tokens(self) -> int:
+        """rows of one vlo_prefill (8 x max_step_tokens) once bf16 layer weights are loaded; 0 before, and on engines
+        with e4m3 layer weights or activations"""
+        return int(self.lib.vlo_max_prefill_tokens(self._h))
+
+    @property
+    def prefills(self) -> bool:
+        """True when one stream's input longer than max_step_tokens runs as a prefill (vlo_prefill: tokens-on-M tensor-core
+        GEMMs over up to max_prefill_tokens rows per call, with the bits of max_step_tokens steps).  Engines with e4m3
+        layer weights or activations chunk such inputs into steps instead."""
+        return self.max_prefill_tokens > 0
+
+    @property
+    def max_pass_tokens(self) -> int:
+        """the most rows one single-stream `step` computes in one pass, so that `last_step_logits` /
+        `last_step_hidden` cover all of them: max_prefill_tokens on a prefilling engine, else max_step_tokens"""
+        return self.max_prefill_tokens if self.prefills else self.max_step_tokens
+
+    @property
     def fp8_activations(self) -> bool:
         """True when the layer GEMMs take e4m3 activations with per-token scales (W8A8; Engine(fp8_activations=True))."""
         return self._fp8_act
@@ -642,6 +661,8 @@ class Engine:
         if segments is not None:
             return self._step_segments(stream_ids, q_lens, segments, embeds, row_ids, interval_id, want_logits)
         if T > self.max_step_tokens:
+            if n == 1 and self.prefills:
+                return self._prefill(stream_ids[0], T, embeds, row_ids, interval_id, want_logits)
             return self._step_chunked(stream_ids, q_lens, embeds, row_ids, interval_id, want_logits)
         iid, pid = self._step_inputs(T, embeds, row_ids, interval_id)
         sid = (C.c_int32 * n)(*stream_ids)
@@ -683,10 +704,31 @@ class Engine:
                                          _ptr(self._dec_dev), iid, self._stream()), "vlo_step_segments")
         return logits, self._dec_dev[:n_rows]
 
+    def _prefill(self, sid, T, embeds, row_ids, interval_id, want_logits):
+        """One stream's input longer than max_step_tokens on a bf16 engine: vlo_prefill calls of up to max_prefill_tokens
+        rows, each giving the bits of the same rows fed as max_step_tokens steps.  The logits / decision come from the
+        last call; if a later call fails (e.g. on an exhausted KV page pool), the earlier ones are taken back, so the
+        call changes nothing and the caller can retry it whole."""
+        iid, pid = self._step_inputs(T, embeds, row_ids, interval_id)
+        cap = self.max_prefill_tokens
+        kv0 = self.kv_len(sid)
+        logits = self._logits[:1] if want_logits else None
+        try:
+            for lo in range(0, T, cap):
+                n = min(cap, T - lo)
+                last = lo + n == T
+                check(self.lib.vlo_prefill(self._h, sid, n, _ptr(None if pid is None else pid[lo:lo + n]),
+                                           _ptr(embeds[lo:lo + n]), _ptr(logits if last else None),
+                                           _ptr(self._dec_dev[:1]), iid, self._stream()), "vlo_prefill")
+        except VloError:
+            self.kv_truncate(sid, kv0)
+            raise
+        return logits, self._dec_dev[:1]
+
     def _step_chunked(self, stream_ids, q_lens, embeds, row_ids, interval_id, want_logits):
-        """Inputs longer than max_step_tokens (the first frame's system prompt, long queries): feed the KV-append
-        forward in pieces — chunked streaming is exactly one causal pass (SURVEY.md Appendix C.1).  Each
-        sequence's logits / decision come from the sub-step that holds its last piece."""
+        """Ragged multi-stream inputs longer than max_step_tokens, and long inputs on engines that do not prefill (e4m3
+        layer weights): feed the KV-append forward in pieces — chunked streaming is exactly one causal pass (SURVEY.md
+        Appendix C.1).  Each sequence's logits / decision come from the sub-step that holds its last piece."""
         n, cap, H = len(stream_ids), self.max_step_tokens, self.cfg.hidden_size
         if row_ids is not None:  # materialise the gathered token rows once; the sub-steps then see plain embeddings
             pid = row_ids.to(self.device).view(-1)

@@ -128,14 +128,15 @@ class LiveLlamaForCausalLM:
 
     # --- evaluation (SURVEY 8(f) row 4)
     def forward_all_logits(self, inputs_embeds: torch.Tensor, past_key_values: StreamKV) -> torch.Tensor:
-        """Teacher-forced KV-append forward returning the logits of EVERY position ([L, V] bf16), fed in chunks of
-        the engine's step capacity (chunked streaming == one causal pass): the reference's
-        `self.forward(..., use_cache=True).logits[0]` (models/modeling_live.py:67) on the engine's cache."""
+        """Teacher-forced KV-append forward returning the logits of EVERY position ([L, V] bf16), fed in pieces of
+        the engine's one-pass capacity (prefills of max_prefill_tokens, or steps of max_step_tokens; chunked streaming
+        == one causal pass): the reference's `self.forward(..., use_cache=True).logits[0]` (models/modeling_live.py:67)
+        on the engine's cache."""
         eng = self.engine
         x = inputs_embeds.reshape(-1, self.config.hidden_size).to(torch.bfloat16)
-        outs = []
-        for lo in range(0, x.shape[0], eng.max_step_tokens):
-            chunk = x[lo:lo + eng.max_step_tokens].contiguous()
+        outs, cap = [], eng.max_pass_tokens
+        for lo in range(0, x.shape[0], cap):
+            chunk = x[lo:lo + cap].contiguous()
             eng.step([past_key_values.stream_id], [chunk.shape[0]], chunk, want_logits=False)
             outs.append(eng.last_step_logits(chunk.shape[0]))
         return torch.cat(outs, 0)
