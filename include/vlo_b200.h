@@ -93,9 +93,17 @@ int vlo_engine_destroy(vlo_engine* e);
  * packing at init).  The engine keeps the pointer; the caller keeps the storage alive. */
 int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t n_bytes);
 /* Resolve and size-check the registered tensors.  Each decoder layer matrix L{i}.{qkv,o,gate_up,down} comes in exactly
- * one form: bf16 `name`, or FP8 weights `name.f8` (e4m3fn bytes [N, K]) + `name.scale` (fp32 [N], one per row).  All
- * 4 x num_layers matrices must share one form; a mixed set, a missing scale or a wrong size fails with a message that
- * names the tensor.  The form decides which GEMM kernels the layer loop runs. */
+ * one form: bf16 `name`, or FP8 weights `name.f8` (e4m3fn bytes [N, K]) + `name.scale` (fp32 [N], one per row), or int4
+ * weights `name.i4` + `name.gscale`.  All 4 x num_layers matrices must share one form; a mixed set, a missing scale or a
+ * wrong size fails with a message that names the tensor.  The form decides which GEMM kernels the layer loop runs.
+ * The int4 form (W4A16, weights.quantize_int4_groups), groups of 128 along K (K % 128 == 0, else finalize fails):
+ *   s[n, g] = bf16_rn(fp32(max_{k in g} |W[n,k]|) / 7), 1 where that is 0;  q[n, k] = clamp(rne(fp32(W) / fp32(s)), -8, 7);
+ *   the weight every kernel multiplies is W4[n, k] = bf16_rn(q * s) (q * s is exact in fp32: one rounding).
+ * `name.gscale` is bf16 [N, K / 128].  `name.i4` holds the codes q + 8, two per byte, ceil(N / 128) x 128 x K / 2 bytes in
+ * the engine byte order: one 4 KB block per (128-row tile, 64-wide k-block), blocks in (tile, k-block) order, and inside a
+ * block thread t of the consumer warpgroup's 16 bytes per 64-row half h at h * 2048 + 16 t (DESIGN.md section 2,
+ * weights.pack_int4_codes).  Every result is bit for bit the bf16 engine's on W4.  An int4 engine does not prefill
+ * (vlo_max_prefill_tokens is 0) and takes no FP8 activations (finalize fails with a message). */
 int vlo_finalize_weights(vlo_engine* e);
 /* bytes of device memory the engine allocated itself (KV + workspaces) */
 int64_t vlo_engine_device_bytes(vlo_engine* e);
@@ -390,6 +398,13 @@ int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const 
  * k-blocks.  d_out == NULL only plans (*h_max_planes).  Asynchronous. */
 int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale, int rows_x,
                       int k, float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream);
+/* The same GEMM in mode 0 on int4 weights (the decoder's W4A16 form, see vlo_finalize_weights): d_w4 the codes in the
+ * engine byte order, d_gscale bf16 [rows_w, k / 128], X bf16 [rows_x, k], 1 <= rows_x <= 128, k % 128 == 0.  Same token
+ * tile and stream-K plan as the bf16 call with these sizes and n_ctas; the codes are dequantized to W4 in registers and
+ * multiplied by the bf16 wgmma chain, so every plane is bit for bit that of the bf16 call on W4.  d_out == NULL only
+ * plans (*h_max_planes).  Asynchronous. */
+int vlo_op_gemm_ws_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
+                      long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream);
 /* ViT trunk GEMM (csrc/gemm_vit.cuh), fp16, 128-token x 128-feature tiles:
  * out[t][n] = act(fp16(sum_k X[t,k] W[n,k] + bias[n])), fp16 out[rows_x][ld_out], ld_out even and >= rows_w;
  * n_ctas <= 0: one CTA per SM. */
@@ -527,6 +542,10 @@ int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, co
 int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale,
                           int rows_x, int k, void* d_act, float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags,
                           void* cuda_stream);
+/* vlo_op_gemm_swiglu on int4 weights (d_w4, d_gscale as in vlo_op_gemm_ws_i4; same row order and plan): bit for bit
+ * vlo_op_gemm_swiglu on W4.  Asynchronous. */
+int vlo_op_gemm_swiglu_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
+                          float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream);
 /* Speak / silent decision over bf16 logits [n_rows, vocab] (vocab a multiple of 8, rows 16-byte aligned), one
  * vlo_decision per row into d_out (device): first-index argmax, max logit, max - second max (a repeated maximum counts
  * as the second), log-sum-exp, p_interval = bf16(softmax[interval_id]) (0 when interval_id is outside the row), and the

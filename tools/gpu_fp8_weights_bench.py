@@ -1,12 +1,13 @@
-"""Dev tool: FP8 (e4m3) decoder weights, and FP8 weights with FP8 activations (W8A8), against bf16 on the full-size
-synthetic model (same seed; the FP8 engines hold the quantized layer matrices of the bf16 engine's weights).  The three
-engines are alternated in one run, REPEATS times.
+"""Dev tool: FP8 (e4m3) decoder weights, FP8 weights with FP8 activations (W8A8) and int4 weights with per-group scales
+(W4A16) against bf16 on the full-size synthetic model (same seed; the quantized engines hold the quantized layer matrices
+of the bf16 engine's weights).  The four engines are alternated in one run, REPEATS times.
 
   card      GPU name and power limit (nvidia-smi), read in the same run
   memory    weight bytes and engine device bytes of each form, and the KV pool tokens / pages the smaller weights free at
-            one memory budget (131 072 B per token, 64-token pages)
-  gemm      vlo_bench_gemm (the 4 x 32 layer GEMMs, planes only; W8A8: on the e4m3 activation copies) at 11 tokens: ms
-            per pass and algorithmic TB/s
+            one memory budget (131 072 B per token, 64-token pages), against bf16: one entry per quantized form (these
+            fields were scalars for FP8 alone before the int4 arm; nothing in the repository reads the records back)
+  gemm      vlo_bench_gemm (the 4 x 32 layer GEMMs, planes only; W8A8: on the e4m3 activation copies; int4: codes and
+            group scales) at 11 tokens: ms per pass and algorithmic TB/s
   step      decoder step device ms (CUDA events), median of STEPS, at q = 11 and q = 1, at 12 288 and 66 048 keys
   backlog   one segmented step of 11 frames (11 x 11 rows) at 12 288 keys: decoder ms per frame
   response  1-token steps at 12 288 keys with the host reading each decision (a greedy response's loop): tokens/s
@@ -25,7 +26,7 @@ cfg = llama3_8b_siglip_l()
 KEYS = (12288, 66048)
 REPEATS, STEPS, GEMM_ITERS, FRAMES = 3, 30, 20, 300
 TOKEN_BYTES, PAGE = 131072, 64
-FORMS = ("bf16", "fp8", "w8a8")
+FORMS = ("bf16", "fp8", "w8a8", "int4")
 
 
 def emit(part, d):
@@ -39,20 +40,22 @@ emit("card", {"gpu": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit
 cap = KEYS[-1] + 256
 engines, wbytes = {}, {}
 for form in FORMS:
-    w = {k: v for k, v in W.synthetic_engine_weights(cfg, dev, cap, seed=0, fp8_weights=form != "bf16").items()
+    w = {k: v for k, v in W.synthetic_engine_weights(cfg, dev, cap, seed=0, fp8_weights=form in ("fp8", "w8a8"),
+                                                     int4_weights=form == "int4").items()
          if not k.startswith("vit.")}
     wbytes[form] = W.engine_weight_bytes(w)
     eng = Engine(cfg, dev, max_streams=1, max_kv_tokens=cap, max_step_tokens=128, max_vit_batch=1,
                  fp8_activations=form == "w8a8")
     eng.load_weights(w)
-    assert eng.fp8_weights == (form != "bf16") and eng.fp8_activations == (form == "w8a8")
+    assert eng.fp8_weights == (form in ("fp8", "w8a8")) and eng.fp8_activations == (form == "w8a8")
+    assert eng.int4_weights == (form == "int4")
     engines[form] = (eng, eng.stream_open())
     del w
     torch.cuda.empty_cache()
-freed = wbytes["bf16"] - wbytes["fp8"]
+freed = {f: wbytes["bf16"] - wbytes[f] for f in FORMS if f != "bf16"}
 emit("memory", {"weight_bytes": wbytes, "device_bytes": {f: engines[f][0].device_bytes() for f in FORMS},
-                "freed_bytes": freed, "extra_pool_tokens": freed // TOKEN_BYTES,
-                "extra_pool_pages": freed // (TOKEN_BYTES * PAGE)})
+                "freed_bytes": freed, "extra_pool_tokens": {f: b // TOKEN_BYTES for f, b in freed.items()},
+                "extra_pool_pages": {f: b // (TOKEN_BYTES * PAGE) for f, b in freed.items()}})
 
 ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 
@@ -134,8 +137,8 @@ from videollm_online_b200.cli import synthetic_clip   # noqa: E402
 from videollm_online_b200.config import LiveArguments   # noqa: E402
 from videollm_online_b200.inference import LiveInfer   # noqa: E402
 
-lis = {f: LiveInfer(LiveArguments(synthetic_weights=True, device="cuda:0", fp8_weights=f != "bf16",
-                                  fp8_activations=f == "w8a8")) for f in FORMS}
+lis = {f: LiveInfer(LiveArguments(synthetic_weights=True, device="cuda:0", fp8_weights=f in ("fp8", "w8a8"),
+                                  fp8_activations=f == "w8a8", int4_weights=f == "int4")) for f in FORMS}
 
 
 def silent_frames(dec, n):

@@ -119,6 +119,7 @@ SIGNATURES = {
     "vlo_op_gemm_ws": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_ws_tiled": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, _I, C.POINTER(C.c_int32), _P]),
     "vlo_op_gemm_ws_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
+    "vlo_op_gemm_ws_i4": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_ws_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),
@@ -143,6 +144,7 @@ SIGNATURES = {
     "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_prefill": (_I, [_I, _P, _I, _P, _I, _I, _I, _P, _P]),
     "vlo_op_gemm_swiglu_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
+    "vlo_op_gemm_swiglu_i4": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_swiglu_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_op_sample": (_I, [_P, _I, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P, _P]),

@@ -19,6 +19,8 @@ device.  A stream that ends inside a frame drops it with a warning.  A camera at
 numbers change, so it is off by default).
 --fp8_activations (with --fp8_weights) also quantizes the layer GEMMs' activations to e4m3 per token and multiplies them on
 the FP8 tensor cores (W8A8); off by default for the same reason.
+--int4_weights serves the decoder layers from 4-bit weights with one bf16 scale per 128 weights of a row (W4A16: a
+quarter of their bf16 bytes per step); the numbers change, so it is off by default, and it excludes the FP8 flags.
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

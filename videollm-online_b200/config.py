@@ -161,6 +161,9 @@ class LiveArguments:
     # with fp8_weights: quantize each layer GEMM's activations to e4m3 per token and multiply on the FP8 tensor cores
     # (W8A8); changes the model's numbers again, so off by default
     fp8_activations: bool = False
+    # serve the decoder layer matrices from 4-bit codes with one bf16 scale per 128 weights of a row (W4A16, a quarter of
+    # the bf16 bytes); changes the model's numbers, so off by default; excludes fp8_weights and fp8_activations
+    int4_weights: bool = False
     # LiveInfer.context_window, tokens: keep the start prompt and drop the oldest cache pages after it so the session's
     # cache never exceeds this many tokens; 0: off (the cache grows until max_kv_tokens)
     context_window: int = 0

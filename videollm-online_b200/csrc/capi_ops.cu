@@ -183,6 +183,29 @@ int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const 
   return rc;
 }
 
+int vlo_op_gemm_ws_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
+                      long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
+  VLO_CHECK(d_out == nullptr || d_gscale != nullptr, "gemm_ws_i4: null group scales");
+  GemmWsCall c{};
+  c.fmt = FMT_I4;
+  c.mode = 0;
+  c.w = d_w4;
+  c.g_scale = static_cast<const uint16_t*>(d_gscale);
+  c.rows_w = rows_w;
+  c.x = d_x;
+  c.rows_x = rows_x;
+  c.k = k;
+  c.out = d_out;
+  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
+  c.ld_out = rows_w;
+  c.plane_stride = plane_stride;
+  c.n_ctas = n_ctas;
+  GemmWsPlan plan{};
+  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
+  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
+  return rc;
+}
+
 int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale, int rows_x,
                       int k, float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
   VLO_CHECK(d_out == nullptr || (d_scale != nullptr && d_xscale != nullptr), "gemm_ws_a8: null row or token scales");
@@ -489,6 +512,14 @@ int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, co
   VLO_CHECK(d_scale != nullptr && d_xscale != nullptr, "gemm_swiglu_a8: null row or token scales");
   return gemm_wsf_launch(d_w8, d_scale, rows_w, d_x8, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
                          n_flags, static_cast<cudaStream_t>(cuda_stream), d_xscale);
+}
+
+int vlo_op_gemm_swiglu_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
+                          float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
+  VLO_CHECK(plane_elems >= 0, "gemm_swiglu_i4: plane_elems");
+  VLO_CHECK(d_gscale != nullptr, "gemm_swiglu_i4: null group scales");
+  return gemm_wsf_launch(d_w4, nullptr, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
+                         n_flags, static_cast<cudaStream_t>(cuda_stream), nullptr, static_cast<const uint16_t*>(d_gscale));
 }
 
 int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream) {

@@ -28,10 +28,12 @@ constexpr int kRotFloats = 128;  // vlo_kv_evict's cos | sin (head_dim / 2 each)
 
 using bf16 = __nv_bfloat16;
 
-// a layer matrix [n, k]: bf16 (scale null) or e4m3 bytes with fp32 row scales [n]
+// a layer matrix [n, k]: bf16 (scale and gscale null), e4m3 bytes with fp32 row scales [n], or int4 codes in the engine
+// byte order with bf16 group scales [n, k / 128]
 struct DecW {
   const void* w;
   const float* scale;
+  const uint16_t* gscale;
 };
 struct DecLayer {
   const bf16 *in_norm, *post_norm;
@@ -63,6 +65,7 @@ struct vlo_engine {
   const bf16 *conn0_w = nullptr, *conn2_w = nullptr;
   bool has_vit = false, has_connector = false, has_decoder = false;
   bool fp8_weights = false;  // the layer matrices are e4m3 + row scales (vlo_finalize_weights)
+  bool int4_weights = false; // the layer matrices are int4 codes + group scales (vlo_finalize_weights)
   bool fp8_act = false;      // vlo_set_fp8_activations: the layer GEMMs take e4m3 activations with token scales
 
   // derived
@@ -234,6 +237,25 @@ int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int
 // e4m3 copy of the activations with these token scales (fp8_act).
 int dec_partial(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, int k, GemmWsPlan* sk, cudaStream_t st,
                 const float* x_scale = nullptr) {
+  if (w.gscale != nullptr) {
+    GemmWsCall c{};
+    c.fmt = FMT_I4;
+    c.g_scale = w.gscale;
+    c.mode = 0;
+    c.w = w.w;
+    c.rows_w = n_out;
+    c.x = x;
+    c.rows_x = T;
+    c.k = k;
+    c.out = e->part;
+    c.out_elems = e->part_elems;
+    c.ld_out = n_out;
+    c.plane_stride = static_cast<long long>(T) * n_out;
+    c.tiling = WS_TILE_FIT;
+    if (gemm_ws_launch(c, st, sk)) return -1;
+    VLO_CHECK(sk->planes <= kFixMaxPlanes, "stream-K produced more partial planes than the fix-up kernels unroll");
+    return 0;
+  }
   return gemm_partial(x_scale ? FMT_E4M3_A8 : w.scale ? FMT_E4M3 : FMT_BF16, w.w, n_out, x, T, k, e->part, e->part_elems,
                       WS_TILE_FIT, sk, st, w.scale, x_scale);
 }
@@ -245,7 +267,8 @@ int dec_partial(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, i
 // its fix-up; q|k|v, o_proj and down_proj go through gemm_partial and a fix-up kernel (DESIGN.md section 5).
 int gemm_swiglu(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, int k, cudaStream_t st,
                 const float* x_scale = nullptr) {
-  return gemm_wsf_launch(w.w, w.scale, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st, x_scale);
+  return gemm_wsf_launch(w.w, w.scale, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st, x_scale,
+                         w.gscale);
 }
 
 // whole-tile persistent GEMM with the 16-bit epilogue: out[T, n_out] = act(x W^T + bias)
@@ -737,20 +760,38 @@ int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t 
 }
 
 namespace {
-// Layer matrix `name` [n, k] in exactly one form: bf16 `name`, or e4m3 bytes `name.f8` with fp32 row scales `name.scale`.
-// *f8 < 0: the first matrix, which sets the form every later one must share.
-int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* f8, DecW* out) {
+// Layer matrix `name` [n, k] in exactly one form: bf16 `name` (form 0), e4m3 bytes `name.f8` with fp32 row scales
+// `name.scale` (form 1), or int4 codes `name.i4` with bf16 group scales `name.gscale` (form 2).  *form < 0: the first
+// matrix, which sets the form every later one must share.
+int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* forms, DecW* out) {
   const bool has16 = e->tensors.count(name) > 0, has8 = e->tensors.count(name + ".f8") > 0,
-             has_s = e->tensors.count(name + ".scale") > 0;
-  if (has16 && (has8 || has_s)) return fail("weight tensor '" + name + "' is loaded both as bf16 and as e4m3");
-  if (!has16 && !has8 && !has_s) return fail("missing weight tensor '" + name + "' (or '" + name + ".f8' + '" + name + ".scale')");
+             has_s = e->tensors.count(name + ".scale") > 0, has4 = e->tensors.count(name + ".i4") > 0,
+             has_g = e->tensors.count(name + ".gscale") > 0;
+  if (static_cast<int>(has16) + static_cast<int>(has8 || has_s) + static_cast<int>(has4 || has_g) > 1)
+    return fail("weight tensor '" + name + "' is loaded in more than one form (bf16, e4m3 '.f8' + '.scale', int4 '.i4' + '.gscale')");
+  if (!has16 && !has8 && !has_s && !has4 && !has_g)
+    return fail("missing weight tensor '" + name + "' (or '" + name + ".f8' + '" + name + ".scale', or '" + name + ".i4' + '" +
+                name + ".gscale')");
   if (has8 != has_s) return fail("missing weight tensor '" + name + (has8 ? ".scale'" : ".f8'"));
-  const int form = has8 ? 1 : 0;
-  if (*f8 >= 0 && form != *f8)
-    return fail("weight tensor '" + name + (form ? ".f8' is e4m3" : "' is bf16") +
-                " but an earlier layer matrix is not: all layer matrices must share one form");
-  *f8 = form;
+  if (has4 != has_g) return fail("missing weight tensor '" + name + (has4 ? ".gscale'" : ".i4'"));
+  const int form = has8 ? 1 : has4 ? 2 : 0;
+  static const char* const kDesc[3] = {"' is bf16", ".f8' is e4m3", ".i4' is int4"};
+  if (*forms >= 0 && form != *forms)
+    return fail("weight tensor '" + name + kDesc[form] + " but an earlier layer matrix is not: all layer matrices must share one form");
+  *forms = form;
   out->scale = nullptr;
+  out->gscale = nullptr;
+  if (form == 2) {
+    if (k % kI4Group != 0)
+      return fail("weight tensor '" + name + ".i4': int4 weights need K (" + std::to_string(k) +
+                  ") to be a multiple of 128, one scale per 128 weights of a row");
+    const uint8_t* w;
+    if (lookup(e, name + ".i4", (n + kGemmBM - 1) / kGemmBM * kGemmBM * (k / 2), &w) ||
+        lookup(e, name + ".gscale", n * (k / kI4Group), &out->gscale))
+      return -1;
+    out->w = w;
+    return 0;
+  }
   if (!form) {
     const bf16* w;
     if (lookup(e, name, n * k, &w)) return -1;
@@ -780,11 +821,11 @@ int vlo_finalize_weights(vlo_engine* e) {
     VLO_CHECK(e->rope_positions >= c.max_kv_tokens, "rope tables shorter than max_kv_tokens");
     if (lookup(e, "rope.cos", e->rope_positions * 64, &e->rope_cos)) return -1;
     if (lookup(e, "rope.sin", e->rope_positions * 64, &e->rope_sin)) return -1;
-    e->dec.resize(c.num_layers);
+    std::vector<DecLayer> dec(c.num_layers);   // installed only once every matrix has resolved
     int f8 = -1;
     for (int l = 0; l < c.num_layers; ++l) {
       const std::string p = "L" + std::to_string(l) + ".";
-      DecLayer& d = e->dec[l];
+      DecLayer& d = dec[l];
       if (lookup(e, p + "in_norm", H, &d.in_norm)) return -1;
       if (lookup_layer_matrix(e, p + "qkv", e->qkv_width, H, &f8, &d.qkv)) return -1;
       if (lookup_layer_matrix(e, p + "o", H, static_cast<int64_t>(c.num_heads) * c.head_dim, &f8, &d.o)) return -1;
@@ -792,10 +833,15 @@ int vlo_finalize_weights(vlo_engine* e) {
       if (lookup_layer_matrix(e, p + "gate_up", 2 * I, H, &f8, &d.gate_up)) return -1;
       if (lookup_layer_matrix(e, p + "down", H, I, &f8, &d.down)) return -1;
     }
-    e->fp8_weights = f8 == 1;
-    VLO_CHECK(!e->fp8_act || e->fp8_weights,
+    VLO_CHECK(!e->fp8_act || f8 != 2,
+              "fp8_activations takes FP8 (e4m3) layer weights, but the layer matrices are int4: 4-bit weights multiply "
+              "bf16 activations");
+    VLO_CHECK(!e->fp8_act || f8 == 1,
               "fp8_activations needs FP8 (e4m3) layer weights, but the layer matrices are bf16: the FP8 tensor cores "
               "take both operands in e4m3");
+    e->dec.swap(dec);
+    e->fp8_weights = f8 == 1;
+    e->int4_weights = f8 == 2;
   }
   e->has_connector = e->tensors.count("conn.0.w") > 0;
   if (e->has_connector) {
@@ -835,7 +881,7 @@ int vlo_finalize_weights(vlo_engine* e) {
   }
   // A bf16 engine prefills (vlo_prefill): its token-row workspaces grow once to max_prefill rows.  Engines with e4m3 layer
   // weights or activations chunk long inputs into steps and keep them at max_step_tokens.
-  if (e->has_decoder && !e->fp8_weights && !e->fp8_act && e->max_prefill == 0) {
+  if (e->has_decoder && !e->fp8_weights && !e->int4_weights && !e->fp8_act && e->max_prefill == 0) {
     VLO_CUDA(cudaDeviceSynchronize());   // no step, copy or staging slot of this engine may be in flight
     if (size_token_rows(e, kFixMaxPlanes * c.max_step_tokens)) return -1;
     e->max_prefill = kFixMaxPlanes * c.max_step_tokens;
@@ -1456,7 +1502,7 @@ int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, co
 int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row_ids, const void* d_embeds,
                 void* d_last_logits, vlo_decision* d_decision, int interval_id, void* cuda_stream) {
   VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
-  VLO_CHECK(!e->fp8_weights && !e->fp8_act && e->max_prefill > 0,
+  VLO_CHECK(!e->fp8_weights && !e->int4_weights && !e->fp8_act && e->max_prefill > 0,
             "prefill: bf16 layer weights and activations only (e4m3 engines chunk long inputs into steps)");
   VLO_CHECK(n_tokens > 0 && n_tokens <= e->max_prefill,
             "prefill: n_tokens must lie in [1, max_prefill_tokens] = [1, " + std::to_string(e->max_prefill) + "]");
@@ -1544,7 +1590,8 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const int H = c.hidden_size, I = c.intermediate_size, A = c.num_heads * c.head_dim;
   double bytes = 0.0;
-  const double w_elem = e->fp8_weights ? 1.0 : 2.0, row_b = e->fp8_weights ? 4.0 : 0.0;   // e4m3: 1 B + a scale per row
+  // e4m3: 1 B + a scale per row; int4: half a byte + a bf16 scale per 128 weights
+  const double w_elem = e->fp8_weights ? 1.0 : e->int4_weights ? 0.5 + 2.0 / kI4Group : 2.0, row_b = e->fp8_weights ? 4.0 : 0.0;
   // fp8_act: the W8A8 GEMMs on the e4m3 activation copies, 1 B per activation + a scale per token
   const bool a8 = e->fp8_act;
   const double x_elem = a8 ? 1.0 : 2.0, tok_b = a8 ? 4.0 : 0.0;

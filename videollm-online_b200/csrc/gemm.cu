@@ -195,9 +195,20 @@ static_assert(GemmWsCfg<16, kA8DecoderStages, FMT_E4M3_A8>::kSmemBytes + GemmVit
 static_assert(GemmWsCfg<16, kA8DecoderStages, FMT_E4M3_A8>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
               "W8A8 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
 
+// The int4 16-token decoder GEMM keeps the pairing too: the deepest ring of 24 KB slots (16 KB of codes, 8 KB of
+// activations) that fits beside the ViT trunk GEMM CTA.
+constexpr int kI4DecoderStages =
+    std::min(16, (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes - GemmWsCfg<16, 0, FMT_I4>::kSmemBytes) /
+                     (i4_slot_units(16) * (kI4BytesUnit + 16 * kGemmBK * 2)));
+static_assert(GemmWsCfg<16, kI4DecoderStages, FMT_I4>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "int4 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
+static_assert(GemmWsCfg<16, kI4DecoderStages, FMT_I4>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
+              "int4 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
+
 namespace {
 template <int FMT, int BN,
-          int STAGES = FMT == FMT_E4M3 ? ws_f8_default_stages(BN) : FMT == FMT_E4M3_A8 ? ws_a8_default_stages(BN) : ws_default_stages(BN)>
+          int STAGES = FMT == FMT_E4M3 ? ws_f8_default_stages(BN) : FMT == FMT_E4M3_A8 ? ws_a8_default_stages(BN)
+                       : FMT == FMT_I4 ? ws_i4_default_stages(BN) : ws_default_stages(BN)>
 int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
   auto kern = gemm_ws_kernel<FMT, BN, STAGES>;
   using Cfg = GemmWsCfg<BN, STAGES, FMT>;
@@ -206,6 +217,7 @@ int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a,
     const double out_b = a.mode == 0 ? 4.0 * a.rows_x * a.rows_w : 2.0 * a.rows_x * a.rows_w;
     const double in_b = FMT == FMT_E4M3      ? (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x   // 1 B per weight + row scales
                         : FMT == FMT_E4M3_A8 ? (a.k + 4.0) * (static_cast<double>(a.rows_w) + a.rows_x)   // + token scales
+                        : FMT == FMT_I4      ? (a.k / 2.0 + a.k / 64.0) * a.rows_w + 2.0 * a.k * a.rows_x   // codes + scales
                                              : 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x);
     prof_begin(FMT == FMT_F16 ? PROF_GEMM_VIT : PROF_GEMM_STREAM, stream, in_b + out_b);
   }
@@ -272,8 +284,12 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   VLO_CHECK(!beside || (c.fmt == FMT_F16 && bn == 64), "gemm_ws: only the 64-token fp16 instance fits beside a decoder CTA");
   const bool a8 = c.fmt == FMT_E4M3_A8;
   const bool f8 = c.fmt == FMT_E4M3 || a8;
+  const bool i4 = c.fmt == FMT_I4;
   VLO_CHECK(!f8 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn)),
             "gemm_ws: e4m3 weights run stream-K partials (mode 0) on the token tile token_tile() picks");
+  VLO_CHECK(!i4 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn) && c.rows_x <= 128),
+            "gemm_ws: int4 weights run stream-K partials (mode 0) of 1..128 token rows on the token tile token_tile() picks");
+  VLO_CHECK(!i4 || c.k % kI4Group == 0, "gemm_ws: int4 weights need K to be a multiple of 128 (one scale per 128 k)");
   const int x_tiles = (c.rows_x + bn - 1) / bn;
   GemmWsArgs a{};
   a.rows_w = c.rows_w;
@@ -297,7 +313,20 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   a.w_scale = c.w_scale;
   VLO_CHECK(!a8 || c.a_scale != nullptr, "gemm_ws: e4m3 activations need their token scales");
   a.a_scale = c.a_scale;
+  VLO_CHECK(!i4 || (c.g_scale != nullptr && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0),
+            "gemm_ws: int4 weights need their group scales and 16-byte aligned codes");
+  a.w4 = static_cast<const uint8_t*>(c.w);
+  a.g_scale = c.g_scale;
   CUtensorMap tw, tx;
+  if (i4) {
+    if (get_tmap(c.x, c.rows_x, c.k, bn, FMT_BF16, &tx) != 0) return -1;
+    tw = tx;   // unused: the codes stream as bulk copies
+    if (bn == 16) return launch_ws<FMT_I4, 16, kI4DecoderStages>(tw, tx, a, stream);
+    if (bn == 32) return launch_ws<FMT_I4, 32>(tw, tx, a, stream);
+    if (bn == 64) return launch_ws<FMT_I4, 64>(tw, tx, a, stream);
+    if (bn == 96) return launch_ws<FMT_I4, 96>(tw, tx, a, stream);
+    return launch_ws<FMT_I4, 128>(tw, tx, a, stream);
+  }
   if (get_tmap(c.w, c.rows_w, c.k, kGemmBM, c.fmt, &tw) != 0) return -1;
   if (get_tmap(c.x, c.rows_x, c.k, bn, a8 ? FMT_E4M3_A8 : f8 ? FMT_BF16 : c.fmt, &tx) != 0) return -1;
 #define VLO_WS_CASE(F, N) \
@@ -403,6 +432,21 @@ int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int r
 // ------------------------------------------------------------------------------------------------
 // stream-K gate|up GEMM with the SwiGLU finisher epilogue (gemm_wsf.cuh)
 namespace {
+template <int BN>
+int launch_wsf_i4(const CUtensorMap& tx, const GemmWsfArgs& a, const void* w4, const uint16_t* g_scale, cudaStream_t stream) {
+  constexpr int S = wsf_i4_default_stages(BN);
+  auto kern = gemm_wsf_i4_kernel<BN, S>;
+  using Cfg = GemmWsfCfg<BN, S, FMT_I4>;
+  if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
+  if (prof_on())   // half a byte per weight + a bf16 scale per 128
+    prof_begin(PROF_GEMM_STREAM, stream, (a.k / 2.0 + a.k / 64.0) * a.rows_w + 2.0 * a.k * a.rows_x + 2.0 * a.rows_x * a.rows_w);
+  VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tx, a,
+                      static_cast<const uint8_t*>(w4), g_scale));
+  prof_end(stream);
+  count_launch();
+  return 0;
+}
+
 // w_scale null: bf16 weights; else e4m3 weights with these row scales, and with a_scale also e4m3 activations
 template <int BN>
 int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, const float* w_scale,
@@ -445,7 +489,8 @@ int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& 
 }  // namespace
 
 int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
-                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream, const float* a_scale) {
+                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream, const float* a_scale,
+                    const uint16_t* g_scale) {
   VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(rows_w > 0 && rows_x > 0 && rows_x <= 128, "gemm_wsf: 1..128 token rows");
   VLO_CHECK(rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
@@ -465,6 +510,18 @@ int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void*
   a.act = static_cast<__nv_bfloat16*>(act);
   a.I = rows_w / 2;
   VLO_CHECK(a_scale == nullptr || w_scale != nullptr, "gemm_wsf: e4m3 activations need e4m3 weights");
+  if (g_scale != nullptr) {
+    VLO_CHECK(w_scale == nullptr && a_scale == nullptr, "gemm_wsf: int4 weights take bf16 activations");
+    VLO_CHECK(k % kI4Group == 0, "gemm_wsf: int4 weights need K to be a multiple of 128 (one scale per 128 k)");
+    VLO_CHECK((reinterpret_cast<uintptr_t>(w) & 15) == 0, "gemm_wsf: int4 codes must be 16-byte aligned");
+    CUtensorMap tx;
+    if (get_tmap(x, rows_x, k, bn, FMT_BF16, &tx) != 0) return -1;
+    if (bn == 16) return launch_wsf_i4<16>(tx, a, w, g_scale, stream);
+    if (bn == 32) return launch_wsf_i4<32>(tx, a, w, g_scale, stream);
+    if (bn == 64) return launch_wsf_i4<64>(tx, a, w, g_scale, stream);
+    if (bn == 96) return launch_wsf_i4<96>(tx, a, w, g_scale, stream);
+    return launch_wsf_i4<128>(tx, a, w, g_scale, stream);
+  }
   const int fw = a_scale ? FMT_E4M3_A8 : w_scale ? FMT_E4M3 : FMT_BF16;
   CUtensorMap tw, tx;
   if (get_tmap(w, rows_w, k, kGemmBM, fw, &tw) != 0) return -1;

@@ -30,7 +30,9 @@ enum GemmAct : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF_PY = 2 };
 // to bf16 exactly and runs the bf16 wgmma chain (weight-streaming kernels, stream-K partials only)
 // FMT_E4M3_A8: e4m3 weights (row scales) x e4m3 activations (token scales), multiplied by the FP8 wgmma (QGMMA) on
 // SWIZZLE_64B stages; each partial is scaled once in the epilogue (weight-streaming kernels, stream-K partials only)
-enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2, FMT_E4M3_A8 = 3 };
+// FMT_I4: 4-bit weight codes with one bf16 scale per 128 k of a row, bf16 activations; the consumer dequantizes the
+// codes into the wgmma A fragment in registers and runs the bf16 wgmma chain (weight-streaming kernels, stream-K only)
+enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2, FMT_E4M3_A8 = 3, FMT_I4 = 4 };
 // epilogues of the prefill GEMM (gemm_prefill.cuh): one fp32 plane for the fix-up kernels, or gate|up + SwiGLU
 enum PrefillEpi : int { PREFILL_PLANE = 0, PREFILL_SWIGLU = 1 };
 
@@ -216,6 +218,181 @@ __device__ __forceinline__ void wg_mainloop_a8(float (&acc)[2][BN / 2], const ui
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
     }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  if (nk > 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+  }
+}
+
+// ---- int4 weights (FMT_I4).  W4[n, k] = bf16_rn(q * s), q = code - 8 in [-8, 7], s = gscale[n, k / 128] (bf16).
+// Engine byte order of the codes: one 4 KB block per (128-row tile, 64-wide k-block) unit, the units of a tile in k order
+// and the tiles in row order, so the unit range of a stream-K CTA is one contiguous byte range.  Inside a unit, thread t
+// of the warpgroup owns 16 bytes per 64-row half h at byte h * 2048 + t * 16: the four 32-bit words of its m64k16
+// A fragments for the k16 steps kk = 0..3.  The word of step kk holds, for row r = 64h + 16(t/32) + (t%32)/4 and
+// column c = 16kk + 2(t%4), the code of element (r + 8e, c + 8f + b) in bits 4(e + 2f) + 16b .. +3, so
+// (word >> 4p) & 0x000F000F is the pair of fragment register p.
+constexpr int kI4BytesUnit = kGemmBM * kGemmBK / 2;   // 4 KB of codes per unit
+constexpr int kI4Group = 128;                           // k per scale
+// A ring slot carries up to this many consecutive k-blocks of one tile (8-16 KB of codes), split at multiples of it, so
+// a slot never spans more than units / 2 scale groups.
+constexpr int i4_slot_units(int bn) { return bn <= 32 ? 4 : 2; }
+
+// the slot that starts at unit u of the range [u, u1): its tile, first k-block and unit count
+template <int KU>
+__device__ __forceinline__ int i4_slot(long long u, long long u1, int kb, int& tile, int& kblk) {
+  tile = static_cast<int>(u / kb);
+  kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
+  return static_cast<int>(min(static_cast<long long>(min(KU - kblk % KU, kb - kblk)), u1 - u));
+}
+
+// producer, before griddepcontrol.wait: the codes of the first S slots of [u0, u1) (they depend on no earlier kernel).
+// Returns the number of slots issued.
+template <int BN, int S, int KU>
+__device__ __forceinline__ int i4_prefetch_codes(const uint8_t* w4, uint8_t* smem_a, uint64_t* full_bar, long long u0,
+                                                 long long u1, int kb, uint64_t hint) {
+  int pre = 0;
+  for (long long u = u0; u < u1 && pre < S; ++pre) {
+    int tile, kblk;
+    const int n = i4_slot<KU>(u, u1, kb, tile, kblk);
+    mbar_arrive_expect_tx(&full_bar[pre], n * (kI4BytesUnit + BN * kGemmBK * 2));
+    bulk_load(smem_a + pre * KU * kI4BytesUnit, w4 + u * kI4BytesUnit, n * kI4BytesUnit, &full_bar[pre], hint);
+    u += n;
+  }
+  return pre;
+}
+
+// producer: the whole slot stream of [u0, u1); slots below `pre` only still need their activation boxes
+template <int BN, int S, int KU>
+__device__ __forceinline__ void i4_produce(const uint8_t* w4, const CUtensorMap* tm_x, uint8_t* smem_a, uint8_t* smem_b,
+                                           uint64_t* full_bar, uint64_t* empty_bar, long long u0, long long u1, int kb,
+                                           int pre, uint64_t hint) {
+  int i = 0;
+  for (long long u = u0; u < u1; ++i) {
+    int tile, kblk;
+    const int n = i4_slot<KU>(u, u1, kb, tile, kblk);
+    const int s = i % S;
+    if (i >= pre) {
+      mbar_wait(&empty_bar[s], ((i / S) & 1) ^ 1);
+      mbar_arrive_expect_tx(&full_bar[s], n * (kI4BytesUnit + BN * kGemmBK * 2));
+      bulk_load(smem_a + s * KU * kI4BytesUnit, w4 + u * kI4BytesUnit, n * kI4BytesUnit, &full_bar[s], hint);
+    }
+    for (int j = 0; j < n; ++j)
+      tma_load_2d(smem_b + (s * KU + j) * BN * kGemmBK * 2, tm_x, &full_bar[s], (kblk + j) * kGemmBK, 0, kEvictLast);
+    u += n;
+  }
+}
+
+// consumer threads, before griddepcontrol.wait: pull the scale rows of their fragment rows over [u0, u1) into L2
+__device__ __forceinline__ void i4_prefetch_scales(const uint16_t* gs, int ng, int rows_w, long long u0, long long u1, int kb) {
+  if (u0 >= u1) return;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int t_lo = static_cast<int>(u0 / kb), t_hi = static_cast<int>((u1 - 1) / kb);
+  for (int t = t_lo; t <= t_hi; ++t) {
+    const int g0 = t == t_lo ? static_cast<int>(u0 - static_cast<long long>(t) * kb) / 2 : 0;
+    const int g1 = t == t_hi ? static_cast<int>(u1 - 1 - static_cast<long long>(t) * kb) / 2 : ng - 1;
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int n = t * kGemmBM + 64 * (r >> 1) + 16 * warp + (lane >> 2) + 8 * (r & 1);
+      if (n >= rows_w) continue;
+      const uint16_t* row = gs + static_cast<size_t>(n) * ng;
+      for (int g = g0; g < g1; g += 64) prefetch_l2(row + g);   // one 128-B line per 64 scales
+      prefetch_l2(row + g1);
+    }
+  }
+}
+
+__device__ __forceinline__ uint32_t bf16x2_bcast(uint16_t s) { return static_cast<uint32_t>(s) * 0x10001u; }
+
+// four codes pairs of `word` -> the bf16x2 registers of one A fragment: (128 + code) by OR into the mantissa of 128,
+// minus 136 = q exactly, times the row's scale = bf16_rn(q * s) (the product is exact in fp32; one rounding)
+__device__ __forceinline__ void i4_fragment(uint32_t word, uint32_t s_lo, uint32_t s_hi, uint32_t (&a)[4]) {
+#pragma unroll
+  for (int p = 0; p < 4; ++p) {
+    const uint32_t v = ((word >> (4 * p)) & 0x000F000Fu) | 0x43004300u;
+    __nv_bfloat162 q = __hsub2(*reinterpret_cast<const __nv_bfloat162*>(&v), __floats2bfloat162_rn(136.f, 136.f));
+    const uint32_t s = (p & 1) ? s_hi : s_lo;
+    q = __hmul2(q, *reinterpret_cast<const __nv_bfloat162*>(&s));
+    a[p] = *reinterpret_cast<const uint32_t*>(&q);
+  }
+}
+
+// wg_mainloop for int4 weights over the nk k-blocks k0 .. of one tile, in the producer's slots (ring position i counts
+// slots).  The codes go shared -> registers -> A fragments; each k-block issues the bf16 kernel's chain (kk = 0..3, half 0
+// then half 1) with A from registers, so the fp32 accumulators are those of the bf16 kernel on W4.  The shared loads of
+// a k-block's codes overlap the previous k-block's MMAs; its conversion waits for them.  A slot goes back to the producer
+// once the MMAs of its last k-block retire (they read its activation boxes).
+template <int BN, int S, int KU>
+__device__ __forceinline__ void wg_mainloop_i4(float (&acc)[2][BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
+                                               uint64_t* full_bar, uint64_t* empty_bar, int& i, int tile, int k0, int nk,
+                                               const uint16_t* gs, int ng, int rows_w) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+  int rows[4];   // fragment rows: half h = r >> 1, +8 for r & 1
+#pragma unroll
+  for (int r = 0; r < 4; ++r) rows[r] = tile * kGemmBM + 64 * (r >> 1) + 16 * warp + (lane >> 2) + 8 * (r & 1);
+  bool first = true;
+  for (int kblk = k0; kblk < k0 + nk; ++i) {
+    const int n = min(KU - kblk % KU, k0 + nk - kblk);
+    const int s = i % S;
+    // the scales of the (at most KU / 2) groups of the slot's KU-aligned window, loaded before the wait
+    const int gw = (kblk - kblk % KU) / 2;
+    uint32_t sc[KU / 2][4];
+#pragma unroll
+    for (int g = 0; g < KU / 2; ++g)
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+        sc[g][r] = bf16x2_bcast(rows[r] < rows_w && gw + g < ng ? __ldg(gs + static_cast<size_t>(rows[r]) * ng + gw + g) : 0);
+    mbar_wait(&full_bar[s], (i / S) & 1);
+#pragma unroll
+    for (int j = 0; j < KU; ++j) {
+      if (j >= n) break;
+      const int gsel = ((kblk + j) % KU) / 2;   // group of this k-block inside the window
+      uint32_t s_r[4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        s_r[r] = sc[0][r];
+#pragma unroll
+        for (int g = 1; g < KU / 2; ++g)
+          if (gsel == g) s_r[r] = sc[g][r];
+      }
+      const uint8_t* unit = smem_a + (s * KU + j) * kI4BytesUnit + threadIdx.x * 16;
+      const uint4 c0 = *reinterpret_cast<const uint4*>(unit);
+      const uint4 c1 = *reinterpret_cast<const uint4*>(unit + kI4BytesUnit / 2);
+      // no MMA in flight while the A registers are written: left to itself, ptxas serializes every wgmma of the loop
+      // behind these writes (C7513), which measured 27 % slower than this one wait per k-block (DESIGN.md section 5)
+      wgmma_wait<0>();
+      uint32_t a[2][4][4];
+      i4_fragment(c0.x, s_r[0], s_r[1], a[0][0]);
+      i4_fragment(c0.y, s_r[0], s_r[1], a[0][1]);
+      i4_fragment(c0.z, s_r[0], s_r[1], a[0][2]);
+      i4_fragment(c0.w, s_r[0], s_r[1], a[0][3]);
+      i4_fragment(c1.x, s_r[2], s_r[3], a[1][0]);
+      i4_fragment(c1.y, s_r[2], s_r[3], a[1][1]);
+      i4_fragment(c1.z, s_r[2], s_r[3], a[1][2]);
+      i4_fragment(c1.w, s_r[2], s_r[3], a[1][3]);
+      wgmma_fence();
+      const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + (s * KU + j) * BN * kGemmBK * 2));
+#pragma unroll
+      for (int kk = 0; kk < kGemmBK / 16; ++kk) {
+        WgmmaRegA<BN>::mma(acc[0], a[0][kk], db + 2 * kk);
+        WgmmaRegA<BN>::mma(acc[1], a[1][kk], db + 2 * kk);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (j == 0 && !first) {   // every MMA of the previous slot has retired
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+      }
+    }
+    first = false;
+    kblk += n;
   }
   wgmma_wait<0>();
   wgmma_fence_regs(acc[0]);

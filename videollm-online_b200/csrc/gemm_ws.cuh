@@ -15,7 +15,10 @@
 //   * FMT_E4M3 (mode 0 only): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop_f8), each partial
 //     multiplied by its row's scale once before it is written;
 //   * FMT_E4M3_A8 (mode 0 only): e4m3 weight and e4m3 activation stages straight into the FP8 wgmma (wg_mainloop_a8);
-//     each partial is multiplied by its row's weight scale, then by its token's activation scale, before it is written.
+//     each partial is multiplied by its row's weight scale, then by its token's activation scale, before it is written;
+//   * FMT_I4 (mode 0, one token tile only): 4-bit codes with per-group bf16 scales, dequantized into the wgmma A fragment in
+//     registers (wg_mainloop_i4); a ring slot carries up to i4_slot_units(BN) consecutive k-blocks of one tile, the codes
+//     as one bulk copy.  The units, their k order and the plane each lands in are those of the bf16 kernel.
 #pragma once
 #include <cuda.h>
 #include "gemm.cuh"
@@ -37,6 +40,8 @@ struct GemmWsArgs {
   unsigned long long hint_w;  // L2 policy for the weight stream (evict-first when read once per launch)
   const float* w_scale;       // FMT_E4M3 / FMT_E4M3_A8: [rows_w] fp32 row scales, applied once to each partial
   const float* a_scale;       // FMT_E4M3_A8: [rows_x] fp32 token scales, applied after the row scale
+  const uint8_t* w4;          // FMT_I4: the codes in the engine byte order (gemm.cuh)
+  const uint16_t* g_scale;    // FMT_I4: bf16 [rows_w][k / 128] group scales
 };
 
 // deepest ring of at most 8 stages that fits next to the staging tile
@@ -50,11 +55,18 @@ constexpr int ws_f8_default_stages(int bn) {
 // e4m3 weights and activations: up to 16 stages of 8 KB + BN x 64 B next to the staging tile (no conversion tiles)
 constexpr int ws_a8_default_stages(int bn) { return fit_stages(kA8BytesW + bn * kGemmBK, kWgStageBytes + 1024 + 256, 16); }
 
+// int4 weights: up to 16 slots of i4_slot_units(BN) k-blocks (codes + activation boxes) next to the staging tile
+constexpr int ws_i4_default_stages(int bn) {
+  return fit_stages(i4_slot_units(bn) * (kI4BytesUnit + bn * kGemmBK * 2), kWgStageBytes + 1024 + 256, 16);
+}
+
 template <int BN, int STAGES = ws_default_stages(BN), int FMT = FMT_BF16>
 struct GemmWsCfg {
   static constexpr int kStages = STAGES;
-  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW : kGemmBM * kGemmBK * 2;
-  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2);
+  // FMT_I4: per ring slot
+  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW
+                                 : FMT == FMT_I4 ? i4_slot_units(BN) * kI4BytesUnit : kGemmBM * kGemmBK * 2;
+  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2) * (FMT == FMT_I4 ? i4_slot_units(BN) : 1);
   static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
   static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kWgStageBytes;
   static_assert(kSmemBytes <= kSmemOptIn, "ring + staging tile exceed the shared memory of one block");
@@ -68,6 +80,8 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   using Cfg = GemmWsCfg<BN, STAGES, FMT>;
   constexpr bool kF8 = FMT == FMT_E4M3;
   constexpr bool kA8 = FMT == FMT_E4M3_A8;
+  constexpr bool kI4 = FMT == FMT_I4;
+  constexpr int KU = i4_slot_units(BN);
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -93,7 +107,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   const bool producer = warp == kGemmProducerWarp && lane == 0;
 
   if (producer) {
-    tma_prefetch_desc(&tm_w);
+    if constexpr (!kI4) tma_prefetch_desc(&tm_w);
     tma_prefetch_desc(&tm_x);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
@@ -107,7 +121,10 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   // The weight operand never depends on any earlier kernel: the producer starts streaming the first S weight
   // k-blocks right away, i.e. while the predecessors are still running.
   int pre = 0;
-  if (producer) {
+  if constexpr (kI4) {
+    if (producer) pre = i4_prefetch_codes<BN, S, KU>(p.w4, smem_a, full_bar, u0, u1, kb, p.hint_w);
+    else if (warp < kGemmProducerWarp) i4_prefetch_scales(p.g_scale, p.k / kI4Group, p.rows_w, u0, u1, kb);
+  } else if (producer) {
     for (long long u = u0; u < u1 && pre < S; ++u, ++pre) {
       const int tile = static_cast<int>(u / kb);
       const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
@@ -120,7 +137,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   pdl_wait();
 
   if (warp == kGemmProducerWarp) {
-    if (lane == 0) {
+    if constexpr (kI4) {
+      if (lane == 0) i4_produce<BN, S, KU>(p.w4, &tm_x, smem_a, smem_b, full_bar, empty_bar, u0, u1, kb, pre, p.hint_w);
+    } else if (lane == 0) {
       // ------------------------------------------------ TMA producer: one continuous stream of k-blocks
       int i = 0;
       for (long long u = u0; u < u1; ++u, ++i) {
@@ -151,6 +170,9 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
       else if constexpr (kA8)
         wg_mainloop_a8<BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      else if constexpr (kI4)
+        wg_mainloop_i4<BN, S, KU>(acc, smem_a, smem_b, full_bar, empty_bar, i, tile, k0, nk, p.g_scale, p.k / kI4Group,
+                                  p.rows_w);
       else
         wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int wt = tile / p.x_tiles, xt = tile - wt * p.x_tiles;

@@ -17,6 +17,8 @@
 // accumulator included, multiplies its fp32 partial of feature n by the row scale w_scale[n] once before the plane sum.
 // gemm_wsf_a8_kernel runs it on e4m3 weights and e4m3 activations (FMT_E4M3_A8): every partial of feature n, token t is
 // fl(fl(P * w_scale[n]) * a_scale[t]) before the plane sum.
+// gemm_wsf_i4_kernel runs it on int4 weights (FMT_I4, gemm.cuh): the same units and planes as the bf16 kernel in the
+// int4 ring slots of gemm_ws_kernel, and the bf16 kernel's epilogue, so its output is the bf16 kernel's on W4.
 // All CTAs of the grid are co-resident or become so without depending on a waiting CTA (grid <= #SMs, the PDL successor
 // cannot start before every CTA of this grid has started), so the finisher's wait cannot dead-lock; it is bounded anyway.
 #pragma once
@@ -42,8 +44,10 @@ constexpr int kWsfXchStride = 17;   // floats per feature row of the exchange ti
 template <int BN, int STAGES, int FMT = FMT_BF16>
 struct GemmWsfCfg {
   static constexpr int kStages = STAGES;
-  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW : kGemmBM * kGemmBK * 2;
-  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2);
+  // FMT_I4: per ring slot
+  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW
+                                 : FMT == FMT_I4 ? i4_slot_units(BN) * kI4BytesUnit : kGemmBM * kGemmBK * 2;
+  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2) * (FMT == FMT_I4 ? i4_slot_units(BN) : 1);
   static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
   static constexpr int kXchBytes = kGemmBM * kWsfXchStride * 4;
   static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kXchBytes + kWgStageBytes;
@@ -63,20 +67,28 @@ constexpr int wsf_a8_default_stages(int bn) {
   return fit_stages(kA8BytesW + bn * kGemmBK, 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 16);
 }
 
+// int4 weights: up to 16 slots of i4_slot_units(bn) k-blocks next to the exchange and the staging tile
+constexpr int wsf_i4_default_stages(int bn) {
+  return fit_stages(i4_slot_units(bn) * (kI4BytesUnit + bn * kGemmBK * 2), 1024 + 256 + kGemmBM * kWsfXchStride * 4 + kWgStageBytes, 16);
+}
+
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
   asm volatile("ld.acquire.gpu.global.s32 %0, [%1];\n" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
 
-// The body of the kernels below; FMT is FMT_BF16, FMT_E4M3 or FMT_E4M3_A8.  p by value: ptxas then still reads
+// The body of the kernels below; FMT is FMT_BF16, FMT_E4M3, FMT_E4M3_A8 or FMT_I4 (tm_w unused: w4 and g_scale instead).  p by value: ptxas then still reads
 // the fields from parameter space where used (the bf16 kernels compile to the same code as with the body inline).
 template <int FMT, int BN, int STAGES>
 __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUtensorMap& tm_x, const GemmWsfArgs p,
-                                              const float* w_scale, const float* a_scale = nullptr) {
+                                              const float* w_scale, const float* a_scale = nullptr,
+                                              const uint8_t* w4 = nullptr, const uint16_t* g_scale = nullptr) {
   using Cfg = GemmWsfCfg<BN, STAGES, FMT>;
   constexpr bool kF8 = FMT == FMT_E4M3;
   constexpr bool kA8 = FMT == FMT_E4M3_A8;
+  constexpr bool kI4 = FMT == FMT_I4;
+  constexpr int KU = i4_slot_units(BN);
   constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -95,7 +107,7 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
   const bool producer = warp == kGemmProducerWarp && lane == 0;
 
   if (producer) {
-    tma_prefetch_desc(&tm_w);
+    if constexpr (!kI4) tma_prefetch_desc(&tm_w);
     tma_prefetch_desc(&tm_x);
     for (int s = 0; s < S; ++s) {
       mbar_init(&full_bar[s], 1);
@@ -107,7 +119,10 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
   pdl_trigger();
   // the weight operand never depends on an earlier kernel: fill the ring while the predecessors are still running
   int pre = 0;
-  if (producer) {
+  if constexpr (kI4) {
+    if (producer) pre = i4_prefetch_codes<BN, S, KU>(w4, smem_a, full_bar, u0, u1, kb, p.hint_w);
+    else if (warp < kGemmProducerWarp) i4_prefetch_scales(g_scale, p.k / kI4Group, p.rows_w, u0, u1, kb);
+  } else if (producer) {
     for (long long u = u0; u < u1 && pre < S; ++u, ++pre) {
       const int tile = static_cast<int>(u / kb);
       const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
@@ -118,7 +133,9 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
   pdl_wait();
 
   if (warp == kGemmProducerWarp) {
-    if (lane == 0) {
+    if constexpr (kI4) {
+      if (lane == 0) i4_produce<BN, S, KU>(w4, &tm_x, smem_a, smem_b, full_bar, empty_bar, u0, u1, kb, pre, p.hint_w);
+    } else if (lane == 0) {
       // ------------------------------------------------ TMA producer: one continuous stream of k-blocks
       int i = 0;
       for (long long u = u0; u < u1; ++u, ++i) {
@@ -148,6 +165,9 @@ __device__ __forceinline__ void gemm_wsf_body(const CUtensorMap& tm_w, const CUt
         wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
       else if constexpr (kA8)
         wg_mainloop_a8<BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      else if constexpr (kI4)
+        wg_mainloop_i4<BN, S, KU>(acc, smem_a, smem_b, full_bar, empty_bar, i, tile, k0, nk, g_scale, p.k / kI4Group,
+                                  p.rows_w);
       else
         wg_mainloop<FMT_BF16, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
       const int pl = c - sk_first_cta(tile, p.sk);
@@ -272,6 +292,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wsf_a8_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
                    const __grid_constant__ GemmWsfArgs p, const float* __restrict__ w_scale, const float* a_scale) {
   gemm_wsf_body<FMT_E4M3_A8, BN, STAGES>(tm_w, tm_x, p, w_scale, a_scale);
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_wsf_i4_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ GemmWsfArgs p,
+                   const uint8_t* __restrict__ w4, const uint16_t* __restrict__ g_scale) {
+  gemm_wsf_body<FMT_I4, BN, STAGES>(tm_x, tm_x, p, nullptr, nullptr, w4, g_scale);
 }
 
 }  // namespace vlo

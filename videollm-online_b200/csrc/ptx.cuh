@@ -120,6 +120,19 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
+// `bytes` contiguous bytes (a multiple of 16, both addresses 16-byte aligned) from global memory into shared memory,
+// completing on bar like a tensor load
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)), "l"(hint)
+      : "memory");
+}
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+  asm volatile("prefetch.global.L2 [%0];\n" ::"l"(reinterpret_cast<uint64_t>(p)));
+}
+
 // The same box written at the same shared-memory offset of every CTA of the cluster in cta_mask; each destination's
 // mbarrier at bar's offset receives the complete_tx of its copy.
 __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0, int32_t c1,

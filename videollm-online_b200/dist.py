@@ -11,9 +11,11 @@ from .config import LiveConfig
 from .weights import layer_matrix_spec
 
 
-def engine_weight_spec(cfg: LiveConfig, max_positions: int, fp8_weights: bool = False) -> Dict[str, tuple]:
+def engine_weight_spec(cfg: LiveConfig, max_positions: int, fp8_weights: bool = False,
+                       int4_weights: bool = False) -> Dict[str, tuple]:
     """name -> (shape, dtype) of every tensor of the engine layout (weights.py docstring), derivable on
-    every rank without materialising anything.  fp8_weights: the layer matrices as e4m3 codes + row scales."""
+    every rank without materialising anything.  fp8_weights: the layer matrices as e4m3 codes + row scales;
+    int4_weights: as packed int4 codes + bf16 group scales."""
     bf, f16, f32 = torch.bfloat16, torch.float16, torch.float32
     H, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
     nh, nkv, hd = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -23,10 +25,10 @@ def engine_weight_spec(cfg: LiveConfig, max_positions: int, fp8_weights: bool = 
     for i in range(cfg.num_hidden_layers):
         s[f"L{i}.in_norm"] = ((H,), bf)
         s[f"L{i}.post_norm"] = ((H,), bf)
-        s.update(layer_matrix_spec(f"L{i}.qkv", ((nh + 2 * nkv) * hd, H), fp8_weights))
-        s.update(layer_matrix_spec(f"L{i}.o", (H, nh * hd), fp8_weights))
-        s.update(layer_matrix_spec(f"L{i}.gate_up", (2 * I, H), fp8_weights))
-        s.update(layer_matrix_spec(f"L{i}.down", (H, I), fp8_weights))
+        s.update(layer_matrix_spec(f"L{i}.qkv", ((nh + 2 * nkv) * hd, H), fp8_weights, int4_weights))
+        s.update(layer_matrix_spec(f"L{i}.o", (H, nh * hd), fp8_weights, int4_weights))
+        s.update(layer_matrix_spec(f"L{i}.gate_up", (2 * I, H), fp8_weights, int4_weights))
+        s.update(layer_matrix_spec(f"L{i}.down", (H, I), fp8_weights, int4_weights))
     s.update({"conn.0.w": ((H, C), bf), "conn.0.b": ((H,), f32), "conn.2.w": ((H, H), bf), "conn.2.b": ((H,), f32),
               "vit.patch.w": ((C, 3 * ps * ps), f16), "vit.patch.b": ((C,), f32), "vit.pos": ((P, C), f32),
               "vit.post_ln.w": ((C,), f32), "vit.post_ln.b": ((C,), f32)})
@@ -72,18 +74,18 @@ def _flat_layout(spec: Dict[str, tuple], n_buckets: int):
 
 def broadcast_weights(cfg: LiveConfig, weights: Optional[Dict[str, torch.Tensor]], device, max_positions: int,
                       dist=None, src: int = 0, n_buckets: int = 8, release_source: bool = False,
-                      fp8_weights: bool = False) -> Dict[str, torch.Tensor]:
+                      fp8_weights: bool = False, int4_weights: bool = False) -> Dict[str, torch.Tensor]:
     """Rank `src` passes its engine-layout dict, the others pass None; everyone returns the full dict on `device`.
     The ~560 tensors (16.7 GB) travel as <= `n_buckets` flat byte buffers, one NCCL broadcast each over NVLink/NVSwitch
     (per-tensor broadcasts cost 1.2 s at 8 GPUs: launch latency, not bandwidth); the returned tensors are views into
     those buffers (256-byte aligned), on the source rank too, so every rank ends with the same memory layout.
     release_source=True empties the source dict entry by entry while packing.  fp8_weights: every rank expects the layer
-    matrices in the FP8 form (engine_weight_spec)."""
+    matrices in the FP8 form (engine_weight_spec); int4_weights: in the int4 form."""
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
         if weights is None:
             raise ValueError("single process: weights must be provided")
         return weights
-    spec = engine_weight_spec(cfg, max_positions, fp8_weights)
+    spec = engine_weight_spec(cfg, max_positions, fp8_weights, int4_weights)
     out: Dict[str, torch.Tensor] = {}
     is_src = dist.get_rank() == src
     if is_src:

@@ -323,6 +323,12 @@ class Engine:
         return "L0.qkv.f8" in self._weights
 
     @property
+    def int4_weights(self) -> bool:
+        """True when the decoder layer matrices were loaded as int4 codes + bf16 group scales
+        (weights.quantize_int4_groups)."""
+        return "L0.qkv.i4" in self._weights
+
+    @property
     def max_prefill_tokens(self) -> int:
         """rows of one vlo_prefill (8 x max_step_tokens) once bf16 layer weights are loaded; 0 before, and on engines
         with e4m3 layer weights or activations"""

@@ -52,6 +52,7 @@ class SessionState:
     fed_ids: Optional[list] = None   # the id fed at every cache position (-1: frame row) when no NgramDrafter holds them
     fp8_weights: bool = False    # the cache was written by a model with FP8 layer weights (Engine.fp8_weights)
     fp8_activations: bool = False   # ... and with FP8 activations (Engine.fp8_activations)
+    int4_weights: bool = False   # ... with int4 layer weights (Engine.int4_weights)
 
 
 torch.serialization.add_safe_globals([SessionState, SamplingConfig])
@@ -237,7 +238,7 @@ class LiveInfer:
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
                 n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling,
                 evicted_tokens=self.evicted_tokens, fp8_weights=self._kv.engine.fp8_weights,
-                fp8_activations=self._kv.engine.fp8_activations, fed_ids=fed)
+                fp8_activations=self._kv.engine.fp8_activations, int4_weights=self._kv.engine.int4_weights, fed_ids=fed)
             self.reset()
             return state
 
@@ -246,14 +247,16 @@ class LiveInfer:
         every queue and counter `__call__` reads is restored.  The video is not part of the state: load it again
         (before or after resuming).  Raises VloError if the pool is short or the image belongs to another config; the
         session's stream is then empty and the rest of the session unchanged.  A state whose cache was written with the
-        other weight form (FP8 or bf16 layer weights: a different model), or with the other activation form (W8A8 or not),
-        is refused before anything changes."""
+        other weight form (bf16, FP8 or int4 layer weights: a different model), or with the other activation form (W8A8 or
+        not), is refused before anything changes.  States saved before the int4 form existed load as not int4."""
         with self._lock:
             eng = self._kv.engine
-            if state.fp8_weights != eng.fp8_weights:
-                form = {True: "FP8", False: "bf16"}
-                raise VloError(f"resume: the state's cache was written with {form[state.fp8_weights]} layer weights, "
-                               f"this model has {form[eng.fp8_weights]} ones")
+            def weight_form(fp8, int4):
+                return "FP8" if fp8 else "int4" if int4 else "bf16"
+            theirs = weight_form(state.fp8_weights, state.int4_weights)
+            ours = weight_form(eng.fp8_weights, eng.int4_weights)
+            if theirs != ours:
+                raise VloError(f"resume: the state's cache was written with {theirs} layer weights, this model has {ours} ones")
             if state.fp8_activations != eng.fp8_activations:
                 form = {True: "FP8", False: "bf16"}
                 raise VloError(f"resume: the state's cache was written with {form[state.fp8_activations]} layer "

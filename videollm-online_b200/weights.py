@@ -20,6 +20,10 @@ Engine layout (name -> tensor), all contiguous on the engine's device:
 FP8 weights (fp8_weights=True): each layer matrix L{i}.{qkv,o,gate_up,down} [N, K] is replaced by L{i}.{m}.f8 (e4m3fn
 bytes [N, K], uint8) and L{i}.{m}.scale (fp32 [N], one scale per output row), quantized by quantize_fp8_rows from the
 bf16 matrix above (after the LoRA merge and the gate|up interleave).  Everything else stays 16-bit.
+Int4 weights (int4_weights=True, W4A16): each layer matrix [N, K] (K % 128 == 0) is replaced by L{i}.{m}.i4 (the codes
+q + 8 in the engine byte order of pack_int4_codes, uint8, ceil(N / 128) * 128 * K / 2 bytes) and L{i}.{m}.gscale (bf16
+[N, K / 128]), quantized by quantize_int4_groups from the same bf16 matrix.  The engine multiplies W4 =
+dequantize_int4_groups(q, s) exactly, so an int4 engine computes the bits of a bf16 engine loaded with W4.
 """
 from __future__ import annotations
 
@@ -201,22 +205,102 @@ def dequantize_fp8_rows(codes: torch.Tensor, scale: torch.Tensor) -> torch.Tenso
     return codes.view(torch.float8_e4m3fn).float() * scale[:, None]
 
 
-def layer_matrix_spec(name: str, shape: tuple, fp8_weights: bool) -> Dict[str, tuple]:
+INT4_GROUP = 128   # weights of a row per int4 scale
+INT4_TILE = 128    # weight rows per engine tile (the GEMM's 128-row M tile)
+
+
+def quantize_int4_groups(w: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """[N, K] weight (K % 128 == 0) -> (int8 q [N, K] in [-8, 7], bf16 scales [N, K / 128]) on w's device:
+    s[n, g] = bf16_rn(fp32(max_{k in group g} |W[n, k]|) / 7) (1 where that is 0), q[n, k] = clamp(rne(fp32(W[n, k]) /
+    fp32(s[n, g])), -8, 7), IEEE fp32 division."""
+    if w.dim() != 2:
+        raise ValueError(f"quantize_int4_groups: a 2-D weight, got shape {tuple(w.shape)}")
+    n, k = w.shape
+    if k % INT4_GROUP != 0:
+        raise ValueError(f"quantize_int4_groups: K = {k} is not a multiple of {INT4_GROUP}")
+    w32 = w.float()
+    if not bool(torch.isfinite(w32).all()):
+        raise ValueError("quantize_int4_groups: the weight holds a non-finite value")
+    g = w32.view(n, k // INT4_GROUP, INT4_GROUP)
+    s = (g.abs().amax(dim=2) / 7).to(torch.bfloat16)
+    s = torch.where(s == 0, torch.ones_like(s), s)
+    q = torch.round(g / s.float()[:, :, None]).clamp_(-8, 7).to(torch.int8)
+    return q.view(n, k), s.contiguous()
+
+
+def dequantize_int4_groups(q: torch.Tensor, s: torch.Tensor) -> torch.Tensor:
+    """bf16 [N, K] = W4 = bf16_rn(q * s): the weight every int4 kernel multiplies (q * s is exact in fp32)."""
+    n, k = q.shape
+    return (q.float().view(n, k // INT4_GROUP, INT4_GROUP) * s.float()[:, :, None]).view(n, k).to(torch.bfloat16)
+
+
+def _int4_code_view(codes: torch.Tensor, n_pad: int, k: int) -> torch.Tensor:
+    # [tile][h][warp][e][lane / 4] rows x [k-block][kk][f][lane % 4][b] columns: row = 64h + 16warp + 8e + lane / 4,
+    # column = 64 k-block + 16kk + 8f + 2(lane % 4) + b (gemm.cuh, FMT_I4)
+    return codes.view(n_pad // INT4_TILE, 2, 4, 2, 8, k // 64, 4, 2, 4, 2)
+
+
+def pack_int4_codes(q: torch.Tensor) -> torch.Tensor:
+    """int8 q [N, K] in [-8, 7] -> uint8 [ceil(N / 128) * 128 * K / 2]: the codes q + 8 in the engine byte order.  One
+    4 KB block per (128-row tile, 64-wide k-block), blocks in (tile, k-block) order; inside a block, consumer thread t =
+    32 warp + lane has 16 bytes per 64-row half h at h * 2048 + 16 t: one 32-bit word per k16 step kk, holding the code of
+    element (row r + 8e, column c + 8f + b) in bits 4(e + 2f) + 16b, r = 64h + 16 warp + lane / 4, c = 16kk + 2(lane % 4).
+    Rows past N are padded with code 8 (q = 0)."""
+    n, k = q.shape
+    n_pad = -(-n // INT4_TILE) * INT4_TILE
+    codes = torch.full((n_pad, k), 8, dtype=torch.int64, device=q.device)
+    codes[:n] = q.to(torch.int64) + 8
+    c = _int4_code_view(codes, n_pad, k)
+    # -> [tile, k-block, h, warp, lane / 4, lane % 4, kk, e, f, b]
+    c = c.permute(0, 5, 1, 2, 4, 8, 6, 3, 7, 9)
+    shift = torch.tensor([[[0, 16], [8, 24]], [[4, 20], [12, 28]]], dtype=torch.int64, device=q.device)   # [e][f][b]
+    words = (c << shift).sum(dim=(-3, -2, -1))
+    return words.to(torch.int32).contiguous().view(torch.uint8).reshape(-1)
+
+
+def unpack_int4_codes(packed: torch.Tensor, n: int, k: int) -> torch.Tensor:
+    """The inverse of pack_int4_codes: int8 q [N, K]."""
+    n_pad = -(-n // INT4_TILE) * INT4_TILE
+    words = packed.contiguous().view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+    words = words.view(n_pad // INT4_TILE, k // 64, 2, 4, 8, 4, 4)   # [tile, k-block, h, warp, lane/4, lane%4, kk]
+    shift = torch.tensor([[[0, 16], [8, 24]], [[4, 20], [12, 28]]], dtype=torch.int64, device=packed.device)
+    c = (words[..., None, None, None] >> shift) & 0xF            # [..., kk, e, f, b]
+    c = c.permute(0, 2, 3, 7, 4, 1, 6, 8, 5, 9)                  # -> [tile, h, warp, e, lane/4, k-block, kk, f, lane%4, b]
+    return (c.reshape(n_pad, k)[:n] - 8).to(torch.int8)
+
+
+def _weight_form(fp8_weights: bool, int4_weights: bool) -> None:
+    if fp8_weights and int4_weights:
+        raise ValueError("fp8_weights and int4_weights are two forms of the layer matrices: choose one")
+
+
+def layer_matrix_spec(name: str, shape: tuple, fp8_weights: bool, int4_weights: bool = False) -> Dict[str, tuple]:
     """Engine tensor name -> (shape, dtype) of one layer matrix [N, K] in the chosen form."""
+    _weight_form(fp8_weights, int4_weights)
+    if int4_weights:
+        n, k = shape
+        n_pad = -(-n // INT4_TILE) * INT4_TILE
+        return {name + ".i4": ((n_pad * k // 2,), torch.uint8), name + ".gscale": ((n, k // INT4_GROUP), torch.bfloat16)}
     if not fp8_weights:
         return {name: (shape, torch.bfloat16)}
     return {name + ".f8": (shape, torch.uint8), name + ".scale": ((shape[0],), torch.float32)}
 
 
-def _put_layer_matrix(out: StateDict, name: str, w: torch.Tensor, fp8_weights: bool) -> None:
+def _put_layer_matrix(out: StateDict, name: str, w: torch.Tensor, fp8_weights: bool, int4_weights: bool = False) -> None:
     # quantized on w's device, one matrix at a time: the bf16 matrix is dropped as soon as its codes exist
-    if fp8_weights:
+    _weight_form(fp8_weights, int4_weights)
+    if int4_weights:
+        q, s = quantize_int4_groups(w)
+        out[name + ".i4"], out[name + ".gscale"] = pack_int4_codes(q), s
+    elif fp8_weights:
         out[name + ".f8"], out[name + ".scale"] = quantize_fp8_rows(w)
     else:
         out[name] = w
 
 
-def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: int, fp8_weights: bool = False) -> StateDict:
+def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: int, fp8_weights: bool = False,
+                        int4_weights: bool = False) -> StateDict:
+    _weight_form(fp8_weights, int4_weights)
     bf = torch.bfloat16
     out: StateDict = {}
 
@@ -234,11 +318,12 @@ def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: i
         out[f"L{i}.post_norm"] = take(p + "post_attention_layernorm.weight")
         _put_layer_matrix(out, f"L{i}.qkv", torch.cat([take(p + "self_attn.q_proj.weight"),
                                                        take(p + "self_attn.k_proj.weight"),
-                                                       take(p + "self_attn.v_proj.weight")], 0).contiguous(), fp8_weights)
-        _put_layer_matrix(out, f"L{i}.o", take(p + "self_attn.o_proj.weight"), fp8_weights)
+                                                       take(p + "self_attn.v_proj.weight")], 0).contiguous(), fp8_weights,
+                          int4_weights)
+        _put_layer_matrix(out, f"L{i}.o", take(p + "self_attn.o_proj.weight"), fp8_weights, int4_weights)
         _put_layer_matrix(out, f"L{i}.gate_up", interleave_gate_up(take(p + "mlp.gate_proj.weight"),
-                                                                   take(p + "mlp.up_proj.weight")), fp8_weights)
-        _put_layer_matrix(out, f"L{i}.down", take(p + "mlp.down_proj.weight"), fp8_weights)
+                                                                   take(p + "mlp.up_proj.weight")), fp8_weights, int4_weights)
+        _put_layer_matrix(out, f"L{i}.down", take(p + "mlp.down_proj.weight"), fp8_weights, int4_weights)
     if "connector.0.weight" in sd:
         out["conn.0.w"] = take("connector.0.weight")
         out["conn.0.b"] = _b32_from16(sd["connector.0.bias"].to(device), bf)
@@ -290,10 +375,11 @@ def pack_vision_for_engine(cfg: LiveConfig, sd: StateDict, device) -> StateDict:
 
 
 def synthetic_engine_weights(cfg: LiveConfig, device, max_positions: int, seed: int = 0, std: float = 0.02,
-                             fp8_weights: bool = False) -> StateDict:
+                             fp8_weights: bool = False, int4_weights: bool = False) -> StateDict:
     """Full-size synthetic weights generated directly in the engine layout on `device` (bench path: no
-    16 GB host round trip).  Same distributions as synthetic_*_state, different random stream.  fp8_weights: the layer
-    matrices of the same seed, quantized."""
+    16 GB host round trip).  Same distributions as synthetic_*_state, different random stream.  fp8_weights /
+    int4_weights: the layer matrices of the same seed, quantized."""
+    _weight_form(fp8_weights, int4_weights)
     g = torch.Generator(device=device).manual_seed(seed)
     bf, f16, f32 = torch.bfloat16, torch.float16, torch.float32
     H, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
@@ -307,10 +393,10 @@ def synthetic_engine_weights(cfg: LiveConfig, device, max_positions: int, seed: 
     for i in range(cfg.num_hidden_layers):
         out[f"L{i}.in_norm"] = _gen((H,), 0.1, g, device, bf, 1.0)
         out[f"L{i}.post_norm"] = _gen((H,), 0.1, g, device, bf, 1.0)
-        _put_layer_matrix(out, f"L{i}.qkv", _gen(((nh + 2 * nkv) * hd, H), std, g, device, bf), fp8_weights)
-        _put_layer_matrix(out, f"L{i}.o", _gen((H, nh * hd), std, g, device, bf), fp8_weights)
-        _put_layer_matrix(out, f"L{i}.gate_up", _gen((2 * I, H), std, g, device, bf), fp8_weights)
-        _put_layer_matrix(out, f"L{i}.down", _gen((H, I), std, g, device, bf), fp8_weights)
+        _put_layer_matrix(out, f"L{i}.qkv", _gen(((nh + 2 * nkv) * hd, H), std, g, device, bf), fp8_weights, int4_weights)
+        _put_layer_matrix(out, f"L{i}.o", _gen((H, nh * hd), std, g, device, bf), fp8_weights, int4_weights)
+        _put_layer_matrix(out, f"L{i}.gate_up", _gen((2 * I, H), std, g, device, bf), fp8_weights, int4_weights)
+        _put_layer_matrix(out, f"L{i}.down", _gen((H, I), std, g, device, bf), fp8_weights, int4_weights)
     out["conn.0.w"] = _gen((H, C), std, g, device, bf)
     out["conn.0.b"] = _gen((H,), std, g, device, bf).float()
     out["conn.2.w"] = _gen((H, H), std, g, device, bf)
