@@ -47,7 +47,7 @@ int op_attn_plan(AttnPlan* plan, void* d_ws, int n_tok, int n_heads, int n_kv_he
 int op_fix_plan(int width, int T, int k, int n_ctas, SkInfo* sk) {
   VLO_CHECK(T > 0 && T <= 128, "fix-up kernels: 1..128 token rows (one token tile)");
   GemmWsCall c{};
-  c.fmt = FMT_BF16;
+  c.w.fmt = FMT_BF16;
   c.mode = 0;
   c.rows_w = width;
   c.rows_x = T;
@@ -68,6 +68,28 @@ __global__ void tanh_approx_kernel(const float* x, float* y, long long n) {
 }
 
 // Device scratch of a synchronous kernel-level entry point, freed on every return path.
+// gemm_ws_launch mode 0 of weights w into the caller-sized planes d_out (null: plan only) on the token tile it picks
+int op_gemm_ws_partials(const WeightOperand& w, int rows_w, const void* d_x, const float* d_xscale, int rows_x, int k,
+                        float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
+  GemmWsCall c{};
+  c.w = w;
+  c.mode = 0;
+  c.rows_w = rows_w;
+  c.x = d_x;
+  c.a_scale = d_xscale;
+  c.rows_x = rows_x;
+  c.k = k;
+  c.out = d_out;
+  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
+  c.ld_out = rows_w;
+  c.plane_stride = plane_stride;
+  c.n_ctas = n_ctas;
+  GemmWsPlan plan{};
+  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
+  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
+  return rc;
+}
+
 struct OpScratch {
   void* p = nullptr;
   ~OpScratch() {
@@ -134,9 +156,8 @@ int vlo_op_gemm_ws_tiled(int fmt, int mode, const void* d_w, int rows_w, const v
                          int32_t* h_plan, void* cuda_stream) {
   VLO_CHECK(tiling == WS_TILE_FIT || tiling == WS_TILE_TRUNK || tiling == WS_TILE_BESIDE_DECODER, "gemm_ws: unknown tiling");
   GemmWsCall c{};
-  c.fmt = fmt;
+  c.w = WeightOperand{fmt, d_w, nullptr, nullptr};
   c.mode = mode;
-  c.w = d_w;
   c.rows_w = rows_w;
   c.x = d_x;
   c.rows_x = rows_x;
@@ -163,71 +184,22 @@ int vlo_op_gemm_ws_tiled(int fmt, int mode, const void* d_w, int rows_w, const v
 int vlo_op_gemm_ws_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
                       long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
   VLO_CHECK(d_out == nullptr || d_scale != nullptr, "gemm_ws_f8: null row scales");
-  GemmWsCall c{};
-  c.fmt = FMT_E4M3;
-  c.mode = 0;
-  c.w = d_w8;
-  c.w_scale = d_scale;
-  c.rows_w = rows_w;
-  c.x = d_x;
-  c.rows_x = rows_x;
-  c.k = k;
-  c.out = d_out;
-  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
-  c.ld_out = rows_w;
-  c.plane_stride = plane_stride;
-  c.n_ctas = n_ctas;
-  GemmWsPlan plan{};
-  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
-  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
-  return rc;
+  return op_gemm_ws_partials(WeightOperand{FMT_E4M3, d_w8, d_scale, nullptr}, rows_w, d_x, nullptr, rows_x, k, d_out,
+                             plane_stride, n_ctas, h_max_planes, cuda_stream);
 }
 
 int vlo_op_gemm_ws_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
                       long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
   VLO_CHECK(d_out == nullptr || d_gscale != nullptr, "gemm_ws_i4: null group scales");
-  GemmWsCall c{};
-  c.fmt = FMT_I4;
-  c.mode = 0;
-  c.w = d_w4;
-  c.g_scale = static_cast<const uint16_t*>(d_gscale);
-  c.rows_w = rows_w;
-  c.x = d_x;
-  c.rows_x = rows_x;
-  c.k = k;
-  c.out = d_out;
-  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
-  c.ld_out = rows_w;
-  c.plane_stride = plane_stride;
-  c.n_ctas = n_ctas;
-  GemmWsPlan plan{};
-  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
-  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
-  return rc;
+  return op_gemm_ws_partials(WeightOperand{FMT_I4, d_w4, nullptr, static_cast<const uint16_t*>(d_gscale)}, rows_w, d_x,
+                             nullptr, rows_x, k, d_out, plane_stride, n_ctas, h_max_planes, cuda_stream);
 }
 
 int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale, int rows_x,
                       int k, float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
   VLO_CHECK(d_out == nullptr || (d_scale != nullptr && d_xscale != nullptr), "gemm_ws_a8: null row or token scales");
-  GemmWsCall c{};
-  c.fmt = FMT_E4M3_A8;
-  c.mode = 0;
-  c.w = d_w8;
-  c.w_scale = d_scale;
-  c.rows_w = rows_w;
-  c.x = d_x8;
-  c.a_scale = d_xscale;
-  c.rows_x = rows_x;
-  c.k = k;
-  c.out = d_out;
-  c.out_elems = SIZE_MAX;  // the caller sizes d_out from the planning query
-  c.ld_out = rows_w;
-  c.plane_stride = plane_stride;
-  c.n_ctas = n_ctas;
-  GemmWsPlan plan{};
-  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
-  if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
-  return rc;
+  return op_gemm_ws_partials(WeightOperand{FMT_E4M3_A8, d_w8, d_scale, nullptr}, rows_w, d_x8, d_xscale, rows_x, k, d_out,
+                             plane_stride, n_ctas, h_max_planes, cuda_stream);
 }
 
 int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
@@ -333,7 +305,7 @@ int vlo_op_vit_tiling(int n_frames, int n_patches, int hidden, int mlp, int32_t*
   // the planning query of each gemm_ws_launch vlo_vit_encode makes (mode, output features, k, tiling)
   auto query = [&](int mode, int n_out, int k, int tiling, int tok_rows, GemmWsPlan* plan) -> int {
     GemmWsCall c{};
-    c.fmt = FMT_F16;
+    c.w.fmt = FMT_F16;
     c.mode = mode;
     c.rows_w = n_out;
     c.rows_x = tok_rows;
@@ -401,7 +373,7 @@ int vlo_op_vit_fix_ln(const float* d_part, int rows, int C, int k, int bn, int n
                 aligned(d_out32, 16) && aligned(d_out16, 8),
             "vit_fix_ln: fp32 arrays 16-byte and out16 8-byte aligned");
   GemmWsCall c{};
-  c.fmt = FMT_F16;
+  c.w.fmt = FMT_F16;
   c.mode = 0;
   c.rows_w = C;
   c.rows_x = rows;
@@ -493,16 +465,16 @@ int vlo_op_gemm_prefill(int epi, const void* d_w, int rows_w, const void* d_x, i
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
                        int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu: plane_elems");
-  return gemm_wsf_launch(d_w, nullptr, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
-                         n_flags, static_cast<cudaStream_t>(cuda_stream));
+  return gemm_wsf_launch(WeightOperand{FMT_BF16, d_w, nullptr, nullptr}, rows_w, d_x, rows_x, k, d_act, d_planes,
+                         static_cast<size_t>(plane_elems), d_flags, n_flags, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
                           float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu_f8: plane_elems");
   VLO_CHECK(d_scale != nullptr, "gemm_swiglu_f8: null row scales");
-  return gemm_wsf_launch(d_w8, d_scale, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
-                         n_flags, static_cast<cudaStream_t>(cuda_stream));
+  return gemm_wsf_launch(WeightOperand{FMT_E4M3, d_w8, d_scale, nullptr}, rows_w, d_x, rows_x, k, d_act, d_planes,
+                         static_cast<size_t>(plane_elems), d_flags, n_flags, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale,
@@ -510,16 +482,17 @@ int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, co
                           void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu_a8: plane_elems");
   VLO_CHECK(d_scale != nullptr && d_xscale != nullptr, "gemm_swiglu_a8: null row or token scales");
-  return gemm_wsf_launch(d_w8, d_scale, rows_w, d_x8, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
-                         n_flags, static_cast<cudaStream_t>(cuda_stream), d_xscale);
+  return gemm_wsf_launch(WeightOperand{FMT_E4M3_A8, d_w8, d_scale, nullptr}, rows_w, d_x8, rows_x, k, d_act, d_planes,
+                         static_cast<size_t>(plane_elems), d_flags, n_flags, static_cast<cudaStream_t>(cuda_stream), d_xscale);
 }
 
 int vlo_op_gemm_swiglu_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, void* d_act,
                           float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu_i4: plane_elems");
   VLO_CHECK(d_gscale != nullptr, "gemm_swiglu_i4: null group scales");
-  return gemm_wsf_launch(d_w4, nullptr, rows_w, d_x, rows_x, k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags,
-                         n_flags, static_cast<cudaStream_t>(cuda_stream), nullptr, static_cast<const uint16_t*>(d_gscale));
+  return gemm_wsf_launch(WeightOperand{FMT_I4, d_w4, nullptr, static_cast<const uint16_t*>(d_gscale)}, rows_w, d_x, rows_x,
+                         k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags, n_flags,
+                         static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream) {

@@ -112,11 +112,18 @@ enum WsTiling : int {
   WS_TILE_BESIDE_DECODER = 2,  // ViT trunk of 1-2 frames, fp16: 64-token tiles on a 3-stage ring (83 KB), so the CTA
                                // shares an SM with a decoder weight-streaming CTA
 };
-struct GemmWsCall {
+// The weight operand of the weight-streaming GEMMs: its format (GemmFmt, gemm.cuh) and what that format stores.
+struct WeightOperand {
   int fmt;            // 0 fp16, 1 bf16, 2 e4m3 weights x bf16 activations, 3 e4m3 weights x e4m3 activations,
-                      // 4 int4 weights x bf16 activations (2, 3, 4: mode 0)
+                      // 4 int4 weights x bf16 activations (2, 3, 4: stream-K partials only)
+  const void* w;      // [rows_w, k]: 16-bit or e4m3 elements, or fmt 4: int4 codes in the engine byte order
+  const float* row_scale;       // fmt 2, 3: [rows_w] fp32 row scales, each partial is multiplied by its row's scale once
+  const uint16_t* group_scale;  // fmt 4: bf16 [rows_w][k / 128] group scales
+};
+
+struct GemmWsCall {
+  WeightOperand w;
   int mode;           // 0 stream-K fp32 partial planes, 1 whole tiles + 16-bit epilogue
-  const void* w;      // [rows_w, k]
   int rows_w;
   const void* x;      // [rows_x, k]
   int rows_x;
@@ -130,9 +137,7 @@ struct GemmWsCall {
   int n_ctas;         // <= 0: one CTA per SM
   int bn;             // token-tile width; 0: chosen by `tiling`
   int tiling;         // WsTiling
-  const float* w_scale;  // fmt 2, 3: [rows_w] fp32 row scales, each partial is multiplied by its row's scale once
-  const float* a_scale;  // fmt 3: [rows_x] fp32 token scales, each partial is then multiplied by its token's scale once
-  const uint16_t* g_scale;  // fmt 4 (w = int4 codes in the engine byte order): bf16 [rows_w][k / 128] group scales
+  const float* a_scale;  // w.fmt 3: [rows_x] fp32 token scales, each partial is then multiplied by its token's scale once
 };
 // What a launch decided, for the kernels that fold its partial planes.
 struct GemmWsPlan {
@@ -149,12 +154,6 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan = 
 int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
                     const float* bias, int act, int n_ctas, cudaStream_t stream);
 
-// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), bf16 x, one CTA per SM:
-// act[rows_x][rows_w / 2] = SwiGLU(x w^T).  w is bf16 (w_scale null) or e4m3 with fp32 row scales w_scale [rows_w];
-// a_scale non-null: x is e4m3 with fp32 token scales a_scale [rows_x] (e4m3 weights only).  g_scale non-null: w is int4
-// codes in the engine byte order with bf16 group scales g_scale [rows_w][k / 128] (w_scale and a_scale null).
-// planes (plane_elems floats) take the partials of the non-finisher CTAs, flags (n_flags counters, zero between
-// launches) their arrivals.
 // ---- prefill GEMM, tokens on wgmma M (gemm_prefill.cuh / gemm.cu): bf16 x [rows_x, k], w [rows_w, k], any rows_x; the
 // k-ranges and plane order of the chunked path's stream-K plan over n_ctas CTAs (<= 0: one per SM).  epi 0: one fp32
 // plane out[rows_x][rows_w] (fill *sk with the one-plane SkInfo its fix-up kernel reads); epi 1: gate|up + SwiGLU into
@@ -162,9 +161,12 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
                         cudaStream_t stream, SkInfo* sk = nullptr);
 
-int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
-                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream,
-                    const float* a_scale = nullptr, const uint16_t* g_scale = nullptr);
+// ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), one CTA per SM:
+// act[rows_x][rows_w / 2] = SwiGLU(x w^T) for weights w of format 1-4; x is bf16, or e4m3 with fp32 token scales
+// a_scale [rows_x] for format 3.  planes (plane_elems floats) take the partials of the non-finisher CTAs, flags (n_flags
+// counters, zero between launches) their arrivals.
+int gemm_wsf_launch(const WeightOperand& w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
+                    size_t plane_elems, int* flags, int n_flags, cudaStream_t stream, const float* a_scale = nullptr);
 
 // ---- decoder fix-up and decision kernels (decoder_kernels.cuh / engine.cu) -----------
 // bf16 tensors; `part` holds fp32 stream-K planes [plane][T][width] of the plan `sk`, as gemm_ws_launch mode 0 leaves

@@ -28,16 +28,9 @@ constexpr int kRotFloats = 128;  // vlo_kv_evict's cos | sin (head_dim / 2 each)
 
 using bf16 = __nv_bfloat16;
 
-// a layer matrix [n, k]: bf16 (scale and gscale null), e4m3 bytes with fp32 row scales [n], or int4 codes in the engine
-// byte order with bf16 group scales [n, k / 128]
-struct DecW {
-  const void* w;
-  const float* scale;
-  const uint16_t* gscale;
-};
 struct DecLayer {
   const bf16 *in_norm, *post_norm;
-  DecW qkv, o, gate_up, down;
+  WeightOperand qkv, o, gate_up, down;   // the layer matrices, all of the engine's layer_fmt
 };
 struct VitLayer {
   const float *ln1_w, *ln1_b, *ln2_w, *ln2_b, *qkv_b, *out_b, *fc1_b, *fc2_b;
@@ -64,8 +57,7 @@ struct vlo_engine {
               *head_fc1_b = nullptr, *head_fc2_b = nullptr, *conn0_b = nullptr, *conn2_b = nullptr;
   const bf16 *conn0_w = nullptr, *conn2_w = nullptr;
   bool has_vit = false, has_connector = false, has_decoder = false;
-  bool fp8_weights = false;  // the layer matrices are e4m3 + row scales (vlo_finalize_weights)
-  bool int4_weights = false; // the layer matrices are int4 codes + group scales (vlo_finalize_weights)
+  int layer_fmt = FMT_BF16;  // GemmFmt of the layer matrices (vlo_finalize_weights; FMT_E4M3_A8 with fp8_act)
   bool fp8_act = false;      // vlo_set_fp8_activations: the layer GEMMs take e4m3 activations with token scales
 
   // derived
@@ -208,17 +200,15 @@ int lookup(vlo_engine* e, const std::string& name, int64_t expect_elems, const T
 }
 
 // weights [n_out, k] x tokens [rows, k] -> stream-K fp32 partial planes part[plane][rows][n_out] (persistent kernel),
-// which a fix-up kernel folds.  The fix-up kernels unroll kFixMaxPlanes planes: this is the one check of that limit,
-// made before the fix-up kernel that would read the planes is launched.
-int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int k, float* part, size_t part_elems,
-                 int tiling, GemmWsPlan* plan, cudaStream_t st, const float* w_scale = nullptr,
-                 const float* a_scale = nullptr) {
+// which a fix-up kernel folds.  x_scale: the token scales of e4m3 activations (w.fmt FMT_E4M3_A8).  The fix-up kernels
+// unroll kFixMaxPlanes planes: this is the one check of that limit, made before the fix-up kernel that would read the
+// planes is launched.
+int gemm_partial(const WeightOperand& w, int n_out, const void* x, const float* x_scale, int rows, int k, float* part,
+                 size_t part_elems, int tiling, GemmWsPlan* plan, cudaStream_t st) {
   GemmWsCall c{};
-  c.fmt = fmt;
-  c.w_scale = w_scale;
-  c.a_scale = a_scale;
-  c.mode = 0;
   c.w = w;
+  c.a_scale = x_scale;
+  c.mode = 0;
   c.rows_w = n_out;
   c.x = x;
   c.rows_x = rows;
@@ -233,51 +223,22 @@ int gemm_partial(int fmt, const void* w, int n_out, const void* x, int rows, int
   return 0;
 }
 
-// the decoder's partial GEMMs: bf16 or e4m3 weights, the step's T tokens, planes in e->part.  x_scale non-null: x is the
-// e4m3 copy of the activations with these token scales (fp8_act).
-int dec_partial(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, int k, GemmWsPlan* sk, cudaStream_t st,
-                const float* x_scale = nullptr) {
-  if (w.gscale != nullptr) {
-    GemmWsCall c{};
-    c.fmt = FMT_I4;
-    c.g_scale = w.gscale;
-    c.mode = 0;
-    c.w = w.w;
-    c.rows_w = n_out;
-    c.x = x;
-    c.rows_x = T;
-    c.k = k;
-    c.out = e->part;
-    c.out_elems = e->part_elems;
-    c.ld_out = n_out;
-    c.plane_stride = static_cast<long long>(T) * n_out;
-    c.tiling = WS_TILE_FIT;
-    if (gemm_ws_launch(c, st, sk)) return -1;
-    VLO_CHECK(sk->planes <= kFixMaxPlanes, "stream-K produced more partial planes than the fix-up kernels unroll");
-    return 0;
-  }
-  return gemm_partial(x_scale ? FMT_E4M3_A8 : w.scale ? FMT_E4M3 : FMT_BF16, w.w, n_out, x, T, k, e->part, e->part_elems,
-                      WS_TILE_FIT, sk, st, w.scale, x_scale);
-}
-
 // gate|up GEMM + SwiGLU: the stream-K finisher CTAs apply the fix-up themselves (gemm_wsf.cuh).  A finisher's epilogue
 // (flag acquire -> plane loads -> stores) is a tail at the end of EVERY CTA during which its SM streams nothing, while a
 // separate fix-up kernel runs next to the next GEMM's CTA, whose ring is already filling.  Only the gate|up GEMM has
 // enough tiles (224, 1.7 per CTA on 132 SMs) to amortise that tail, and fusing it removes the 3.6 MB plane round trip of
 // its fix-up; q|k|v, o_proj and down_proj go through gemm_partial and a fix-up kernel (DESIGN.md section 5).
-int gemm_swiglu(vlo_engine* e, const DecW& w, int n_out, const void* x, int T, int k, cudaStream_t st,
+int gemm_swiglu(vlo_engine* e, const WeightOperand& w, int n_out, const void* x, int T, int k, cudaStream_t st,
                 const float* x_scale = nullptr) {
-  return gemm_wsf_launch(w.w, w.scale, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st, x_scale,
-                         w.gscale);
+  return gemm_wsf_launch(w, n_out, x, T, k, e->act, e->part, e->part_elems, e->sk_flags, kSkFlags, st, x_scale);
 }
 
 // whole-tile persistent GEMM with the 16-bit epilogue: out[T, n_out] = act(x W^T + bias)
 int gemm_ws_store16(int fmt, const void* w, int n_out, const void* x, int T, int k, void* out, int ld, const float* bias,
                     int act, cudaStream_t st, int tiling = WS_TILE_FIT) {
   GemmWsCall c{};
-  c.fmt = fmt;
+  c.w = WeightOperand{fmt, w, nullptr, nullptr};
   c.mode = 1;
-  c.w = w;
   c.rows_w = n_out;
   c.x = x;
   c.rows_x = T;
@@ -760,10 +721,10 @@ int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t 
 }
 
 namespace {
-// Layer matrix `name` [n, k] in exactly one form: bf16 `name` (form 0), e4m3 bytes `name.f8` with fp32 row scales
-// `name.scale` (form 1), or int4 codes `name.i4` with bf16 group scales `name.gscale` (form 2).  *form < 0: the first
-// matrix, which sets the form every later one must share.
-int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* forms, DecW* out) {
+// Layer matrix `name` [n, k] in exactly one form: bf16 `name` (FMT_BF16), e4m3 bytes `name.f8` with fp32 row scales
+// `name.scale` (FMT_E4M3, or FMT_E4M3_A8 with fp8_act), or int4 codes `name.i4` with bf16 group scales `name.gscale`
+// (FMT_I4).  *fmt < 0: the first matrix, which sets the format every later one must share.
+int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* fmt, WeightOperand* out) {
   const bool has16 = e->tensors.count(name) > 0, has8 = e->tensors.count(name + ".f8") > 0,
              has_s = e->tensors.count(name + ".scale") > 0, has4 = e->tensors.count(name + ".i4") > 0,
              has_g = e->tensors.count(name + ".gscale") > 0;
@@ -774,32 +735,32 @@ int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64
                 name + ".gscale')");
   if (has8 != has_s) return fail("missing weight tensor '" + name + (has8 ? ".scale'" : ".f8'"));
   if (has4 != has_g) return fail("missing weight tensor '" + name + (has4 ? ".gscale'" : ".i4'"));
-  const int form = has8 ? 1 : has4 ? 2 : 0;
-  static const char* const kDesc[3] = {"' is bf16", ".f8' is e4m3", ".i4' is int4"};
-  if (*forms >= 0 && form != *forms)
-    return fail("weight tensor '" + name + kDesc[form] + " but an earlier layer matrix is not: all layer matrices must share one form");
-  *forms = form;
-  out->scale = nullptr;
-  out->gscale = nullptr;
-  if (form == 2) {
+  out->fmt = has8 ? (e->fp8_act ? FMT_E4M3_A8 : FMT_E4M3) : has4 ? FMT_I4 : FMT_BF16;
+  if (*fmt >= 0 && out->fmt != *fmt)
+    return fail("weight tensor '" + name + (has8 ? ".f8' is e4m3" : has4 ? ".i4' is int4" : "' is bf16") +
+                " but an earlier layer matrix is not: all layer matrices must share one form");
+  *fmt = out->fmt;
+  out->row_scale = nullptr;
+  out->group_scale = nullptr;
+  if (has4) {
     if (k % kI4Group != 0)
       return fail("weight tensor '" + name + ".i4': int4 weights need K (" + std::to_string(k) +
                   ") to be a multiple of 128, one scale per 128 weights of a row");
     const uint8_t* w;
     if (lookup(e, name + ".i4", (n + kGemmBM - 1) / kGemmBM * kGemmBM * (k / 2), &w) ||
-        lookup(e, name + ".gscale", n * (k / kI4Group), &out->gscale))
+        lookup(e, name + ".gscale", n * (k / kI4Group), &out->group_scale))
       return -1;
     out->w = w;
     return 0;
   }
-  if (!form) {
+  if (!has8) {
     const bf16* w;
     if (lookup(e, name, n * k, &w)) return -1;
     out->w = w;
     return 0;
   }
   const uint8_t* w;
-  if (lookup(e, name + ".f8", n * k, &w) || lookup(e, name + ".scale", n, &out->scale)) return -1;
+  if (lookup(e, name + ".f8", n * k, &w) || lookup(e, name + ".scale", n, &out->row_scale)) return -1;
   out->w = w;
   return 0;
 }
@@ -822,26 +783,25 @@ int vlo_finalize_weights(vlo_engine* e) {
     if (lookup(e, "rope.cos", e->rope_positions * 64, &e->rope_cos)) return -1;
     if (lookup(e, "rope.sin", e->rope_positions * 64, &e->rope_sin)) return -1;
     std::vector<DecLayer> dec(c.num_layers);   // installed only once every matrix has resolved
-    int f8 = -1;
+    int fmt = -1;
     for (int l = 0; l < c.num_layers; ++l) {
       const std::string p = "L" + std::to_string(l) + ".";
       DecLayer& d = dec[l];
       if (lookup(e, p + "in_norm", H, &d.in_norm)) return -1;
-      if (lookup_layer_matrix(e, p + "qkv", e->qkv_width, H, &f8, &d.qkv)) return -1;
-      if (lookup_layer_matrix(e, p + "o", H, static_cast<int64_t>(c.num_heads) * c.head_dim, &f8, &d.o)) return -1;
+      if (lookup_layer_matrix(e, p + "qkv", e->qkv_width, H, &fmt, &d.qkv)) return -1;
+      if (lookup_layer_matrix(e, p + "o", H, static_cast<int64_t>(c.num_heads) * c.head_dim, &fmt, &d.o)) return -1;
       if (lookup(e, p + "post_norm", H, &d.post_norm)) return -1;
-      if (lookup_layer_matrix(e, p + "gate_up", 2 * I, H, &f8, &d.gate_up)) return -1;
-      if (lookup_layer_matrix(e, p + "down", H, I, &f8, &d.down)) return -1;
+      if (lookup_layer_matrix(e, p + "gate_up", 2 * I, H, &fmt, &d.gate_up)) return -1;
+      if (lookup_layer_matrix(e, p + "down", H, I, &fmt, &d.down)) return -1;
     }
-    VLO_CHECK(!e->fp8_act || f8 != 2,
+    VLO_CHECK(!e->fp8_act || fmt != FMT_I4,
               "fp8_activations takes FP8 (e4m3) layer weights, but the layer matrices are int4: 4-bit weights multiply "
               "bf16 activations");
-    VLO_CHECK(!e->fp8_act || f8 == 1,
+    VLO_CHECK(!e->fp8_act || fmt == FMT_E4M3_A8,
               "fp8_activations needs FP8 (e4m3) layer weights, but the layer matrices are bf16: the FP8 tensor cores "
               "take both operands in e4m3");
     e->dec.swap(dec);
-    e->fp8_weights = f8 == 1;
-    e->int4_weights = f8 == 2;
+    e->layer_fmt = fmt;
   }
   e->has_connector = e->tensors.count("conn.0.w") > 0;
   if (e->has_connector) {
@@ -881,7 +841,7 @@ int vlo_finalize_weights(vlo_engine* e) {
   }
   // A bf16 engine prefills (vlo_prefill): its token-row workspaces grow once to max_prefill rows.  Engines with e4m3 layer
   // weights or activations chunk long inputs into steps and keep them at max_step_tokens.
-  if (e->has_decoder && !e->fp8_weights && !e->int4_weights && !e->fp8_act && e->max_prefill == 0) {
+  if (e->has_decoder && e->layer_fmt == FMT_BF16 && e->max_prefill == 0) {
     VLO_CUDA(cudaDeviceSynchronize());   // no step, copy or staging slot of this engine may be in flight
     if (size_token_rows(e, kFixMaxPlanes * c.max_step_tokens)) return -1;
     e->max_prefill = kFixMaxPlanes * c.max_step_tokens;
@@ -1250,7 +1210,7 @@ int vlo_vit_encode(vlo_engine* e, const uint8_t* d_frames, int B, void* d_out, f
     return gemm_ws_store16(FMT_F16, w, n_out, x, rows, k, out, n_out, bias, act, st, WS_TILE_TRUNK);
   };
   auto partial_gemm = [&](const __half* x, const __half* w, int k, GemmWsPlan* plan) -> int {
-    return gemm_partial(FMT_F16, w, C, x, rows, k, e->v_part, e->v_part_elems,
+    return gemm_partial(WeightOperand{FMT_F16, w, nullptr, nullptr}, C, x, nullptr, rows, k, e->v_part, e->v_part_elems,
                         small ? WS_TILE_BESIDE_DECODER : WS_TILE_TRUNK, plan, st);
   };
   auto fix_ln = [&](const GemmWsPlan& plan, const float* bias, const float* lw, const float* lb, float* out32) -> int {
@@ -1436,12 +1396,12 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   const void* attn_in = a8 ? static_cast<const void*>(e->aq) : e->attn_out;
   const void* act_in = a8 ? static_cast<const void*>(e->actq) : e->act;
   // the layer GEMMs: stream-K partial planes of the step's plan, or the prefill GEMM's one plane (fix-up plan: G = 1)
-  auto partial = [&](const DecW& w, int n_out, const void* x, int k, GemmWsPlan* sk, const float* x_scale) -> int {
-    if (!prefill) return dec_partial(e, w, n_out, x, T, k, sk, st, x_scale);
+  auto partial = [&](const WeightOperand& w, int n_out, const void* x, int k, GemmWsPlan* sk, const float* x_scale) -> int {
+    if (!prefill) return gemm_partial(w, n_out, x, x_scale, T, k, e->part, e->part_elems, WS_TILE_FIT, sk, st);
     VLO_CHECK(static_cast<size_t>(T) * n_out <= e->part_elems, "prefill: the plane exceeds the partial workspace");
     return gemm_prefill_launch(PREFILL_PLANE, w.w, n_out, x, T, k, 0, e->part, st, &sk->sk);
   };
-  auto swiglu = [&](const DecW& w) -> int {
+  auto swiglu = [&](const WeightOperand& w) -> int {
     if (!prefill) return gemm_swiglu(e, w, 2 * c.intermediate_size, xn_in, T, H, st, a8 ? e->xs : nullptr);
     return gemm_prefill_launch(PREFILL_SWIGLU, w.w, 2 * c.intermediate_size, e->xn, T, H, 0, e->act, st);
   };
@@ -1502,7 +1462,7 @@ int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, co
 int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row_ids, const void* d_embeds,
                 void* d_last_logits, vlo_decision* d_decision, int interval_id, void* cuda_stream) {
   VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
-  VLO_CHECK(!e->fp8_weights && !e->int4_weights && !e->fp8_act && e->max_prefill > 0,
+  VLO_CHECK(e->layer_fmt == FMT_BF16 && e->max_prefill > 0,
             "prefill: bf16 layer weights and activations only (e4m3 engines chunk long inputs into steps)");
   VLO_CHECK(n_tokens > 0 && n_tokens <= e->max_prefill,
             "prefill: n_tokens must lie in [1, max_prefill_tokens] = [1, " + std::to_string(e->max_prefill) + "]");
@@ -1590,30 +1550,25 @@ int vlo_bench_gemm(vlo_engine* e, int n_tok, int iters, double* h_algo_bytes_per
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   const int H = c.hidden_size, I = c.intermediate_size, A = c.num_heads * c.head_dim;
   double bytes = 0.0;
-  // e4m3: 1 B + a scale per row; int4: half a byte + a bf16 scale per 128 weights
-  const double w_elem = e->fp8_weights ? 1.0 : e->int4_weights ? 0.5 + 2.0 / kI4Group : 2.0, row_b = e->fp8_weights ? 4.0 : 0.0;
-  // fp8_act: the W8A8 GEMMs on the e4m3 activation copies, 1 B per activation + a scale per token
+  // fp8_act: the W8A8 GEMMs on the e4m3 activation copies with their token scales
   const bool a8 = e->fp8_act;
-  const double x_elem = a8 ? 1.0 : 2.0, tok_b = a8 ? 4.0 : 0.0;
+  const void* xn = a8 ? static_cast<const void*>(e->xq) : e->xn;
+  const void* attn = a8 ? static_cast<const void*>(e->aq) : e->attn_out;
+  const void* act = a8 ? static_cast<const void*>(e->actq) : e->act;
+  auto gemm = [&](const WeightOperand& w, int n_out, const void* x, const float* x_scale, int k) -> int {
+    GemmWsPlan sk{};
+    return gemm_partial(w, n_out, x, a8 ? x_scale : nullptr, n_tok, k, e->part, e->part_elems, WS_TILE_FIT, &sk, st);
+  };
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < c.num_layers; ++l) {
       const DecLayer& d = e->dec[l];
-      GemmWsPlan sk{};
-      if (a8) {
-        if (dec_partial(e, d.qkv, e->qkv_width, e->xq, n_tok, H, &sk, st, e->xs)) return -1;
-        if (dec_partial(e, d.o, H, e->aq, n_tok, A, &sk, st, e->as)) return -1;
-        if (dec_partial(e, d.gate_up, 2 * I, e->xq, n_tok, H, &sk, st, e->xs)) return -1;
-        if (dec_partial(e, d.down, H, e->actq, n_tok, I, &sk, st, e->acts)) return -1;
-      } else {
-        if (dec_partial(e, d.qkv, e->qkv_width, e->xn, n_tok, H, &sk, st)) return -1;
-        if (dec_partial(e, d.o, H, e->attn_out, n_tok, A, &sk, st)) return -1;
-        if (dec_partial(e, d.gate_up, 2 * I, e->xn, n_tok, H, &sk, st)) return -1;
-        if (dec_partial(e, d.down, H, e->act, n_tok, I, &sk, st)) return -1;
-      }
+      if (gemm(d.qkv, e->qkv_width, xn, e->xs, H)) return -1;
+      if (gemm(d.o, H, attn, e->as, A)) return -1;
+      if (gemm(d.gate_up, 2 * I, xn, e->xs, H)) return -1;
+      if (gemm(d.down, H, act, e->acts, I)) return -1;
       if (it == 0)
-        bytes += w_elem * (static_cast<double>(e->qkv_width) * H + static_cast<double>(H) * A + 2.0 * I * H + static_cast<double>(H) * I) +
-                 row_b * (static_cast<double>(e->qkv_width) + H + 2.0 * I + H) + x_elem * n_tok * (2.0 * H + A + I) +
-                 tok_b * 4.0 * n_tok;
+        bytes += ws_in_bytes(e->layer_fmt, e->qkv_width, n_tok, H) + ws_in_bytes(e->layer_fmt, H, n_tok, A) +
+                 ws_in_bytes(e->layer_fmt, 2 * I, n_tok, H) + ws_in_bytes(e->layer_fmt, H, n_tok, I);
     }
   if (h_algo_bytes_per_iter) *h_algo_bytes_per_iter = bytes;
   if (h_launches_per_iter) *h_launches_per_iter = 4 * c.num_layers;

@@ -165,66 +165,68 @@ int gemm_launch(const GemmCall& c, cudaStream_t stream) {
 // persistent weight-streaming GEMM (gemm_ws.cuh)
 
 // The default single-stream frame step runs the ViT of frame i+1 (gemm_vit_kernel for QKV / fc1, the 64-token
-// small-tile configuration of gemm_ws_kernel for out_proj / fc2) next to the decoder step of frame i (16-token tiles,
-// 6 stages).  One CTA of each fits on one sm_90 SM: 228 KB of shared memory per SM, of which 1 KB is reserved per
-// resident block.  The fused gate|up GEMM's 8-stage ring leaves no room for a gemm_vit_kernel CTA (a 6-stage ring
-// would, and measured no faster: DESIGN.md section 5).
+// small-tile configuration of gemm_ws_kernel for out_proj / fc2) next to the decoder step of frame i (16-token tiles).
+// One CTA of each fits on one sm_90 SM: 228 KB of shared memory per SM, of which 1 KB is reserved per resident block.
+// The fused gate|up GEMM's 8-stage ring leaves no room for a gemm_vit_kernel CTA (a 6-stage ring would, and measured no
+// faster: DESIGN.md section 5).
 constexpr int kSmemPerSm = 233472, kSmemReservedPerBlock = 1024;
-static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
-static_assert(GemmWsCfg<16, 6>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
-static_assert(GemmWsfCfg<16, wsf_default_stages(16)>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
+constexpr int kVitBesideBytes = GemmWsCfg<FMT_F16, 64, 3>::kSmemBytes;   // the 64-token ViT GEMM CTA (83 KB)
+// Ring depth of the 16-token decoder GEMM of each weight format.  bf16: 6 x 18 KB, measured.  The others: the deepest
+// ring that fits beside the ViT trunk GEMM CTA, up to the format's cap (e4m3: 8 stages of 10 KB next to the two
+// converted 16 KB tiles, 64 KB of weights in flight; W8A8: 9 KB stages; int4: 24 KB slots of 16 KB of codes and 8 KB of
+// activations; DESIGN.md section 5).
+constexpr int decoder_stages(int fmt) {
+  return fmt == FMT_BF16 ? 6
+                         : std::min(ws_max_stages(fmt), (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes -
+                                                         ws_fixed_bytes(fmt, 0)) /
+                                                            (ws_slot_bytes_w(fmt, 16) + ws_slot_bytes_x(fmt, 16)));
+}
+template <int FMT>
+constexpr bool decoder_shares_sm() {
+  constexpr int dec = GemmWsCfg<FMT, 16, decoder_stages(FMT)>::kSmemBytes + 2 * kSmemReservedPerBlock;
+  return dec + GemmVitCfg::kSmemBytes <= kSmemPerSm && dec + kVitBesideBytes <= kSmemPerSm;
+}
+static_assert(decoder_shares_sm<FMT_BF16>(), "bf16 decoder GEMM CTA and a ViT GEMM CTA no longer share an SM");
+static_assert(decoder_shares_sm<FMT_E4M3>(), "e4m3 decoder GEMM CTA and a ViT GEMM CTA no longer share an SM");
+static_assert(decoder_shares_sm<FMT_E4M3_A8>(), "W8A8 decoder GEMM CTA and a ViT GEMM CTA no longer share an SM");
+static_assert(decoder_shares_sm<FMT_I4>(), "int4 decoder GEMM CTA and a ViT GEMM CTA no longer share an SM");
+static_assert(GemmWsCfg<FMT_BF16, 16, ws_default_stages(FMT_BF16, 16, kWsfXchBytes), kWsfXchBytes>::kSmemBytes +
+                      GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
               "the 8-stage fused decoder GEMM now shares its SM with a ViT trunk GEMM CTA: update the comment above");
-// The e4m3 16-token decoder GEMM keeps that pairing: the deepest ring of 10 KB stages that fits beside the ViT trunk GEMM
-// CTA next to the two converted 16 KB tiles (8 stages, 64 KB of weights in flight; DESIGN.md section 5).
-constexpr int kF8DecoderStages =
-    std::min(16, (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes - GemmWsCfg<16, 0, FMT_E4M3>::kSmemBytes) /
-                     (kF8BytesW + 16 * kGemmBK * 2));
-static_assert(GemmWsCfg<16, kF8DecoderStages, FMT_E4M3>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "e4m3 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
-static_assert(GemmWsCfg<16, kF8DecoderStages, FMT_E4M3>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "e4m3 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
-// The W8A8 16-token decoder GEMM keeps the pairing too.  Without conversion tiles its 9 KB stages (8 KB of weights, 1 KB
-// of activations) go as deep as the ViT trunk GEMM CTA leaves room for, up to the 16 barrier pairs.
-constexpr int kA8DecoderStages =
-    std::min(16, (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes - GemmWsCfg<16, 0, FMT_E4M3_A8>::kSmemBytes) /
-                     (kA8BytesW + 16 * kGemmBK));
-static_assert(GemmWsCfg<16, kA8DecoderStages, FMT_E4M3_A8>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "W8A8 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
-static_assert(GemmWsCfg<16, kA8DecoderStages, FMT_E4M3_A8>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "W8A8 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
-
-// The int4 16-token decoder GEMM keeps the pairing too: the deepest ring of 24 KB slots (16 KB of codes, 8 KB of
-// activations) that fits beside the ViT trunk GEMM CTA.
-constexpr int kI4DecoderStages =
-    std::min(16, (kSmemPerSm - 2 * kSmemReservedPerBlock - GemmVitCfg::kSmemBytes - GemmWsCfg<16, 0, FMT_I4>::kSmemBytes) /
-                     (i4_slot_units(16) * (kI4BytesUnit + 16 * kGemmBK * 2)));
-static_assert(GemmWsCfg<16, kI4DecoderStages, FMT_I4>::kSmemBytes + GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "int4 decoder GEMM CTA and ViT trunk GEMM CTA no longer share an SM");
-static_assert(GemmWsCfg<16, kI4DecoderStages, FMT_I4>::kSmemBytes + GemmWsCfg<64, 3>::kSmemBytes + 2 * kSmemReservedPerBlock <= kSmemPerSm,
-              "int4 decoder GEMM CTA and 64-token ViT GEMM CTA no longer share an SM");
 
 namespace {
-template <int FMT, int BN,
-          int STAGES = FMT == FMT_E4M3 ? ws_f8_default_stages(BN) : FMT == FMT_E4M3_A8 ? ws_a8_default_stages(BN)
-                       : FMT == FMT_I4 ? ws_i4_default_stages(BN) : ws_default_stages(BN)>
+template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN)>
 int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
   auto kern = gemm_ws_kernel<FMT, BN, STAGES>;
-  using Cfg = GemmWsCfg<BN, STAGES, FMT>;
+  using Cfg = GemmWsCfg<FMT, BN, STAGES>;
   if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
   if (prof_on()) {
     const double out_b = a.mode == 0 ? 4.0 * a.rows_x * a.rows_w : 2.0 * a.rows_x * a.rows_w;
-    const double in_b = FMT == FMT_E4M3      ? (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x   // 1 B per weight + row scales
-                        : FMT == FMT_E4M3_A8 ? (a.k + 4.0) * (static_cast<double>(a.rows_w) + a.rows_x)   // + token scales
-                        : FMT == FMT_I4      ? (a.k / 2.0 + a.k / 64.0) * a.rows_w + 2.0 * a.k * a.rows_x   // codes + scales
-                                             : 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x);
-    prof_begin(FMT == FMT_F16 ? PROF_GEMM_VIT : PROF_GEMM_STREAM, stream, in_b + out_b);
+    prof_begin(FMT == FMT_F16 ? PROF_GEMM_VIT : PROF_GEMM_STREAM, stream, ws_in_bytes(FMT, a.rows_w, a.rows_x, a.k) + out_b);
   }
   VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a));
   prof_end(stream);
   count_launch();
   return 0;
+}
+
+// the instances of one format: every decoder token tile, the 16-token one at its decoder ring depth; fp16 also has the
+// 192-wide ViT trunk tile and the 3-stage 64-token ring that fits beside a decoder CTA
+template <int FMT>
+int launch_ws_fmt(int bn, bool beside, const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a,
+                  cudaStream_t stream) {
+  if constexpr (FMT == FMT_F16) {
+    if (beside) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);
+    if (bn == 192) return launch_ws<FMT_F16, 192>(tw, tx, a, stream);
+  }
+  switch (bn) {
+    case 16: return launch_ws<FMT, 16, FMT == FMT_F16 ? ws_default_stages(FMT, 16) : decoder_stages(FMT)>(tw, tx, a, stream);
+    case 32: return launch_ws<FMT, 32>(tw, tx, a, stream);
+    case 64: return launch_ws<FMT, 64>(tw, tx, a, stream);
+    case 96: return launch_ws<FMT, 96>(tw, tx, a, stream);
+    case 128: return launch_ws<FMT, 128>(tw, tx, a, stream);
+  }
+  return fail("gemm_ws_launch: no kernel instance");
 }
 
 // Token-tile width for rows_x token rows, of both weight-streaming kernels: the smallest instance covering them (a
@@ -276,15 +278,16 @@ int gemm_ws_plan(int tiles, int k, int mode, int n_ctas, SkInfo* sk) {
 int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   VLO_CHECK(c.k > 0 && c.k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(c.rows_w > 0 && c.rows_x > 0, "empty GEMM operand");
+  const int fmt = c.w.fmt;
   const bool beside = c.tiling == WS_TILE_BESIDE_DECODER;
   const int bn = c.bn > 0 ? c.bn
                  : beside ? 64
                  : c.tiling == WS_TILE_TRUNK ? trunk_token_tile(c.rows_x, c.rows_w, c.mode)
-                 : token_tile(c.rows_x, c.fmt);
-  VLO_CHECK(!beside || (c.fmt == FMT_F16 && bn == 64), "gemm_ws: only the 64-token fp16 instance fits beside a decoder CTA");
-  const bool a8 = c.fmt == FMT_E4M3_A8;
-  const bool f8 = c.fmt == FMT_E4M3 || a8;
-  const bool i4 = c.fmt == FMT_I4;
+                 : token_tile(c.rows_x, fmt);
+  VLO_CHECK(!beside || (fmt == FMT_F16 && bn == 64), "gemm_ws: only the 64-token fp16 instance fits beside a decoder CTA");
+  const bool a8 = fmt == FMT_E4M3_A8;
+  const bool f8 = fmt == FMT_E4M3 || a8;
+  const bool i4 = fmt == FMT_I4;
   VLO_CHECK(!f8 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn)),
             "gemm_ws: e4m3 weights run stream-K partials (mode 0) on the token tile token_tile() picks");
   VLO_CHECK(!i4 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn) && c.rows_x <= 128),
@@ -302,6 +305,7 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   if (c.out == nullptr) return 0;
   VLO_CHECK(c.mode != 0 || static_cast<size_t>(planes) * static_cast<size_t>(c.plane_stride) <= c.out_elems,
             "stream-K workspace too small for " + std::to_string(planes) + " partial planes");
+  VLO_CHECK(fmt >= FMT_F16 && fmt <= FMT_I4, "gemm_ws_launch: no kernel instance for fmt " + std::to_string(fmt));
   a.hint_w = x_tiles > 1 ? kEvictNormal : kEvictFirst;   // weights re-read by several token tiles stay in L2
   a.mode = c.mode;
   a.out = c.out;
@@ -309,53 +313,22 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   a.plane_stride = c.plane_stride;
   a.bias = c.bias;
   a.act = c.act;
-  VLO_CHECK(!f8 || c.w_scale != nullptr, "gemm_ws: e4m3 weights need their row scales");
-  a.w_scale = c.w_scale;
+  VLO_CHECK(!f8 || c.w.row_scale != nullptr, "gemm_ws: e4m3 weights need their row scales");
   VLO_CHECK(!a8 || c.a_scale != nullptr, "gemm_ws: e4m3 activations need their token scales");
-  a.a_scale = c.a_scale;
-  VLO_CHECK(!i4 || (c.g_scale != nullptr && (reinterpret_cast<uintptr_t>(c.w) & 15) == 0),
+  VLO_CHECK(!i4 || (c.w.group_scale != nullptr && (reinterpret_cast<uintptr_t>(c.w.w) & 15) == 0),
             "gemm_ws: int4 weights need their group scales and 16-byte aligned codes");
-  a.w4 = static_cast<const uint8_t*>(c.w);
-  a.g_scale = c.g_scale;
+  a.wt = WsWeightArgs{c.w.row_scale, c.a_scale, static_cast<const uint8_t*>(c.w.w), c.w.group_scale};
   CUtensorMap tw, tx;
-  if (i4) {
-    if (get_tmap(c.x, c.rows_x, c.k, bn, FMT_BF16, &tx) != 0) return -1;
-    tw = tx;   // unused: the codes stream as bulk copies
-    if (bn == 16) return launch_ws<FMT_I4, 16, kI4DecoderStages>(tw, tx, a, stream);
-    if (bn == 32) return launch_ws<FMT_I4, 32>(tw, tx, a, stream);
-    if (bn == 64) return launch_ws<FMT_I4, 64>(tw, tx, a, stream);
-    if (bn == 96) return launch_ws<FMT_I4, 96>(tw, tx, a, stream);
-    return launch_ws<FMT_I4, 128>(tw, tx, a, stream);
+  if (!i4 && get_tmap(c.w.w, c.rows_w, c.k, kGemmBM, kWsFmtInfo[fmt].w_map, &tw) != 0) return -1;
+  if (get_tmap(c.x, c.rows_x, c.k, bn, kWsFmtInfo[fmt].x_map, &tx) != 0) return -1;
+  if (i4) tw = tx;   // unused: the codes stream as bulk copies
+  switch (fmt) {
+    case FMT_F16: return launch_ws_fmt<FMT_F16>(bn, beside, tw, tx, a, stream);
+    case FMT_BF16: return launch_ws_fmt<FMT_BF16>(bn, beside, tw, tx, a, stream);
+    case FMT_E4M3: return launch_ws_fmt<FMT_E4M3>(bn, beside, tw, tx, a, stream);
+    case FMT_E4M3_A8: return launch_ws_fmt<FMT_E4M3_A8>(bn, beside, tw, tx, a, stream);
+    default: return launch_ws_fmt<FMT_I4>(bn, beside, tw, tx, a, stream);
   }
-  if (get_tmap(c.w, c.rows_w, c.k, kGemmBM, c.fmt, &tw) != 0) return -1;
-  if (get_tmap(c.x, c.rows_x, c.k, bn, a8 ? FMT_E4M3_A8 : f8 ? FMT_BF16 : c.fmt, &tx) != 0) return -1;
-#define VLO_WS_CASE(F, N) \
-  if (c.fmt == F && bn == N) return launch_ws<F, N>(tw, tx, a, stream);
-  // the single-stream decoder GEMM: 6 x 18 KB leaves room on the SM for a co-resident ViT CTA (static_asserts above)
-  if (c.fmt == FMT_BF16 && bn == 16) return launch_ws<FMT_BF16, 16, 6>(tw, tx, a, stream);
-  if (a8 && bn == 16) return launch_ws<FMT_E4M3_A8, 16, kA8DecoderStages>(tw, tx, a, stream);
-  if (f8 && bn == 16) return launch_ws<FMT_E4M3, 16, kF8DecoderStages>(tw, tx, a, stream);
-  if (beside) return launch_ws<FMT_F16, 64, 3>(tw, tx, a, stream);    // 83 KB
-  VLO_WS_CASE(FMT_BF16, 32)
-  VLO_WS_CASE(FMT_BF16, 64)
-  VLO_WS_CASE(FMT_BF16, 96)
-  VLO_WS_CASE(FMT_BF16, 128)
-  VLO_WS_CASE(FMT_F16, 16)
-  VLO_WS_CASE(FMT_F16, 32)
-  VLO_WS_CASE(FMT_F16, 64)
-  VLO_WS_CASE(FMT_F16, 128)
-  VLO_WS_CASE(FMT_F16, 96)
-  VLO_WS_CASE(FMT_F16, 192)
-  VLO_WS_CASE(FMT_E4M3, 32)
-  VLO_WS_CASE(FMT_E4M3, 64)
-  VLO_WS_CASE(FMT_E4M3, 96)
-  VLO_WS_CASE(FMT_E4M3, 128)
-  VLO_WS_CASE(FMT_E4M3_A8, 32)
-  VLO_WS_CASE(FMT_E4M3_A8, 64)
-  VLO_WS_CASE(FMT_E4M3_A8, 96)
-  VLO_WS_CASE(FMT_E4M3_A8, 128)
-#undef VLO_WS_CASE
-  return fail("gemm_ws_launch: no kernel instance");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -432,68 +405,38 @@ int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int r
 // ------------------------------------------------------------------------------------------------
 // stream-K gate|up GEMM with the SwiGLU finisher epilogue (gemm_wsf.cuh)
 namespace {
-template <int BN>
-int launch_wsf_i4(const CUtensorMap& tx, const GemmWsfArgs& a, const void* w4, const uint16_t* g_scale, cudaStream_t stream) {
-  constexpr int S = wsf_i4_default_stages(BN);
-  auto kern = gemm_wsf_i4_kernel<BN, S>;
-  using Cfg = GemmWsfCfg<BN, S, FMT_I4>;
+template <int FMT, int BN>
+int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, cudaStream_t stream) {
+  constexpr int S = ws_default_stages(FMT, BN, kWsfXchBytes);
+  auto kern = gemm_wsf_kernel<FMT, BN, S>;
+  using Cfg = GemmWsCfg<FMT, BN, S, kWsfXchBytes>;
   if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
-  if (prof_on())   // half a byte per weight + a bf16 scale per 128
-    prof_begin(PROF_GEMM_STREAM, stream, (a.k / 2.0 + a.k / 64.0) * a.rows_w + 2.0 * a.k * a.rows_x + 2.0 * a.rows_x * a.rows_w);
-  VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tx, a,
-                      static_cast<const uint8_t*>(w4), g_scale));
-  prof_end(stream);
-  count_launch();
-  return 0;
-}
-
-// w_scale null: bf16 weights; else e4m3 weights with these row scales, and with a_scale also e4m3 activations
-template <int BN>
-int launch_wsf(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, const float* w_scale,
-               const float* a_scale, cudaStream_t stream) {
-  if (a_scale != nullptr) {
-    constexpr int S = wsf_a8_default_stages(BN);
-    auto kern = gemm_wsf_a8_kernel<BN, S>;
-    using Cfg = GemmWsfCfg<BN, S, FMT_E4M3_A8>;
-    if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
-    if (prof_on())   // 1 B per weight and activation + their scales
-      prof_begin(PROF_GEMM_STREAM, stream, (a.k + 4.0) * (static_cast<double>(a.rows_w) + a.rows_x) + 2.0 * a.rows_x * a.rows_w);
-    VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a, w_scale, a_scale));
-    prof_end(stream);
-    count_launch();
-    return 0;
-  }
-  if (w_scale != nullptr) {
-    constexpr int S = wsf_f8_default_stages(BN);
-    auto kern = gemm_wsf_f8_kernel<BN, S>;
-    using Cfg = GemmWsfCfg<BN, S, FMT_E4M3>;
-    if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
-    if (prof_on())   // 1 B per weight + the row scales
-      prof_begin(PROF_GEMM_STREAM, stream, (a.k + 4.0) * a.rows_w + 2.0 * a.k * a.rows_x + 2.0 * a.rows_x * a.rows_w);
-    VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a, w_scale));
-    prof_end(stream);
-    count_launch();
-    return 0;
-  }
-  constexpr int S = wsf_default_stages(BN);
-  auto kern = gemm_wsf_kernel<BN, S>;
-  using Cfg = GemmWsfCfg<BN, S>;
-  if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
-  if (prof_on())
-    prof_begin(PROF_GEMM_STREAM, stream, 2.0 * a.k * (static_cast<double>(a.rows_w) + a.rows_x) + 2.0 * a.rows_x * a.rows_w);
+  if (prof_on()) prof_begin(PROF_GEMM_STREAM, stream, ws_in_bytes(FMT, a.rows_w, a.rows_x, a.k) + 2.0 * a.rows_x * a.rows_w);
   VLO_CUDA(launch_pdl(kern, dim3(a.sk.G), dim3(kGemmThreads), Cfg::kSmemBytes, stream, tw, tx, a));
   prof_end(stream);
   count_launch();
   return 0;
 }
+
+template <int FMT>
+int launch_wsf_fmt(int bn, const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsfArgs& a, cudaStream_t stream) {
+  switch (bn) {
+    case 16: return launch_wsf<FMT, 16>(tw, tx, a, stream);
+    case 32: return launch_wsf<FMT, 32>(tw, tx, a, stream);
+    case 64: return launch_wsf<FMT, 64>(tw, tx, a, stream);
+    case 96: return launch_wsf<FMT, 96>(tw, tx, a, stream);
+    default: return launch_wsf<FMT, 128>(tw, tx, a, stream);
+  }
+}
 }  // namespace
 
-int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void* x, int rows_x, int k, void* act,
-                    float* planes, size_t plane_elems, int* flags, int n_flags, cudaStream_t stream, const float* a_scale,
-                    const uint16_t* g_scale) {
+int gemm_wsf_launch(const WeightOperand& w, int rows_w, const void* x, int rows_x, int k, void* act, float* planes,
+                    size_t plane_elems, int* flags, int n_flags, cudaStream_t stream, const float* a_scale) {
   VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(rows_w > 0 && rows_x > 0 && rows_x <= 128, "gemm_wsf: 1..128 token rows");
   VLO_CHECK(rows_w % kGemmBM == 0, "gemm_wsf: the SwiGLU epilogue needs whole 128-row tiles");
+  const int fmt = w.fmt;
+  VLO_CHECK(fmt >= FMT_BF16 && fmt <= FMT_I4, "gemm_wsf: bf16, e4m3 or int4 weights");
   const int bn = token_tile(rows_x, FMT_BF16);
   GemmWsfArgs a{};
   a.rows_w = rows_w;
@@ -509,28 +452,22 @@ int gemm_wsf_launch(const void* w, const float* w_scale, int rows_w, const void*
   a.hint_w = kEvictFirst;
   a.act = static_cast<__nv_bfloat16*>(act);
   a.I = rows_w / 2;
-  VLO_CHECK(a_scale == nullptr || w_scale != nullptr, "gemm_wsf: e4m3 activations need e4m3 weights");
-  if (g_scale != nullptr) {
-    VLO_CHECK(w_scale == nullptr && a_scale == nullptr, "gemm_wsf: int4 weights take bf16 activations");
-    VLO_CHECK(k % kI4Group == 0, "gemm_wsf: int4 weights need K to be a multiple of 128 (one scale per 128 k)");
-    VLO_CHECK((reinterpret_cast<uintptr_t>(w) & 15) == 0, "gemm_wsf: int4 codes must be 16-byte aligned");
-    CUtensorMap tx;
-    if (get_tmap(x, rows_x, k, bn, FMT_BF16, &tx) != 0) return -1;
-    if (bn == 16) return launch_wsf_i4<16>(tx, a, w, g_scale, stream);
-    if (bn == 32) return launch_wsf_i4<32>(tx, a, w, g_scale, stream);
-    if (bn == 64) return launch_wsf_i4<64>(tx, a, w, g_scale, stream);
-    if (bn == 96) return launch_wsf_i4<96>(tx, a, w, g_scale, stream);
-    return launch_wsf_i4<128>(tx, a, w, g_scale, stream);
-  }
-  const int fw = a_scale ? FMT_E4M3_A8 : w_scale ? FMT_E4M3 : FMT_BF16;
+  VLO_CHECK(fmt != FMT_E4M3 && fmt != FMT_E4M3_A8 || w.row_scale != nullptr, "gemm_wsf: e4m3 weights need their row scales");
+  VLO_CHECK(fmt != FMT_E4M3_A8 || a_scale != nullptr, "gemm_wsf: e4m3 activations need their token scales");
+  VLO_CHECK(fmt != FMT_I4 || w.group_scale != nullptr, "gemm_wsf: int4 weights need their group scales");
+  VLO_CHECK(fmt != FMT_I4 || k % kI4Group == 0, "gemm_wsf: int4 weights need K to be a multiple of 128 (one scale per 128 k)");
+  VLO_CHECK(fmt != FMT_I4 || (reinterpret_cast<uintptr_t>(w.w) & 15) == 0, "gemm_wsf: int4 codes must be 16-byte aligned");
+  a.wt = WsWeightArgs{w.row_scale, a_scale, static_cast<const uint8_t*>(w.w), w.group_scale};
   CUtensorMap tw, tx;
-  if (get_tmap(w, rows_w, k, kGemmBM, fw, &tw) != 0) return -1;
-  if (get_tmap(x, rows_x, k, bn, a_scale ? FMT_E4M3_A8 : FMT_BF16, &tx) != 0) return -1;
-  if (bn == 16) return launch_wsf<16>(tw, tx, a, w_scale, a_scale, stream);
-  if (bn == 32) return launch_wsf<32>(tw, tx, a, w_scale, a_scale, stream);
-  if (bn == 64) return launch_wsf<64>(tw, tx, a, w_scale, a_scale, stream);
-  if (bn == 96) return launch_wsf<96>(tw, tx, a, w_scale, a_scale, stream);
-  return launch_wsf<128>(tw, tx, a, w_scale, a_scale, stream);
+  if (fmt != FMT_I4 && get_tmap(w.w, rows_w, k, kGemmBM, kWsFmtInfo[fmt].w_map, &tw) != 0) return -1;
+  if (get_tmap(x, rows_x, k, bn, kWsFmtInfo[fmt].x_map, &tx) != 0) return -1;
+  if (fmt == FMT_I4) tw = tx;   // unused: the codes stream as bulk copies
+  switch (fmt) {
+    case FMT_BF16: return launch_wsf_fmt<FMT_BF16>(bn, tw, tx, a, stream);
+    case FMT_E4M3: return launch_wsf_fmt<FMT_E4M3>(bn, tw, tx, a, stream);
+    case FMT_E4M3_A8: return launch_wsf_fmt<FMT_E4M3_A8>(bn, tw, tx, a, stream);
+    default: return launch_wsf_fmt<FMT_I4>(bn, tw, tx, a, stream);
+  }
 }
 
 }  // namespace vlo

@@ -74,52 +74,75 @@ struct GemmCfg {
 
 __device__ __forceinline__ void wg_sync() { asm volatile("bar.sync 1, 128;\n" ::: "memory"); }  // the MMA warpgroup
 
-// The warpgroup's part of the ring protocol: accumulate the nk k-blocks at ring positions i, i+1, ... into acc
-// (zeroed first; acc[h] is the 64-row half h of the 128 x BN tile).  A stage goes back to the producer (one arrival per
-// warp, empty barriers count 4) once the MMAs reading it have retired; one k-block of MMAs stays in flight.
-template <int FMT, int BN, int S>
-__device__ __forceinline__ void wg_mainloop(float (&acc)[2][BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
-                                            uint64_t* full_bar, uint64_t* empty_bar, int& i, int nk) {
-  constexpr int kBytesA = kGemmBM * kGemmBK * 2, kBytesB = BN * kGemmBK * 2;
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
-  for (int j = 0; j < nk; ++j, ++i) {
-    const int s = i % S;
-    mbar_wait(&full_bar[s], (i / S) & 1);
-    wgmma_fence();
-    const uint64_t da = wgmma_desc_sw128(smem_u32(smem_a + s * kBytesA));
-    const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + s * kBytesB));
-#pragma unroll
-    for (int kk = 0; kk < kGemmBK / 16; ++kk) {
-      // +2 per 16 elements (32 B) along K; the second 64-row half of A starts 8 KB (+512) further
-      Wgmma<FMT, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
-      Wgmma<FMT, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
-    }
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (j > 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
-    }
-  }
-  wgmma_wait<0>();
-  wgmma_fence_regs(acc[0]);
-  wgmma_fence_regs(acc[1]);
-  if (nk > 0) {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
-  }
+// ---- the weight formats of the weight-streaming kernels (gemm_ws.cuh, gemm_wsf.cuh)
+// FMT_E4M3: a weight stage is a 128 x 64-byte TMA box without swizzle.  Every finite e4m3 value is a bf16 value, so the
+// upcast is exact; the MMAs then read a bf16 tile laid out as a SWIZZLE_128B TMA box would leave it and issue the same
+// wgmma chain as FMT_BF16, so the fp32 accumulators are those of the bf16 kernel on the upcast weights.
+// FMT_E4M3_A8: a weight stage is a 128 x 64-byte TMA box and an activation stage a BN x 64-byte box, both with the 64-byte
+// swizzle the FP8 wgmma descriptor reads directly: no conversion, no generic-proxy stores, no warpgroup barrier.
+// FMT_I4: W4[n, k] = bf16_rn(q * s), q = code - 8 in [-8, 7], s = gscale[n, k / 128] (bf16).  Engine byte order of the
+// codes: one 4 KB block per (128-row tile, 64-wide k-block) unit, the units of a tile in k order and the tiles in row
+// order, so the unit range of a stream-K CTA is one contiguous byte range.  Inside a unit, thread t of the warpgroup owns
+// 16 bytes per 64-row half h at byte h * 2048 + t * 16: the four 32-bit words of its m64k16 A fragments for the k16 steps
+// kk = 0..3.  The word of step kk holds, for row r = 64h + 16(t/32) + (t%32)/4 and column c = 16kk + 2(t%4), the code of
+// element (r + 8e, c + 8f + b) in bits 4(e + 2f) + 16b .. +3, so (word >> 4p) & 0x000F000F is the pair of fragment
+// register p.
+constexpr int kF8BytesCvt = 2 * kGemmBM * kGemmBK * 2;  // two bf16 tiles: k-block j converts while the MMAs of j - 1 run
+constexpr int kI4BytesUnit = kGemmBM * kGemmBK / 2;     // 4 KB of codes per unit
+constexpr int kI4Group = 128;                           // k per scale
+// An int4 ring slot carries up to this many consecutive k-blocks of one tile (8-16 KB of codes), split at multiples of
+// it, so a slot never spans more than units / 2 scale groups.
+constexpr int i4_slot_units(int bn) { return bn <= 32 ? 4 : 2; }
+
+// k-blocks per ring slot, the weight and activation bytes of one slot, the conversion tiles and the deepest ring of a
+// format at token-tile width bn.  16-bit weights stop at 8 stages; the others have smaller stages and go up to the 16
+// full / empty barrier pairs of the barrier block.
+constexpr int ws_slot_units(int fmt, int bn) { return fmt == FMT_I4 ? i4_slot_units(bn) : 1; }
+constexpr int ws_slot_bytes_w(int fmt, int bn) {
+  return fmt == FMT_I4 ? i4_slot_units(bn) * kI4BytesUnit : kGemmBM * kGemmBK * (fmt == FMT_E4M3 || fmt == FMT_E4M3_A8 ? 1 : 2);
+}
+constexpr int ws_slot_bytes_x(int fmt, int bn) { return ws_slot_units(fmt, bn) * bn * kGemmBK * (fmt == FMT_E4M3_A8 ? 1 : 2); }
+constexpr int ws_cvt_bytes(int fmt) { return fmt == FMT_E4M3 ? kF8BytesCvt : 0; }
+constexpr int ws_max_stages(int fmt) { return fmt == FMT_F16 || fmt == FMT_BF16 ? 8 : 16; }
+// shared memory besides the ring: conversion tiles, 1024 B of alignment slack, 256 B of barriers, the staging tile and
+// `extra` bytes of the kernel's own (the fused kernel's exchange tile)
+constexpr int ws_fixed_bytes(int fmt, int extra) { return ws_cvt_bytes(fmt) + 1024 + 256 + extra + kWgStageBytes; }
+// the deepest ring that fits
+constexpr int ws_default_stages(int fmt, int bn, int extra = 0) {
+  return fit_stages(ws_slot_bytes_w(fmt, bn) + ws_slot_bytes_x(fmt, bn), ws_fixed_bytes(fmt, extra), ws_max_stages(fmt));
 }
 
-// ---- e4m3 weights (FMT_E4M3).  A weight stage is a 128 x 64-byte TMA box without swizzle.  Every finite e4m3 value is
-// a bf16 value, so the upcast is exact; the MMAs then read a bf16 tile laid out as a SWIZZLE_128B TMA box would leave it
-// and issue the same wgmma chain as wg_mainloop<FMT_BF16>, so the fp32 accumulators are those of the bf16 kernel on the
-// upcast weights.
-constexpr int kF8BytesW = kGemmBM * kGemmBK;          // one e4m3 weight stage
-constexpr int kF8BytesCvt = 2 * kGemmBM * kGemmBK * 2;  // two bf16 tiles: k-block j converts while the MMAs of j - 1 run
+template <int FMT, int BN, int STAGES, int EXTRA = 0>
+struct GemmWsCfg {
+  static constexpr int kStages = STAGES;
+  static constexpr int kBytesA = ws_slot_bytes_w(FMT, BN);
+  static constexpr int kBytesB = ws_slot_bytes_x(FMT, BN);
+  static constexpr int kBytesCvt = ws_cvt_bytes(FMT);
+  static constexpr int kSmemBytes = kStages * (kBytesA + kBytesB) + ws_fixed_bytes(FMT, EXTRA);
+  static_assert(kSmemBytes <= kSmemOptIn, "ring + staging tiles exceed the shared memory of one block");
+  static_assert(kStages <= 16, "the barrier block holds 16 full / empty pairs");
+};
+
+// What the host needs of a format: the get_tmap kind (a GemmFmt) of the weight and activation maps (-1: the int4 codes
+// stream as bulk copies) and the HBM bytes of one weight, one activation, one weight row's scale, one token's scale and
+// one 128-k group's scale.
+struct WsFmtInfo {
+  int w_map, x_map;
+  double w_elem, x_elem;
+  int row_scale, tok_scale, group_scale;
+};
+constexpr WsFmtInfo kWsFmtInfo[] = {
+    {FMT_F16, FMT_F16, 2.0, 2.0, 0, 0, 0},              // FMT_F16
+    {FMT_BF16, FMT_BF16, 2.0, 2.0, 0, 0, 0},            // FMT_BF16
+    {FMT_E4M3, FMT_BF16, 1.0, 2.0, 4, 0, 0},            // FMT_E4M3
+    {FMT_E4M3_A8, FMT_E4M3_A8, 1.0, 1.0, 4, 4, 0},      // FMT_E4M3_A8
+    {-1, FMT_BF16, 0.5, 2.0, 0, 0, 2},                  // FMT_I4
+};
+// the weight and activation bytes a weight-streaming GEMM of W [rows_w, k] by X [rows_x, k] reads (profiler, benches)
+inline double ws_in_bytes(int fmt, int rows_w, int rows_x, int k) {
+  const WsFmtInfo& f = kWsFmtInfo[fmt];
+  return (k * f.w_elem + f.row_scale + f.group_scale * (k / kI4Group)) * rows_w + (k * f.x_elem + f.tok_scale) * rows_x;
+}
 
 __device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t two) {
   const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two & 0xFFFF), __NV_E4M3);
@@ -140,35 +163,77 @@ __device__ __forceinline__ void f8_tile_to_bf16_sw128(const uint8_t* src, uint8_
   }
 }
 
-// wg_mainloop for e4m3 weight stages: k-block j is converted into cvt tile j % 2, then multiplied exactly as the bf16
-// mainloop does.  The barrier before a conversion makes every warp's MMAs of k-block j - 2 (the tile's last readers)
-// retired: each warp has passed wgmma_wait<1> of iteration j - 1 by then.  A stage goes back to the producer when the
-// MMAs of its k-block retire, as in wg_mainloop, since they read its activation tile.
-template <int BN, int S>
-__device__ __forceinline__ void wg_mainloop_f8(float (&acc)[2][BN / 2], uint8_t* smem_cvt, const uint8_t* smem_w8,
-                                               const uint8_t* smem_b, uint64_t* full_bar, uint64_t* empty_bar, int& i,
-                                               int nk) {
-  constexpr int kBytesB = BN * kGemmBK * 2;
-  const int lane = threadIdx.x & 31;
+template <int BN>
+__device__ __forceinline__ void wg_zero(float (&acc)[2][BN / 2]) {
 #pragma unroll
   for (int h = 0; h < 2; ++h)
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+}
+
+// after the last k-block: retire every MMA and give the last stage (ring position i - 1) back to the producer
+template <int BN, int S>
+__device__ __forceinline__ void wg_drain(float (&acc)[2][BN / 2], uint64_t* empty_bar, int i, int nk) {
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc[0]);
+  wgmma_fence_regs(acc[1]);
+  if (nk > 0) {
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
+  }
+}
+
+// The warpgroup's part of the ring protocol: accumulate the nk k-blocks at ring positions i, i+1, ... into acc
+// (zeroed first; acc[h] is the 64-row half h of the 128 x BN tile).  A stage goes back to the producer (one arrival per
+// warp, empty barriers count 4) once the MMAs reading it have retired; one k-block of MMAs stays in flight.
+// FMT_E4M3 converts k-block j into the bf16 tile j % 2 of smem_cvt first, then multiplies exactly as FMT_BF16 does.  The
+// barrier before a conversion makes every warp's MMAs of k-block j - 2 (the tile's last readers) retired: each warp has
+// passed wgmma_wait<1> of iteration j - 1 by then.  FMT_E4M3_A8 issues two k32 FP8 MMAs per 64-wide k-block on each
+// 64-row half, in k order.
+template <int FMT, int BN, int S>
+__device__ __forceinline__ void wg_mainloop(float (&acc)[2][BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
+                                            uint64_t* full_bar, uint64_t* empty_bar, int& i, int nk,
+                                            uint8_t* smem_cvt = nullptr) {
+  constexpr int kBytesA = ws_slot_bytes_w(FMT, BN), kBytesB = ws_slot_bytes_x(FMT, BN);
+  const int lane = threadIdx.x & 31;
+  wg_zero<BN>(acc);
   for (int j = 0; j < nk; ++j, ++i) {
     const int s = i % S;
-    uint8_t* cvt = smem_cvt + (j & 1) * (kF8BytesCvt / 2);
+    uint8_t* cvt = smem_cvt + (j & 1) * (kF8BytesCvt / 2);   // FMT_E4M3
     mbar_wait(&full_bar[s], (i / S) & 1);
-    if (j >= 2) wg_sync();
-    f8_tile_to_bf16_sw128(smem_w8 + s * kF8BytesW, cvt);
-    fence_proxy_async();   // the generic-proxy stores become visible to the wgmma operand reads
-    wg_sync();
-    wgmma_fence();
-    const uint64_t da = wgmma_desc_sw128(smem_u32(cvt));
-    const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + s * kBytesB));
+    if constexpr (FMT == FMT_E4M3) {
+      if (j >= 2) wg_sync();
+      f8_tile_to_bf16_sw128(smem_a + s * kBytesA, cvt);
+      fence_proxy_async();   // the generic-proxy stores become visible to the wgmma operand reads
+      wg_sync();
+      wgmma_fence();
+      const uint64_t da = wgmma_desc_sw128(smem_u32(cvt));
+      const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + s * kBytesB));
 #pragma unroll
-    for (int kk = 0; kk < kGemmBK / 16; ++kk) {
-      Wgmma<FMT_BF16, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
-      Wgmma<FMT_BF16, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
+      for (int kk = 0; kk < kGemmBK / 16; ++kk) {
+        Wgmma<FMT_BF16, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
+        Wgmma<FMT_BF16, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
+      }
+    } else if constexpr (FMT == FMT_E4M3_A8) {
+      wgmma_fence();
+      const uint64_t da = wgmma_desc_sw64(smem_u32(smem_a + s * kBytesA));
+      const uint64_t db = wgmma_desc_sw64(smem_u32(smem_b + s * kBytesB));
+#pragma unroll
+      for (int kk = 0; kk < kGemmBK / 32; ++kk) {
+        // +2 per 32 elements (32 B) along K; the second 64-row half of A starts 4 KB (+256) further
+        WgmmaE4M3<BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
+        WgmmaE4M3<BN>::mma(acc[1], da + 256 + 2 * kk, db + 2 * kk);
+      }
+    } else {
+      wgmma_fence();
+      const uint64_t da = wgmma_desc_sw128(smem_u32(smem_a + s * kBytesA));
+      const uint64_t db = wgmma_desc_sw128(smem_u32(smem_b + s * kBytesB));
+#pragma unroll
+      for (int kk = 0; kk < kGemmBK / 16; ++kk) {
+        // +2 per 16 elements (32 B) along K; the second 64-row half of A starts 8 KB (+512) further
+        Wgmma<FMT, BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
+        Wgmma<FMT, BN>::mma(acc[1], da + 512 + 2 * kk, db + 2 * kk);
+      }
     }
     wgmma_commit();
     wgmma_wait<1>();
@@ -177,69 +242,10 @@ __device__ __forceinline__ void wg_mainloop_f8(float (&acc)[2][BN / 2], uint8_t*
       if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
     }
   }
-  wgmma_wait<0>();
-  wgmma_fence_regs(acc[0]);
-  wgmma_fence_regs(acc[1]);
-  if (nk > 0) {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
-  }
+  wg_drain<BN, S>(acc, empty_bar, i, nk);
 }
 
-// ---- e4m3 weights x e4m3 activations (FMT_E4M3_A8).  A weight stage is a 128 x 64-byte TMA box and an activation stage
-// a BN x 64-byte box, both with the 64-byte swizzle the FP8 wgmma descriptor reads directly: no conversion, no
-// generic-proxy stores, no warpgroup barrier.  Two k32 MMAs per 64-wide k-block on each 64-row half, in k order.
-constexpr int kA8BytesW = kGemmBM * kGemmBK;   // one e4m3 weight stage (8 KB)
-
-template <int BN, int S>
-__device__ __forceinline__ void wg_mainloop_a8(float (&acc)[2][BN / 2], const uint8_t* smem_a, const uint8_t* smem_b,
-                                               uint64_t* full_bar, uint64_t* empty_bar, int& i, int nk) {
-  constexpr int kBytesB = BN * kGemmBK;
-  const int lane = threadIdx.x & 31;
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
-  for (int j = 0; j < nk; ++j, ++i) {
-    const int s = i % S;
-    mbar_wait(&full_bar[s], (i / S) & 1);
-    wgmma_fence();
-    const uint64_t da = wgmma_desc_sw64(smem_u32(smem_a + s * kA8BytesW));
-    const uint64_t db = wgmma_desc_sw64(smem_u32(smem_b + s * kBytesB));
-#pragma unroll
-    for (int kk = 0; kk < kGemmBK / 32; ++kk) {
-      // +2 per 32 elements (32 B) along K; the second 64-row half of A starts 4 KB (+256) further
-      WgmmaE4M3<BN>::mma(acc[0], da + 2 * kk, db + 2 * kk);
-      WgmmaE4M3<BN>::mma(acc[1], da + 256 + 2 * kk, db + 2 * kk);
-    }
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (j > 0) {
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
-    }
-  }
-  wgmma_wait<0>();
-  wgmma_fence_regs(acc[0]);
-  wgmma_fence_regs(acc[1]);
-  if (nk > 0) {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
-  }
-}
-
-// ---- int4 weights (FMT_I4).  W4[n, k] = bf16_rn(q * s), q = code - 8 in [-8, 7], s = gscale[n, k / 128] (bf16).
-// Engine byte order of the codes: one 4 KB block per (128-row tile, 64-wide k-block) unit, the units of a tile in k order
-// and the tiles in row order, so the unit range of a stream-K CTA is one contiguous byte range.  Inside a unit, thread t
-// of the warpgroup owns 16 bytes per 64-row half h at byte h * 2048 + t * 16: the four 32-bit words of its m64k16
-// A fragments for the k16 steps kk = 0..3.  The word of step kk holds, for row r = 64h + 16(t/32) + (t%32)/4 and
-// column c = 16kk + 2(t%4), the code of element (r + 8e, c + 8f + b) in bits 4(e + 2f) + 16b .. +3, so
-// (word >> 4p) & 0x000F000F is the pair of fragment register p.
-constexpr int kI4BytesUnit = kGemmBM * kGemmBK / 2;   // 4 KB of codes per unit
-constexpr int kI4Group = 128;                           // k per scale
-// A ring slot carries up to this many consecutive k-blocks of one tile (8-16 KB of codes), split at multiples of it, so
-// a slot never spans more than units / 2 scale groups.
-constexpr int i4_slot_units(int bn) { return bn <= 32 ? 4 : 2; }
+// ---- int4 weights (FMT_I4): the byte order of the codes is described above
 
 // the slot that starts at unit u of the range [u, u1): its tile, first k-block and unit count
 template <int KU>
@@ -330,10 +336,7 @@ __device__ __forceinline__ void wg_mainloop_i4(float (&acc)[2][BN / 2], const ui
                                                uint64_t* full_bar, uint64_t* empty_bar, int& i, int tile, int k0, int nk,
                                                const uint16_t* gs, int ng, int rows_w) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+  wg_zero<BN>(acc);
   int rows[4];   // fragment rows: half h = r >> 1, +8 for r & 1
 #pragma unroll
   for (int r = 0; r < 4; ++r) rows[r] = tile * kGemmBM + 64 * (r >> 1) + 16 * warp + (lane >> 2) + 8 * (r & 1);
@@ -394,13 +397,7 @@ __device__ __forceinline__ void wg_mainloop_i4(float (&acc)[2][BN / 2], const ui
     first = false;
     kblk += n;
   }
-  wgmma_wait<0>();
-  wgmma_fence_regs(acc[0]);
-  wgmma_fence_regs(acc[1]);
-  if (nk > 0) {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[(i - 1) % S]);
-  }
+  wg_drain<BN, S>(acc, empty_bar, i, nk);
 }
 
 // columns c0 .. c0 + 15 of the accumulators -> staging tile (row r of the tile at stage[r * kWgStageLd]); c0 must be a

@@ -12,9 +12,9 @@
 //   * TILES mode (lm_head, connector): whole tiles per CTA, direct 16-bit epilogue, no partials;
 //   * the producer warp keeps the ring full across items, so the weight stream continues while the warpgroup
 //     runs the epilogue of an item;
-//   * FMT_E4M3 (mode 0 only): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop_f8), each partial
+//   * FMT_E4M3 (mode 0 only): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop), each partial
 //     multiplied by its row's scale once before it is written;
-//   * FMT_E4M3_A8 (mode 0 only): e4m3 weight and e4m3 activation stages straight into the FP8 wgmma (wg_mainloop_a8);
+//   * FMT_E4M3_A8 (mode 0 only): e4m3 weight and e4m3 activation stages straight into the FP8 wgmma (wg_mainloop);
 //     each partial is multiplied by its row's weight scale, then by its token's activation scale, before it is written;
 //   * FMT_I4 (mode 0, one token tile only): 4-bit codes with per-group bf16 scales, dequantized into the wgmma A fragment in
 //     registers (wg_mainloop_i4); a ring slot carries up to i4_slot_units(BN) consecutive k-blocks of one tile, the codes
@@ -25,6 +25,14 @@
 #include "streamk.h"
 
 namespace vlo {
+
+// The weight side of a weight-streaming launch beyond the TMA map of 16-bit and e4m3 weights
+struct WsWeightArgs {
+  const float* w_scale;       // FMT_E4M3 / FMT_E4M3_A8: [rows_w] fp32 row scales, applied once to each partial
+  const float* a_scale;       // FMT_E4M3_A8: [rows_x] fp32 token scales, applied after the row scale
+  const uint8_t* w4;          // FMT_I4: the codes in the engine byte order (gemm.cuh)
+  const uint16_t* g_scale;    // FMT_I4: bf16 [rows_w][k / 128] group scales
+};
 
 struct GemmWsArgs {
   int rows_w, rows_x, k;   // W [rows_w, k], X [rows_x, k]
@@ -38,60 +46,136 @@ struct GemmWsArgs {
   const float* bias;
   int act;
   unsigned long long hint_w;  // L2 policy for the weight stream (evict-first when read once per launch)
-  const float* w_scale;       // FMT_E4M3 / FMT_E4M3_A8: [rows_w] fp32 row scales, applied once to each partial
-  const float* a_scale;       // FMT_E4M3_A8: [rows_x] fp32 token scales, applied after the row scale
-  const uint8_t* w4;          // FMT_I4: the codes in the engine byte order (gemm.cuh)
-  const uint16_t* g_scale;    // FMT_I4: bf16 [rows_w][k / 128] group scales
+  WsWeightArgs wt;
 };
 
-// deepest ring of at most 8 stages that fits next to the staging tile
-constexpr int ws_default_stages(int bn) { return fit_stages(kGemmBM * kGemmBK * 2 + bn * kGemmBK * 2, kWgStageBytes + 1024 + 256, 8); }
-// e4m3 weights: stages of half the weight bytes, so up to 16 of them (the barrier block holds 16 pairs), next to the
-// staging tile and the two converted bf16 tiles
-constexpr int ws_f8_default_stages(int bn) {
-  return fit_stages(kF8BytesW + bn * kGemmBK * 2, kF8BytesCvt + kWgStageBytes + 1024 + 256, 16);
-}
+// ---- the front half of the weight-streaming kernels (this file and gemm_wsf.cuh).  A CTA owns the units [u0, u1) of
+// its plan; unit u is k-block u % kb of tile u / kb, and tile t multiplies weight tile t / x_tiles by token tile
+// t % x_tiles (the fused kernel passes x_tiles = 1).  Args is GemmWsArgs or GemmWsfArgs: the helpers read the fields
+// both have (rows_w, k, hint_w, wt) where they use them, as the kernel bodies did.
 
-// e4m3 weights and activations: up to 16 stages of 8 KB + BN x 64 B next to the staging tile (no conversion tiles)
-constexpr int ws_a8_default_stages(int bn) { return fit_stages(kA8BytesW + bn * kGemmBK, kWgStageBytes + 1024 + 256, 16); }
-
-// int4 weights: up to 16 slots of i4_slot_units(BN) k-blocks (codes + activation boxes) next to the staging tile
-constexpr int ws_i4_default_stages(int bn) {
-  return fit_stages(i4_slot_units(bn) * (kI4BytesUnit + bn * kGemmBK * 2), kWgStageBytes + 1024 + 256, 16);
-}
-
-template <int BN, int STAGES = ws_default_stages(BN), int FMT = FMT_BF16>
-struct GemmWsCfg {
-  static constexpr int kStages = STAGES;
-  // FMT_I4: per ring slot
-  static constexpr int kBytesA = FMT == FMT_E4M3 ? kF8BytesW : FMT == FMT_E4M3_A8 ? kA8BytesW
-                                 : FMT == FMT_I4 ? i4_slot_units(BN) * kI4BytesUnit : kGemmBM * kGemmBK * 2;
-  static constexpr int kBytesB = BN * kGemmBK * (FMT == FMT_E4M3_A8 ? 1 : 2) * (FMT == FMT_I4 ? i4_slot_units(BN) : 1);
-  static constexpr int kBytesCvt = FMT == FMT_E4M3 ? kF8BytesCvt : 0;
-  static constexpr int kSmemBytes = kBytesCvt + kStages * (kBytesA + kBytesB) + 1024 + 256 + kWgStageBytes;
-  static_assert(kSmemBytes <= kSmemOptIn, "ring + staging tile exceed the shared memory of one block");
-  static_assert(kStages <= 16, "the barrier block holds 16 full / empty pairs");
+// Shared memory: [conversion tiles][S weight slots][S activation slots][barriers, 256 B][the kernel's own tiles at tail]
+struct WsRing {
+  uint8_t *cvt, *a, *b;
+  uint64_t *full_bar, *empty_bar;
+  float* tail;
 };
+template <class Cfg>
+__device__ __forceinline__ WsRing ws_ring() {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  constexpr int S = Cfg::kStages;
+  WsRing r;
+  r.cvt = smem;   // FMT_E4M3: the converted bf16 weight tiles
+  r.a = smem + Cfg::kBytesCvt;
+  r.b = smem + Cfg::kBytesCvt + S * Cfg::kBytesA;
+  r.full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBytesCvt + S * (Cfg::kBytesA + Cfg::kBytesB));
+  r.empty_bar = r.full_bar + S;
+  r.tail = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(r.full_bar) + 256);
+  return r;
+}
 
-template <int FMT, int BN, int STAGES = ws_default_stages(BN)>
+// Barrier init and the PDL trigger, then the weight prefetch, then pdl_wait.  The weight operand never depends on an
+// earlier kernel: the producer fills the first S slots with weights (and the consumer warps pull the int4 group scales
+// into L2) while the predecessors are still running.  Returns the number of slots the producer has filled.
+template <int FMT, int BN, int S, class Args>
+__device__ __forceinline__ int ws_prologue(const CUtensorMap& tm_w, const CUtensorMap& tm_x, const WsRing& r, const Args& p,
+                                           long long u0, long long u1, int kb, int x_tiles, int warp, bool producer) {
+  constexpr int kBytesA = ws_slot_bytes_w(FMT, BN), kBytesB = ws_slot_bytes_x(FMT, BN);
+  if (producer) {
+    if constexpr (FMT != FMT_I4) tma_prefetch_desc(&tm_w);
+    tma_prefetch_desc(&tm_x);
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&r.full_bar[s], 1);
+      mbar_init(&r.empty_bar[s], 4);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  // Early triggering lets the next kernels of the step become resident and prefetch while this one streams.
+  pdl_trigger();
+  int pre = 0;
+  if constexpr (FMT == FMT_I4) {
+    if (producer) pre = i4_prefetch_codes<BN, S, i4_slot_units(BN)>(p.wt.w4, r.a, r.full_bar, u0, u1, kb, p.hint_w);
+    else if (warp < kGemmProducerWarp) i4_prefetch_scales(p.wt.g_scale, p.k / kI4Group, p.rows_w, u0, u1, kb);
+  } else if (producer) {
+    for (long long u = u0; u < u1 && pre < S; ++u, ++pre) {
+      const int tile = static_cast<int>(u / kb);
+      const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
+      const int wt = tile / x_tiles;
+      mbar_arrive_expect_tx(&r.full_bar[pre], kBytesA + kBytesB);
+      tma_load_2d(r.a + pre * kBytesA, &tm_w, &r.full_bar[pre], kblk * kGemmBK, wt * kGemmBM, p.hint_w);
+    }
+  }
+  // everything above overlapped the predecessors; their results (the activations) are needed from here on
+  pdl_wait();
+  return pre;
+}
+
+// The producer (lane 0 of the producer warp): one continuous stream of ring slots; the first `pre` slots only still
+// need their activation boxes.
+template <int FMT, int BN, int S, class Args>
+__device__ __forceinline__ void ws_produce(const CUtensorMap& tm_w, const CUtensorMap& tm_x, const WsRing& r, const Args& p,
+                                           long long u0, long long u1, int kb, int x_tiles, int pre) {
+  constexpr int kBytesA = ws_slot_bytes_w(FMT, BN), kBytesB = ws_slot_bytes_x(FMT, BN);
+  if constexpr (FMT == FMT_I4) {
+    i4_produce<BN, S, i4_slot_units(BN)>(p.wt.w4, &tm_x, r.a, r.b, r.full_bar, r.empty_bar, u0, u1, kb, pre, p.hint_w);
+  } else {
+    int i = 0;
+    for (long long u = u0; u < u1; ++u, ++i) {
+      const int tile = static_cast<int>(u / kb);
+      const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
+      const int wt = tile / x_tiles, xt = tile - wt * x_tiles;
+      const int s = i % S;
+      if (i >= pre) {
+        const uint32_t ph = (i / S) & 1;
+        mbar_wait(&r.empty_bar[s], ph ^ 1);
+        mbar_arrive_expect_tx(&r.full_bar[s], kBytesA + kBytesB);
+        tma_load_2d(r.a + s * kBytesA, &tm_w, &r.full_bar[s], kblk * kGemmBK, wt * kGemmBM, p.hint_w);
+      }
+      tma_load_2d(r.b + s * kBytesB, &tm_x, &r.full_bar[s], kblk * kGemmBK, xt * BN, kEvictLast);
+    }
+  }
+}
+
+// The warpgroup's main loop over the nk k-blocks k0 .. of tile `tile`, in the format's ring slots
+template <int FMT, int BN, int S, class Args>
+__device__ __forceinline__ void ws_mainloop(float (&acc)[2][BN / 2], const WsRing& r, const Args& p, int& i, int tile,
+                                            int k0, int nk) {
+  if constexpr (FMT == FMT_I4)
+    wg_mainloop_i4<BN, S, i4_slot_units(BN)>(acc, r.a, r.b, r.full_bar, r.empty_bar, i, tile, k0, nk, p.wt.g_scale,
+                                             p.k / kI4Group, p.rows_w);
+  else
+    wg_mainloop<FMT, BN, S>(acc, r.a, r.b, r.full_bar, r.empty_bar, i, nk, r.cvt);
+}
+
+// The scaling of a partial of weight row n and token t before it is written or summed: once by the row scale for e4m3
+// weights, then by the token scale for e4m3 activations (a_scale is the quantizer's output: a plain load, after
+// pdl_wait); the other formats' partials are the accumulators
+template <int FMT>
+__device__ __forceinline__ float scale_partial(float v, float scale_n, const float* a_scale, int t) {
+  if constexpr (FMT == FMT_E4M3) return __fmul_rn(v, scale_n);
+  if constexpr (FMT == FMT_E4M3_A8) return __fmul_rn(__fmul_rn(v, scale_n), a_scale[t]);
+  return v;
+}
+// the row scale of feature n (e4m3 weights; 0 for the others and for rows past rows_w)
+template <int FMT>
+__device__ __forceinline__ float ws_row_scale(const float* w_scale, int n, bool n_ok) {
+  float scale_n = 0.f;
+  if constexpr (FMT == FMT_E4M3 || FMT == FMT_E4M3_A8) {
+    if (n_ok) scale_n = __ldg(w_scale + n);
+  }
+  return scale_n;
+}
+
+template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN)>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
                const GemmWsArgs p) {
-  using Cfg = GemmWsCfg<BN, STAGES, FMT>;
-  constexpr bool kF8 = FMT == FMT_E4M3;
-  constexpr bool kA8 = FMT == FMT_E4M3_A8;
-  constexpr bool kI4 = FMT == FMT_I4;
-  constexpr int KU = i4_slot_units(BN);
+  using Cfg = GemmWsCfg<FMT, BN, STAGES>;
   constexpr int S = Cfg::kStages;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
-  uint8_t* smem_cvt = smem;               // kF8: the converted bf16 weight tiles
-  uint8_t* smem_a = smem + Cfg::kBytesCvt;
-  uint8_t* smem_b = smem + Cfg::kBytesCvt + S * Cfg::kBytesA;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBytesCvt + S * (Cfg::kBytesA + Cfg::kBytesB));
-  uint64_t* empty_bar = full_bar + S;
-  float* stage = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(full_bar) + 256);
+  const WsRing r = ws_ring<Cfg>();
+  float* stage = r.tail;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = blockIdx.x;
@@ -105,57 +189,10 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
     u1 = ((static_cast<long long>(c + 1) * p.tiles) / p.sk.G) * kb;
   }
   const bool producer = warp == kGemmProducerWarp && lane == 0;
-
-  if (producer) {
-    if constexpr (!kI4) tma_prefetch_desc(&tm_w);
-    tma_prefetch_desc(&tm_x);
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 4);
-    }
-    fence_mbar_init();
-  }
-  __syncthreads();
-  // Early triggering lets the next kernels of the step become resident and prefetch while this one streams.
-  pdl_trigger();
-  // The weight operand never depends on any earlier kernel: the producer starts streaming the first S weight
-  // k-blocks right away, i.e. while the predecessors are still running.
-  int pre = 0;
-  if constexpr (kI4) {
-    if (producer) pre = i4_prefetch_codes<BN, S, KU>(p.w4, smem_a, full_bar, u0, u1, kb, p.hint_w);
-    else if (warp < kGemmProducerWarp) i4_prefetch_scales(p.g_scale, p.k / kI4Group, p.rows_w, u0, u1, kb);
-  } else if (producer) {
-    for (long long u = u0; u < u1 && pre < S; ++u, ++pre) {
-      const int tile = static_cast<int>(u / kb);
-      const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
-      const int wt = tile / p.x_tiles;
-      mbar_arrive_expect_tx(&full_bar[pre], Cfg::kBytesA + Cfg::kBytesB);
-      tma_load_2d(smem_a + pre * Cfg::kBytesA, &tm_w, &full_bar[pre], kblk * kGemmBK, wt * kGemmBM, p.hint_w);
-    }
-  }
-  // everything above overlapped the predecessors; their results (the activations) are needed from here on
-  pdl_wait();
+  const int pre = ws_prologue<FMT, BN, S>(tm_w, tm_x, r, p, u0, u1, kb, p.x_tiles, warp, producer);
 
   if (warp == kGemmProducerWarp) {
-    if constexpr (kI4) {
-      if (lane == 0) i4_produce<BN, S, KU>(p.w4, &tm_x, smem_a, smem_b, full_bar, empty_bar, u0, u1, kb, pre, p.hint_w);
-    } else if (lane == 0) {
-      // ------------------------------------------------ TMA producer: one continuous stream of k-blocks
-      int i = 0;
-      for (long long u = u0; u < u1; ++u, ++i) {
-        const int tile = static_cast<int>(u / kb);
-        const int kblk = static_cast<int>(u - static_cast<long long>(tile) * kb);
-        const int wt = tile / p.x_tiles, xt = tile - wt * p.x_tiles;
-        const int s = i % S;
-        if (i >= pre) {
-          const uint32_t ph = (i / S) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          mbar_arrive_expect_tx(&full_bar[s], Cfg::kBytesA + Cfg::kBytesB);
-          tma_load_2d(smem_a + s * Cfg::kBytesA, &tm_w, &full_bar[s], kblk * kGemmBK, wt * kGemmBM, p.hint_w);
-        }
-        tma_load_2d(smem_b + s * Cfg::kBytesB, &tm_x, &full_bar[s], kblk * kGemmBK, xt * BN, kEvictLast);
-      }
-    }
+    if (lane == 0) ws_produce<FMT, BN, S>(tm_w, tm_x, r, p, u0, u1, kb, p.x_tiles, pre);
   } else {
     // -------------------------------------------------- MMA + epilogue warpgroup (warps 0-3)
     const int row = threadIdx.x;  // tile row (output feature inside the weight tile) this thread finishes
@@ -166,25 +203,14 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       const int nk = static_cast<int>(min(static_cast<long long>(kb - k0), u1 - u));
       u += nk;
       float acc[2][BN / 2];
-      if constexpr (kF8)
-        wg_mainloop_f8<BN, S>(acc, smem_cvt, smem_a, smem_b, full_bar, empty_bar, i, nk);
-      else if constexpr (kA8)
-        wg_mainloop_a8<BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
-      else if constexpr (kI4)
-        wg_mainloop_i4<BN, S, KU>(acc, smem_a, smem_b, full_bar, empty_bar, i, tile, k0, nk, p.g_scale, p.k / kI4Group,
-                                  p.rows_w);
-      else
-        wg_mainloop<FMT, BN, S>(acc, smem_a, smem_b, full_bar, empty_bar, i, nk);
+      ws_mainloop<FMT, BN, S>(acc, r, p, i, tile, k0, nk);
       const int wt = tile / p.x_tiles, xt = tile - wt * p.x_tiles;
       const int n = wt * kGemmBM + row;  // output feature (row of W)
       const int t0 = xt * BN;            // first token row of this tile
       const bool n_ok = n < p.rows_w;
       float* plane = nullptr;
       float bias_n = 0.f;
-      float scale_n = 0.f;
-      if constexpr (kF8 || kA8) {
-        if (n_ok) scale_n = __ldg(p.w_scale + n);
-      }
+      const float scale_n = ws_row_scale<FMT>(p.wt.w_scale, n, n_ok);
       if (p.mode == 0) {
         const int pl = c - sk_first_cta(tile, p.sk);
         plane = reinterpret_cast<float*>(p.out) + static_cast<size_t>(pl) * p.plane_stride;
@@ -203,16 +229,11 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         for (int j = 0; j < 16; ++j) {
           const int t = t0 + c0 + j;
           if (t >= p.rows_x) break;
-          const float acc = v[j];
-          if constexpr (kF8) {
-            plane[static_cast<size_t>(t) * p.rows_w + n] = __fmul_rn(acc, scale_n);   // the one rounding of the scale
-          } else if constexpr (kA8) {
-            // a_scale is the quantizer's output: a plain load, after pdl_wait
-            plane[static_cast<size_t>(t) * p.rows_w + n] = __fmul_rn(__fmul_rn(acc, scale_n), p.a_scale[t]);
-          } else if (p.mode == 0) {
-            plane[static_cast<size_t>(t) * p.rows_w + n] = acc;
+          // e4m3 formats run mode 0 only
+          if (FMT == FMT_E4M3 || FMT == FMT_E4M3_A8 || p.mode == 0) {
+            plane[static_cast<size_t>(t) * p.rows_w + n] = scale_partial<FMT>(v[j], scale_n, p.wt.a_scale, t);
           } else {
-            float x = r16<FMT>(acc + bias_n);
+            float x = r16<FMT>(v[j] + bias_n);
             x = apply_act<FMT>(x, p.act);
             reinterpret_cast<uint16_t*>(p.out)[static_cast<size_t>(t) * p.ld_out + n] = to16<FMT>(x);
           }
