@@ -103,8 +103,22 @@ int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t 
  * the engine byte order: one 4 KB block per (128-row tile, 64-wide k-block), blocks in (tile, k-block) order, and inside a
  * block thread t of the consumer warpgroup's 16 bytes per 64-row half h at h * 2048 + 16 t (DESIGN.md section 2,
  * weights.pack_int4_codes).  Every result is bit for bit the bf16 engine's on W4.  An int4 engine does not prefill
- * (vlo_max_prefill_tokens is 0) and takes no FP8 activations (finalize fails with a message). */
+ * (vlo_max_prefill_tokens is 0) and takes no FP8 activations (finalize fails with a message).
+ * The vocabulary matrices `embed` and `lm_head` ([vocab, hidden] each) come either in bf16 (`embed`, `lm_head`) or, on
+ * an engine with quantized layer matrices, both in the layers' quantized form, quantized by the same rules:
+ *   int4 layers: `embed.i4` + `embed.gscale`, `lm_head.i4` + `lm_head.gscale` (engine byte order, as above).  lm_head
+ *     writes bf16(acc), acc the bf16 lm_head's fp32 chain over W4; the embedding of id i is row i of W4.  Every result is
+ *     bit for bit that of the same int4 engine loaded with the dequantized vocabulary matrices in bf16.
+ *   e4m3 layers (also with FP8 activations): `embed.f8` + `embed.scale`, `lm_head.f8` + `lm_head.scale`.  lm_head
+ *     multiplies the bf16 final-norm rows by the exactly upcast codes (bf16 MMAs) and writes bf16(fl(acc * s[n])); the
+ *     embedding of id i is bf16_rn(fp32(q[i, k]) * s[i]).
+ * Finalize fails with a message on a vocabulary matrix in the other quantized form, on embed and lm_head in different
+ * forms, on quantized vocabulary matrices next to bf16 layers, and on missing or wrongly sized tensors.  A failed
+ * finalize leaves the previous tables untouched.  vlo_vocab_format tells the form the engine loaded. */
 int vlo_finalize_weights(vlo_engine* e);
+/* GemmFmt of the vocabulary matrices the last successful vlo_finalize_weights installed: 1 bf16, 2 e4m3, 4 int4; -1
+ * before one with a decoder.  A failed finalize does not change it. */
+int vlo_vocab_format(vlo_engine* e);
 /* bytes of device memory the engine allocated itself (KV + workspaces) */
 int64_t vlo_engine_device_bytes(vlo_engine* e);
 /* FP8 activations (W8A8), on top of FP8 layer weights.  Valid before vlo_finalize_weights (fails after it); finalize then
@@ -259,7 +273,8 @@ int vlo_letterbox_planes(vlo_engine* e, const vlo_frame_planes* h_frames, int n_
  * pre-extracted features). d_tokens: bf16 [n_rows, vit_hidden] */
 int vlo_connector(vlo_engine* e, const void* d_tokens, int n_rows, void* d_out, void* cuda_stream);
 /* replaces model.get_input_embeddings()(ids) (demo/inference.py:46,66; models/modeling_live.py:181).
- * ids are clamped to vocab-1 like joint_embed does (models/modeling_live.py:38). */
+ * ids are clamped to vocab-1 like joint_embed does (models/modeling_live.py:38).  With quantized vocabulary matrices the
+ * rows are dequantized by the rules of vlo_finalize_weights. */
 int vlo_embed_tokens(vlo_engine* e, const int64_t* d_ids, int n, void* d_out, void* cuda_stream);
 /* KV-append forward for a ragged batch — replaces LiveLlamaForCausalLM.forward(inputs_embeds=...,
  * past_key_values=..., use_cache=True) (models/live_llama/modeling_live_llama.py:24-67 ->
@@ -344,7 +359,8 @@ int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row
 int vlo_max_prefill_tokens(vlo_engine* e);
 
 /* all-position logits for the last vlo_step's tokens (the reference's logits_to_keep=0 behaviour,
- * HF:models/llama/modeling_llama.py:485-487); d_logits bf16 [sum(q_lens), vocab]. Test/compat path. */
+ * HF:models/llama/modeling_llama.py:485-487); d_logits bf16 [sum(q_lens), vocab]. Test/compat path.  A quantized lm_head
+ * runs in pieces of at most 128 rows; every row's logits are those a step of its own would give. */
 int vlo_last_step_logits(vlo_engine* e, void* d_logits, void* cuda_stream);
 /* final hidden states (post model.norm) of the last step, bf16 [sum(q_lens), hidden] (tests) */
 int vlo_last_step_hidden(vlo_engine* e, void* d_hidden, void* cuda_stream);
@@ -405,6 +421,21 @@ int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const 
  * plans (*h_max_planes).  Asynchronous. */
 int vlo_op_gemm_ws_i4(const void* d_w4, const void* d_gscale, int rows_w, const void* d_x, int rows_x, int k, float* d_out,
                       long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream);
+/* Whole tiles (mode 1) of e4m3 or int4 weights with the bf16 store: the lm_head of engines with quantized vocabulary
+ * matrices.  fmt 2: d_w e4m3 bytes [rows_w, k], d_scale fp32 [rows_w], out = bf16(fl(acc * s[n])), acc the fp32 chain of
+ * the bf16 kernel on the upcast codes.  fmt 4: d_w int4 codes in the engine byte order, d_scale bf16 [rows_w, k / 128],
+ * k % 128 == 0, rows_x <= 128, out = bf16(acc) = the bf16 whole-tile call on W4.  X bf16 [rows_x, k]; out bf16
+ * [rows_x][ld_out].  One CTA covers all of k for each of its tiles, so a row's logits depend on no other row and on no
+ * token tile.  n_ctas <= 0: one CTA per SM.  h_plan (optional): {token tile, token tiles, CTAs}.  d_out == NULL only
+ * plans.  Asynchronous. */
+int vlo_op_gemm_ws_tiles_q(int fmt, const void* d_w, const void* d_scale, int rows_w, const void* d_x, int rows_x, int k,
+                           void* d_out, int ld_out, int n_ctas, int32_t* h_plan, void* cuda_stream);
+/* The token-embedding gather of vlo_embed_tokens on a bare table: fmt 1 bf16 [vocab, hidden] (d_scale unused), 2 e4m3
+ * bytes + fp32 row scales, 4 int4 codes in the engine byte order + bf16 group scales; hidden % 128 == 0.  Row i of
+ * d_out (bf16 [n, hidden]) = row min(ids[i], vocab - 1), dequantized; a row with ids[i] < 0 is left alone.
+ * Asynchronous. */
+int vlo_op_embed_rows_q(int fmt, const void* d_table, const void* d_scale, int vocab, int hidden, const int64_t* d_ids, int n,
+                        void* d_out, void* cuda_stream);
 /* ViT trunk GEMM (csrc/gemm_vit.cuh), fp16, 128-token x 128-feature tiles:
  * out[t][n] = act(fp16(sum_k X[t,k] W[n,k] + bias[n])), fp16 out[rows_x][ld_out], ld_out even and >= rows_w;
  * n_ctas <= 0: one CTA per SM. */

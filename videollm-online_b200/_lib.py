@@ -111,6 +111,7 @@ SIGNATURES = {
     "vlo_sample": (_I, [_P, _P, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P]),
     "vlo_prefill": (_I, [_P, _I, _I, _P, _P, _P, _P, _I, _P]),
     "vlo_max_prefill_tokens": (_I, [_P]),
+    "vlo_vocab_format": (_I, [_P]),
     "vlo_last_step_logits": (_I, [_P, _P, _P]),
     "vlo_last_step_hidden": (_I, [_P, _P, _P]),
     "vlo_bench_attn": (_I, [_P, _I, C.POINTER(C.c_int32), _I, _I, _I, C.POINTER(C.c_double), _P]),
@@ -120,6 +121,8 @@ SIGNATURES = {
     "vlo_op_gemm_ws_tiled": (_I, [_I, _I, _P, _I, _P, _I, _I, _P, _I, _LL, _P, _I, _I, _I, _I, C.POINTER(C.c_int32), _P]),
     "vlo_op_gemm_ws_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_ws_i4": (_I, [_P, _P, _I, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
+    "vlo_op_gemm_ws_tiles_q": (_I, [_I, _P, _P, _I, _P, _I, _I, _P, _I, _I, C.POINTER(C.c_int32), _P]),
+    "vlo_op_embed_rows_q": (_I, [_I, _P, _P, _I, _I, _P, _I, _P, _P]),
     "vlo_op_gemm_ws_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _LL, _I, C.POINTER(_I), _P]),
     "vlo_op_gemm_vit": (_I, [_P, _I, _P, _I, _I, _P, _I, _P, _I, _I, _P]),
     "vlo_op_attn_ws_bytes": (C.c_int64, [_I, _I, _I, _I]),

@@ -21,6 +21,8 @@ numbers change, so it is off by default).
 the FP8 tensor cores (W8A8); off by default for the same reason.
 --int4_weights serves the decoder layers from 4-bit weights with one bf16 scale per 128 weights of a row (W4A16: a
 quarter of their bf16 bytes per step); the numbers change, so it is off by default, and it excludes the FP8 flags.
+--quantize_vocab (with --fp8_weights or --int4_weights) also serves the token embeddings and lm_head in that quantized
+form, which frees their memory for the KV cache; the numbers change, so it is off by default.
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

@@ -195,6 +195,45 @@ int vlo_op_gemm_ws_i4(const void* d_w4, const void* d_gscale, int rows_w, const 
                              nullptr, rows_x, k, d_out, plane_stride, n_ctas, h_max_planes, cuda_stream);
 }
 
+int vlo_op_gemm_ws_tiles_q(int fmt, const void* d_w, const void* d_scale, int rows_w, const void* d_x, int rows_x, int k,
+                           void* d_out, int ld_out, int n_ctas, int32_t* h_plan, void* cuda_stream) {
+  VLO_CHECK(fmt == FMT_E4M3 || fmt == FMT_I4, "gemm_ws_tiles_q: fmt 2 (e4m3 weights, fp32 row scales) or 4 (int4 weights, "
+                                              "bf16 group scales)");
+  VLO_CHECK(d_out == nullptr || d_scale != nullptr, "gemm_ws_tiles_q: null scales");
+  GemmWsCall c{};
+  c.w = fmt == FMT_E4M3 ? WeightOperand{fmt, d_w, static_cast<const float*>(d_scale), nullptr}
+                        : WeightOperand{fmt, d_w, nullptr, static_cast<const uint16_t*>(d_scale)};
+  c.mode = 1;
+  c.rows_w = rows_w;
+  c.x = d_x;
+  c.rows_x = rows_x;
+  c.k = k;
+  c.out = d_out;
+  c.ld_out = ld_out;
+  c.n_ctas = n_ctas;
+  GemmWsPlan plan{};
+  const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
+  if (rc == 0 && h_plan) {
+    h_plan[0] = plan.bn;
+    h_plan[1] = plan.x_tiles;
+    h_plan[2] = plan.sk.G;
+  }
+  return rc;
+}
+
+int vlo_op_embed_rows_q(int fmt, const void* d_table, const void* d_scale, int vocab, int hidden, const int64_t* d_ids, int n,
+                        void* d_out, void* cuda_stream) {
+  VLO_CHECK(fmt == FMT_BF16 || fmt == FMT_E4M3 || fmt == FMT_I4, "embed_rows_q: fmt 1 (bf16), 2 (e4m3) or 4 (int4)");
+  VLO_CHECK(d_table != nullptr && d_ids != nullptr && d_out != nullptr && (fmt == FMT_BF16 || d_scale != nullptr),
+            "embed_rows_q: null argument");
+  VLO_CHECK(n > 0 && vocab > 0 && hidden > 0 && hidden % 128 == 0, "embed_rows_q: n, vocab > 0, hidden a multiple of 128");
+  const WeightOperand t = fmt == FMT_E4M3 ? WeightOperand{fmt, d_table, static_cast<const float*>(d_scale), nullptr}
+                          : fmt == FMT_I4 ? WeightOperand{fmt, d_table, nullptr, static_cast<const uint16_t*>(d_scale)}
+                                          : WeightOperand{fmt, d_table, nullptr, nullptr};
+  return embed_rows_launch(t, reinterpret_cast<const long long*>(d_ids), n, vocab, hidden, d_out,
+                           static_cast<cudaStream_t>(cuda_stream));
+}
+
 int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const void* d_x8, const float* d_xscale, int rows_x,
                       int k, float* d_out, long long plane_stride, int n_ctas, int* h_max_planes, void* cuda_stream) {
   VLO_CHECK(d_out == nullptr || (d_scale != nullptr && d_xscale != nullptr), "gemm_ws_a8: null row or token scales");

@@ -115,7 +115,7 @@ enum WsTiling : int {
 // The weight operand of the weight-streaming GEMMs: its format (GemmFmt, gemm.cuh) and what that format stores.
 struct WeightOperand {
   int fmt;            // 0 fp16, 1 bf16, 2 e4m3 weights x bf16 activations, 3 e4m3 weights x e4m3 activations,
-                      // 4 int4 weights x bf16 activations (2, 3, 4: stream-K partials only)
+                      // 4 int4 weights x bf16 activations (3: stream-K partials only; 2, 4: also whole tiles)
   const void* w;      // [rows_w, k]: 16-bit or e4m3 elements, or fmt 4: int4 codes in the engine byte order
   const float* row_scale;       // fmt 2, 3: [rows_w] fp32 row scales, each partial is multiplied by its row's scale once
   const uint16_t* group_scale;  // fmt 4: bf16 [rows_w][k / 128] group scales
@@ -148,6 +148,11 @@ struct GemmWsPlan {
 };
 // Picks the token tile, plans the stream-K split and launches; out == null only fills *plan.
 int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan = nullptr);
+
+// ---- token-embedding gather (decoder_kernels.cuh / engine.cu): dst row i = row min(ids[i], vocab - 1) of the table
+// [vocab, H] (rows with ids[i] < 0 are left alone), from a bf16 table, or dequantized from an e4m3 table (row scales:
+// bf16_rn(fp32(q) * s)) or an int4 table (codes in the engine byte order, group scales: bf16_rn(q * s)).  H % 128 == 0.
+int embed_rows_launch(const WeightOperand& table, const long long* ids, int n, int vocab, int H, void* dst, cudaStream_t st);
 
 // ---- ViT trunk GEMM, 128-token x 128-feature tiles (gemm_vit.cuh / gemm.cu): fp16 x [rows_x, k], w [rows_w, k] ->
 // fp16 out[rows_x][ld_out] = act(fp16(x w^T + bias)); n_ctas <= 0 -> one CTA per SM

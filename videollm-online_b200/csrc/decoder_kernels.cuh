@@ -281,6 +281,66 @@ __global__ void __launch_bounds__(256) embed_rows_kernel(const long long* ids, c
   for (int j = threadIdx.x; j < H / 8; j += blockDim.x) out[j] = src[j];
 }
 
+// The same gather from a quantized table [vocab, H]: the ids are taken as embed_rows_kernel takes them, and the row is
+// dequantized on the way.
+//   I4 = false (e4m3): codes [vocab][H] bytes, fp32 row scales; element k of row n = bf16_rn(fp32(q[n, k]) * s[n])
+//   I4 = true:  codes in the engine byte order (gemm.cuh), bf16 group scales [vocab][H / 128]; element k of row n =
+//               bf16_rn(q * s[n, k / 128]), q = code - 8 (the W4 of the int4 GEMMs).  In each (tile, k-block) unit the
+//               row's 64 codes lie in the 16 bytes of four consumer threads (lane % 4 = 0..3) at h * 2048 + 16 t, t = 32
+//               warp + lane; one thread here decodes one of those 16-byte pieces: 16 codes, columns 16 kk + 8 f + 2 (lane
+//               % 4) + b.
+template <bool I4>
+__global__ void __launch_bounds__(256) embed_rows_q_kernel(const long long* ids, const int* dst_rows, int n,
+                                                           const uint8_t* codes, const void* scale, int vocab, int H,
+                                                           __nv_bfloat16* dst) {
+  const int i = blockIdx.x;
+  if (i >= n) return;
+  long long id = ids[i];
+  if (id < 0) return;
+  if (id > vocab - 1) id = vocab - 1;
+  const int r = dst_rows ? dst_rows[i] : i;
+  __nv_bfloat16* out = dst + static_cast<size_t>(r) * H;
+  if constexpr (!I4) {
+    const float s = __ldg(static_cast<const float*>(scale) + id);
+    const uint2* src = reinterpret_cast<const uint2*>(codes + static_cast<size_t>(id) * H);
+    for (int j = threadIdx.x; j < H / 8; j += blockDim.x) {
+      const uint2 v = src[j];
+      uint32_t w[4];
+#pragma unroll
+      for (int p = 0; p < 4; ++p) {
+        const uint32_t two = (p < 2 ? v.x : v.y) >> (16 * (p & 1));
+        const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(two & 0xFFFF), __NV_E4M3);
+        const float2 q = __half22float2(__half2(h));   // exact
+        const __nv_bfloat162 b = __floats2bfloat162_rn(__fmul_rn(q.x, s), __fmul_rn(q.y, s));
+        w[p] = *reinterpret_cast<const uint32_t*>(&b);
+      }
+      reinterpret_cast<uint4*>(out)[j] = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+  } else {
+    const int kb = H / 64, ng = H / 128;
+    const int tile = static_cast<int>(id / 128), rr = static_cast<int>(id % 128);
+    const int h = rr / 64, warp = (rr % 64) / 16, e = (rr % 16) / 8, lane_hi = rr % 8;
+    const uint16_t* gs = static_cast<const uint16_t*>(scale) + static_cast<size_t>(id) * ng;
+    for (int j = threadIdx.x; j < kb * 4; j += blockDim.x) {
+      const int kblk = j / 4, l4 = j % 4;
+      const uint8_t* unit = codes + (static_cast<size_t>(tile) * kb + kblk) * 4096;
+      const uint4 c = *reinterpret_cast<const uint4*>(unit + h * 2048 + (32 * warp + 4 * lane_hi + l4) * 16);
+      const float s = __bfloat162float(__ushort_as_bfloat16(__ldg(gs + kblk / 2)));
+      const uint32_t words[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int f = 0; f < 2; ++f) {
+          const int sh = 4 * (e + 2 * f);
+          const float q0 = static_cast<float>(static_cast<int>((words[kk] >> sh) & 0xF) - 8);
+          const float q1 = static_cast<float>(static_cast<int>((words[kk] >> (sh + 16)) & 0xF) - 8);
+          const __nv_bfloat162 b = __floats2bfloat162_rn(q0 * s, q1 * s);   // q * s is exact in fp32: one rounding
+          *reinterpret_cast<__nv_bfloat162*>(out + kblk * 64 + 16 * kk + 8 * f + 2 * l4) = b;
+        }
+    }
+  }
+}
+
 // copy packed rows (bf16) src[i] -> dst[rows[i]]
 __global__ void __launch_bounds__(256) scatter_rows_kernel(const __nv_bfloat16* src, const int* rows, int n, int H,
                                                            __nv_bfloat16* dst) {

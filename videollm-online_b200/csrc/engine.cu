@@ -47,7 +47,9 @@ struct vlo_engine {
 
   // resolved weights
   std::vector<DecLayer> dec;
-  const bf16 *embed = nullptr, *final_norm = nullptr, *lm_head = nullptr, *rope_cos = nullptr, *rope_sin = nullptr;
+  // the vocabulary matrices [vocab, hidden]: bf16, or both in the layer matrices' quantized form (vocab_fmt)
+  WeightOperand embed{}, lm_head{};
+  const bf16 *final_norm = nullptr, *rope_cos = nullptr, *rope_sin = nullptr;
   int64_t rope_positions = 0;
   std::vector<VitLayer> vit;
   const __half *patch_w = nullptr, *head_kv_w = nullptr, *head_out_w = nullptr, *head_fc1_w = nullptr,
@@ -58,6 +60,7 @@ struct vlo_engine {
   const bf16 *conn0_w = nullptr, *conn2_w = nullptr;
   bool has_vit = false, has_connector = false, has_decoder = false;
   int layer_fmt = FMT_BF16;  // GemmFmt of the layer matrices (vlo_finalize_weights; FMT_E4M3_A8 with fp8_act)
+  int vocab_fmt = FMT_BF16;  // GemmFmt of embed and lm_head (vlo_finalize_weights): FMT_BF16, FMT_E4M3 or FMT_I4
   bool fp8_act = false;      // vlo_set_fp8_activations: the layer GEMMs take e4m3 activations with token scales
 
   // derived
@@ -113,6 +116,25 @@ struct vlo_engine {
   size_t v_part_elems = 0;
   bf16 *tokens16 = nullptr, *conn_mid = nullptr;
 };
+
+namespace vlo {
+int embed_rows_launch(const WeightOperand& table, const long long* ids, int n, int vocab, int H, void* dst, cudaStream_t st) {
+  bf16* out = static_cast<bf16*>(dst);
+  if (table.fmt == FMT_BF16)
+    embed_rows_kernel<<<n, 256, 0, st>>>(ids, nullptr, n, static_cast<const bf16*>(table.w), vocab, H, out);
+  else if (table.fmt == FMT_E4M3)
+    embed_rows_q_kernel<false><<<n, 256, 0, st>>>(ids, nullptr, n, static_cast<const uint8_t*>(table.w), table.row_scale,
+                                                  vocab, H, out);
+  else if (table.fmt == FMT_I4)
+    embed_rows_q_kernel<true><<<n, 256, 0, st>>>(ids, nullptr, n, static_cast<const uint8_t*>(table.w), table.group_scale,
+                                                 vocab, H, out);
+  else
+    return fail("embed_rows: no gather for weight format " + std::to_string(table.fmt));
+  VLO_LAUNCH_CHECK();
+  count_launch();
+  return 0;
+}
+}  // namespace vlo
 
 namespace {
 
@@ -249,6 +271,28 @@ int gemm_ws_store16(int fmt, const void* w, int n_out, const void* x, int T, int
   c.act = act;
   c.tiling = tiling;
   return gemm_ws_launch(c, st);
+}
+
+// logits [rows, vocab] bf16 = x [rows, hidden] lm_head^T, whole tiles (each row independent of the others).  bf16:
+// one launch.  e4m3 / int4: the format's whole-tile instances, in pieces of at most 128 rows (one token tile of int4).
+int lm_head_launch(vlo_engine* e, const void* x, int rows, void* out, cudaStream_t st) {
+  const vlo_config& c = e->cfg;
+  if (e->lm_head.fmt == FMT_BF16)
+    return gemm_ws_store16(FMT_BF16, e->lm_head.w, c.vocab_size, x, rows, c.hidden_size, out, c.vocab_size, nullptr,
+                           ACT_NONE, st);
+  for (int r0 = 0; r0 < rows; r0 += kGemmBM) {
+    GemmWsCall g{};
+    g.w = e->lm_head;
+    g.mode = 1;
+    g.rows_w = c.vocab_size;
+    g.x = static_cast<const bf16*>(x) + static_cast<size_t>(r0) * c.hidden_size;
+    g.rows_x = std::min(kGemmBM, rows - r0);
+    g.k = c.hidden_size;
+    g.out = static_cast<bf16*>(out) + static_cast<size_t>(r0) * c.vocab_size;
+    g.ld_out = c.vocab_size;
+    if (gemm_ws_launch(g, st)) return -1;
+  }
+  return 0;
 }
 
 // one-tile fp16 GEMM with the 16-bit epilogue: out[rows_a, rows_b] = act(a b^T + bias)
@@ -724,7 +768,8 @@ namespace {
 // Layer matrix `name` [n, k] in exactly one form: bf16 `name` (FMT_BF16), e4m3 bytes `name.f8` with fp32 row scales
 // `name.scale` (FMT_E4M3, or FMT_E4M3_A8 with fp8_act), or int4 codes `name.i4` with bf16 group scales `name.gscale`
 // (FMT_I4).  *fmt < 0: the first matrix, which sets the format every later one must share.
-int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* fmt, WeightOperand* out) {
+int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64_t k, int* fmt, WeightOperand* out,
+                        const char* one = "layer matrix", const char* group = "layer matrices") {
   const bool has16 = e->tensors.count(name) > 0, has8 = e->tensors.count(name + ".f8") > 0,
              has_s = e->tensors.count(name + ".scale") > 0, has4 = e->tensors.count(name + ".i4") > 0,
              has_g = e->tensors.count(name + ".gscale") > 0;
@@ -738,7 +783,7 @@ int lookup_layer_matrix(vlo_engine* e, const std::string& name, int64_t n, int64
   out->fmt = has8 ? (e->fp8_act ? FMT_E4M3_A8 : FMT_E4M3) : has4 ? FMT_I4 : FMT_BF16;
   if (*fmt >= 0 && out->fmt != *fmt)
     return fail("weight tensor '" + name + (has8 ? ".f8' is e4m3" : has4 ? ".i4' is int4" : "' is bf16") +
-                " but an earlier layer matrix is not: all layer matrices must share one form");
+                " but an earlier " + one + " is not: all " + group + " must share one form");
   *fmt = out->fmt;
   out->row_scale = nullptr;
   out->group_scale = nullptr;
@@ -771,11 +816,10 @@ int vlo_finalize_weights(vlo_engine* e) {
   VLO_CHECK(e != nullptr, "null engine");
   const vlo_config& c = e->cfg;
   const int64_t H = c.hidden_size, I = c.intermediate_size, V = c.vocab_size;
-  e->has_decoder = e->tensors.count("embed") > 0;
+  e->has_decoder = false;   // any tensor of the embedding table, in any form (a partial form then fails with a message)
+  for (const char* n : {"embed", "embed.f8", "embed.scale", "embed.i4", "embed.gscale"}) e->has_decoder |= e->tensors.count(n) > 0;
   if (e->has_decoder) {
-    if (lookup(e, "embed", V * H, &e->embed)) return -1;
     if (lookup(e, "final_norm", H, &e->final_norm)) return -1;
-    if (lookup(e, "lm_head", V * H, &e->lm_head)) return -1;
     auto it = e->tensors.find("rope.cos");
     if (it == e->tensors.end()) return fail("missing weight tensor 'rope.cos'");
     e->rope_positions = it->second.second / (64 * 2);
@@ -800,8 +844,27 @@ int vlo_finalize_weights(vlo_engine* e) {
     VLO_CHECK(!e->fp8_act || fmt == FMT_E4M3_A8,
               "fp8_activations needs FP8 (e4m3) layer weights, but the layer matrices are bf16: the FP8 tensor cores "
               "take both operands in e4m3");
+    // the vocabulary matrices: both bf16, or both in the layer matrices' quantized form (e4m3 on bf16 activations also
+    // under fp8_act: the lm_head multiplies the bf16 final-norm rows)
+    WeightOperand embed{}, lm_head{};
+    int vfmt = -1;
+    if (lookup_layer_matrix(e, "embed", V, H, &vfmt, &embed, "vocabulary matrix", "vocabulary matrices") ||
+        lookup_layer_matrix(e, "lm_head", V, H, &vfmt, &lm_head, "vocabulary matrix", "vocabulary matrices"))
+      return -1;
+    if (vfmt == FMT_E4M3_A8) vfmt = embed.fmt = lm_head.fmt = FMT_E4M3;
+    const int lfmt = fmt == FMT_E4M3_A8 ? FMT_E4M3 : fmt;
+    const char* form_name[] = {"fp16", "bf16", "e4m3", "e4m3", "int4"};
+    VLO_CHECK(vfmt == FMT_BF16 || lfmt != FMT_BF16,
+              std::string("the vocabulary matrices (embed, lm_head) are ") + form_name[vfmt] +
+                  " but the layer matrices are bf16: quantized vocabulary matrices take the layer matrices' form");
+    VLO_CHECK(vfmt == FMT_BF16 || vfmt == lfmt,
+              std::string("the vocabulary matrices (embed, lm_head) are ") + form_name[vfmt] + " but the layer matrices are " +
+                  form_name[lfmt] + ": quantized vocabulary matrices take the layer matrices' form");
     e->dec.swap(dec);
     e->layer_fmt = fmt;
+    e->embed = embed;
+    e->lm_head = lm_head;
+    e->vocab_fmt = vfmt;
   }
   e->has_connector = e->tensors.count("conn.0.w") > 0;
   if (e->has_connector) {
@@ -1280,12 +1343,8 @@ int vlo_embed_tokens(vlo_engine* e, const int64_t* d_ids, int n, void* d_out, vo
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
   VLO_CHECK(n > 0, "embed_tokens: n must be positive");
-  embed_rows_kernel<<<n, 256, 0, static_cast<cudaStream_t>(cuda_stream)>>>(
-      reinterpret_cast<const long long*>(d_ids), nullptr, n, e->embed, e->cfg.vocab_size, e->cfg.hidden_size,
-      static_cast<bf16*>(d_out));
-  VLO_LAUNCH_CHECK();
-  count_launch();
-  return 0;
+  return embed_rows_launch(e->embed, reinterpret_cast<const long long*>(d_ids), n, e->cfg.vocab_size, e->cfg.hidden_size,
+                           d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
 namespace {
@@ -1375,12 +1434,9 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
 
   // ---- residual stream <- packed input embeddings (+ prefix-token rows gathered by id)
   VLO_CUDA(cudaMemcpyAsync(e->h, d_embeds, static_cast<size_t>(T) * H * sizeof(bf16), cudaMemcpyDeviceToDevice, st));
-  if (d_row_ids != nullptr) {
-    embed_rows_kernel<<<T, 256, 0, st>>>(reinterpret_cast<const long long*>(d_row_ids), nullptr, T, e->embed, c.vocab_size,
-                                         H, e->h);
-    VLO_LAUNCH_CHECK();
-    count_launch();
-  }
+  if (d_row_ids != nullptr &&
+      embed_rows_launch(e->embed, reinterpret_cast<const long long*>(d_row_ids), T, c.vocab_size, H, e->h, st))
+    return -1;
 
   // sk == null: no partials (the first layer's input norm).  With fp8_act every norm but the final one also writes the
   // e4m3 copy of xn that the next GEMM reads.
@@ -1431,8 +1487,7 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   }
   // ---- last-position lm_head + on-device decision (one row per segment)
   bf16* logits = d_last_logits ? static_cast<bf16*>(d_last_logits) : e->logits;
-  if (gemm_ws_store16(FMT_BF16, e->lm_head, c.vocab_size, e->xn_last, n_rows, H, logits, c.vocab_size, nullptr, ACT_NONE, st))
-    return -1;
+  if (lm_head_launch(e, e->xn_last, n_rows, logits, st)) return -1;
   if (decision_launch(logits, n_rows, c.vocab_size, interval_id, d_decisions ? static_cast<void*>(d_decisions) : e->decisions,
                       st))
     return -1;
@@ -1586,9 +1641,9 @@ int vlo_last_step_hidden(vlo_engine* e, void* d_hidden, void* cuda_stream) {
 int vlo_last_step_logits(vlo_engine* e, void* d_logits, void* cuda_stream) {
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr && e->last_step_tokens > 0, "no decoder step has run");
-  const vlo_config& c = e->cfg;
-  return gemm_ws_store16(FMT_BF16, e->lm_head, c.vocab_size, e->xn, e->last_step_tokens, c.hidden_size, d_logits,
-                         c.vocab_size, nullptr, ACT_NONE, static_cast<cudaStream_t>(cuda_stream));
+  return lm_head_launch(e, e->xn, e->last_step_tokens, d_logits, static_cast<cudaStream_t>(cuda_stream));
 }
+
+int vlo_vocab_format(vlo_engine* e) { return e != nullptr && e->embed.w != nullptr ? e->vocab_fmt : -1; }
 
 }  // extern "C"

@@ -194,10 +194,21 @@ static_assert(GemmWsCfg<FMT_BF16, 16, ws_default_stages(FMT_BF16, 16, kWsfXchByt
                       GemmVitCfg::kSmemBytes + 2 * kSmemReservedPerBlock > kSmemPerSm,
               "the 8-stage fused decoder GEMM now shares its SM with a ViT trunk GEMM CTA: update the comment above");
 
+// The whole-tile e4m3 and int4 instances (the vocabulary matrices) take the decoder instances' ring depths, so the
+// 16-token one still shares its SM with a ViT trunk GEMM CTA next to the frame step.
+template <int FMT>
+constexpr bool tiles_share_sm() {
+  constexpr int dec = GemmWsCfg<FMT, 16, decoder_stages(FMT)>::kSmemBytes + 2 * kSmemReservedPerBlock;
+  return ws_tiles_own_instances(FMT) && dec + GemmVitCfg::kSmemBytes <= kSmemPerSm && dec + kVitBesideBytes <= kSmemPerSm;
+}
+static_assert(tiles_share_sm<FMT_E4M3>(), "16-token whole-tile e4m3 GEMM CTA and a ViT GEMM CTA no longer share an SM");
+static_assert(tiles_share_sm<FMT_I4>(), "16-token whole-tile int4 GEMM CTA and a ViT GEMM CTA no longer share an SM");
+
 namespace {
-template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN)>
+template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN), bool TILES = false>
 int launch_ws(const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
   auto kern = gemm_ws_kernel<FMT, BN, STAGES>;
+  if constexpr (TILES) kern = gemm_ws_tiles_kernel<FMT, BN, STAGES>;
   using Cfg = GemmWsCfg<FMT, BN, STAGES>;
   if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
   if (prof_on()) {
@@ -227,6 +238,19 @@ int launch_ws_fmt(int bn, bool beside, const CUtensorMap& tw, const CUtensorMap&
     case 128: return launch_ws<FMT, 128>(tw, tx, a, stream);
   }
   return fail("gemm_ws_launch: no kernel instance");
+}
+
+// the whole-tile instances of e4m3 and int4 weights, at the token tiles and ring depths of the format's decoder instances
+template <int FMT>
+int launch_ws_tiles_fmt(int bn, const CUtensorMap& tw, const CUtensorMap& tx, const GemmWsArgs& a, cudaStream_t stream) {
+  switch (bn) {
+    case 16: return launch_ws<FMT, 16, decoder_stages(FMT), true>(tw, tx, a, stream);
+    case 32: return launch_ws<FMT, 32, ws_default_stages(FMT, 32), true>(tw, tx, a, stream);
+    case 64: return launch_ws<FMT, 64, ws_default_stages(FMT, 64), true>(tw, tx, a, stream);
+    case 96: return launch_ws<FMT, 96, ws_default_stages(FMT, 96), true>(tw, tx, a, stream);
+    case 128: return launch_ws<FMT, 128, ws_default_stages(FMT, 128), true>(tw, tx, a, stream);
+  }
+  return fail("gemm_ws_launch: no whole-tile kernel instance");
 }
 
 // Token-tile width for rows_x token rows, of both weight-streaming kernels: the smallest instance covering them (a
@@ -288,10 +312,14 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   const bool a8 = fmt == FMT_E4M3_A8;
   const bool f8 = fmt == FMT_E4M3 || a8;
   const bool i4 = fmt == FMT_I4;
-  VLO_CHECK(!f8 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn)),
-            "gemm_ws: e4m3 weights run stream-K partials (mode 0) on the token tile token_tile() picks");
-  VLO_CHECK(!i4 || (c.mode == 0 && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn) && c.rows_x <= 128),
-            "gemm_ws: int4 weights run stream-K partials (mode 0) of 1..128 token rows on the token tile token_tile() picks");
+  VLO_CHECK(!f8 || ((c.mode == 0 || (c.mode == 1 && !a8)) && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn)),
+            "gemm_ws: e4m3 weights run stream-K partials (mode 0), or whole tiles (mode 1) on bf16 activations, on the "
+            "token tile token_tile() picks");
+  VLO_CHECK(!i4 || ((c.mode == 0 || c.mode == 1) && c.tiling == WS_TILE_FIT && (c.bn == 0 || c.bn == bn) && c.rows_x <= 128),
+            "gemm_ws: int4 weights run stream-K partials (mode 0) or whole tiles (mode 1) of 1..128 token rows on the token "
+            "tile token_tile() picks");
+  VLO_CHECK(!(f8 || i4) || c.mode == 0 || (c.bias == nullptr && c.act == ACT_NONE),
+            "gemm_ws: whole tiles of e4m3 or int4 weights store bf16 logits: no bias, no activation");
   VLO_CHECK(!i4 || c.k % kI4Group == 0, "gemm_ws: int4 weights need K to be a multiple of 128 (one scale per 128 k)");
   const int x_tiles = (c.rows_x + bn - 1) / bn;
   GemmWsArgs a{};
@@ -322,6 +350,8 @@ int gemm_ws_launch(const GemmWsCall& c, cudaStream_t stream, GemmWsPlan* plan) {
   if (!i4 && get_tmap(c.w.w, c.rows_w, c.k, kGemmBM, kWsFmtInfo[fmt].w_map, &tw) != 0) return -1;
   if (get_tmap(c.x, c.rows_x, c.k, bn, kWsFmtInfo[fmt].x_map, &tx) != 0) return -1;
   if (i4) tw = tx;   // unused: the codes stream as bulk copies
+  if (c.mode == 1 && ws_tiles_own_instances(fmt))
+    return fmt == FMT_I4 ? launch_ws_tiles_fmt<FMT_I4>(bn, tw, tx, a, stream) : launch_ws_tiles_fmt<FMT_E4M3>(bn, tw, tx, a, stream);
   switch (fmt) {
     case FMT_F16: return launch_ws_fmt<FMT_F16>(bn, beside, tw, tx, a, stream);
     case FMT_BF16: return launch_ws_fmt<FMT_BF16>(bn, beside, tw, tx, a, stream);

@@ -27,11 +27,13 @@ enum GemmEpi : int {
 };
 enum GemmAct : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF_PY = 2 };
 // FMT_E4M3: e4m3 weights with one fp32 scale per weight row, bf16 activations; the consumer upcasts each weight k-block
-// to bf16 exactly and runs the bf16 wgmma chain (weight-streaming kernels, stream-K partials only)
+// to bf16 exactly and runs the bf16 wgmma chain (weight-streaming kernels: stream-K partials, and whole tiles in
+// instances of their own)
 // FMT_E4M3_A8: e4m3 weights (row scales) x e4m3 activations (token scales), multiplied by the FP8 wgmma (QGMMA) on
 // SWIZZLE_64B stages; each partial is scaled once in the epilogue (weight-streaming kernels, stream-K partials only)
 // FMT_I4: 4-bit weight codes with one bf16 scale per 128 k of a row, bf16 activations; the consumer dequantizes the
-// codes into the wgmma A fragment in registers and runs the bf16 wgmma chain (weight-streaming kernels, stream-K only)
+// codes into the wgmma A fragment in registers and runs the bf16 wgmma chain (weight-streaming kernels: stream-K
+// partials, and whole tiles in instances of their own)
 enum GemmFmt : int { FMT_F16 = 0, FMT_BF16 = 1, FMT_E4M3 = 2, FMT_E4M3_A8 = 3, FMT_I4 = 4 };
 // epilogues of the prefill GEMM (gemm_prefill.cuh): one fp32 plane for the fix-up kernels, or gate|up + SwiGLU
 enum PrefillEpi : int { PREFILL_PLANE = 0, PREFILL_SWIGLU = 1 };
@@ -111,6 +113,13 @@ constexpr int ws_fixed_bytes(int fmt, int extra) { return ws_cvt_bytes(fmt) + 10
 constexpr int ws_default_stages(int fmt, int bn, int extra = 0) {
   return fit_stages(ws_slot_bytes_w(fmt, bn) + ws_slot_bytes_x(fmt, bn), ws_fixed_bytes(fmt, extra), ws_max_stages(fmt));
 }
+
+// Whole tiles (mode 1) with the 16-bit store: every format but FMT_E4M3_A8.  The 16-bit formats run it in the
+// instances the layers run (a runtime mode); e4m3 and int4 weights run it in instances of their own
+// (gemm_ws_tiles_kernel: the vocabulary matrices of engines whose layers take those forms), which store bf16(acc) for
+// int4 and bf16(fl(acc * s[n])) for e4m3, with no bias and no activation.  One CTA covers all of K for each of its
+// tiles, so a logits row depends on no other row and on no token tile.  int4: at most 128 token rows (one token tile).
+constexpr bool ws_tiles_own_instances(int fmt) { return fmt == FMT_E4M3 || fmt == FMT_I4; }
 
 template <int FMT, int BN, int STAGES, int EXTRA = 0>
 struct GemmWsCfg {

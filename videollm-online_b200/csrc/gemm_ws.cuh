@@ -12,12 +12,14 @@
 //   * TILES mode (lm_head, connector): whole tiles per CTA, direct 16-bit epilogue, no partials;
 //   * the producer warp keeps the ring full across items, so the weight stream continues while the warpgroup
 //     runs the epilogue of an item;
-//   * FMT_E4M3 (mode 0 only): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop), each partial
-//     multiplied by its row's scale once before it is written;
+//   * FMT_E4M3 and FMT_I4 also run whole tiles (the vocabulary matrices), in gemm_ws_tiles_kernel instances of their own
+//     so that the instances the layers run keep their code (gemm.cuh, ws_tiles_own_instances);
+//   * FMT_E4M3 (mode 0 only in gemm_ws_kernel): e4m3 weight stages, upcast to bf16 by the warpgroup (wg_mainloop), each
+//     partial multiplied by its row's scale once before it is written;
 //   * FMT_E4M3_A8 (mode 0 only): e4m3 weight and e4m3 activation stages straight into the FP8 wgmma (wg_mainloop);
 //     each partial is multiplied by its row's weight scale, then by its token's activation scale, before it is written;
-//   * FMT_I4 (mode 0, one token tile only): 4-bit codes with per-group bf16 scales, dequantized into the wgmma A fragment in
-//     registers (wg_mainloop_i4); a ring slot carries up to i4_slot_units(BN) consecutive k-blocks of one tile, the codes
+//   * FMT_I4 (mode 0 only in gemm_ws_kernel, one token tile only): 4-bit codes with per-group bf16 scales, dequantized
+//     into the wgmma A fragment in registers (wg_mainloop_i4); a ring slot carries up to i4_slot_units(BN) consecutive k-blocks of one tile, the codes
 //     as one bulk copy.  The units, their k order and the plane each lands in are those of the bf16 kernel.
 #pragma once
 #include <cuda.h>
@@ -168,10 +170,11 @@ __device__ __forceinline__ float ws_row_scale(const float* w_scale, int n, bool 
   return scale_n;
 }
 
-template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN)>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
-               const GemmWsArgs p) {
+// The body of both kernels.  TILES = false: the runtime mode of p (the instances the layers run); TILES = true: whole
+// tiles of e4m3 or int4 weights with the bf16 store (ws_tiles_own_instances, gemm.cuh).
+template <int FMT, int BN, int STAGES, bool TILES>
+__device__ __forceinline__ void gemm_ws_body(const CUtensorMap& tm_w, const CUtensorMap& tm_x, const GemmWsArgs& p) {
+  static_assert(!TILES || ws_tiles_own_instances(FMT), "whole-tile instances of their own: e4m3 and int4 weights");
   using Cfg = GemmWsCfg<FMT, BN, STAGES>;
   constexpr int S = Cfg::kStages;
   const WsRing r = ws_ring<Cfg>();
@@ -181,7 +184,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
   const int c = blockIdx.x;
   const int kb = p.sk.kb;
   long long u0, u1;
-  if (p.mode == 0) {
+  if (!TILES && p.mode == 0) {
     u0 = sk_lo(c, p.sk);
     u1 = sk_lo(c + 1, p.sk);
   } else {
@@ -211,7 +214,7 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       float* plane = nullptr;
       float bias_n = 0.f;
       const float scale_n = ws_row_scale<FMT>(p.wt.w_scale, n, n_ok);
-      if (p.mode == 0) {
+      if (!TILES && p.mode == 0) {
         const int pl = c - sk_first_cta(tile, p.sk);
         plane = reinterpret_cast<float*>(p.out) + static_cast<size_t>(pl) * p.plane_stride;
       } else if (p.bias != nullptr && n_ok) {
@@ -229,8 +232,10 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
         for (int j = 0; j < 16; ++j) {
           const int t = t0 + c0 + j;
           if (t >= p.rows_x) break;
-          // e4m3 formats run mode 0 only
-          if (FMT == FMT_E4M3 || FMT == FMT_E4M3_A8 || p.mode == 0) {
+          if (TILES) {   // bf16(acc) for int4, bf16(fl(acc * s[n])) for e4m3
+            reinterpret_cast<uint16_t*>(p.out)[static_cast<size_t>(t) * p.ld_out + n] =
+                to16<FMT_BF16>(scale_partial<FMT>(v[j], scale_n, nullptr, t));
+          } else if (FMT == FMT_E4M3 || FMT == FMT_E4M3_A8 || p.mode == 0) {   // e4m3 formats run mode 0 only here
             plane[static_cast<size_t>(t) * p.rows_w + n] = scale_partial<FMT>(v[j], scale_n, p.wt.a_scale, t);
           } else {
             float x = r16<FMT>(v[j] + bias_n);
@@ -241,6 +246,21 @@ gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__
       }
     }
   }
+}
+
+template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN)>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_ws_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
+               const GemmWsArgs p) {
+  gemm_ws_body<FMT, BN, STAGES, false>(tm_w, tm_x, p);
+}
+
+// whole tiles of e4m3 or int4 weights (p.mode is ignored)
+template <int FMT, int BN, int STAGES = ws_default_stages(FMT, BN)>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_ws_tiles_kernel(const __grid_constant__ CUtensorMap tm_w, const __grid_constant__ CUtensorMap tm_x,
+                     const GemmWsArgs p) {
+  gemm_ws_body<FMT, BN, STAGES, true>(tm_w, tm_x, p);
 }
 
 }  // namespace vlo

@@ -8,20 +8,22 @@ from typing import Dict, Optional
 import torch
 
 from .config import LiveConfig
-from .weights import layer_matrix_spec
+from .weights import layer_matrix_spec, vocab_matrix_spec
 
 
 def engine_weight_spec(cfg: LiveConfig, max_positions: int, fp8_weights: bool = False,
-                       int4_weights: bool = False) -> Dict[str, tuple]:
+                       int4_weights: bool = False, quantize_vocab: bool = False) -> Dict[str, tuple]:
     """name -> (shape, dtype) of every tensor of the engine layout (weights.py docstring), derivable on
     every rank without materialising anything.  fp8_weights: the layer matrices as e4m3 codes + row scales;
-    int4_weights: as packed int4 codes + bf16 group scales."""
+    int4_weights: as packed int4 codes + bf16 group scales; quantize_vocab: embed and lm_head in that form too."""
     bf, f16, f32 = torch.bfloat16, torch.float16, torch.float32
     H, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
     nh, nkv, hd = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     C, M, ps, P = cfg.vision_hidden_size, cfg.vision_intermediate_size, cfg.vision_patch_size, cfg.num_patches
-    s: Dict[str, tuple] = {"embed": ((V, H), bf), "final_norm": ((H,), bf), "lm_head": ((V, H), bf),
-                           "rope.cos": ((max_positions, hd // 2), bf), "rope.sin": ((max_positions, hd // 2), bf)}
+    s: Dict[str, tuple] = dict(vocab_matrix_spec("embed", (V, H), fp8_weights, int4_weights, quantize_vocab))
+    s["final_norm"] = ((H,), bf)
+    s.update(vocab_matrix_spec("lm_head", (V, H), fp8_weights, int4_weights, quantize_vocab))
+    s.update({"rope.cos": ((max_positions, hd // 2), bf), "rope.sin": ((max_positions, hd // 2), bf)})
     for i in range(cfg.num_hidden_layers):
         s[f"L{i}.in_norm"] = ((H,), bf)
         s[f"L{i}.post_norm"] = ((H,), bf)
@@ -74,18 +76,19 @@ def _flat_layout(spec: Dict[str, tuple], n_buckets: int):
 
 def broadcast_weights(cfg: LiveConfig, weights: Optional[Dict[str, torch.Tensor]], device, max_positions: int,
                       dist=None, src: int = 0, n_buckets: int = 8, release_source: bool = False,
-                      fp8_weights: bool = False, int4_weights: bool = False) -> Dict[str, torch.Tensor]:
+                      fp8_weights: bool = False, int4_weights: bool = False,
+                      quantize_vocab: bool = False) -> Dict[str, torch.Tensor]:
     """Rank `src` passes its engine-layout dict, the others pass None; everyone returns the full dict on `device`.
     The ~560 tensors (16.7 GB) travel as <= `n_buckets` flat byte buffers, one NCCL broadcast each over NVLink/NVSwitch
     (per-tensor broadcasts cost 1.2 s at 8 GPUs: launch latency, not bandwidth); the returned tensors are views into
     those buffers (256-byte aligned), on the source rank too, so every rank ends with the same memory layout.
     release_source=True empties the source dict entry by entry while packing.  fp8_weights: every rank expects the layer
-    matrices in the FP8 form (engine_weight_spec); int4_weights: in the int4 form."""
+    matrices in the FP8 form (engine_weight_spec); int4_weights: in the int4 form; quantize_vocab: embed and lm_head too."""
     if dist is None or not dist.is_initialized() or dist.get_world_size() == 1:
         if weights is None:
             raise ValueError("single process: weights must be provided")
         return weights
-    spec = engine_weight_spec(cfg, max_positions, fp8_weights, int4_weights)
+    spec = engine_weight_spec(cfg, max_positions, fp8_weights, int4_weights, quantize_vocab)
     out: Dict[str, torch.Tensor] = {}
     is_src = dist.get_rank() == src
     if is_src:

@@ -329,6 +329,12 @@ class Engine:
         return "L0.qkv.i4" in self._weights
 
     @property
+    def quantized_vocab(self) -> bool:
+        """True when embed and lm_head were loaded in the layer matrices' quantized form (e4m3 or int4, quantize_vocab)
+        rather than in bf16."""
+        return "embed.f8" in self._weights or "embed.i4" in self._weights
+
+    @property
     def max_prefill_tokens(self) -> int:
         """rows of one vlo_prefill (8 x max_step_tokens) once bf16 layer weights are loaded; 0 before, and on engines
         with e4m3 layer weights or activations"""

@@ -53,6 +53,7 @@ class SessionState:
     fp8_weights: bool = False    # the cache was written by a model with FP8 layer weights (Engine.fp8_weights)
     fp8_activations: bool = False   # ... and with FP8 activations (Engine.fp8_activations)
     int4_weights: bool = False   # ... with int4 layer weights (Engine.int4_weights)
+    quantized_vocab: bool = False   # ... with quantized token embeddings and lm_head (Engine.quantized_vocab)
 
 
 torch.serialization.add_safe_globals([SessionState, SamplingConfig])
@@ -238,7 +239,8 @@ class LiveInfer:
                 drafter_ids=list(self.drafter.ids) if isinstance(self.drafter, NgramDrafter) else None,
                 n_calls=self._n_calls, started=self.past_key_values is not None, sampling=self.sampling,
                 evicted_tokens=self.evicted_tokens, fp8_weights=self._kv.engine.fp8_weights,
-                fp8_activations=self._kv.engine.fp8_activations, int4_weights=self._kv.engine.int4_weights, fed_ids=fed)
+                fp8_activations=self._kv.engine.fp8_activations, int4_weights=self._kv.engine.int4_weights,
+                quantized_vocab=self._kv.engine.quantized_vocab, fed_ids=fed)
             self.reset()
             return state
 
@@ -248,7 +250,9 @@ class LiveInfer:
         (before or after resuming).  Raises VloError if the pool is short or the image belongs to another config; the
         session's stream is then empty and the rest of the session unchanged.  A state whose cache was written with the
         other weight form (bf16, FP8 or int4 layer weights: a different model), or with the other activation form (W8A8 or
-        not), is refused before anything changes.  States saved before the int4 form existed load as not int4."""
+        not), or with the other form of the vocabulary matrices (quantized or bf16: the cache holds rows computed from
+        the text embeddings), is refused before anything changes.  States saved before the int4 form existed load as not
+        int4, and states saved before quantized vocabulary matrices existed load as not quantized."""
         with self._lock:
             eng = self._kv.engine
             def weight_form(fp8, int4):
@@ -261,6 +265,10 @@ class LiveInfer:
                 form = {True: "FP8", False: "bf16"}
                 raise VloError(f"resume: the state's cache was written with {form[state.fp8_activations]} layer "
                                f"activations, this model has {form[eng.fp8_activations]} ones")
+            if state.quantized_vocab != eng.quantized_vocab:
+                form = {True: "quantized", False: "bf16"}
+                raise VloError(f"resume: the state's cache was written with {form[state.quantized_vocab]} vocabulary "
+                               f"matrices, this model has {form[eng.quantized_vocab]} ones")
             self._drop_prefetch()
             eng.stream_reset(self._kv.stream_id)
             eng.kv_swap_in(self._kv.stream_id, state.kv)

@@ -61,8 +61,12 @@ class _Embedding:
         return self.engine.embed_tokens(ids).view(*shape, self.engine.cfg.hidden_size)
 
     @property
-    def weight(self):
-        return self.engine.weights["embed"]
+    def weight(self) -> torch.Tensor:
+        """bf16 [V, H], the table the engine gathers from.  With quantized vocabulary matrices it is dequantized on every
+        access into a new tensor (1.05 GB at Llama-3-8B's shape): keep it only as long as it is needed."""
+        from .weights import dequantized_vocab_matrix
+        cfg = self.engine.cfg
+        return dequantized_vocab_matrix(self.engine.weights, "embed", cfg.vocab_size, cfg.hidden_size)
 
 
 class LiveLlamaForCausalLM:
@@ -297,7 +301,7 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
                synthetic_weights: bool = False, seed: int = 0, max_streams: int = 1, max_kv_tokens: int = 16384,
                max_step_tokens: int = 128, max_vit_batch: int = 8, llm_state=None, vision_state=None,
                lora_r: int = 128, lora_alpha: int = 256, kv_pool_tokens: Optional[int] = None, fp8_weights: bool = False,
-               fp8_activations: bool = False, int4_weights: bool = False, **kwargs):
+               fp8_activations: bool = False, int4_weights: bool = False, quantize_vocab: bool = False, **kwargs):
     """models/modeling_live.py:184-222 for inference: build config + tokenizer, load (or synthesise)
     weights, merge LoRA, hand everything to the engine.  kv_pool_tokens: size of the KV page pool the streams
     share (None or <= 0: max_streams * max_kv_tokens).  fp8_weights: quantize the decoder layer matrices to e4m3 with
@@ -305,7 +309,8 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
     fp8_activations (needs fp8_weights): the layer GEMMs also quantize their activations to e4m3 per token and run on
     the FP8 tensor cores (W8A8).  int4_weights: quantize the layer matrices to 4-bit codes with one bf16 scale per 128
     weights of a row (weights.quantize_int4_groups, W4A16); the engine computes the bits of a bf16 engine on the
-    dequantized weights.  It excludes fp8_weights and fp8_activations."""
+    dequantized weights.  It excludes fp8_weights and fp8_activations.  quantize_vocab (needs fp8_weights or
+    int4_weights): embed and lm_head take the layer matrices' quantized form too (weights.pack_llm_for_engine)."""
     if is_training:
         raise NotImplementedError("the vlo_b200 engine covers the streaming-inference path only")
     if int4_weights and (fp8_weights or fp8_activations):
@@ -313,6 +318,9 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
                          "4-bit weights multiply bf16 activations")
     if fp8_activations and not fp8_weights:
         raise ValueError("fp8_activations needs fp8_weights: the FP8 tensor cores take both operands in e4m3")
+    if quantize_vocab and not (fp8_weights or int4_weights):
+        raise ValueError("quantize_vocab needs fp8_weights or int4_weights: the vocabulary matrices take the layer "
+                         "matrices' quantized form")
     cfg = config or llama3_8b_siglip_l()
     for k in ("frame_resolution", "frame_token_cls", "frame_token_pooled", "frame_num_tokens", "frame_token_interval",
               "vision_pretrained"):
@@ -324,28 +332,29 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
                     fp8_activations=fp8_activations)
     if llm_state is not None:
         packed = W.pack_llm_for_engine(cfg, llm_state, engine.device, max_kv_tokens, fp8_weights=fp8_weights,
-                                       int4_weights=int4_weights)
+                                       int4_weights=int4_weights, quantize_vocab=quantize_vocab)
         if set_vision_inside:
             if vision_state is None:
                 raise VloError("set_vision_inside=True needs vision_state")
             packed.update(W.pack_vision_for_engine(cfg, vision_state, engine.device))
     elif synthetic_weights:
         packed = W.synthetic_engine_weights(cfg, engine.device, max_kv_tokens, seed=seed, fp8_weights=fp8_weights,
-                                            int4_weights=int4_weights)
+                                            int4_weights=int4_weights, quantize_vocab=quantize_vocab)
         if not set_vision_inside:
             packed = {k: v for k, v in packed.items() if not k.startswith("vit.")}
     else:
         packed = _load_checkpoints(cfg, llm_pretrained, resume_from_checkpoint, set_vision_inside, engine.device,
-                                   max_kv_tokens, lora_r, lora_alpha, fp8_weights, int4_weights)
+                                   max_kv_tokens, lora_r, lora_alpha, fp8_weights, int4_weights, quantize_vocab)
     engine.load_weights(packed)
     model = LiveLlamaForCausalLM(cfg, engine)
     return model, tokenizer
 
 
 def _load_checkpoints(cfg, llm_pretrained, adapter, with_vision, device, max_positions, lora_r, lora_alpha,
-                      fp8_weights=False, int4_weights=False):
+                      fp8_weights=False, int4_weights=False, quantize_vocab=False):
     """Real weights: base Llama safetensors + PEFT adapter (+ SigLIP), local files only.  fp8_weights / int4_weights:
-    the layer matrices are quantized after the LoRA merge, one at a time on `device`."""
+    the layer matrices are quantized after the LoRA merge, one at a time on `device`; quantize_vocab: embed and lm_head
+    too."""
     import glob
     import os
     try:
@@ -370,7 +379,8 @@ def _load_checkpoints(cfg, llm_pretrained, adapter, with_vision, device, max_pos
                 aj = json.load(fh)
             lora_r, lora_alpha = int(aj.get("r", lora_r)), float(aj.get("lora_alpha", lora_alpha))
         sd = W.merge_lora(sd, ad, lora_alpha=lora_alpha, lora_r=lora_r)
-    packed = W.pack_llm_for_engine(cfg, sd, device, max_positions, fp8_weights=fp8_weights, int4_weights=int4_weights)
+    packed = W.pack_llm_for_engine(cfg, sd, device, max_positions, fp8_weights=fp8_weights, int4_weights=int4_weights,
+                                   quantize_vocab=quantize_vocab)
     if with_vision:
         vdir = cfg.vision_pretrained
         vs = {}

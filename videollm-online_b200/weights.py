@@ -24,6 +24,10 @@ Int4 weights (int4_weights=True, W4A16): each layer matrix [N, K] (K % 128 == 0)
 q + 8 in the engine byte order of pack_int4_codes, uint8, ceil(N / 128) * 128 * K / 2 bytes) and L{i}.{m}.gscale (bf16
 [N, K / 128]), quantized by quantize_int4_groups from the same bf16 matrix.  The engine multiplies W4 =
 dequantize_int4_groups(q, s) exactly, so an int4 engine computes the bits of a bf16 engine loaded with W4.
+Quantized vocabulary matrices (quantize_vocab=True, with fp8_weights or int4_weights): embed and lm_head [V, H] are
+quantized after the LoRA merge by the same rule as the layer matrices and stored under the same suffixes (embed.f8 +
+embed.scale, lm_head.f8 + lm_head.scale; or embed.i4 + embed.gscale, lm_head.i4 + lm_head.gscale).  The engine's
+embedding of id i is row i of dequantize_fp8_rows_bf16 / dequantize_int4_groups (dequantized_vocab_matrix).
 """
 from __future__ import annotations
 
@@ -205,6 +209,12 @@ def dequantize_fp8_rows(codes: torch.Tensor, scale: torch.Tensor) -> torch.Tenso
     return codes.view(torch.float8_e4m3fn).float() * scale[:, None]
 
 
+def dequantize_fp8_rows_bf16(codes: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
+    """bf16 [N, K] = bf16_rn(fp32(q) * s): the rows of an e4m3 embedding table as the engine's gather returns them (one
+    fp32 product, then one rounding to bf16)."""
+    return dequantize_fp8_rows(codes, scale).to(torch.bfloat16)
+
+
 INT4_GROUP = 128   # weights of a row per int4 scale
 INT4_TILE = 128    # weight rows per engine tile (the GEMM's 128-row M tile)
 
@@ -274,6 +284,12 @@ def _weight_form(fp8_weights: bool, int4_weights: bool) -> None:
         raise ValueError("fp8_weights and int4_weights are two forms of the layer matrices: choose one")
 
 
+def _vocab_form(fp8_weights: bool, int4_weights: bool, quantize_vocab: bool) -> None:
+    _weight_form(fp8_weights, int4_weights)
+    if quantize_vocab and not (fp8_weights or int4_weights):
+        raise ValueError("quantize_vocab takes the layer matrices' quantized form: it needs fp8_weights or int4_weights")
+
+
 def layer_matrix_spec(name: str, shape: tuple, fp8_weights: bool, int4_weights: bool = False) -> Dict[str, tuple]:
     """Engine tensor name -> (shape, dtype) of one layer matrix [N, K] in the chosen form."""
     _weight_form(fp8_weights, int4_weights)
@@ -284,6 +300,24 @@ def layer_matrix_spec(name: str, shape: tuple, fp8_weights: bool, int4_weights: 
     if not fp8_weights:
         return {name: (shape, torch.bfloat16)}
     return {name + ".f8": (shape, torch.uint8), name + ".scale": ((shape[0],), torch.float32)}
+
+
+def vocab_matrix_spec(name: str, shape: tuple, fp8_weights: bool, int4_weights: bool = False,
+                      quantize_vocab: bool = False) -> Dict[str, tuple]:
+    """Engine tensor name -> (shape, dtype) of a vocabulary matrix (embed, lm_head): bf16, or with quantize_vocab in the
+    layer matrices' form."""
+    _vocab_form(fp8_weights, int4_weights, quantize_vocab)
+    return layer_matrix_spec(name, shape, fp8_weights and quantize_vocab, int4_weights and quantize_vocab)
+
+
+def dequantized_vocab_matrix(weights: StateDict, name: str, n: int, k: int) -> torch.Tensor:
+    """bf16 [n, k] of vocabulary matrix `name` in whichever form `weights` holds it: the matrix every engine kernel
+    multiplies or gathers (the bf16 tensor itself when it is not quantized; a new tensor otherwise)."""
+    if name + ".i4" in weights:
+        return dequantize_int4_groups(unpack_int4_codes(weights[name + ".i4"], n, k), weights[name + ".gscale"])
+    if name + ".f8" in weights:
+        return dequantize_fp8_rows_bf16(weights[name + ".f8"].view(n, k), weights[name + ".scale"])
+    return weights[name]
 
 
 def _put_layer_matrix(out: StateDict, name: str, w: torch.Tensor, fp8_weights: bool, int4_weights: bool = False) -> None:
@@ -299,17 +333,20 @@ def _put_layer_matrix(out: StateDict, name: str, w: torch.Tensor, fp8_weights: b
 
 
 def pack_llm_for_engine(cfg: LiveConfig, sd: StateDict, device, max_positions: int, fp8_weights: bool = False,
-                        int4_weights: bool = False) -> StateDict:
-    _weight_form(fp8_weights, int4_weights)
+                        int4_weights: bool = False, quantize_vocab: bool = False) -> StateDict:
+    """quantize_vocab (with fp8_weights or int4_weights): embed and lm_head in the layer matrices' form too, quantized
+    after the LoRA merge (the adapter targets lm_head)."""
+    _vocab_form(fp8_weights, int4_weights, quantize_vocab)
+    qf8, qi4 = fp8_weights and quantize_vocab, int4_weights and quantize_vocab
     bf = torch.bfloat16
     out: StateDict = {}
 
     def take(k):
         return sd[k].to(device=device, dtype=bf).contiguous()
 
-    out["embed"] = take("model.embed_tokens.weight")
+    _put_layer_matrix(out, "embed", take("model.embed_tokens.weight"), qf8, qi4)
     out["final_norm"] = take("model.norm.weight")
-    out["lm_head"] = take("lm_head.weight")
+    _put_layer_matrix(out, "lm_head", take("lm_head.weight"), qf8, qi4)
     cos, sin = rope_tables(cfg, max_positions, device)
     out["rope.cos"], out["rope.sin"] = cos, sin
     for i in range(cfg.num_hidden_layers):
@@ -375,20 +412,21 @@ def pack_vision_for_engine(cfg: LiveConfig, sd: StateDict, device) -> StateDict:
 
 
 def synthetic_engine_weights(cfg: LiveConfig, device, max_positions: int, seed: int = 0, std: float = 0.02,
-                             fp8_weights: bool = False, int4_weights: bool = False) -> StateDict:
+                             fp8_weights: bool = False, int4_weights: bool = False, quantize_vocab: bool = False) -> StateDict:
     """Full-size synthetic weights generated directly in the engine layout on `device` (bench path: no
     16 GB host round trip).  Same distributions as synthetic_*_state, different random stream.  fp8_weights /
-    int4_weights: the layer matrices of the same seed, quantized."""
-    _weight_form(fp8_weights, int4_weights)
+    int4_weights: the layer matrices of the same seed, quantized; quantize_vocab: embed and lm_head too."""
+    _vocab_form(fp8_weights, int4_weights, quantize_vocab)
+    qf8, qi4 = fp8_weights and quantize_vocab, int4_weights and quantize_vocab
     g = torch.Generator(device=device).manual_seed(seed)
     bf, f16, f32 = torch.bfloat16, torch.float16, torch.float32
     H, I, V = cfg.hidden_size, cfg.intermediate_size, cfg.vocab_size
     nh, nkv, hd = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     C, M, ps, P = cfg.vision_hidden_size, cfg.vision_intermediate_size, cfg.vision_patch_size, cfg.num_patches
     out: StateDict = {}
-    out["embed"] = _gen((V, H), 1.0, g, device, bf)
+    _put_layer_matrix(out, "embed", _gen((V, H), 1.0, g, device, bf), qf8, qi4)
     out["final_norm"] = _gen((H,), 0.1, g, device, bf, 1.0)
-    out["lm_head"] = _gen((V, H), std, g, device, bf)
+    _put_layer_matrix(out, "lm_head", _gen((V, H), std, g, device, bf), qf8, qi4)
     out["rope.cos"], out["rope.sin"] = rope_tables(cfg, max_positions, device)
     for i in range(cfg.num_hidden_layers):
         out[f"L{i}.in_norm"] = _gen((H,), 0.1, g, device, bf, 1.0)
