@@ -102,8 +102,9 @@ int vlo_load_tensor(vlo_engine* e, const char* name, const void* d_ptr, int64_t 
  * `name.gscale` is bf16 [N, K / 128].  `name.i4` holds the codes q + 8, two per byte, ceil(N / 128) x 128 x K / 2 bytes in
  * the engine byte order: one 4 KB block per (128-row tile, 64-wide k-block), blocks in (tile, k-block) order, and inside a
  * block thread t of the consumer warpgroup's 16 bytes per 64-row half h at h * 2048 + 16 t (DESIGN.md section 2,
- * weights.pack_int4_codes).  Every result is bit for bit the bf16 engine's on W4.  An int4 engine does not prefill
- * (vlo_max_prefill_tokens is 0) and takes no FP8 activations (finalize fails with a message).
+ * weights.pack_int4_codes).  Every result is bit for bit the bf16 engine's on W4.  An int4 engine prefills only with
+ * vlo_set_quantized_prefill (vlo_max_prefill_tokens is 0 without it) and takes no FP8 activations (finalize fails with a
+ * message).
  * The vocabulary matrices `embed` and `lm_head` ([vocab, hidden] each) come either in bf16 (`embed`, `lm_head`) or, on
  * an engine with quantized layer matrices, both in the layers' quantized form, quantized by the same rules:
  *   int4 layers: `embed.i4` + `embed.gscale`, `lm_head.i4` + `lm_head.gscale` (engine byte order, as above).  lm_head
@@ -137,6 +138,14 @@ int64_t vlo_engine_device_bytes(vlo_engine* e);
  * xn_last and vlo_last_step_hidden) is still written in bf16.  Two more launches per layer: the quantizers of the
  * attention output and of act (the norms write the e4m3 xn themselves). */
 int vlo_set_fp8_activations(vlo_engine* e, int on);
+/* Prefill on quantized layer matrices (FP8 weights, W8A8, int4), opt-in.  Valid before vlo_finalize_weights (fails after
+ * it).  With on != 0, finalize grows the token-row workspaces to vlo_max_prefill_tokens rows as it does on a bf16 engine
+ * and, under FP8 activations, the e4m3 activation copies and their token scales too; vlo_prefill then runs the layer
+ * GEMMs on gemm_prefill_q_kernel (csrc/gemm_prefill_q.cuh), with the bits of the same rows fed as max_step_tokens steps
+ * on the same engine.  Finalize fails with a message if the mode is on and the layer matrices are bf16 (a bf16 engine
+ * always prefills).  Off (the default), a quantized engine keeps its workspaces at max_step_tokens rows and does not
+ * prefill. */
+int vlo_set_quantized_prefill(vlo_engine* e, int on);
 
 /* ------------------------------------------------------------------ streams (KV ownership)
  * replaces: the DynamicCache handed around as past_key_values (HF:cache_utils.py:88-121;
@@ -349,13 +358,16 @@ int vlo_sample(vlo_engine* e, const void* d_logits, int n_rows, const vlo_sample
  * attention is one vlo_step_segments-style launch whose segments are the max_step_tokens pieces, each planned as its own
  * step.  d_row_ids (device int64 [n_tokens] or NULL) as in vlo_step_ids; d_last_logits: bf16 [1, vocab] or NULL;
  * d_decision: one vlo_decision or NULL, at the last row.  vlo_last_step_logits / vlo_last_step_hidden then cover all
- * n_tokens rows.  The stream's pages are taken all or none; on any error the stream is unchanged.  bf16 layer weights
- * only: an engine with e4m3 weights (or W8A8) returns an error. */
+ * n_tokens rows.  The stream's pages are taken all or none; on any error the stream is unchanged.  An engine with
+ * quantized layer matrices (e4m3 weights, W8A8, int4) prefills only with vlo_set_quantized_prefill: its layer GEMMs then
+ * run on gemm_prefill_q_kernel (weights on wgmma M, the chunked kernels' MMAs and partial scaling, csrc/gemm_prefill_q.cuh);
+ * without it vlo_prefill returns an error. */
 int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row_ids, const void* d_embeds,
                 void* d_last_logits, vlo_decision* d_decision, int interval_id, void* cuda_stream);
-/* 8 x max_step_tokens once vlo_finalize_weights has loaded bf16 layer weights on an engine without fp8 activations: it
- * then grows the token-row workspaces (h, xn, q, attn_out, act, attention workspace, step tables) to that many rows.
- * 0 before, and on engines with e4m3 layer weights or activations, which keep them at max_step_tokens rows. */
+/* 8 x max_step_tokens once vlo_finalize_weights has loaded bf16 layer weights, or quantized ones with
+ * vlo_set_quantized_prefill: it then grows the token-row workspaces (h, xn, q, attn_out, act, attention workspace, step
+ * tables; under FP8 activations also their e4m3 copies and token scales) to that many rows.  0 before, and on engines
+ * with quantized layer matrices without vlo_set_quantized_prefill, which keep them at max_step_tokens rows. */
 int vlo_max_prefill_tokens(vlo_engine* e);
 
 /* all-position logits for the last vlo_step's tokens (the reference's logits_to_keep=0 behaviour,
@@ -562,6 +574,16 @@ int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x,
  * (rows_w % 128 == 0, all SMs' plan) on g, u = P0 + P1 + ....  Rows past rows_x are not written.  Asynchronous. */
 int vlo_op_gemm_prefill(int epi, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, int n_ctas, void* d_out,
                         void* cuda_stream);
+/* Prefill GEMM of quantized weights (csrc/gemm_prefill_q.cuh), with the operands of vlo_op_gemm_ws_f8 (fmt 2: d_w e4m3
+ * [rows_w, k], d_scale fp32 [rows_w]), vlo_op_gemm_ws_a8 (fmt 3: the same weights, d_x e4m3 [rows_x, k] with fp32 token
+ * scales d_xscale [rows_x]) or vlo_op_gemm_ws_i4 (fmt 4: d_w the codes, d_gscale bf16 [rows_w, k / 128]); the unused
+ * pointers may be NULL.  Any rows_x; plan and epilogues as vlo_op_gemm_prefill, with each range's partial scaled as the
+ * chunked kernels scale a partial before it is summed (fmt 2: fl(P * d_scale[n]); fmt 3: fl(fl(P * d_scale[n]) *
+ * d_xscale[t]); fmt 4: P).  So epi 0 equals vlo_op_gemm_ws_{f8,a8,i4} mode 0 on each 128-row chunk of X summed
+ * 0 + plane 0 + plane 1 + ..., and epi 1 equals vlo_op_gemm_swiglu_{f8,a8,i4} on each chunk.  Asynchronous. */
+int vlo_op_gemm_prefill_q(int fmt, int epi, const void* d_w, const float* d_scale, const void* d_gscale, int rows_w,
+                          const void* d_x, const float* d_xscale, int rows_x, int k, int n_ctas, void* d_out,
+                          void* cuda_stream);
 /* vlo_op_gemm_swiglu on e4m3 weights d_w8 [rows_w, k] with fp32 row scales d_scale [rows_w] (same row order and plan):
  * g, u = bf16(sum_p fl(P_p * d_scale[n])) summed in plane order, P_p the fp32 partials of the bf16 kernel on the exactly
  * upcast weights (the finisher's own partial is plane 0).  Asynchronous. */

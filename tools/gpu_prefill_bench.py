@@ -5,7 +5,10 @@ the chunked path (max_step_tokens steps).  One JSON line per measurement:
   pass      T-token input from kv_len `kv`, prefill and chunked alternated, `reps` repeats each: ms, and the layer-GEMM
             TFLOP/s of the whole pass (2 x layer parameters x T over the pass time); the outputs are checked equal
   evaluate  stream_evaluate on a synthetic conversation of `frames` frames, end to end, prefill and chunked alternated
-  python tools/gpu_prefill_bench.py [--reps 3] [--frames 1200]"""
+--form picks the layer matrices: bf16 (the default), or fp8 (e4m3 weights), w8a8 (e4m3 weights and activations) or int4,
+which run with quantized_prefill; the chunked path is then the same engine's max_step_tokens steps, and the quantized
+forms measure the passes of 1024 and 4096 tokens from an empty cache and 4096 after 12k keys.
+  python tools/gpu_prefill_bench.py [--form bf16] [--reps 3] [--frames 1200]"""
 import argparse, json, pathlib, subprocess, sys, time
 import torch
 sys.path.insert(0, str(pathlib.Path(__file__).resolve().parents[1]))
@@ -17,6 +20,7 @@ from videollm_online_b200.modeling_live import build_live
 ap = argparse.ArgumentParser()
 ap.add_argument("--reps", type=int, default=3)
 ap.add_argument("--frames", type=int, default=1200)
+ap.add_argument("--form", choices=["bf16", "fp8", "w8a8", "int4"], default="bf16")
 args = ap.parse_args()
 
 
@@ -26,20 +30,23 @@ def emit(kind, rec):
 
 smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                      text=True).stdout.strip()
-emit("card", {"gpu": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit": smi})
+emit("card", {"gpu": torch.cuda.get_device_name(0), "nvidia_smi_name_power_limit": smi, "form": args.form})
 
 dev = torch.device("cuda:0")
 cfg = llama3_8b_siglip_l()
 CAP = 12000 + 13200 + 1024
+quant = args.form != "bf16"
+a8 = args.form == "w8a8"
 model, _ = build_live(config=cfg, synthetic_weights=True, set_vision_inside=False, device="cuda:0", max_streams=2,
-                      max_kv_tokens=CAP, max_step_tokens=128, max_vit_batch=1)
+                      max_kv_tokens=CAP, max_step_tokens=128, max_vit_batch=1, fp8_weights=args.form in ("fp8", "w8a8"),
+                      fp8_activations=a8, int4_weights=args.form == "int4", quantized_prefill=quant)
 eng = model.engine
 H, I, A = cfg.hidden_size, cfg.intermediate_size, cfg.num_attention_heads * cfg.head_dim
 QKV = (cfg.num_attention_heads + 2 * cfg.num_key_value_heads) * cfg.head_dim
 layer_params = cfg.num_hidden_layers * (QKV * H + H * A + 2 * I * H + H * I)
-fresh = Engine(cfg, dev, max_streams=2, max_kv_tokens=CAP, max_step_tokens=128, max_vit_batch=1)
-emit("engine", {"device_bytes": eng.device_bytes(), "max_prefill_tokens": eng.max_prefill_tokens,
-                "prefill_workspace_bytes": eng.device_bytes() - fresh.device_bytes()})   # grown by loading bf16 weights
+fresh = Engine(cfg, dev, max_streams=2, max_kv_tokens=CAP, max_step_tokens=128, max_vit_batch=1, fp8_activations=a8)
+emit("engine", {"form": args.form, "device_bytes": eng.device_bytes(), "max_prefill_tokens": eng.max_prefill_tokens,
+                "prefill_workspace_bytes": eng.device_bytes() - fresh.device_bytes()})   # grown by finalize
 fresh.close()
 PREFILL = Engine.prefills
 
@@ -64,14 +71,15 @@ bytes_ = C.c_double()
 launches = C.c_int()
 eng.lib.vlo_bench_gemm(eng._h, 128, 2, C.byref(bytes_), C.byref(launches), eng._stream())
 ms, _ = timed(lambda: eng.lib.vlo_bench_gemm(eng._h, 128, 10, C.byref(bytes_), C.byref(launches), eng._stream()))
-emit("gemm128", {"ms_per_step": ms / 10, "algo_GB": bytes_.value / 1e9, "TB_per_s": bytes_.value / (ms / 10) / 1e9})
+emit("gemm128", {"form": args.form, "ms_per_step": ms / 10, "algo_GB": bytes_.value / 1e9, "TB_per_s": bytes_.value / (ms / 10) / 1e9})
 
 # ---- whole passes
 sid = eng.stream_open()
 g = torch.Generator(device=dev).manual_seed(0)
-for T, kv in [(1024, 0), (4096, 0), (4096, 12000), (13200, 0), (13200, 12000)]:
+PASSES = [(1024, 0), (4096, 0), (4096, 12000)] + ([] if quant else [(13200, 0), (13200, 12000)])
+for T, kv in PASSES:
     emb = (torch.randn(T, H, device=dev, generator=g) * 0.02).bfloat16()
-    rec = {"T": T, "kv": kv, "prefill_ms": [], "chunked_ms": []}
+    rec = {"form": args.form, "T": T, "kv": kv, "prefill_ms": [], "chunked_ms": []}
     outs = {}
     for r in range(args.reps + 1):            # the first round warms both paths up
         for mode in ("prefill", "chunked"):
@@ -108,7 +116,7 @@ input_ids, label_ids = torch.tensor([ids], device=dev), torch.tensor([labels], d
 feats = (torch.randn(args.frames, fnt, cfg.vision_hidden_size, generator=gc) * 0.5).to(dev)
 # the engine's connector takes max_vit_batch frames per call
 model.visual_embed = lambda f: torch.cat([eng.connector(f[i:i + eng.max_vit_batch]) for i in range(0, f.shape[0], eng.max_vit_batch)])
-rec = {"frames": args.frames, "tokens": len(ids), "prefill_s": [], "chunked_s": []}
+rec = {"form": args.form, "frames": args.frames, "tokens": len(ids), "prefill_s": [], "chunked_s": []}
 res = {}
 for r in range(args.reps + 1):
     for mode in ("prefill", "chunked"):

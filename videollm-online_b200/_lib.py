@@ -85,6 +85,7 @@ SIGNATURES = {
     "vlo_finalize_weights": (_I, [_P]),
     "vlo_engine_device_bytes": (C.c_int64, [_P]),
     "vlo_set_fp8_activations": (_I, [_P, _I]),
+    "vlo_set_quantized_prefill": (_I, [_P, _I]),
     "vlo_stream_open": (_I, [_P, C.POINTER(_I)]),
     "vlo_stream_reset": (_I, [_P, _I]),
     "vlo_stream_close": (_I, [_P, _I]),
@@ -146,6 +147,7 @@ SIGNATURES = {
                                     _I, _I, _I, _P]),
     "vlo_op_gemm_swiglu": (_I, [_P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_prefill": (_I, [_I, _P, _I, _P, _I, _I, _I, _P, _P]),
+    "vlo_op_gemm_prefill_q": (_I, [_I, _I, _P, _P, _P, _I, _P, _P, _I, _I, _I, _P, _P]),
     "vlo_op_gemm_swiglu_f8": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_swiglu_i4": (_I, [_P, _P, _I, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),
     "vlo_op_gemm_swiglu_a8": (_I, [_P, _P, _I, _P, _P, _I, _I, _P, _P, C.c_int64, _P, _I, _P]),

@@ -23,6 +23,8 @@ the FP8 tensor cores (W8A8); off by default for the same reason.
 quarter of their bf16 bytes per step); the numbers change, so it is off by default, and it excludes the FP8 flags.
 --quantize_vocab (with --fp8_weights or --int4_weights) also serves the token embeddings and lm_head in that quantized
 form, which frees their memory for the KV cache; the numbers change, so it is off by default.
+--quantized_prefill (with --fp8_weights or --int4_weights) runs long prompts and clips as prefills on the quantized
+layers, with the same numbers as without; it grows the engine's token-row workspaces, so it is off by default.
 
 Loads (or synthesises) a clip, asks for narration at t=0 and runs N iterations of
 (encode 1 frame -> KV-append step -> maybe respond), reporting the reference's

@@ -167,6 +167,9 @@ class LiveArguments:
     # with fp8_weights or int4_weights: also serve embed and lm_head in that quantized form (frees 1.05 GB with FP8 and
     # 1.56 GB with int4 weights at Llama-3-8B); changes the model's numbers, so off by default
     quantize_vocab: bool = False
+    # with fp8_weights or int4_weights: prefill long single-stream inputs on the quantized layers too, with the bits of
+    # max_step_tokens steps; grows the token-row workspaces to 8 x max_step_tokens rows, so off by default
+    quantized_prefill: bool = False
     # LiveInfer.context_window, tokens: keep the start prompt and drop the oldest cache pages after it so the session's
     # cache never exceeds this many tokens; 0: off (the cache grows until max_kv_tokens)
     context_window: int = 0

@@ -498,7 +498,18 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
 int vlo_op_gemm_prefill(int epi, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, int n_ctas, void* d_out,
                         void* cuda_stream) {
   VLO_CHECK(n_ctas >= 0, "gemm_prefill: n_ctas");
-  return gemm_prefill_launch(epi, d_w, rows_w, d_x, rows_x, k, n_ctas, d_out, static_cast<cudaStream_t>(cuda_stream));
+  return gemm_prefill_launch(epi, WeightOperand{FMT_BF16, d_w, nullptr, nullptr}, rows_w, d_x, rows_x, k, n_ctas, d_out,
+                             static_cast<cudaStream_t>(cuda_stream));
+}
+
+int vlo_op_gemm_prefill_q(int fmt, int epi, const void* d_w, const float* d_scale, const void* d_gscale, int rows_w,
+                          const void* d_x, const float* d_xscale, int rows_x, int k, int n_ctas, void* d_out,
+                          void* cuda_stream) {
+  VLO_CHECK(n_ctas >= 0, "gemm_prefill_q: n_ctas");
+  VLO_CHECK(fmt == FMT_E4M3 || fmt == FMT_E4M3_A8 || fmt == FMT_I4, "gemm_prefill_q: fmt 2 (e4m3), 3 (W8A8) or 4 (int4)");
+  VLO_CHECK(d_w != nullptr && d_x != nullptr, "gemm_prefill_q: null operand");
+  return gemm_prefill_launch(epi, WeightOperand{fmt, d_w, d_scale, static_cast<const uint16_t*>(d_gscale)}, rows_w, d_x,
+                             rows_x, k, n_ctas, d_out, static_cast<cudaStream_t>(cuda_stream), nullptr, d_xscale);
 }
 
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,

@@ -159,12 +159,14 @@ int embed_rows_launch(const WeightOperand& table, const long long* ids, int n, i
 int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k, void* out, int ld_out,
                     const float* bias, int act, int n_ctas, cudaStream_t stream);
 
-// ---- prefill GEMM, tokens on wgmma M (gemm_prefill.cuh / gemm.cu): bf16 x [rows_x, k], w [rows_w, k], any rows_x; the
-// k-ranges and plane order of the chunked path's stream-K plan over n_ctas CTAs (<= 0: one per SM).  epi 0: one fp32
-// plane out[rows_x][rows_w] (fill *sk with the one-plane SkInfo its fix-up kernel reads); epi 1: gate|up + SwiGLU into
-// bf16 out[rows_x][rows_w / 2] (rows_w % 128 == 0)
-int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
-                        cudaStream_t stream, SkInfo* sk = nullptr);
+// ---- prefill GEMMs (gemm.cu): weights w [rows_w, k] of format 1-4 by x [rows_x, k], any rows_x; bf16 weights run
+// gemm_prefill_kernel (tokens on wgmma M, gemm_prefill.cuh), the others gemm_prefill_q_kernel (weights on wgmma M,
+// gemm_prefill_q.cuh).  x is bf16, or e4m3 with fp32 token scales a_scale [rows_x] for format 3.  The k-ranges and plane
+// order of the chunked path's stream-K plan over n_ctas CTAs (<= 0: one per SM).  epi 0: one fp32 plane
+// out[rows_x][rows_w] (fill *sk with the one-plane SkInfo its fix-up kernel reads); epi 1: gate|up + SwiGLU into bf16
+// out[rows_x][rows_w / 2] (rows_w % 128 == 0)
+int gemm_prefill_launch(int epi, const WeightOperand& w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
+                        cudaStream_t stream, SkInfo* sk = nullptr, const float* a_scale = nullptr);
 
 // ---- stream-K gate|up GEMM with the fused SwiGLU finisher (gemm_wsf.cuh / gemm.cu), one CTA per SM:
 // act[rows_x][rows_w / 2] = SwiGLU(x w^T) for weights w of format 1-4; x is bf16, or e4m3 with fp32 token scales

@@ -62,6 +62,7 @@ struct vlo_engine {
   int layer_fmt = FMT_BF16;  // GemmFmt of the layer matrices (vlo_finalize_weights; FMT_E4M3_A8 with fp8_act)
   int vocab_fmt = FMT_BF16;  // GemmFmt of embed and lm_head (vlo_finalize_weights): FMT_BF16, FMT_E4M3 or FMT_I4
   bool fp8_act = false;      // vlo_set_fp8_activations: the layer GEMMs take e4m3 activations with token scales
+  bool quant_prefill = false;  // vlo_set_quantized_prefill: quantized layer matrices prefill too
 
   // derived
   int qkv_width = 0, grid = 0, n_patches = 0, n_frame_tokens = 0, patch_k = 0;
@@ -80,7 +81,8 @@ struct vlo_engine {
        *logits = nullptr;
   float* part = nullptr;
   size_t part_elems = 0;
-  // fp8_act only: e4m3 copies of xn, attn_out and act with their fp32 token scales
+  // fp8_act only: e4m3 copies of xn, attn_out and act with their fp32 token scales, act_rows rows
+  int act_rows = 0;
   uint8_t *xq = nullptr, *aq = nullptr, *actq = nullptr;
   float *xs = nullptr, *as = nullptr, *acts = nullptr;
   int* sk_flags = nullptr;          // kSkFlags counters, zero between launches
@@ -106,7 +108,8 @@ struct vlo_engine {
   int last_step_tokens = 0;
   int token_rows = 0;    // rows the token-row workspaces hold (size_token_rows)
   // rows of one vlo_prefill: kFixMaxPlanes x max_step_tokens (one fp32 plane fits `part`) once vlo_finalize_weights has
-  // grown the token-row workspaces of a bf16 engine; 0 before, and on engines with e4m3 layer weights or activations
+  // grown the token-row workspaces of a bf16 engine, or of a quantized one with quant_prefill; 0 before, and on
+  // quantized engines without quant_prefill
   int max_prefill = 0;
 
   // ViT workspaces
@@ -165,8 +168,8 @@ void dev_free(vlo_engine* e, T** p, size_t bytes) {
 }
 
 // The workspaces whose size follows the rows of one pass: h, xn, q, attn_out, act, the attention workspace, the step
-// tables (and with them the layout of every pinned staging slot).  `rows` = max_step_tokens at creation; a bf16 engine
-// grows them to max_prefill rows in vlo_finalize_weights.  Growing frees the old buffers: no work may be in flight.
+// tables (and with them the layout of every pinned staging slot).  `rows` = max_step_tokens at creation; a prefilling
+// engine grows them to max_prefill rows in vlo_finalize_weights.  Growing frees the old buffers: no work may be in flight.
 int size_token_rows(vlo_engine* e, int rows) {
   const vlo_config& c = e->cfg;
   const size_t H = c.hidden_size, A = static_cast<size_t>(c.num_heads) * c.head_dim, I = c.intermediate_size;
@@ -740,19 +743,45 @@ int vlo_engine_destroy(vlo_engine* e) {
 
 int64_t vlo_engine_device_bytes(vlo_engine* e) { return e ? e->device_bytes : 0; }
 
+namespace {
+// The e4m3 copies of xn, attn_out and act and their fp32 token scales, for `rows` token rows (zeroed: vlo_bench_gemm).
+// Growing frees the old buffers: no work may be in flight.
+int size_fp8_act_rows(vlo_engine* e, int rows) {
+  const vlo_config& c = e->cfg;
+  const size_t H = c.hidden_size, A = static_cast<size_t>(c.num_heads) * c.head_dim, I = c.intermediate_size;
+  if (e->xq != nullptr) {
+    const size_t old = e->act_rows;
+    dev_free(e, &e->xq, old * H);
+    dev_free(e, &e->aq, old * A);
+    dev_free(e, &e->actq, old * I);
+    dev_free(e, &e->xs, old * sizeof(float));
+    dev_free(e, &e->as, old * sizeof(float));
+    dev_free(e, &e->acts, old * sizeof(float));
+  }
+  e->act_rows = rows;
+  const size_t T = rows;
+  if (dev_alloc_t(e, &e->xq, T * H, true)) return -1;
+  if (dev_alloc_t(e, &e->aq, T * A, true)) return -1;
+  if (dev_alloc_t(e, &e->actq, T * I, true)) return -1;
+  if (dev_alloc_t(e, &e->xs, T, true) || dev_alloc_t(e, &e->as, T, true) || dev_alloc_t(e, &e->acts, T, true)) return -1;
+  return 0;
+}
+}  // namespace
+
 int vlo_set_fp8_activations(vlo_engine* e, int on) {
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr, "null engine");
   VLO_CHECK(!e->finalized, "set_fp8_activations: the mode is chosen before vlo_finalize_weights");
   e->fp8_act = on != 0;
-  if (e->fp8_act && e->xq == nullptr) {   // the e4m3 activation copies exist only in this mode (zeroed: vlo_bench_gemm)
-    const vlo_config& c = e->cfg;
-    const size_t T = c.max_step_tokens;
-    if (dev_alloc_t(e, &e->xq, T * c.hidden_size, true)) return -1;
-    if (dev_alloc_t(e, &e->aq, T * c.num_heads * c.head_dim, true)) return -1;
-    if (dev_alloc_t(e, &e->actq, T * c.intermediate_size, true)) return -1;
-    if (dev_alloc_t(e, &e->xs, T, true) || dev_alloc_t(e, &e->as, T, true) || dev_alloc_t(e, &e->acts, T, true)) return -1;
-  }
+  // the e4m3 activation copies exist only in this mode
+  if (e->fp8_act && e->xq == nullptr && size_fp8_act_rows(e, e->cfg.max_step_tokens)) return -1;
+  return 0;
+}
+
+int vlo_set_quantized_prefill(vlo_engine* e, int on) {
+  VLO_CHECK(e != nullptr, "null engine");
+  VLO_CHECK(!e->finalized, "set_quantized_prefill: the mode is chosen before vlo_finalize_weights");
+  e->quant_prefill = on != 0;
   return 0;
 }
 
@@ -844,6 +873,9 @@ int vlo_finalize_weights(vlo_engine* e) {
     VLO_CHECK(!e->fp8_act || fmt == FMT_E4M3_A8,
               "fp8_activations needs FP8 (e4m3) layer weights, but the layer matrices are bf16: the FP8 tensor cores "
               "take both operands in e4m3");
+    VLO_CHECK(!e->quant_prefill || fmt != FMT_BF16,
+              "quantized_prefill needs quantized (FP8 or int4) layer matrices, but they are bf16: a bf16 engine always "
+              "prefills");
     // the vocabulary matrices: both bf16, or both in the layer matrices' quantized form (e4m3 on bf16 activations also
     // under fp8_act: the lm_head multiplies the bf16 final-norm rows)
     WeightOperand embed{}, lm_head{};
@@ -902,12 +934,15 @@ int vlo_finalize_weights(vlo_engine* e) {
       if (lookup(e, "vit.head.fc2.w", C * M, &e->head_fc2_w) || lookup(e, "vit.head.fc2.b", C, &e->head_fc2_b)) return -1;
     }
   }
-  // A bf16 engine prefills (vlo_prefill): its token-row workspaces grow once to max_prefill rows.  Engines with e4m3 layer
-  // weights or activations chunk long inputs into steps and keep them at max_step_tokens.
-  if (e->has_decoder && e->layer_fmt == FMT_BF16 && e->max_prefill == 0) {
+  // A bf16 engine prefills (vlo_prefill): its token-row workspaces grow once to max_prefill rows, and so do those of a
+  // quantized engine with quant_prefill (W8A8: with the e4m3 activation copies).  The other quantized engines chunk long
+  // inputs into steps and keep them at max_step_tokens.
+  if (e->has_decoder && (e->layer_fmt == FMT_BF16 || e->quant_prefill) && e->max_prefill == 0) {
     VLO_CUDA(cudaDeviceSynchronize());   // no step, copy or staging slot of this engine may be in flight
-    if (size_token_rows(e, kFixMaxPlanes * c.max_step_tokens)) return -1;
-    e->max_prefill = kFixMaxPlanes * c.max_step_tokens;
+    const int rows = kFixMaxPlanes * c.max_step_tokens;
+    if (size_token_rows(e, rows)) return -1;
+    if (e->fp8_act && size_fp8_act_rows(e, rows)) return -1;
+    e->max_prefill = rows;
   }
   e->finalized = true;
   return 0;
@@ -1352,7 +1387,7 @@ namespace {
 // The decoder step.  Sequence i carries h_seg_counts[i] consecutive segments (h_seg_counts == NULL: one each) whose
 // lengths follow one another in h_seg_lens; one lm_head row and one decision per segment, read at its last row.
 // prefill (vlo_prefill): one sequence of one segment, up to max_prefill rows, whose layer GEMMs run on
-// gemm_prefill_kernel and whose attention plans each max_step_tokens piece as a step of its own: the bits of the same
+// gemm_prefill_kernel (bf16) or gemm_prefill_q_kernel (quantized formats) and whose attention plans each max_step_tokens piece as a step of its own: the bits of the same
 // rows fed as max_step_tokens steps.
 int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const int32_t* h_seg_counts,
                   const int32_t* h_seg_lens, const int64_t* d_row_ids, const void* d_embeds, void* d_last_logits,
@@ -1455,11 +1490,12 @@ int step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, const 
   auto partial = [&](const WeightOperand& w, int n_out, const void* x, int k, GemmWsPlan* sk, const float* x_scale) -> int {
     if (!prefill) return gemm_partial(w, n_out, x, x_scale, T, k, e->part, e->part_elems, WS_TILE_FIT, sk, st);
     VLO_CHECK(static_cast<size_t>(T) * n_out <= e->part_elems, "prefill: the plane exceeds the partial workspace");
-    return gemm_prefill_launch(PREFILL_PLANE, w.w, n_out, x, T, k, 0, e->part, st, &sk->sk);
+    return gemm_prefill_launch(PREFILL_PLANE, w, n_out, x, T, k, 0, e->part, st, &sk->sk, x_scale);
   };
   auto swiglu = [&](const WeightOperand& w) -> int {
     if (!prefill) return gemm_swiglu(e, w, 2 * c.intermediate_size, xn_in, T, H, st, a8 ? e->xs : nullptr);
-    return gemm_prefill_launch(PREFILL_SWIGLU, w.w, 2 * c.intermediate_size, e->xn, T, H, 0, e->act, st);
+    return gemm_prefill_launch(PREFILL_SWIGLU, w, 2 * c.intermediate_size, xn_in, T, H, 0, e->act, st, nullptr,
+                               a8 ? e->xs : nullptr);
   };
 
   if (resid_norm(nullptr, e->dec[0].in_norm, false)) return -1;
@@ -1517,8 +1553,9 @@ int vlo_step_segments(vlo_engine* e, int n_seqs, const int32_t* h_stream_ids, co
 int vlo_prefill(vlo_engine* e, int stream_id, int n_tokens, const int64_t* d_row_ids, const void* d_embeds,
                 void* d_last_logits, vlo_decision* d_decision, int interval_id, void* cuda_stream) {
   VLO_CHECK(e != nullptr && e->finalized && e->has_decoder, "decoder weights not loaded");
-  VLO_CHECK(e->layer_fmt == FMT_BF16 && e->max_prefill > 0,
-            "prefill: bf16 layer weights and activations only (e4m3 engines chunk long inputs into steps)");
+  VLO_CHECK(e->max_prefill > 0,
+            "prefill: quantized layer matrices prefill only with quantized_prefill (vlo_set_quantized_prefill); without "
+            "it long inputs run as max_step_tokens steps");
   VLO_CHECK(n_tokens > 0 && n_tokens <= e->max_prefill,
             "prefill: n_tokens must lie in [1, max_prefill_tokens] = [1, " + std::to_string(e->max_prefill) + "]");
   VLO_CHECK(d_embeds != nullptr, "prefill: null embeddings");

@@ -3,6 +3,7 @@
 // selection, stream-K planning and kernel dispatch.
 #include "gemm.cuh"
 #include "gemm_prefill.cuh"
+#include "gemm_prefill_q.cuh"
 #include "gemm_vit.cuh"
 #include "gemm_ws.cuh"
 #include "gemm_wsf.cuh"
@@ -394,15 +395,43 @@ int gemm_vit_launch(const void* x, int rows_x, const void* w, int rows_w, int k,
 }
 
 // ------------------------------------------------------------------------------------------------
-// prefill GEMM, tokens on wgmma M, with the chunked path's stream-K k-ranges (gemm_prefill.cuh)
+// prefill GEMMs with the chunked path's stream-K k-ranges: bf16 weights with tokens on wgmma M (gemm_prefill.cuh), the
+// quantized formats with weights on wgmma M (gemm_prefill_q.cuh)
 
-int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
-                        cudaStream_t stream, SkInfo* sk) {
+namespace {
+// the quantized instances (gemm_prefill_q.cuh)
+template <int FMT, int EPI>
+int launch_prefill_q(const CUtensorMap& tx, const CUtensorMap& tw, const GemmPrefillQArgs& a, int G, double prof_bytes,
+                     cudaStream_t stream) {
+  using Cfg = GemmPrefillQCfg<FMT, EPI>;
+  auto kern = gemm_prefill_q_kernel<FMT, EPI>;
+  if (ensure_max_smem(reinterpret_cast<const void*>(kern), Cfg::kSmemBytes)) return -1;
+  if (prof_on()) prof_begin(PROF_GEMM_STREAM, stream, prof_bytes);
+  VLO_CUDA(launch_pdl(kern, dim3(G), dim3(kPrefillQThreads), Cfg::kSmemBytes, stream, tx, tw, a));
+  return 0;
+}
+template <int FMT>
+int launch_prefill_q_fmt(int epi, const CUtensorMap& tx, const CUtensorMap& tw, const GemmPrefillQArgs& a, int G,
+                         double prof_bytes, cudaStream_t stream) {
+  return epi == PREFILL_PLANE ? launch_prefill_q<FMT, PREFILL_PLANE>(tx, tw, a, G, prof_bytes, stream)
+                              : launch_prefill_q<FMT, PREFILL_SWIGLU>(tx, tw, a, G, prof_bytes, stream);
+}
+}  // namespace
+
+int gemm_prefill_launch(int epi, const WeightOperand& w, int rows_w, const void* x, int rows_x, int k, int n_ctas, void* out,
+                        cudaStream_t stream, SkInfo* sk, const float* a_scale) {
   VLO_CHECK(k > 0 && k % kGemmBK == 0, "K must be a positive multiple of 64");
   VLO_CHECK(rows_w > 0 && rows_x > 0, "empty GEMM operand");
   VLO_CHECK(epi == PREFILL_PLANE || epi == PREFILL_SWIGLU, "gemm_prefill: unknown epilogue");
   VLO_CHECK(epi != PREFILL_SWIGLU || rows_w % kGemmBM == 0, "gemm_prefill: the SwiGLU epilogue needs whole 128-row tiles");
   VLO_CHECK(out != nullptr, "gemm_prefill: null output");
+  const int fmt = w.fmt;
+  VLO_CHECK(fmt == FMT_BF16 || fmt == FMT_E4M3 || fmt == FMT_E4M3_A8 || fmt == FMT_I4,
+            "gemm_prefill: bf16, e4m3, W8A8 or int4 weights");
+  VLO_CHECK(fmt != FMT_E4M3 && fmt != FMT_E4M3_A8 || w.row_scale != nullptr, "gemm_prefill: e4m3 weights need their row scales");
+  VLO_CHECK(fmt != FMT_E4M3_A8 || a_scale != nullptr, "gemm_prefill: e4m3 activations need their token scales");
+  VLO_CHECK(fmt != FMT_I4 || (w.group_scale != nullptr && k % kI4Group == 0 && (reinterpret_cast<uintptr_t>(w.w) & 15) == 0),
+            "gemm_prefill: int4 weights need their group scales, K a multiple of 128 and 16-byte aligned codes");
   GemmPrefillArgs a{};
   a.rows_x = rows_x;
   a.rows_w = rows_w;
@@ -418,15 +447,22 @@ int gemm_prefill_launch(int epi, const void* w, int rows_w, const void* x, int r
   if (sk) *sk = SkInfo{a.sk.U, a.sk.kb, 1};      // G = 1: every tile has one plane
   const int G = std::min(num_sms(), a.tiles);
   CUtensorMap tx, tw;
-  if (get_tmap(x, rows_x, k, kGemmBM, FMT_BF16, &tx) != 0) return -1;
-  if (get_tmap(w, rows_w, k, kGemmBM, FMT_BF16, &tw) != 0) return -1;
-  auto kern = epi == PREFILL_PLANE ? gemm_prefill_kernel<PREFILL_PLANE> : gemm_prefill_kernel<PREFILL_SWIGLU>;
-  if (ensure_max_smem(reinterpret_cast<const void*>(kern), GemmPrefillCfg::kSmemBytes)) return -1;
-  if (prof_on()) {
-    const double out_b = epi == PREFILL_PLANE ? 4.0 * rows_x * rows_w : 1.0 * rows_x * rows_w;
-    prof_begin(PROF_GEMM_STREAM, stream, 2.0 * k * (static_cast<double>(rows_w) + rows_x) + out_b);
+  if (get_tmap(x, rows_x, k, kGemmBM, kWsFmtInfo[fmt].x_map, &tx) != 0) return -1;
+  if (fmt != FMT_I4 && get_tmap(w.w, rows_w, k, kGemmBM, kWsFmtInfo[fmt].w_map, &tw) != 0) return -1;
+  if (fmt == FMT_I4) tw = tx;   // unused: the codes stream as bulk copies
+  const double prof_bytes = ws_in_bytes(fmt, rows_w, rows_x, k) + (epi == PREFILL_PLANE ? 4.0 : 1.0) * rows_x * rows_w;
+  if (fmt == FMT_BF16) {
+    auto kern = epi == PREFILL_PLANE ? gemm_prefill_kernel<PREFILL_PLANE> : gemm_prefill_kernel<PREFILL_SWIGLU>;
+    if (ensure_max_smem(reinterpret_cast<const void*>(kern), GemmPrefillCfg::kSmemBytes)) return -1;
+    if (prof_on()) prof_begin(PROF_GEMM_STREAM, stream, prof_bytes);
+    VLO_CUDA(launch_pdl(kern, dim3(G), dim3(kPrefillThreads), GemmPrefillCfg::kSmemBytes, stream, tx, tw, a));
+  } else {
+    const GemmPrefillQArgs qa{a, WsWeightArgs{w.row_scale, a_scale, static_cast<const uint8_t*>(w.w), w.group_scale}};
+    const int rc = fmt == FMT_E4M3      ? launch_prefill_q_fmt<FMT_E4M3>(epi, tx, tw, qa, G, prof_bytes, stream)
+                   : fmt == FMT_E4M3_A8 ? launch_prefill_q_fmt<FMT_E4M3_A8>(epi, tx, tw, qa, G, prof_bytes, stream)
+                                        : launch_prefill_q_fmt<FMT_I4>(epi, tx, tw, qa, G, prof_bytes, stream);
+    if (rc) return -1;
   }
-  VLO_CUDA(launch_pdl(kern, dim3(G), dim3(kPrefillThreads), GemmPrefillCfg::kSmemBytes, stream, tx, tw, a));
   prof_end(stream);
   count_launch();
   return 0;

@@ -234,12 +234,15 @@ class SampleRow:
 class Engine:
     def __init__(self, cfg: LiveConfig, device: str | torch.device = "cuda:0", *, max_streams: int = 1,
                  max_kv_tokens: int = 16384, max_step_tokens: int = 128, max_vit_batch: int = 8,
-                 kv_pool_tokens: Optional[int] = None, fp8_activations: bool = False):
+                 kv_pool_tokens: Optional[int] = None, fp8_activations: bool = False, quantized_prefill: bool = False):
         """kv_pool_tokens: size of the KV page pool all streams share (rounded up to 64-token pages); None reserves
         max_streams * max_kv_tokens, so every stream can reach max_kv_tokens at once.  A smaller pool over-subscribes:
         a step that needs more pages than are free raises VloError and leaves every stream as it was.
         fp8_activations: the layer GEMMs quantize their activations to e4m3 per token and multiply on the FP8 tensor
-        cores (W8A8, vlo_set_fp8_activations); load_weights then needs FP8 layer weights."""
+        cores (W8A8, vlo_set_fp8_activations); load_weights then needs FP8 layer weights.
+        quantized_prefill: an engine with quantized layer matrices (FP8 weights, W8A8 or int4) prefills long inputs too
+        (vlo_set_quantized_prefill), at the cost of token-row workspaces of max_prefill_tokens rows; load_weights then
+        needs quantized layer weights."""
         self.lib = _lib.load()
         self.cfg = cfg
         self.device = torch.device(device)
@@ -271,6 +274,8 @@ class Engine:
             self._fp8_act = bool(fp8_activations)
             if self._fp8_act:
                 check(self.lib.vlo_set_fp8_activations(self._h, 1), "vlo_set_fp8_activations")
+            if quantized_prefill:
+                check(self.lib.vlo_set_quantized_prefill(self._h, 1), "vlo_set_quantized_prefill")
         # device scratch for results (decisions, last logits): one row per sequence, or per segment of a segmented step
         # and the sampled ids right behind the decisions, so that one copy brings both back
         rows = max(max_streams, max_step_tokens)
@@ -336,15 +341,16 @@ class Engine:
 
     @property
     def max_prefill_tokens(self) -> int:
-        """rows of one vlo_prefill (8 x max_step_tokens) once bf16 layer weights are loaded; 0 before, and on engines
-        with e4m3 layer weights or activations"""
+        """rows of one vlo_prefill (8 x max_step_tokens) once bf16 layer weights are loaded, or quantized ones on an
+        Engine(quantized_prefill=True); 0 before, and on quantized engines without quantized_prefill"""
         return int(self.lib.vlo_max_prefill_tokens(self._h))
 
     @property
     def prefills(self) -> bool:
-        """True when one stream's input longer than max_step_tokens runs as a prefill (vlo_prefill: tokens-on-M tensor-core
-        GEMMs over up to max_prefill_tokens rows per call, with the bits of max_step_tokens steps).  Engines with e4m3
-        layer weights or activations chunk such inputs into steps instead."""
+        """True when one stream's input longer than max_step_tokens runs as a prefill (vlo_prefill: tensor-core GEMMs
+        over up to max_prefill_tokens rows per call, with the bits of max_step_tokens steps on the same engine): bf16
+        engines, and quantized ones built with quantized_prefill.  The other quantized engines chunk such inputs into
+        steps instead."""
         return self.max_prefill_tokens > 0
 
     @property
@@ -717,7 +723,7 @@ class Engine:
         return logits, self._dec_dev[:n_rows]
 
     def _prefill(self, sid, T, embeds, row_ids, interval_id, want_logits):
-        """One stream's input longer than max_step_tokens on a bf16 engine: vlo_prefill calls of up to max_prefill_tokens
+        """One stream's input longer than max_step_tokens on a prefilling engine: vlo_prefill calls of up to max_prefill_tokens
         rows, each giving the bits of the same rows fed as max_step_tokens steps.  The logits / decision come from the
         last call; if a later call fails (e.g. on an exhausted KV page pool), the earlier ones are taken back, so the
         call changes nothing and the caller can retry it whole."""
@@ -738,8 +744,8 @@ class Engine:
         return logits, self._dec_dev[:1]
 
     def _step_chunked(self, stream_ids, q_lens, embeds, row_ids, interval_id, want_logits):
-        """Ragged multi-stream inputs longer than max_step_tokens, and long inputs on engines that do not prefill (e4m3
-        layer weights): feed the KV-append forward in pieces — chunked streaming is exactly one causal pass (SURVEY.md
+        """Ragged multi-stream inputs longer than max_step_tokens, and long inputs on engines that do not prefill (quantized
+        layer matrices without quantized_prefill): feed the KV-append forward in pieces — chunked streaming is exactly one causal pass (SURVEY.md
         Appendix C.1).  Each sequence's logits / decision come from the sub-step that holds its last piece."""
         n, cap, H = len(stream_ids), self.max_step_tokens, self.cfg.hidden_size
         if row_ids is not None:  # materialise the gathered token rows once; the sub-steps then see plain embeddings

@@ -301,7 +301,8 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
                synthetic_weights: bool = False, seed: int = 0, max_streams: int = 1, max_kv_tokens: int = 16384,
                max_step_tokens: int = 128, max_vit_batch: int = 8, llm_state=None, vision_state=None,
                lora_r: int = 128, lora_alpha: int = 256, kv_pool_tokens: Optional[int] = None, fp8_weights: bool = False,
-               fp8_activations: bool = False, int4_weights: bool = False, quantize_vocab: bool = False, **kwargs):
+               fp8_activations: bool = False, int4_weights: bool = False, quantize_vocab: bool = False,
+               quantized_prefill: bool = False, **kwargs):
     """models/modeling_live.py:184-222 for inference: build config + tokenizer, load (or synthesise)
     weights, merge LoRA, hand everything to the engine.  kv_pool_tokens: size of the KV page pool the streams
     share (None or <= 0: max_streams * max_kv_tokens).  fp8_weights: quantize the decoder layer matrices to e4m3 with
@@ -310,7 +311,10 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
     the FP8 tensor cores (W8A8).  int4_weights: quantize the layer matrices to 4-bit codes with one bf16 scale per 128
     weights of a row (weights.quantize_int4_groups, W4A16); the engine computes the bits of a bf16 engine on the
     dequantized weights.  It excludes fp8_weights and fp8_activations.  quantize_vocab (needs fp8_weights or
-    int4_weights): embed and lm_head take the layer matrices' quantized form too (weights.pack_llm_for_engine)."""
+    int4_weights): embed and lm_head take the layer matrices' quantized form too (weights.pack_llm_for_engine).
+    quantized_prefill (needs fp8_weights or int4_weights): long single-stream inputs run as prefills on the quantized
+    layers too (Engine(quantized_prefill=True)), with the bits of max_step_tokens steps; it grows the engine's token-row
+    workspaces to max_prefill_tokens rows."""
     if is_training:
         raise NotImplementedError("the vlo_b200 engine covers the streaming-inference path only")
     if int4_weights and (fp8_weights or fp8_activations):
@@ -321,6 +325,8 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
     if quantize_vocab and not (fp8_weights or int4_weights):
         raise ValueError("quantize_vocab needs fp8_weights or int4_weights: the vocabulary matrices take the layer "
                          "matrices' quantized form")
+    if quantized_prefill and not (fp8_weights or int4_weights):
+        raise ValueError("quantized_prefill needs fp8_weights or int4_weights: a bf16 engine always prefills")
     cfg = config or llama3_8b_siglip_l()
     for k in ("frame_resolution", "frame_token_cls", "frame_token_pooled", "frame_num_tokens", "frame_token_interval",
               "vision_pretrained"):
@@ -329,7 +335,7 @@ def build_live(*, is_training: bool = False, config: Optional[LiveConfig] = None
     tokenizer = build_live_tokenizer_and_update_config(llm_pretrained or "", cfg)
     engine = Engine(cfg, device, max_streams=max_streams, max_kv_tokens=max_kv_tokens,
                     max_step_tokens=max_step_tokens, max_vit_batch=max_vit_batch, kv_pool_tokens=kv_pool_tokens,
-                    fp8_activations=fp8_activations)
+                    fp8_activations=fp8_activations, quantized_prefill=quantized_prefill)
     if llm_state is not None:
         packed = W.pack_llm_for_engine(cfg, llm_state, engine.device, max_kv_tokens, fp8_weights=fp8_weights,
                                        int4_weights=int4_weights, quantize_vocab=quantize_vocab)
