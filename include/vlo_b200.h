@@ -618,6 +618,25 @@ int vlo_op_attn_bench(const void* d_q, const void* d_k, const void* d_v, void* d
                       int n_kv_heads, int head_dim, int kv_len, long long kv_stride, int n_layers,
                       long long layer_stride_rows, int iters, int skip_merge, double* h_algo_bytes, void* cuda_stream);
 
+/* Test hooks for the PDL contract (csrc/ptx.cuh): before its grid dependency resolves, a kernel reads nothing an
+ * earlier kernel of the step writes and writes nothing to global memory.
+ * vlo_op_pdl_arm arms a one-shot probe.  Every vlo_op_* entry above that launches a PDL kernel, and vlo_letterbox /
+ * vlo_letterbox_planes, launch the armed probe on their stream right before their first PDL launch (after their own
+ * table uploads) and disarm it.  The probe kernel runs on a few CTAs, lets its dependents launch at once, spins on the
+ * global timer for spin_ns (0 < spin_ns <= 2 ms), then copies n_chunks chunks of `bytes` bytes, chunk i at byte offset
+ * i * chunk_stride of both pointers: mode VLO_PDL_LATE_WRITE src -> dst (the operand arrives after the kernel under test
+ * has started); VLO_PDL_LATE_READ exchanges them: src receives a snapshot of what that kernel had written to dst by
+ * then, dst what src held (so a region can hold a marker before the launch and the values the kernel expects after
+ * its wait, e.g. zero arrival counters).  Ranges must not overlap.  vlo_op_pdl_probe_count: probes that ran to completion (synchronises the device); -1 on error. */
+enum { VLO_PDL_LATE_WRITE = 1, VLO_PDL_LATE_READ = 2 };
+int vlo_op_pdl_arm(int mode, void* d_dst, void* d_src, long long bytes, int n_chunks, long long chunk_stride,
+                   long long spin_ns);
+long long vlo_op_pdl_probe_count(void);
+/* A PDL canary through the product's launch helper: n_words 32-bit words d_src -> d_dst.  variant 0 waits for the grid
+ * dependency, then copies; 1 reads d_src before the wait (a read violation); 2 writes d_dst before the wait (a write
+ * violation).  Asynchronous. */
+int vlo_op_pdl_canary(int variant, const void* d_src, void* d_dst, int n_words, void* cuda_stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -154,7 +154,13 @@ SIGNATURES = {
     "vlo_op_decision": (_I, [_P, _I, _I, _I, _P, _P]),
     "vlo_op_sample": (_I, [_P, _I, _I, C.POINTER(VloSampleRow), _P, _I, _P, _P, _P]),
     "vlo_op_attn_bench": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _LL, _I, _LL, _I, _I, C.POINTER(C.c_double), _P]),
+    "vlo_op_pdl_arm": (_I, [_I, _P, _P, _LL, _I, _LL, _LL]),
+    "vlo_op_pdl_probe_count": (_LL, []),
+    "vlo_op_pdl_canary": (_I, [_I, _P, _P, _I, _P]),
 }
+
+# vlo_op_pdl_arm modes (include/vlo_b200.h)
+PDL_LATE_WRITE, PDL_LATE_READ = 1, 2
 
 _lock = threading.Lock()
 _lib = None

@@ -85,6 +85,7 @@ int op_gemm_ws_partials(const WeightOperand& w, int rows_w, const void* d_x, con
   c.plane_stride = plane_stride;
   c.n_ctas = n_ctas;
   GemmWsPlan plan{};
+  if (d_out != nullptr && pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
   if (rc == 0 && h_max_planes) *h_max_planes = plan.planes;
   return rc;
@@ -97,7 +98,74 @@ struct OpScratch {
   }
 };
 
+// ---- the PDL-contract probe and canary (vlo_op_pdl_arm, vlo_op_pdl_canary): test hooks, not used by the engine
+struct PdlProbe {
+  int mode = 0;   // 0: not armed
+  uint8_t* dst = nullptr;
+  uint8_t* src = nullptr;
+  long long bytes = 0, stride = 0, spin_ns = 0;
+  int n_chunks = 0;
+};
+PdlProbe g_probe;
+constexpr int kProbeCtas = 4;   // a few CTAs: the kernel under test becomes resident on the other SMs
+constexpr long long kProbeMaxSpinNs = 2000000;
+__device__ unsigned long long g_probes_done;
+
+// Lets its dependents launch, spins on the global timer (nothing else is waited for), then copies the chunks src -> dst,
+// or late_read: exchanges them.
+__global__ void __launch_bounds__(256) pdl_probe_kernel(int late_read, uint8_t* dst, uint8_t* src, long long bytes,
+                                                        int n_chunks, long long stride, long long spin_ns) {
+  pdl_trigger();
+  const unsigned long long t0 = globaltimer_ns();
+  while (globaltimer_ns() - t0 < static_cast<unsigned long long>(spin_ns)) {
+  }
+  const long long tid = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const long long nth = static_cast<long long>(gridDim.x) * blockDim.x;
+  const bool vec = ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src) | bytes | stride) & 15) == 0;
+  for (int c = 0; c < n_chunks; ++c) {
+    uint8_t* d = dst + c * stride;
+    uint8_t* s = src + c * stride;
+    if (vec) {
+      uint4* d4 = reinterpret_cast<uint4*>(d);
+      uint4* s4 = reinterpret_cast<uint4*>(s);
+      for (long long i = tid; i < bytes / 16; i += nth) {
+        const uint4 v = s4[i];
+        if (late_read) s4[i] = d4[i];
+        d4[i] = v;
+      }
+    } else {
+      for (long long i = tid; i < bytes; i += nth) {
+        const uint8_t v = s[i];
+        if (late_read) s[i] = d[i];
+        d[i] = v;
+      }
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&g_probes_done, 1ull);
+}
+
+__global__ void __launch_bounds__(256) pdl_canary_kernel(int variant, const uint32_t* src, uint32_t* dst, int n) {
+  pdl_trigger();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  uint32_t early = 0;
+  if (i < n && variant == 1) early = src[i];   // seeded read violation
+  if (i < n && variant == 2) dst[i] = src[i];  // seeded write violation
+  pdl_wait();
+  if (i < n && variant == 0) dst[i] = src[i];
+  if (i < n && variant == 1) dst[i] = early;
+}
+
 }  // namespace
+
+int vlo::pdl_probe_fire(cudaStream_t st) {
+  if (g_probe.mode == 0) return 0;
+  const PdlProbe p = g_probe;
+  g_probe = PdlProbe{};
+  pdl_probe_kernel<<<kProbeCtas, 256, 0, st>>>(p.mode == VLO_PDL_LATE_READ, p.dst, p.src, p.bytes, p.n_chunks, p.stride,
+                                                p.spin_ns);
+  VLO_LAUNCH_CHECK();
+  return 0;
+}
 
 extern "C" {
 
@@ -138,6 +206,7 @@ int vlo_op_gemm(int epi, int act, const void* d_x, int rows_x, const void* d_w, 
   c.pos = d_pos;
   c.pos_rows = pos_rows;
   c.bn = bn > 0 ? bn : 128;
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_launch(c, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -172,6 +241,7 @@ int vlo_op_gemm_ws_tiled(int fmt, int mode, const void* d_w, int rows_w, const v
   c.bn = bn;
   c.tiling = tiling;
   GemmWsPlan plan{};
+  if (d_out != nullptr && pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
   if (rc == 0 && h_plan) {
     h_plan[0] = plan.bn;
@@ -212,6 +282,7 @@ int vlo_op_gemm_ws_tiles_q(int fmt, const void* d_w, const void* d_scale, int ro
   c.ld_out = ld_out;
   c.n_ctas = n_ctas;
   GemmWsPlan plan{};
+  if (d_out != nullptr && pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   const int rc = gemm_ws_launch(c, static_cast<cudaStream_t>(cuda_stream), &plan);
   if (rc == 0 && h_plan) {
     h_plan[0] = plan.bn;
@@ -243,6 +314,7 @@ int vlo_op_gemm_ws_a8(const void* d_w8, const float* d_scale, int rows_w, const 
 
 int vlo_op_gemm_vit(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_out, int ld_out,
                     const float* d_bias, int act, int n_ctas, void* cuda_stream) {
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_vit_launch(d_x, rows_x, d_w, rows_w, k, d_out, ld_out, d_bias, act, n_ctas, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -261,6 +333,7 @@ int vlo_op_attn_kvappend(const void* d_q, const void* d_k, const void* d_v, void
   AttnPlan plan{};
   const int* pt = nullptr;
   if (op_attn_plan(&plan, d_ws, n_tok, n_heads, n_kv_heads, head_dim, kv_len, true, &pt, st)) return -1;
+  if (pdl_probe_fire(st)) return -1;
   if (attn_run(plan, d_q, d_k, d_v, static_cast<long long>(n_kv_heads) * kv_stride, pt, kKvPageTokens, kv_stride, d_out,
                n_heads, n_kv_heads, head_dim, st))
     return -1;
@@ -275,6 +348,7 @@ int vlo_op_attn_kvappend_paged(const void* d_q, const void* d_k_pool, const void
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   AttnPlan plan{};
   if (op_attn_plan(&plan, d_ws, n_tok, n_heads, n_kv_heads, head_dim, kv_len, false, nullptr, st)) return -1;
+  if (pdl_probe_fire(st)) return -1;
   const long long page_rows = static_cast<long long>(n_kv_heads) * kKvPageTokens;
   if (attn_run(plan, d_q, d_k_pool, d_v_pool, n_pages * page_rows, d_page_table, page_rows, kKvPageTokens, d_out, n_heads,
                n_kv_heads, head_dim, st))
@@ -299,6 +373,7 @@ int vlo_op_attn_kvappend_segments(const void* d_q, const void* d_k_pool, const v
   AttnPlan plan{};
   if (op_attn_plan(&plan, ws.p, n_tok, n_heads, n_kv_heads, head_dim, kv_len, false, nullptr, st, n_segs, h_seg_lens))
     return -1;
+  if (pdl_probe_fire(st)) return -1;
   const long long page_rows = static_cast<long long>(n_kv_heads) * kKvPageTokens;
   if (attn_run(plan, d_q, d_k_pool, d_v_pool, n_pages * page_rows, d_page_table, page_rows, kKvPageTokens, d_out, n_heads,
                n_kv_heads, head_dim, st))
@@ -328,6 +403,7 @@ int vlo_op_attn_plan_counts(int n_segs, const int32_t* h_seg_lens, int n_heads, 
 
 int vlo_op_vit_attn(const void* d_qkv, void* d_out, int n_frames, int n_tok, int hidden, void* cuda_stream) {
   VLO_CHECK(d_qkv != nullptr && d_out != nullptr, "vit_attn: null argument");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return vit_attn_launch(d_qkv, d_out, n_frames, n_tok, hidden, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -387,6 +463,7 @@ int vlo_op_patchify(const uint8_t* d_frames, int n_frames, int image_size, int p
             "patchify: n_frames > 0, patch_size a multiple of 8 dividing image_size");
   VLO_CHECK((reinterpret_cast<uintptr_t>(d_frames) & 7) == 0 && (reinterpret_cast<uintptr_t>(d_out) & 15) == 0,
             "patchify: frames 8-byte and patches 16-byte aligned");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return patchify_launch(d_frames, d_out, n_frames, image_size, patch_size, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -396,6 +473,7 @@ int vlo_op_vit_layernorm(const void* d_in, int in_is_f16, int rows, int C, const
             "vit_layernorm: null argument");
   // the row is staged in shared memory without an opt-in beyond the default 48 KB
   VLO_CHECK(rows > 0 && C > 0 && C * sizeof(float) <= 48 * 1024, "vit_layernorm: rows > 0, 0 < C <= 12288");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return vit_layernorm_launch(d_in, in_is_f16 != 0, rows, C, d_w, d_b, d_out16, d_out32, eps,
                               static_cast<cudaStream_t>(cuda_stream));
 }
@@ -423,6 +501,7 @@ int vlo_op_vit_fix_ln(const float* d_part, int rows, int C, int k, int bn, int n
   if (gemm_ws_launch(c, nullptr, &plan)) return -1;
   VLO_CHECK(plan.planes <= kFixMaxPlanes, "the plan needs " + std::to_string(plan.planes) +
                                               " partial planes, more than the fix-up kernels unroll");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return vit_fix_ln_launch(d_part, plan, rows, C, d_bias, d_h, d_ln_w, d_ln_b, d_out16, d_out32, eps,
                            static_cast<cudaStream_t>(cuda_stream));
 }
@@ -450,6 +529,7 @@ int vlo_op_resid_rmsnorm(const float* d_part, int k, int n_ctas, void* d_h, cons
   VLO_CHECK(d_last_index == nullptr || d_xn_last != nullptr, "resid_rmsnorm: last_index without xn_last");
   SkInfo sk{};
   if (d_part != nullptr && op_fix_plan(H, T, k, n_ctas, &sk)) return -1;
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return resid_rmsnorm_launch(d_part, &sk, d_h, d_w, d_xn, d_xn_last, d_last_index, T, H, eps,
                               static_cast<cudaStream_t>(cuda_stream));
 }
@@ -461,12 +541,14 @@ int vlo_op_resid_rmsnorm_q8(const float* d_part, int k, int n_ctas, void* d_h, c
   VLO_CHECK(d_xn != nullptr && d_xq != nullptr && d_xs != nullptr, "resid_rmsnorm_q8: null xn, xq or xs");
   SkInfo sk{};
   if (d_part != nullptr && op_fix_plan(H, T, k, n_ctas, &sk)) return -1;
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return resid_rmsnorm_q8_launch(d_part, &sk, d_h, d_w, d_xn, d_xn_last, d_last_index, static_cast<uint8_t*>(d_xq), d_xs, T,
                                  H, eps, static_cast<cudaStream_t>(cuda_stream));
 }
 
 int vlo_op_quant_rows_e4m3(const void* d_x, int T, int K, void* d_q, float* d_s, void* cuda_stream) {
   VLO_CHECK(d_x != nullptr && d_q != nullptr && d_s != nullptr, "quant_rows_e4m3: null argument");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return quant_rows_launch(d_x, T, K, static_cast<uint8_t*>(d_q), d_s, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -489,6 +571,7 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
   long long* d_kvrow = reinterpret_cast<long long*>(static_cast<uint8_t*>(tables.p) + pos_bytes);
   VLO_CUDA(cudaMemcpyAsync(d_pos, h_tok_pos, sizeof(int) * T, cudaMemcpyHostToDevice, st));
   VLO_CUDA(cudaMemcpyAsync(d_kvrow, h_tok_kvrow, sizeof(long long) * T, cudaMemcpyHostToDevice, st));
+  if (pdl_probe_fire(st)) return -1;  // after the table uploads, which serialise the stream
   if (qkv_rope_launch(d_part, sk, d_cos, d_sin, d_pos, d_kvrow, kv_head_stride, d_q, d_k, d_v, T, n_heads, n_kv_heads, st))
     return -1;
   VLO_CUDA(cudaStreamSynchronize(st));  // the tables are freed on return
@@ -498,6 +581,7 @@ int vlo_op_qkv_rope_append(const float* d_part, int k, int n_ctas, const void* d
 int vlo_op_gemm_prefill(int epi, const void* d_w, int rows_w, const void* d_x, int rows_x, int k, int n_ctas, void* d_out,
                         void* cuda_stream) {
   VLO_CHECK(n_ctas >= 0, "gemm_prefill: n_ctas");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_prefill_launch(epi, WeightOperand{FMT_BF16, d_w, nullptr, nullptr}, rows_w, d_x, rows_x, k, n_ctas, d_out,
                              static_cast<cudaStream_t>(cuda_stream));
 }
@@ -508,6 +592,7 @@ int vlo_op_gemm_prefill_q(int fmt, int epi, const void* d_w, const float* d_scal
   VLO_CHECK(n_ctas >= 0, "gemm_prefill_q: n_ctas");
   VLO_CHECK(fmt == FMT_E4M3 || fmt == FMT_E4M3_A8 || fmt == FMT_I4, "gemm_prefill_q: fmt 2 (e4m3), 3 (W8A8) or 4 (int4)");
   VLO_CHECK(d_w != nullptr && d_x != nullptr, "gemm_prefill_q: null operand");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_prefill_launch(epi, WeightOperand{fmt, d_w, d_scale, static_cast<const uint16_t*>(d_gscale)}, rows_w, d_x,
                              rows_x, k, n_ctas, d_out, static_cast<cudaStream_t>(cuda_stream), nullptr, d_xscale);
 }
@@ -515,6 +600,7 @@ int vlo_op_gemm_prefill_q(int fmt, int epi, const void* d_w, const float* d_scal
 int vlo_op_gemm_swiglu(const void* d_w, int rows_w, const void* d_x, int rows_x, int k, void* d_act, float* d_planes,
                        int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu: plane_elems");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_wsf_launch(WeightOperand{FMT_BF16, d_w, nullptr, nullptr}, rows_w, d_x, rows_x, k, d_act, d_planes,
                          static_cast<size_t>(plane_elems), d_flags, n_flags, static_cast<cudaStream_t>(cuda_stream));
 }
@@ -523,6 +609,7 @@ int vlo_op_gemm_swiglu_f8(const void* d_w8, const float* d_scale, int rows_w, co
                           float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu_f8: plane_elems");
   VLO_CHECK(d_scale != nullptr, "gemm_swiglu_f8: null row scales");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_wsf_launch(WeightOperand{FMT_E4M3, d_w8, d_scale, nullptr}, rows_w, d_x, rows_x, k, d_act, d_planes,
                          static_cast<size_t>(plane_elems), d_flags, n_flags, static_cast<cudaStream_t>(cuda_stream));
 }
@@ -532,6 +619,7 @@ int vlo_op_gemm_swiglu_a8(const void* d_w8, const float* d_scale, int rows_w, co
                           void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu_a8: plane_elems");
   VLO_CHECK(d_scale != nullptr && d_xscale != nullptr, "gemm_swiglu_a8: null row or token scales");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_wsf_launch(WeightOperand{FMT_E4M3_A8, d_w8, d_scale, nullptr}, rows_w, d_x8, rows_x, k, d_act, d_planes,
                          static_cast<size_t>(plane_elems), d_flags, n_flags, static_cast<cudaStream_t>(cuda_stream), d_xscale);
 }
@@ -540,6 +628,7 @@ int vlo_op_gemm_swiglu_i4(const void* d_w4, const void* d_gscale, int rows_w, co
                           float* d_planes, int64_t plane_elems, int32_t* d_flags, int n_flags, void* cuda_stream) {
   VLO_CHECK(plane_elems >= 0, "gemm_swiglu_i4: plane_elems");
   VLO_CHECK(d_gscale != nullptr, "gemm_swiglu_i4: null group scales");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return gemm_wsf_launch(WeightOperand{FMT_I4, d_w4, nullptr, static_cast<const uint16_t*>(d_gscale)}, rows_w, d_x, rows_x,
                          k, d_act, d_planes, static_cast<size_t>(plane_elems), d_flags, n_flags,
                          static_cast<cudaStream_t>(cuda_stream));
@@ -548,6 +637,7 @@ int vlo_op_gemm_swiglu_i4(const void* d_w4, const void* d_gscale, int rows_w, co
 int vlo_op_decision(const void* d_logits, int n_rows, int vocab, int interval_id, vlo_decision* d_out, void* cuda_stream) {
   VLO_CHECK(n_rows > 0 && vocab > 0 && vocab % 8 == 0, "decision: rows of a positive multiple of 8 logits");
   VLO_CHECK((reinterpret_cast<uintptr_t>(d_logits) & 15) == 0, "decision: logits must be 16-byte aligned");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return decision_launch(d_logits, n_rows, vocab, interval_id, d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -567,6 +657,7 @@ int vlo_op_sample(const void* d_logits, int n_rows, int vocab, const vlo_sample_
                                         cudaMemcpyHostToDevice) != cudaSuccess)
                ? fail("sample: parameter upload failed")
                : 0;
+  if (rc == 0) rc = pdl_probe_fire(st);
   if (rc == 0) rc = sample_launch(d_logits, n_rows, vocab, d_par, reinterpret_cast<const int*>(d_par + rows_bytes),
                                   d_out_ids, d_info, st);
   if (rc == 0 && cudaStreamSynchronize(st) != cudaSuccess) rc = fail("sample: kernel failed");
@@ -588,12 +679,42 @@ int vlo_op_attn_bench(const void* d_q, const void* d_k, const void* d_v, void* d
   plan.skip_merge = skip_merge;
   if (h_algo_bytes) *h_algo_bytes = plan.algo_bytes;
   const size_t lstride = static_cast<size_t>(layer_stride_rows) * head_dim * 2;
+  if (pdl_probe_fire(st)) return -1;
   for (int it = 0; it < iters; ++it)
     for (int l = 0; l < n_layers; ++l)
       if (attn_run(plan, d_q, static_cast<const uint8_t*>(d_k) + l * lstride, static_cast<const uint8_t*>(d_v) + l * lstride,
                    static_cast<long long>(n_kv_heads) * kv_stride, pt, kKvPageTokens, kv_stride, d_out, n_heads,
                    n_kv_heads, head_dim, st))
         return -1;
+  return 0;
+}
+
+int vlo_op_pdl_arm(int mode, void* d_dst, void* d_src, long long bytes, int n_chunks, long long chunk_stride,
+                   long long spin_ns) {
+  VLO_CHECK(mode == VLO_PDL_LATE_WRITE || mode == VLO_PDL_LATE_READ, "pdl_arm: mode 1 (late write) or 2 (late read)");
+  VLO_CHECK(d_dst != nullptr && d_src != nullptr && bytes > 0 && n_chunks > 0, "pdl_arm: null pointer or empty range");
+  VLO_CHECK(n_chunks == 1 || chunk_stride >= bytes, "pdl_arm: chunks must not overlap");
+  VLO_CHECK(spin_ns > 0 && spin_ns <= kProbeMaxSpinNs, "pdl_arm: spin_ns must lie in (0, 2 ms]");
+  g_probe = PdlProbe{mode, static_cast<uint8_t*>(d_dst), static_cast<uint8_t*>(d_src), bytes, chunk_stride, spin_ns,
+                     n_chunks};
+  return 0;
+}
+
+long long vlo_op_pdl_probe_count(void) {
+  unsigned long long n = 0;
+  if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(&n, g_probes_done, sizeof(n)) != cudaSuccess) {
+    fail("pdl_probe_count: " + std::string(cudaGetErrorString(cudaGetLastError())));
+    return -1;
+  }
+  return static_cast<long long>(n);
+}
+
+int vlo_op_pdl_canary(int variant, const void* d_src, void* d_dst, int n_words, void* cuda_stream) {
+  VLO_CHECK(variant >= 0 && variant <= 2 && d_src != nullptr && d_dst != nullptr && n_words > 0, "pdl_canary: arguments");
+  cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+  if (pdl_probe_fire(st)) return -1;
+  VLO_CUDA(launch_pdl(pdl_canary_kernel, dim3((n_words + 255) / 256), dim3(256), 0, st, variant,
+                      static_cast<const uint32_t*>(d_src), static_cast<uint32_t*>(d_dst), n_words));
   return 0;
 }
 

@@ -55,6 +55,9 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
+// Test hook (vlo_op_pdl_arm, capi_ops.cu): launch the armed probe on st and disarm it; nothing when no probe is armed.
+// Entry points call it right before their first PDL launch.
+int pdl_probe_fire(cudaStream_t st);
 
 inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 

@@ -1363,6 +1363,7 @@ int vlo_letterbox(vlo_engine* e, const vlo_letterbox_frame* h_frames, int n_fram
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr, "null engine");
   VLO_CHECK(n_frames > 0 && n_frames <= e->cfg.max_vit_batch, "letterbox: n_frames must lie in [1, max_vit_batch]");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return letterbox_launch(h_frames, n_frames, e->cfg.image_size, d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
@@ -1370,6 +1371,7 @@ int vlo_letterbox_planes(vlo_engine* e, const vlo_frame_planes* h_frames, int n_
   DevGuard dev_guard(e);
   VLO_CHECK(e != nullptr, "null engine");
   VLO_CHECK(n_frames > 0 && n_frames <= e->cfg.max_vit_batch, "letterbox: n_frames must lie in [1, max_vit_batch]");
+  if (pdl_probe_fire(static_cast<cudaStream_t>(cuda_stream))) return -1;
   return letterbox_planes_launch(h_frames, n_frames, e->cfg.image_size, d_out, static_cast<cudaStream_t>(cuda_stream));
 }
 
